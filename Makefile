@@ -1,7 +1,7 @@
-# Builds libfi_epp.so (sm_100a CUDA + host C++) in-tree, and the CPU oracle.
+# Builds libfi_epp.so (sm_90a CUDA + host C++) in-tree, and the CPU oracle.
 NVCC ?= /usr/local/cuda/bin/nvcc
 CXX ?= g++
-ARCH := -gencode arch=compute_100a,code=sm_100a
+ARCH := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC,-Wall,-Wextra,-Wno-unused-parameter -Xptxas -v
 CSRC := fusioninfer_b200/csrc
 OBJDIR := build

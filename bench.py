@@ -2,7 +2,7 @@
 """bench.py — routing decisions/s of the prefix-cache-aware Endpoint Picker hot path.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
-                    [--cfg 2|3|4|5] [--mode replicas|sharded] [--scale F]
+                    [--cfg 2|3|4|5] [--mode replicas|sharded] [--scale F] [--dump-outputs DIR]
 
 One "step" = one pass of the hot path (hash → index lookup → weighted score → argmax)
 over one batch of synthetic requests.  Default workload = BASELINE.json's headline
@@ -16,8 +16,8 @@ Prints ONE JSON line (rank 0):
   roofline  dominant kernel: algorithmic bytes per launch ÷ its CUDA-event duration,
             against MEASURED_PEAKS.json's HBM copy bandwidth
   cpu_baseline  the CPU oracle (C++ restatement of the upstream algorithm; the
-            reference's Go path is neither in /root/reference nor compilable here,
-            SURVEY.md §0 F1/F2) timed on a bounded sample on the host cores
+            upstream Go path is not available to build, SURVEY.md §0 F1/F2) timed
+            on a bounded sample on the host cores
 
 Multi-GPU (torchrun, one rank per GPU): --mode replicas (default: the 1 024-endpoint
 pool fits one GPU, so every GPU is an independent replica serving its own batches —
@@ -42,9 +42,10 @@ if ROOT not in sys.path:
 import numpy as np  # noqa: E402
 
 METRIC = "routing decisions/sec (4K-tok prompts x 1024 endpoints); achieved HBM GB/s"
-ORACLE_LABEL = ("C++ restatement of the upstream EPP v1.2.1 algorithm (oracle/epp_oracle.cpp); the reference's Go "
-                "path is not in /root/reference and cannot be compiled here (SURVEY.md F1/F2); parity unpinned by "
+ORACLE_LABEL = ("C++ restatement of the upstream EPP v1.2.1 algorithm (oracle/epp_oracle.cpp); the upstream Go "
+                "path is not part of the project this one was modelled on (SURVEY.md F1/F2); parity unpinned by "
                 "reference tests")
+PICK_RECORD = np.dtype([("endpoint", "<u4"), ("match_blocks", "<u2"), ("n_blocks", "<u2"), ("score", "<f8")])
 
 
 def log(*a):
@@ -58,15 +59,15 @@ def measured_peak_gbs():
         with open(p) as f:
             return float(json.load(f)["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (copy, read+write)"
     except Exception:
-        return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md); MEASURED_PEAKS.json absent"
+        return 3350.0, "fallback 3.35 TB/s (H100 SXM data sheet HBM3 bandwidth); MEASURED_PEAKS.json absent"
 
 
 class ClockSampler:
     """SM clock + throttle reasons around and DURING the timed region: in-process NVML, one sample right
     before the region, one every 10 ms inside it (the default run's region is ~30 ms — too short for
     `nvidia-smi -lms`), one right after; nvidia-smi as fallback.  Only the rank that prints the line samples
-    (its own GPU), and sparsely: NVML calls contend with kernel launches on the driver — every rank polling at
-    2 kHz took a 4-rank sharded step from 0.29 to 0.78 ms, rank 0 alone at 500 Hz still to 0.43 ms."""
+    (its own GPU), and sparsely: NVML calls contend with kernel launches on the driver, so frequent polling on
+    every rank slows a multi-rank step."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -195,16 +196,6 @@ def algorithmic_bytes(wl, picks_nprobe_total, R, E_local, hashed_requests=None):
     return {"hash_blocks": hr * 4 * wl.T, "match_pick": picks_nprobe_total * (8 + E_local / 8.0) + 16.0 * R}
 
 
-def load_traffic():
-    """dram bytes per launch of the dominant kernels from the committed ncu summary, if any."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        with open(p) as f:
-            return json.load(f)
-    except Exception:
-        return {}
-
-
 def host_cores():
     """Cores the CPU legs may use: the affinity mask capped by the cgroup CPU quota (os.cpu_count() ignores both)."""
     from oracle import epp_oracle as eo
@@ -302,8 +293,8 @@ def workload_config(wl, cfg_id, parallelism):
 
 def bind_to_gpu_numa(local):
     """Run this rank on the cores of its GPU's NUMA node while it allocates and fills its pinned host buffers
-    (pages are placed where the allocating thread runs), so that they are local to the GPU's PCIe root: on the
-    8-GPU node GPUs 4-7 hang off NUMA node 1 (round 1: e2e 6.19 ms/step at N = 8 vs 5.04 at N = 1).
+    (pages are placed where the allocating thread runs), so that they are local to the GPU's PCIe root: on a
+    two-socket node the GPUs of the second socket hang off another NUMA node than those of the first.
     Returns (note for the JSON line, function that restores the original affinity)."""
     try:
         original = os.sched_getaffinity(0)
@@ -512,9 +503,22 @@ class Scenario:
                 self.submit(i)
             self.submit_us = (time.perf_counter() - t0) * 1e6 / max(k, 1)  # host time per submit (launch-bound if ~ the step)
             self.picker.pick_wait(self.stream)
+            self.last_out = self.d_outs[(k - 1) & 1]
         else:
             for i in range(k):
                 self.step(i)
+            self.last_out = self.d_out
+
+    def dump_last_outputs(self, out_dir):
+        """The picks of the last step run_steps made, one array per record field, as DIR/<field>.npy (float64:
+        endpoint ids and block counts are exact in it)."""
+        import torch
+
+        torch.cuda.synchronize()
+        picks = self.last_out.cpu().numpy().view(PICK_RECORD).reshape(self.wl.R, self.P)
+        os.makedirs(out_dir, exist_ok=True)
+        for name in PICK_RECORD.names:
+            np.save(os.path.join(out_dir, f"{name}.npy"), picks[name].astype(np.float64))
 
     def time_steps(self, steps, warmup, pipelined=False, clocks=None):
         """-> (ms per step: CUDA events on the launching stream, max over ranks; launches of this library)"""
@@ -661,7 +665,12 @@ def main():
                     help="how the main run's index was built (the default run reports all three in roofline.index_order)")
     ap.add_argument("--churn-rounds", type=int, default=6, help="pick + indexer.Add rounds that age the 'churned' index")
     ap.add_argument("--extra-steps", type=int, default=30)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the picks of the last timed step as DIR/<field>.npy (float64), for comparing two builds "
+                         "output for output on the same seeded inputs")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl == "reference":
+        ap.error("--dump-outputs writes the GPU path's picks; --impl reference times the CPU oracle on a sample")
 
     from fusioninfer_b200 import synth
 
@@ -718,6 +727,8 @@ def main():
     ms_step, launches = sc.time_steps(args.steps, args.warmup, pipelined,
                                       clocks if (rank == 0 and os.environ.get("FI_BENCH_NO_CLOCKS") != "1") else None)
     clk = clocks.stop()
+    if args.dump_outputs and rank == 0:
+        sc.dump_last_outputs(args.dump_outputs)
     units = R * (world if mode == "replicas" else 1)
     value = units / (ms_step * 1e-3)
     stream_ordered = None
@@ -735,18 +746,17 @@ def main():
     alg = algorithmic_bytes(wl, nprobe_per_step, R, sc.count, hashed)
     dom = max(("hash_blocks", "match_pick"), key=lambda k: avg_ms[k])
     achieved = alg[dom] / (avg_ms[dom] * 1e-3) / 1e9 if avg_ms[dom] else 0.0
-    traffic = load_traffic() if (cfg_id == 3 and mode == "replicas" and args.scale == 1.0) else {}  # captured for cfg 3 only
     step_alg = alg["hash_blocks"] + alg["match_pick"]
     roofline = {
         "bound": "hbm", "kernel": dom, "achieved": achieved, "peak": peak, "unit": "GB/s",
-        "frac": achieved / peak if peak else None, "traffic": traffic.get(dom),
+        "frac": achieved / peak if peak else None,
         "peak_source": peak_src + " (burst figure: kernel timed alone with CUDA events)",
         "algorithmic_bytes_per_launch": alg[dom],
         "kernel_ms": avg_ms, "n_probe_per_decision": nprobe_per_step / R,
         "step_algorithmic_gbs": step_alg / (ms_step * 1e-3) / 1e9,
         "step_frac": step_alg / (ms_step * 1e-3) / 1e9 / peak,
-        "other_kernels": {k: {"achieved": (alg[k] / (avg_ms[k] * 1e-3) / 1e9 if avg_ms[k] else 0.0),
-                              "traffic": traffic.get(k)} for k in ("hash_blocks", "match_pick") if k != dom},
+        "other_kernels": {k: {"achieved": (alg[k] / (avg_ms[k] * 1e-3) / 1e9 if avg_ms[k] else 0.0)}
+                          for k in ("hash_blocks", "match_pick") if k != dom},
         "index": sc.index_stats, "index_order_of_value": args.index_order, "stream_ordered": stream_ordered,
     }
 

@@ -1,4 +1,4 @@
-"""fusioninfer_b200 — B200-native prefix-cache-aware Endpoint Picker hot path.
+"""fusioninfer_b200 — H100-native prefix-cache-aware Endpoint Picker hot path.
 
 One path only (BASELINE.json north_star, SURVEY.md §8): hash prompts into chained
 block keys → look them up in a GPU-resident (endpoint, block-hash) index →

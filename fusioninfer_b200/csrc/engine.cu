@@ -133,7 +133,7 @@ struct fi_epp {
   fi_epp_config cfg;
   std::mutex mu;
   std::string err;
-  int sm_count = 148;
+  int sm_count = 132;
   uint32_t MP = 0;  // chain pitch
   uint32_t W = 0;   // words per index row
   uint32_t P = 0;   // profiles
@@ -160,15 +160,16 @@ struct fi_epp {
   uint64_t pipe_seq = 0;          // batches submitted
   uint32_t pipe_hash_ctas = 0;    // per-SM caps of the pipelined path's two co-running kernels (0 = uncapped);
   uint32_t pipe_match_ctas = 0;   // FI_EPP_PIPE_HASH_CTAS / FI_EPP_PIPE_MATCH_CTAS, option "pipe_hash_ctas" / "pipe_match_ctas"
-  // SM-partitioned pipeline (green contexts, CUDA 12.4+): the chain walk is serial latency that fills 6 % of the
-  // warp slots but cannot share schedulers with a busy kernel (it slows 3x), so nothing overlapped it and every
-  // batch paid its 27 us.  With the GPU split into a 40-SM partition for the walker (three or four of its warps per
-  // scheduler) and a 108-SM partition for hash_blocks / match_pick, batch k is matched while batch k+1's chains
-  // are walked and batch k+2 is hashed: three batches in flight, 131 -> 116 us per batch.
-  // FI_EPP_PIPE_PARTITION=<SMs> / option "pipe_partition" (0 = off: two batches in flight on the whole GPU).
-  // SMs asked for the walker partition.  Measured at cfg 3 (us per step; no partition: 131.1): 8 -> 240, 16 -> 125.6,
-  // 24 -> 123.0, 32 -> 129.0, 40 -> 116.2 (three runs), 48 -> 124.3, 56 -> 133.7
-  int part_want = 40;
+  // SM-partitioned pipeline (green contexts, CUDA 12.4+): the chain walk is serial latency that fills a few % of
+  // the warp slots but cannot share schedulers with a busy kernel, so without a partition nothing overlaps it.
+  // With the GPU split into a partition for the walker and one for hash_blocks / match_pick, batch k is matched
+  // while batch k+1's chains are walked and batch k+2 is hashed: three batches in flight.
+  // FI_EPP_PIPE_PARTITION=<SMs> / option "pipe_partition": SMs asked for the walker partition (0 = off: two
+  // batches in flight on the whole GPU).  Off by default: on an H100 (132 SMs) hash_blocks dominates the step
+  // and loses more on the smaller partition than the overlapped walk saves.  Measured at cfg 3 on one H100 SXM
+  // (700 W), us per step: off 219.7; 24 -> 261.5, 32 -> 255.1, 40 -> 259.1, 48 -> 256.7, 56 -> 261.5; with the
+  // L1-allocating prompt loads of hash_kernels.cu: off 201.0-201.5, 40 -> 243.9-245.6.
+  int part_want = 0;
   int part_compact = -1;        // walker shape on the partition: -1 = the 64-register shape only where the 78-register one does
                                 // not fit (fewer than 24 SMs); FI_EPP_WALK_COMPACT=0/1 forces it
   int part_state = 0;           // 0: not tried, 1: active, -1: unavailable (fallback to the unpartitioned pipeline)
@@ -202,8 +203,8 @@ struct fi_epp {
   uint8_t* d_xchg = nullptr;     // this rank's exchange buffer
   volatile uint32_t* h_xerr = nullptr;  // poll-timeout flag of the exchange (mapped pinned host word the kernels set)
   void* peer_ipc[FI_MAX_RANKS] = {};  // mappings opened with cudaIpcOpenMemHandle (closed in destroy)
-  // sharded mode: every rank hashes every prompt (the default: 149 vs 141 M decisions/s at cfg 4 on 8 GPUs, 131 vs
-  // 119 on 2 — hashing 16 KiB from local HBM costs less than receiving 2 KiB of chain over NVLink); FI_EPP_SHARD_HASH=
+  // sharded mode: every rank hashes every prompt (the default: hashing 16 KiB from local HBM is expected to cost
+  // less than receiving 2 KiB of chain over NVLink; not measured on H100s, bench.py --gpus N times both); FI_EPP_SHARD_HASH=
   // split / option "shard_hash" = 1: every rank hashes R/world requests and the chains are all-gathered
   bool split_hash = false;
   uint32_t chain_rows = 0;  // rows allocated in d_chain / d_pre / d_nblocks (max_batch padded for the gather)
@@ -685,7 +686,7 @@ int alloc_dev_lru(fi_epp* h) {
   // conservative sub-batch + tombstones); a table takes a batch's DISTINCT keys on top of its entries, and an
   // endpoint that attracts a popular prefix can receive a large share of a batch — so the tables get as much as
   // a quarter of the free HBM buys, up to 32 C slots (1 Mi slots = 16 MiB per endpoint at lruCapacityPerServer
-  // 31 250: 17 GB for 1 024 endpoints of a B200's 180).  Option "lru_table_slots" / FI_EPP_LRU_TABLE_SLOTS pins it.
+  // 31 250: 17 GB for 1 024 endpoints, a fifth of an H100's 80).  Option "lru_table_slots" / FI_EPP_LRU_TABLE_SLOTS pins it.
   d.L = std::max<uint32_t>(pow2_ceil32(4u * C), 64u);
   const uint32_t ts_min = d.L;
   uint32_t ts = pow2_ceil32(32u * C);
@@ -1387,14 +1388,14 @@ void setup_partition(fi_epp* h) {
     return;
   }
   // hash_blocks(k+2) and match_pick(k) become runnable at the same moment (both wait for match_pick(k-1)) and share
-  // the big partition; which of them gets its CTAs resident first decided the step — 116 us on some boxes, 138 us
-  // on others with the same code.  Stream priorities make the block scheduler prefer one of them whenever SMs free
-  // up (FI_EPP_PIPE_PRIO=match | hash | none).
+  // the big partition; with one hashing CTA per request, which of them gets its CTAs resident first can decide the
+  // step.  Stream priorities make the block scheduler prefer one of them whenever SMs free up
+  // (FI_EPP_PIPE_PRIO=match | hash | none; none by default).
   int prio_lo = 0, prio_hi = 0;
   cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);  // lo = least (numerically greatest), hi = greatest priority
   int pa = 0, pb = 0;
   const char* pe = std::getenv("FI_EPP_PIPE_PRIO");
-  const std::string prio = pe ? pe : "none";  // (measured on a 116-us box: none 116.1, hash 116.2, match 121.2 us)
+  const std::string prio = pe ? pe : "none";
   if (prio == "match") {
     pa = prio_lo;
     pb = prio_hi;
@@ -1456,11 +1457,10 @@ int submit_pick_partitioned(fi_epp* h, const uint8_t* d_prompts, const uint64_t*
     LaunchScope ls(h, h->s_pa, K_HASH);
     // (the kernel also zeroes the request-queue counter of this batch's match_pick: one runtime call less per batch)
     // hash_blocks runs as 4 persistent CTAs per SM here (FI_EPP_PIPE_HASH_CTAS / option "pipe_hash_ctas" overrides;
-    // a large value = one CTA per request).  With one CTA per request the step is bimodal: 116 us on most boxes,
-    // 138 us on others (among them the 8-GPU node) with the same binary — depending on which of the two kernels
-    // gets its CTAs resident first, hash_blocks' 16 384 short CTAs and match_pick's 324 long ones (80 registers
-    // x 256 threads x 3 per SM) lock each other out of the SMs.  Four hashing CTAs (32 K registers) always leave
-    // room for one matching CTA next to them: 122.6-123.3 us on both kinds of box.
+    // a large value = one CTA per request).  With one CTA per request the step depends on which of the two kernels
+    // gets its CTAs resident first: hash_blocks' 16 384 short CTAs and match_pick's long ones (80 registers x 256
+    // threads x 3 per SM) can lock each other out of the SMs.  Four hashing CTAs (32 K registers) always leave room
+    // for one matching CTA next to them.
     const uint32_t hash_ctas = h->pipe_hash_ctas ? h->pipe_hash_ctas : 4u;
     FI_CUDA(launch_hash_blocks(d_prompts, d_offsets, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, pre, nb,
                                hash_ctas * (uint32_t)h->part_main_sms, h->s_pa, h->d_work + 8 + s3));
@@ -1564,7 +1564,7 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
                                h->pipe_hash_ctas * (uint32_t)h->sm_count, h->s_a));
   }
   // The chain walk is serial latency — a warp per scheduler that wants an issue slot every few cycles — and
-  // runs 3x slower next to a busy kernel (measured: 30 -> 100 us under match_pick), so it waits for the
+  // slows several-fold next to a busy kernel that competes for the same schedulers, so it waits for the
   // previous batch's match to drain; what overlaps is this batch's block hashing with that match.
   if (h->pipe_seq >= 1) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot ^ 1u], 0));
   {
@@ -1831,10 +1831,6 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
   if (const char* e = std::getenv("FI_EPP_PIPE_PARTITION")) {
     h->part_want = (int)std::strtol(e, nullptr, 10);
   }
-  // (8 ranks on the 8-GPU node ran the partitioned pipeline at 138.5 us per batch with one hashing CTA per request,
-  // slower than unpartitioned (133.4 us).  That was first taken for host starvation — 16 cgroup cores for 8 ranks —
-  // and the partition switched off there; a single-GPU box then showed the same 138 us with one rank: it is the
-  // bimodal co-scheduling that the 4-CTA hashing default removes, so the partition stays on at any rank count.)
   if (const char* e = std::getenv("FI_EPP_WALK_COMPACT")) h->part_compact = std::strtol(e, nullptr, 10) != 0 ? 1 : 0;
   if (const char* e = std::getenv("FI_EPP_PIPE_HASH_CTAS")) h->pipe_hash_ctas = (uint32_t)std::strtol(e, nullptr, 10);
   if (const char* e = std::getenv("FI_EPP_PIPE_MATCH_CTAS")) h->pipe_match_ctas = (uint32_t)std::strtol(e, nullptr, 10);

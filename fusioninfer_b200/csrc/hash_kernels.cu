@@ -1,4 +1,4 @@
-// hash_kernels.cu — batched token-block hashing for sm_100a (integer, HBM-stream bound).
+// hash_kernels.cu — batched token-block hashing for sm_90a (integer, HBM-stream bound).
 //
 // Computes the chained block keys of SURVEY.md Appendix A.1 (upstream
 // prefix.hashPrompt; block size / cap from /root/reference/pkg/router/
@@ -22,7 +22,7 @@ __device__ __forceinline__ uint64_t pack64(uint32_t lo, uint32_t hi) { return (u
 
 // Prompt bytes are read exactly once: stream them through L2 with an evict-first policy so they
 // do not push out the index rows/keys of the popular prefixes, which the match kernel re-reads
-// every batch (its latency is L2-hit-rate bound; the hot set is ~80 MB of the 126 MB L2).
+// every batch (its latency is L2-hit-rate bound, and the 50 MB L2 of an H100 holds only part of the hot set).
 __device__ __forceinline__ uint64_t make_evict_first_policy() {
   uint64_t pol;
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;\n" : "=l"(pol));
@@ -30,7 +30,7 @@ __device__ __forceinline__ uint64_t make_evict_first_policy() {
 }
 __device__ __forceinline__ uint4 ld_stream_v4(const uint4* p, uint64_t pol) {
   uint4 v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;\n"
+  asm volatile("ld.global.nc.L1::evict_first.L2::cache_hint.v4.u32 {%0, %1, %2, %3}, [%4], %5;\n"
                : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w)
                : "l"(p), "l"(pol));
   return v;
@@ -39,25 +39,18 @@ __device__ __forceinline__ uint4 ld_stream_v4(const uint4* p, uint64_t pol) {
 // Pre-state layout: tiled request-minor within groups of 32 requests, in 16-byte units
 // (two consecutive blocks):  unit u of request r lives at  ((r/32)*MP2 + u)*32 + r%32.
 // The chain walker (one lane per request) then reads 512 contiguous bytes per warp load — 4 L1TEX
-// wavefronts instead of the 32 of a row-major layout, which saturated the wavefront rate
-// (measured: 17.6 of the kernel's 45 us were those loads).
+// wavefronts instead of the 32 of a row-major layout, which would saturate the wavefront rate.
 __device__ __forceinline__ uint64_t pre_index(uint32_t r, uint32_t i, uint32_t MP2) {
   return ((((uint64_t)(r >> 5) * MP2 + (i >> 1)) * 32 + (r & 31)) << 1) + (i & 1);
 }
 
-// one 32-byte stripe per load: every lane fetches whole 32-byte sectors exactly once (with 16-byte loads the
-// two halves of a sector were requested by two instructions, and with L1::no_allocate both went to L2: ncu
-// counted 2x the prompt bytes between L2 and L1)
+// one 32-byte stripe = two 16-byte loads: 128 bits is the widest global load of sm_90.  The loads allocate in L1
+// (evict-first) so that the second half of each 32-byte sector is an L1 hit: with L1::no_allocate both halves went
+// to L2: at cfg 3 on one H100 SXM (700 W), hash_blocks took 121-123 us that way against 105-107 us with these
+// loads (one run alternating the two builds, two bench runs each).
 struct Stripe {
   uint32_t w[8];
 };
-__device__ __forceinline__ Stripe ld_stream_v8(const void* p, uint64_t pol) {
-  Stripe v;
-  asm volatile("ld.global.nc.L1::no_allocate.L2::cache_hint.v8.u32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8], %9;\n"
-               : "=r"(v.w[0]), "=r"(v.w[1]), "=r"(v.w[2]), "=r"(v.w[3]), "=r"(v.w[4]), "=r"(v.w[5]), "=r"(v.w[6]), "=r"(v.w[7])
-               : "l"(p), "l"(pol));
-  return v;
-}
 __device__ __forceinline__ void xacc2_stripe(XAcc2& a, const Stripe& q) {
   a.v1 = xround2(a.v1, U2{q.w[0], q.w[1]});
   a.v2 = xround2(a.v2, U2{q.w[2], q.w[3]});
@@ -83,19 +76,8 @@ __global__ void __launch_bounds__(256, STRIPES <= 2 ? 8 : 5) hash_blocks_kernel(
     const uint32_t n = nb64 > M ? M : (uint32_t)nb64;
     if (threadIdx.x == 0) nblocks[r] = n;
     const uint8_t* base = prompts + off;
-    const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(base) & 31);
+    const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(base) & 15);
     if (mis == 0) {
-      for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
-        const uint8_t* p = base + (uint64_t)i * B;
-        Stripe q[STRIPES];
-#pragma unroll
-        for (int s = 0; s < STRIPES; ++s) q[s] = ld_stream_v8(p + 32 * s, pol);
-        XAcc2 a = xacc2_init();
-#pragma unroll
-        for (int s = 0; s < STRIPES; ++s) xacc2_stripe(a, q[s]);
-        pre[pre_index(r, i, MP2)] = xacc2_finish(a, (uint64_t)B + 8);
-      }
-    } else if ((mis & 15) == 0) {
       for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
         const uint4* p = reinterpret_cast<const uint4*>(base + (uint64_t)i * B);
         uint4 q[2 * STRIPES];
@@ -173,10 +155,9 @@ __global__ void __launch_bounds__(256) hash_blocks_any_kernel(const uint8_t* __r
 }
 
 // One lane per request, one warp per group of 32 requests: h_i = chain_step(pre_i, h_{i-1}), in
-// groups of 8 links.  The walk is a pure dependency chain — 40 integer instructions per link, 5 dependent
-// 64-bit multiplies, ~110 cycles by ptxas' own stall counts — run by ONE warp per scheduler, in order: every
-// other instruction in the loop and every scoreboard wait adds straight to the batch's critical path (ncu,
-// round 1: 59 instructions and 222 cycles per link).  What the loop is built around:
+// groups of 8 links.  The walk is a pure dependency chain — 5 dependent 64-bit multiplies per link — run by ONE
+// warp per scheduler, in order: every other instruction in the loop and every scoreboard wait adds straight to the
+// batch's critical path.  What the loop is built around:
 //   * pre-states are prefetched kAhead groups ahead with cp.async into a shared-memory ring (register
 //     prefetching does not work: ptxas puts every ring load on one counting scoreboard, so waiting for the
 //     oldest also waits for the newest; cp.async commit/wait groups have the needed "all but the N newest"
@@ -184,16 +165,16 @@ __global__ void __launch_bounds__(256) hash_blocks_any_kernel(const uint8_t* __r
 //     iteration), so neither the wait nor the shared-memory latency sits between two links;
 //   * each lane stores its 8 hashes straight to its chain row as four 16-byte stores (row-major [r][i]: what
 //     the match kernel stages and chains_out returns) — but one group LATE, at the top of the next iteration,
-//     from registers nothing else writes for a whole group.  Stored right after the links (first version of
-//     this kernel: 197 cycles per link) the four scattered STG.128 shared one set of data registers, and each
-//     had to wait for the previous one's operand read behind 32 L1 wavefronts;
+//     from registers nothing else writes for a whole group.  Stored right after the links, the four scattered
+//     STG.128 would share one set of data registers, and each would
+//     have to wait for the previous one's operand read behind 32 L1 wavefronts;
 //   * the loop is unrolled by two groups with the register roles swapped, so no buffer is ever copied;
 //   * the buffers are padded to whole groups (MP % 8 == 0): no per-unit predicates.
 // Entries [n, MP) of every row are zeroed.
 // kRing ring slots, prefetch distance kRing - 1 groups.  Two shapes: RING = 4 with the whole register file (one warp
-// per scheduler on 128 SMs: nothing else hides the pre-state loads), and RING = 3 capped at 64 registers / 24 KB so
-// that ALL 128 CTAs fit on the 16 SMs of the pipelined path's walker partition (eight warps per scheduler hide each
-// other's latency there).
+// per scheduler when the 128 CTAs of a 16 384-request batch spread over the whole GPU: nothing else hides the
+// pre-state loads), and RING = 3 capped at 64 registers / 24 KB so that all 128 CTAs fit on a walker partition of
+// 16 SMs (eight warps per scheduler hide each other's latency there).
 
 __device__ __forceinline__ void cp_async16_cg(void* smem, const void* gmem) {
   const unsigned sa = (unsigned)__cvta_generic_to_shared(smem);

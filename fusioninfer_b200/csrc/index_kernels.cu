@@ -1,5 +1,5 @@
 // index_kernels.cu — GPU-resident open-addressed hash index of (endpoint, block-hash)
-// membership, sm_100a.
+// membership, sm_90a.
 //
 // Logical content = upstream's prefix indexer (SURVEY.md Appendix A.2: hashToPods),
 // physically a table keyed by block hash whose value is a bitset row over the local
@@ -280,7 +280,7 @@ __global__ void __launch_bounds__(256) index_contains_kernel(IndexView ix, const
 
 inline unsigned grid_for(uint64_t n) {
   uint64_t g = (n + 255) / 256;
-  if (g > 148ull * 16) g = 148ull * 16;
+  if (g > 132ull * 16) g = 132ull * 16;  // 16 CTAs per SM of an H100
   if (g == 0) g = 1;
   return (unsigned)g;
 }

@@ -1,10 +1,9 @@
-// lru_kernels.cu — the per-endpoint LRU of block hashes, resident on the GPU (sm_100a).
+// lru_kernels.cu — the per-endpoint LRU of block hashes, resident on the GPU (sm_90a).
 //
 // Upstream keeps one LRU per pod (podToLRU, SURVEY.md Appendix A.2; capacity lruCapacityPerServer,
 // /root/reference/pkg/router/strategy.go:59,149) and runs indexer.Add(chain, pod) for every routed request.
-// On a host that is a pointer chase per block — a few DRAM misses each, ~95 M touches/s on the 16 usable
-// cores of the GPU box, 330 K decisions/s at 256 blocks per prompt — three orders of magnitude below the pick
-// rate.  Here the recency order lives in HBM next to the index and a whole batch of Adds is applied by a handful
+// On a host that is a pointer chase per block — a few DRAM misses each — orders of magnitude below the pick
+// rate at 256 blocks per prompt.  Here the recency order lives in HBM next to the index and a whole batch of Adds is applied by a handful
 // of wide kernels; only the request → endpoint assignment (two small arrays) comes from the host.
 //
 // Exactness.  An LRU of capacity C always holds the C most recently touched distinct keys, whatever it evicted
@@ -17,7 +16,7 @@
 // in between.
 //
 // Capacity.  A table takes the batch's distinct keys on top of its C entries; it holds 0.85 TS, with TS between
-// 4 C and 32 C slots depending on how much HBM is free (engine.cu: a B200 gives 1 024 endpoints 1 Mi slots each).
+// 4 C and 32 C slots depending on how much HBM is free (engine.cu: sized at handle creation from the free HBM).
 // An endpoint that receives more NEW distinct keys than that in a single batch is detected while inserting
 // (slots are reserved before they are claimed), its touches are rolled back and its requests are re-run in
 // sub-batches of at most C touches, which always fit (lru_plan.h; endpoints are independent of each other, so

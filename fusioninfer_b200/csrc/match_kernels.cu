@@ -1,5 +1,5 @@
 // match_kernels.cu — batched longest-prefix-match + weighted score + warp-shuffle
-// argmax over all endpoints, sm_100a.  Bound by per-warp latency (dependent index / row reads and the
+// argmax over all endpoints, sm_90a.  Bound by per-warp latency (dependent index / row reads and the
 // counting arithmetic); no tensor cores (there is no dense contraction on this path).
 //
 // One warp per request (persistent grid, dynamic queue):
@@ -165,10 +165,9 @@ __device__ __forceinline__ void load_row_words(const uint32_t* __restrict__ p, b
 // 64 at a time, as a plain hash index would.
 // Returns m = number of leading blocks the index holds (the first miss, or n); s_node[0 .. m) = their nodes.
 //
-// (Round 1 resolved chunk c+1 while chunk c's rows were in flight: a request's serial chain was two dependent
-// memory round trips per 32 blocks, ~5 800 cycles per chunk and 23 us for a fully cached 256-block prompt — a
-// third of the whole kernel, which is how long the last such request kept the other warps waiting.  With the
-// nodes known up front the rows of a request are independent loads.)
+// (Resolving chunk c+1 while chunk c's rows are in flight makes a request's serial chain two dependent memory
+// round trips per 32 blocks, and the last fully cached prompt keeps the other warps waiting.  With the nodes
+// known up front the rows of a request are independent loads.)
 constexpr int kSpecTries = 4;
 constexpr int kSpecChunks = 8;  // chunks of 32 blocks verified per round (256 blocks; longer chains loop)
 
@@ -237,7 +236,7 @@ __device__ __forceinline__ uint32_t resolve_request_nodes(const IndexView& ix, c
 
 // next request of the launch's dynamic queue.  Plain PTX on purpose: for `if (lane == 0) atomicAdd(..)` the
 // compiler emits its warp-aggregated form — ATOMG followed at once by a SHFL of the result — which makes every
-// request wait out the atomic's round trip (15 % of the kernel's stall samples in round 1).  Here the result
+// request wait out the atomic's round trip.  Here the result
 // register is not touched until the shuffle at the end of the request.
 __device__ __forceinline__ uint32_t take_ticket(uint32_t* counter, uint32_t opaque_zero) {
   uint32_t t;
@@ -276,7 +275,7 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 ? FI_MATCH_MIN_BLOCKS :
   // while request r is matched, the ticket of the request after next is in flight, the chain of the next one is
   // being staged into the other buffer, and the home bucket of its first block is being fetched (lanes 0-3:
   // one key + node each) — a request starts with its chain and its first node already there instead of waiting
-  // out three dependent round trips (ticket -> chain -> table), a third of a request's time in round 1.
+  // out three dependent round trips (ticket -> chain -> table).
   const uint32_t row_units = p.MP / 2;  // 16-byte units of a chain row (rows are zero-padded to MP by the walker)
   auto stage = [&](uint32_t rr, uint64_t* dst) {
     const uint64_t* crow = p.chain + (uint64_t)rr * p.MP;
@@ -793,9 +792,9 @@ cudaError_t launch_match_t(const MatchParams& p, int sm_count, cudaStream_t s) {
 cudaError_t launch_match_pick(const MatchParams& p, int sm_count, cudaStream_t s) {
   if (p.R == 0) return cudaSuccess;
   // Words per row = LPR * VEC.  Two words per lane (half the counter registers of VEC = 4 -> three CTAs
-  // = 24 warps per SM instead of 16) is the measured optimum since lookups stopped saturating the memory
-  // system: the kernel is bound by per-warp instruction latency and wants warps, not wide loads
-  // (E = 1024: 76 us vs 88 us; FI_EPP_MATCH_VEC=4 selects the four-word shape there for comparison).
+  // = 24 warps per SM instead of 16): the kernel is bound by per-warp instruction latency and wants warps, not
+  // wide loads (E = 1024, cfg 3 on one H100 SXM, 700 W: match_pick 74.5 us with two words per lane vs 98.1-98.4 us with four, two runs each; FI_EPP_MATCH_VEC=4 selects the four-word shape
+  // there for comparison).
   static const int vec = [] { const char* e = std::getenv("FI_EPP_MATCH_VEC"); return e ? std::atoi(e) : 2; }();
   switch (p.ix.W) {
     case 1: return launch_match_t<1, 1>(p, sm_count, s);

@@ -1,4 +1,4 @@
-// xxh64.cuh — XXH64 arithmetic shared by the sm_100a kernels and the host side of
+// xxh64.cuh — XXH64 arithmetic shared by the sm_90a kernels and the host side of
 // libfi_epp (chain seed h0, host unit checks).  Pure integer; no tensor cores.
 //
 // Follows the public xxHash specification (SURVEY.md Appendix A.7), the function

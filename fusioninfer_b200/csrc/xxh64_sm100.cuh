@@ -1,13 +1,12 @@
 // xxh64_sm100.cuh — the XXH64 arithmetic of xxh64.cuh (same functions, same results bit for bit) written on
-// 32-bit halves for the SASS it should become on sm_100a.  Device only; xxh64.cuh stays the host/device
+// 32-bit halves for the SASS it should become on sm_90a.  Device only; xxh64.cuh stays the host/device
 // definition the oracle-facing unit tests pin.
 //
-// Why: nvcc turns the 28 64-bit constant multiplies of a 64-byte block into ~136 IMADs (it splits the rotates
-// into extra products and moves halves around with IMAD.MOV / IMAD.IADD: 260 instructions per block, 65 % issue
-// utilisation while the HBM stream idles at 58 %), and a chain link into 59 instructions that a lone warp issues
-// at one per two cycles (tools/microbench/chainlat: 126 cycles per link, and two independent chains in one
-// thread take twice as long: the walk is issue-bound, not latency-bound).  Spelled as IMAD.WIDE + IMADs (addend
-// folded in) and two funnel shifts per rotate, a block costs ~165 instructions and a link 33.
+// Why: nvcc turns the 64-bit constant multiplies of a block into many more IMADs than they need (it splits the
+// rotates into extra products and moves halves around with IMAD.MOV / IMAD.IADD), and the chain walk is
+// issue-bound rather than latency-bound (tools/microbench/chainlat: two independent chains in one thread take
+// twice as long as one).  Spelled as IMAD.WIDE + IMADs (addend folded in) and two funnel shifts per rotate, a
+// block and a link take far fewer instructions.
 #pragma once
 #include <stdint.h>
 #include "xxh64.cuh"
@@ -61,7 +60,7 @@ __device__ __forceinline__ uint64_t xacc2_finish(const XAcc2& a, uint64_t total_
 
 // ---- the serial link --------------------------------------------------------------------------------------
 // x * P + a with the high half as ONE three-input add of independent products: lo after 1 IMAD.WIDE, hi after
-// IMAD + IADD3 (9 cycles instead of the 12 of three chained IMADs) — the form for the chain walker, where a lone
+// IMAD + IADD3 (two dependent steps instead of three chained IMADs) — the form for the chain walker, where a lone
 // warp per scheduler runs one dependency chain and the latency of every product is on the batch's critical path
 template <uint64_t P>
 __device__ __forceinline__ U2 mulc_par(U2 x, U2 a) {

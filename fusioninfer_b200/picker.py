@@ -5,7 +5,7 @@ ONE path this repo implements: it is configured from the EndpointPickerConfig
 YAML that FusionInfer's router role generates
 (/root/reference/pkg/router/strategy.go:27-165), receives pod-state refreshes
 and prefix-index updates, and schedules batches of requests.  Every call goes
-through include/fi_epp.h into the sm_100a kernels; nothing is computed in Python.
+through include/fi_epp.h into the sm_90a kernels; nothing is computed in Python.
 """
 from __future__ import annotations
 

@@ -1,5 +1,5 @@
 /*
- * fi_epp.h — C ABI of the B200-native prefix-cache-aware Endpoint Picker.
+ * fi_epp.h — C ABI of the H100-native prefix-cache-aware Endpoint Picker.
  *
  * This is the drop-in boundary for the ONE hot path this repo implements
  * (BASELINE.json north_star; SURVEY.md §8): per request, hash the prompt into
@@ -358,8 +358,8 @@ int fi_epp_comm_init(fi_epp* h, const uint8_t id[FI_EPP_UNIQUE_ID_BYTES], uint32
  * pick into every rank's buffer over NVLink peer memory / CUDA IPC and the merge kernel polls tagged words —
  * no collective call for the reduction) or FI_EXCHANGE_NCCL (one ncclAllGather: env FI_EPP_EXCHANGE=nccl,
  * more than 16 ranks, or a rank that cannot map a peer's buffer).  Every rank hashes every prompt (env
- * FI_EPP_SHARD_HASH=split: hashing split over the ranks and the chains all-gathered instead — slower on NVLink-
- * connected B200s: 16 KiB from local HBM cost less than 2 KiB over the link). */
+ * FI_EPP_SHARD_HASH=split: hashing split over the ranks and the chains all-gathered instead — measured slower on
+ * NVLink-connected GPUs: hashing 16 KiB from local HBM costs less than receiving 2 KiB over the link). */
 #define FI_EXCHANGE_NONE 0
 #define FI_EXCHANGE_PEER 1
 #define FI_EXCHANGE_NCCL 2
@@ -372,7 +372,7 @@ int fi_epp_comm_exchange(fi_epp* h);
  *   "lru_table_slots"  slots per endpoint table of the device LRU (0 = sized by free HBM, 4..32 x lru_capacity)
  *   "feed_slices"  slices of a host-buffer pick's prompt copy, 1..16 (default 8)
  *   "lru_threads"  host worker threads of fi_epp_index_add_chains (takes effect at the next call)
- *   "pipe_partition"  SMs of the chain-walk partition of the pipelined path (default 40; 0 = no partition)
+ *   "pipe_partition"  SMs of the chain-walk partition of the pipelined path (default 0 = no partition)
  *   "pipe_hash_ctas", "pipe_match_ctas"  CTAs per SM of the two kernels the pipelined path runs side by side (0 = default:
  *                  partitioned GPU 4 hashing CTAs per SM, otherwise one CTA per request; match_pick as many as fit)
  *                  (fi_epp_pick_submit: batch k+1's block hashing next to batch k's match; 0 = uncapped)

@@ -1,4 +1,4 @@
-"""GPU (-m gpu): parity of the sm_100a path against the CPU oracle, through the C ABI.
+"""GPU (-m gpu): parity of the sm_90a path against the CPU oracle, through the C ABI.
 
 Bit-exact for every integer/byte/index output (block hashes, index membership,
 endpoint, match length) and for the fp64 score (compared as raw 64-bit patterns —
@@ -501,10 +501,11 @@ def test_pick_parity_after_churn_and_rebuild():
     gpu.close()
 
 
-@pytest.mark.parametrize("partition", [None, 0, 16])
+@pytest.mark.parametrize("partition", [None, 0, 16, 40])
 def test_pipelined_submit_equals_oracle_with_index_updates_in_between(partition):
     """fi_epp_pick_submit keeps two batches in flight (batch k+1 is hashed while batch k is matched) — three on a
-    partitioned GPU (the default where green contexts exist: chain walk on its own SMs; 0 = unpartitioned).  Seven
+    partitioned GPU (option pipe_partition = SMs of the chain walk's own partition: 16 runs the compact walker shape,
+    40 the full one; None = the default, unpartitioned, like 0).  Seven
     different batches of different sizes are submitted back to back, index updates and a pod-state refresh
     are interleaved (each batch must see the index and the pod states as of ITS submit call), stream-ordered
     picks are mixed in; after one fi_epp_pick_wait every output equals the oracle's."""
@@ -836,11 +837,13 @@ def test_device_lru_from_device_chains():
     gpu.close()
 
 
-@pytest.mark.parametrize("partition", [None, 0])
+@pytest.mark.parametrize("partition", [None, 0, 40])
 def test_pipelined_back_to_back_batches(partition):
     """Twelve batches of different sizes submitted back to back with nothing in between (so that the pipeline really
     has its two — partitioned GPU: three — batches in flight and reuses every slot buffer several times), one wait
-    at the end, every output equal to the oracle's; then the same again after a stream-ordered pick."""
+    at the end, every output equal to the oracle's; then the same again after a stream-ordered pick.  With a 40-SM
+    walker partition, R = 512 exceeds the 4 hashing CTAs per SM of the other partition, so hash_blocks' CTAs each
+    take several requests."""
     import torch
 
     wl = H.small_workload(E=200, R=512, T=2048, max_blocks=128)
@@ -877,8 +880,11 @@ def test_pipelined_back_to_back_batches(partition):
             tok, offs = wl.prompts(batch=99)
             assert H.picks_equal(gpu.pick_batch(tok, offs, wl.h0), cpu.pick_batch(tok, offs, wl.h0))
     info = gpu.pipeline_info()
-    if partition == 0:
+    if partition in (None, 0):
         assert not info["partitioned"]
+    else:
+        assert info["partitioned"] and info["walk_sms"] == partition, info
+        assert 4 * info["main_sms"] < max(sizes), info
     gpu.close()
 
 

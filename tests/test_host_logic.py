@@ -1,7 +1,7 @@
 """CPU: the product's host-side logic and the arithmetic its kernels share with the host.
 
 libfi_hostcheck.so is a host build of fusioninfer_b200/csrc/{xxh64.cuh,bitslice.cuh,lru.h}
-— the same headers the sm_100a kernels compile — so the split pre-state/chain-step
+— the same headers the sm_90a kernels compile — so the split pre-state/chain-step
 hashing, the bit-plane counters and the LRU are checked here without a GPU.
 """
 import ctypes as C
@@ -372,7 +372,7 @@ plugins:
   name: gpu-filter
   parameters:
     label: "nvidia.com/gpu.product"
-    validValues: ["B200"]
+    validValues: ["H100"]
 schedulingProfiles:
 - name: default
   plugins:
@@ -399,7 +399,7 @@ def test_config_by_label_with_arbitrary_labels_and_chained_filters():
     assert table[("fusioninfer.io/component-type", "decoder")] == abi.FI_ROLE_DECODER
     assert table[("fusioninfer.io/component-type", "worker")] == abi.FI_ROLE_WORKER
     za, zb = table[("topology.kubernetes.io/zone", "us-east-1a")], table[("topology.kubernetes.io/zone", "us-east-1b")]
-    gb = table[("nvidia.com/gpu.product", "B200")]
+    gb = table[("nvidia.com/gpu.product", "H100")]
     assert {za, zb, gb} == {8, 16, 32} and p.more_filters[0] == za | zb and p.more_filters[1] == gb
     # two filters on the same label with disjoint values: ANDed -> nothing passes (round 1 read that as "no filter")
     doc = PD_YAML.replace("  - pluginRef: prefill-pods\n", "  - pluginRef: prefill-pods\n  - pluginRef: decode-pods\n", 1)

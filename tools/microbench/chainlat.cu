@@ -1,6 +1,6 @@
 // chainlat.cu — how many cycles does ONE link of the block-hash chain cost a lone warp?
 // (chain_finalize_kernel measured ~200 cycles per link although ptxas' stall counts add up to ~115.)
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -I fusioninfer_b200/csrc -o tools/microbench/chainlat tools/microbench/chainlat.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I fusioninfer_b200/csrc -o tools/microbench/chainlat tools/microbench/chainlat.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 #include "xxh64.cuh"

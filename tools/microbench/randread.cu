@@ -1,6 +1,6 @@
-// randread.cu — random-read throughput/latency of B200 HBM vs table size, access size and
+// randread.cu — random-read throughput/latency of HBM vs table size, access size and
 // parallelism: grounds the latency model of the index lookups (keys: 32 B sectors, rows: 128 B).
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o randread randread.cu
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o randread randread.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -38,7 +38,7 @@ int main() {
     uint64_t mask16 = S / 16 - 1;
     for (int warps_per_sm : {8, 16, 32, 64}) {
       for (int variant = 0; variant < 4; ++variant) {
-        int grid = 148 * warps_per_sm / 8, block = 256, iters = 64;
+        int grid = 132 * warps_per_sm / 8, block = 256, iters = 64;
         float ms = 0; double bytes = 0; const char* name = "";
         for (int rep = 0; rep < 2; ++rep) {
           cudaEventRecord(e0);

@@ -38,7 +38,7 @@ int main() {
     uint4* tab; if (cudaMalloc(&tab, S) != cudaSuccess) { printf("alloc failed\n"); return 1; }
     cudaMemset(tab, 1, S);
     for (int wps : {16, 32, 64}) for (int mode = 0; mode < 3; ++mode) {
-      int grid = 148 * wps / 8, block = 256, iters = 64; float ms = 0;
+      int grid = 132 * wps / 8, block = 256, iters = 64; float ms = 0;
       for (int rep = 0; rep < 2; ++rep) {
         cudaEventRecord(e0);
         if (mode == 0) k<0, 8><<<grid, block>>>(tab, nrec, stride / 16, iters, 3 + rep, out);

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (read on the CPU box): per kernel, the metrics B200_PROFILING.md names."""
+"""Summarise an .ncu-rep: per kernel, the DRAM, L2 and issue metrics."""
 import csv, io, subprocess, sys
 
 rep = sys.argv[1]

@@ -1,5 +1,7 @@
 #!/usr/bin/env python
-"""Decode per-instruction stall counts (control bits 105..108, B300_MICROARCH.md) from
+"""Decode per-instruction stall counts (control bits 105..108 of the 128-bit instruction word: the layout of Volta
+through Hopper SASS, Jia et al., "Dissecting the NVIDIA Volta GPU Architecture via Microbenchmarking", 2018; on
+sm_90a builds the fields decode to stall counts of 0-15, barrier indices 0-5 and write barriers on the loads) from
 `cuobjdump -sass` output and sum them over an address range: a single-warp, in-order issue-time
 estimate for fixed-latency regions (e.g. the serial link of the chain walker).
 usage: sass_stalls.py <obj> <function-substring> [start_hex end_hex]"""
