@@ -158,8 +158,12 @@ struct fi_epp {
   cudaEvent_t ev_pick_own = nullptr;
   cudaEvent_t ev_plain = nullptr;  // completion of the most recent stream-ordered (not pipelined) pick
   uint64_t pipe_seq = 0;          // batches submitted
-  uint32_t pipe_hash_ctas = 0;    // per-SM caps of the pipelined path's two co-running kernels (0 = uncapped);
-  uint32_t pipe_match_ctas = 0;   // FI_EPP_PIPE_HASH_CTAS / FI_EPP_PIPE_MATCH_CTAS, option "pipe_hash_ctas" / "pipe_match_ctas"
+  // per-SM caps of the pipelined path's two co-running kernels (0 = uncapped); FI_EPP_PIPE_HASH_CTAS /
+  // FI_EPP_PIPE_MATCH_CTAS, option "pipe_hash_ctas" / "pipe_match_ctas".  The hash cap applies where stage A is
+  // hash_blocks (the partitioned pipeline, block sizes hash_chain does not take): hash_chain CTAs (32 to 128
+  // requests each) fill a whole SM, whatever the cap.
+  uint32_t pipe_hash_ctas = 0;
+  uint32_t pipe_match_ctas = 0;
   // SM-partitioned pipeline (green contexts, CUDA 12.4+): the chain walk is serial latency that fills a few % of
   // the warp slots but cannot share schedulers with a busy kernel, so without a partition nothing overlaps it.
   // With the GPU split into a partition for the walker and one for hash_blocks / match_pick, batch k is matched
@@ -976,10 +980,14 @@ int upload_lora(fi_epp* h) {
 // hash kernels for the request slice [r0, r0+R): prompts → chain (device buffers), on stream s
 int run_hash(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0, uint32_t r0,
              uint32_t R, cudaStream_t s) {
-  uint64_t* pre = h->d_pre + (size_t)r0 * h->MP;  // tiled by groups of 32 requests: r0 % 32 == 0
   uint64_t* chain = h->d_chain + (size_t)r0 * h->MP;
   uint32_t* nb = h->d_nblocks + r0;
-  if (h->fast_hash) {
+  if (hash_chain_fused(h->cfg.block_bytes)) {  // block hashing and chain walk in one kernel, no pre-states in HBM
+    LaunchScope ls(h, s, K_HASH);
+    FI_CUDA(launch_hash_chain(d_prompts, d_offsets + r0, d_h0 + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP,
+                              chain, nb, h->sm_count, s));
+  } else if (h->fast_hash) {
+    uint64_t* pre = h->d_pre + (size_t)r0 * h->MP;  // tiled by groups of 32 requests: r0 % 32 == 0
     {
       LaunchScope ls(h, s, K_HASH);
       FI_CUDA(launch_hash_blocks(d_prompts, d_offsets + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, pre, nb, 0, s));
@@ -1549,25 +1557,33 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
   uint64_t* chain = slot ? h->d_chain2 : h->d_chain;
   uint32_t* nb = slot ? h->d_nblocks2 : h->d_nblocks;
   // ---- stage A: inputs are ready in the caller's stream order; the slot's buffers are free once the
-  // match of two batches ago is done; d_pre is free once the previous plain pick (if any) is done
+  // match of two batches ago is done; d_pre and slot 0's d_chain / d_nblocks are free once the previous plain pick
+  // (if any) is done
   FI_CUDA(cudaEventRecord(h->ev_in, us));
   FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_in, 0));
   if (h->pipe_seq >= 2) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot], 0));
   FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_plain, 0));
   if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_lru, 0));  // a device-LRU Add may still be reading d_chain
-  {
+  if (hash_chain_fused(h->cfg.block_bytes)) {
+    // Block hashing and chain walk in one kernel (hash_kernels.cu hash_chain).  It does not wait for the previous
+    // batch's match_pick: its CTAs fill whole SMs, so they take the SMs that match's CTAs leave as its queue drains
+    // (DESIGN.md §4.0: 180.0 us per step this way, 190.8 us waiting for the match).
     LaunchScope ls(h, h->s_a, K_HASH);
-    // The SM split of the pipeline: this batch's block hashing runs BESIDE the previous batch's match_pick —
-    // hash_blocks as at most pipe_hash_ctas CTAs per SM, match_pick as at most pipe_match_ctas (its three CTAs of
-    // 79 registers would leave no room) — instead of one after the other.
-    FI_CUDA(launch_hash_blocks(d_prompts, d_offsets, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, h->d_pre, nb,
-                               h->pipe_hash_ctas * (uint32_t)h->sm_count, h->s_a));
-  }
-  // The chain walk is serial latency — a warp per scheduler that wants an issue slot every few cycles — and
-  // slows several-fold next to a busy kernel that competes for the same schedulers, so it waits for the
-  // previous batch's match to drain; what overlaps is this batch's block hashing with that match.
-  if (h->pipe_seq >= 1) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot ^ 1u], 0));
-  {
+    FI_CUDA(launch_hash_chain(d_prompts, d_offsets, d_h0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, chain, nb,
+                              h->sm_count, h->s_a));
+  } else {
+    {
+      LaunchScope ls(h, h->s_a, K_HASH);
+      // The SM split of the pipeline: this batch's block hashing runs BESIDE the previous batch's match_pick —
+      // hash_blocks as at most pipe_hash_ctas CTAs per SM, match_pick as at most pipe_match_ctas (its three CTAs of
+      // 79 registers would leave no room) — instead of one after the other.
+      FI_CUDA(launch_hash_blocks(d_prompts, d_offsets, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, h->d_pre, nb,
+                                 h->pipe_hash_ctas * (uint32_t)h->sm_count, h->s_a));
+    }
+    // The chain walk is serial latency — a warp per scheduler that wants an issue slot every few cycles — and
+    // slows several-fold next to a busy kernel that competes for the same schedulers, so it waits for the
+    // previous batch's match to drain; what overlaps is this batch's block hashing with that match.
+    if (h->pipe_seq >= 1) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot ^ 1u], 0));
     LaunchScope ls(h, h->s_a, K_CHAIN);
     FI_CUDA(launch_chain_finalize(h->d_pre, nb, d_h0, R, h->MP, chain, false, h->s_a));
   }
@@ -2405,7 +2421,7 @@ int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets
   if (rc != FI_OK) return rc;
   rc = stage_inputs(h, prompts, offsets, h0, R, total);
   if (rc != FI_OK) return rc;
-  if (h->pipe_seq)  // a pipelined batch's stage A (on s_a) shares d_pre with us
+  if (h->pipe_seq)  // a pipelined batch's stage A (on s_a) shares d_chain (slot 0) and d_pre with us
     FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[(h->pipe_seq - 1) & 1], 0));
   if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_lru, 0));  // a device-LRU Add may still be reading d_chain
   h->last_plain_R = 0;  // d_chain no longer holds a pick batch's chains

@@ -8,6 +8,8 @@
 //                   and length add — everything that does not depend on h_{i-1}.
 //                   128-bit loads, 64 B per thread, a warp covers 2 KiB contiguous.
 //   chain_finalize  one thread per request walks the serial tail+avalanche link.
+//   hash_chain      both in one kernel (block sizes 32, 64, 128): hashing warps fill a shared-memory ring of
+//                   pre-states, walker warps of the same CTA walk the chains as it fills.
 //   hash_generic    block sizes that are not a multiple of 32 (e.g. the reference's
 //                   blockSize: 5): fully serial per request, byte loads.
 #include "kernels.cuh"
@@ -324,6 +326,235 @@ __global__ void __launch_bounds__(kChainWarps * 32, MINB) chain_finalize_kernel(
   }
 }
 
+// ---- hash_chain: hash_blocks + chain_finalize in one kernel -------------------------------------------------
+// One CTA owns a tile of 32 * WALK requests and runs on an SM of its own (1 024 threads at 64 registers fill the
+// register file).  Warps WALK-31 hash the tile's blocks column chunk by column chunk: group g = blocks [8g, 8g+8) of
+// all the tile's requests is one slot of a shared-memory ring, laid out as chain_finalize's cp.async ring ([walker
+// warp][unit][lane], conflict-free for the walker).  Warps 0 .. WALK-1, on different SM sub-partitions, walk the
+// chains of 32 requests each in groups of 8 links, taking the pre-states from the ring as they land.  The walk
+// (~43 us at cfg 3) then runs under the tile's prompt stream (~120 us) instead of after it, and the pre-states never
+// go to HBM.  WALK = 4 (128 requests per CTA) when the batch has at least ~4 requests per 128 per SM; smaller
+// batches take smaller tiles so that they still spread over every SM (launch_hash_chain).
+// Handshake per slot: mbarrier `full` (every hashing lane that filled part of the slot arrives; the walkers wait)
+// and `empty` (every walker lane arrives once it has the slot in registers; the hashers wait before they refill it).
+constexpr int kFuseWarps = 32;           // warps 0 .. WALK-1 walk, the rest hash
+constexpr int kFuseRingBytes = 32768;    // ring of 8 KiB (WALK = 4) to 2 KiB (WALK = 1) slots
+
+__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count)
+               : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("{\n .reg .b64 st;\n mbarrier.arrive.shared::cta.b64 st, [%0];\n}\n" ::"r"(
+                   (unsigned)__cvta_generic_to_shared(bar))
+               : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
+  asm volatile(
+      "{\n .reg .pred p;\n"
+      "WAIT_%=:\n"
+      " mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
+      " @!p bra WAIT_%=;\n}\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)),
+      "r"(parity)
+      : "memory");
+}
+
+// Pre-state of one block at arbitrary byte alignment: aligned 64-bit windows + funnel shift (hash_blocks' slow path).
+template <int STRIPES>
+__device__ __forceinline__ uint64_t pre_unaligned(const uint8_t* blk) {
+  const uintptr_t addr = reinterpret_cast<uintptr_t>(blk);
+  const uint64_t* wp = reinterpret_cast<const uint64_t*>(addr & ~(uintptr_t)7);
+  const uint32_t sh = (uint32_t)(addr & 7) * 8;
+  XAcc2 a = xacc2_init();
+#pragma unroll
+  for (int s = 0; s < STRIPES; ++s) {
+    uint64_t w[5];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) w[k] = __ldg(wp + 4 * s + k);
+    w[4] = sh ? __ldg(wp + 4 * s + 4) : 0;
+    if (sh) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) w[k] = (w[k] >> sh) | (w[k + 1] << (64 - sh));
+    }
+    xacc2_stripe(a, Stripe{{(uint32_t)w[0], (uint32_t)(w[0] >> 32), (uint32_t)w[1], (uint32_t)(w[1] >> 32),
+                            (uint32_t)w[2], (uint32_t)(w[2] >> 32), (uint32_t)w[3], (uint32_t)(w[3] >> 32)}});
+  }
+  return xacc2_finish(a, (uint64_t)STRIPES * 32 + 8);
+}
+
+template <int STRIPES, int WALK>
+__global__ void __launch_bounds__(kFuseWarps * 32, 1) hash_chain_kernel(const uint8_t* __restrict__ prompts,
+                                                                   const uint64_t* __restrict__ offsets,
+                                                                   const uint64_t* __restrict__ h0, uint32_t R,
+                                                                   uint32_t M, uint32_t MP,
+                                                                   uint64_t* __restrict__ chain,
+                                                                   uint32_t* __restrict__ nblocks,
+                                                                   uint32_t* __restrict__ zero_word) {
+  constexpr uint32_t B = STRIPES * 32;
+  // A hashing warp's job: 8 blocks of 4 * BPL requests, BPL blocks per lane (two blocks' loads in flight per
+  // thread, one at 128-byte blocks).  Lanes 8j .. 8j+7 read one request's 8 blocks: 512 contiguous bytes.
+  constexpr uint32_t BPL = STRIPES == 4 ? 1 : 2;
+  constexpr uint32_t kFuseReq = 32 * WALK;  // requests per CTA
+  constexpr uint32_t kFuseHashWarps = kFuseWarps - WALK;
+  constexpr uint32_t kFuseRing = kFuseRingBytes / (WALK * 4 * 32 * 16);
+  constexpr uint32_t kJobs = kFuseReq / (4 * BPL);  // jobs per group
+  __shared__ __align__(16) ulonglong2 s_ring[kFuseRing][WALK][4][32];
+  __shared__ uint64_t s_full[kFuseRing], s_empty[kFuseRing];
+  __shared__ const uint8_t* s_base[kFuseReq];
+  __shared__ uint32_t s_n[kFuseReq];
+  __shared__ uint32_t s_groups;
+
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t r_tile = blockIdx.x * kFuseReq;
+  if (zero_word && blockIdx.x == 0 && tid == 0) *zero_word = 0;
+  if (tid == 0) {
+    s_groups = 0;
+    for (uint32_t s = 0; s < kFuseRing; ++s) {
+      mbar_init(&s_full[s], kJobs * 32);
+      mbar_init(&s_empty[s], WALK * 32);
+    }
+  }
+  __syncthreads();
+  if (tid < kFuseReq) {
+    const uint32_t r = r_tile + tid;
+    uint32_t n = 0;
+    const uint8_t* base = prompts;
+    if (r < R) {
+      const uint64_t off = offsets[r];
+      const uint64_t nb64 = (offsets[r + 1] - off) / B;
+      n = nb64 > M ? M : (uint32_t)nb64;
+      base = prompts + off;
+      nblocks[r] = n;
+    }
+    s_n[tid] = n;
+    s_base[tid] = base;
+    atomicMax(&s_groups, (n + 7) / 8);
+  }
+  __syncthreads();
+  const uint32_t ng = s_groups;  // groups of the tile's longest request: every slot up to it is produced and consumed
+
+  if (warp >= WALK) {
+    // ---------------- hashing warps
+    const uint64_t pol = make_evict_first_policy();
+    const uint32_t b = lane & 7;
+#pragma unroll 1
+    for (uint32_t t = warp - WALK; t < ng * kJobs; t += kFuseHashWarps) {
+      const uint32_t g = t / kJobs, job = t % kJobs;
+      const uint32_t i = g * 8 + b;  // block index within the row
+      uint32_t q[BPL];
+      bool ok[BPL], al[BPL], mis = false;
+      const uint8_t* src[BPL];
+      uint64_t pre[BPL];
+#pragma unroll
+      for (uint32_t k = 0; k < BPL; ++k) {
+        q[k] = job * 4 * BPL + k * 4 + (lane >> 3);
+        ok[k] = i < s_n[q[k]];
+        src[k] = s_base[q[k]] + (uint64_t)i * B;
+        al[k] = (reinterpret_cast<uintptr_t>(src[k]) & 15) == 0;
+        mis = mis || (ok[k] && !al[k]);
+      }
+      if (__any_sync(0xFFFFFFFFu, mis)) {
+        // some prompt of the job is not 16-byte aligned: the whole warp takes the 8-byte path (it is right for
+        // aligned blocks too), so the 128-bit loads below never share registers with it
+#pragma unroll
+        for (uint32_t k = 0; k < BPL; ++k)
+          if (ok[k]) pre[k] = pre_unaligned<STRIPES>(src[k]);
+      } else {
+        uint4 v[BPL][2 * STRIPES];
+#pragma unroll
+        for (uint32_t k = 0; k < BPL; ++k)
+          if (ok[k]) {
+#pragma unroll
+            for (int s = 0; s < 2 * STRIPES; ++s) v[k][s] = ld_stream_v4(reinterpret_cast<const uint4*>(src[k]) + s, pol);
+          }
+#pragma unroll
+        for (uint32_t k = 0; k < BPL; ++k)
+          if (ok[k]) {
+            XAcc2 a = xacc2_init();
+#pragma unroll
+            for (int s = 0; s < STRIPES; ++s)
+              xacc2_stripe(a, Stripe{{v[k][2 * s].x, v[k][2 * s].y, v[k][2 * s].z, v[k][2 * s].w, v[k][2 * s + 1].x,
+                                      v[k][2 * s + 1].y, v[k][2 * s + 1].z, v[k][2 * s + 1].w}});
+            pre[k] = xacc2_finish(a, (uint64_t)B + 8);
+          }
+      }
+      const uint32_t slot = g % kFuseRing;
+      if (g >= kFuseRing) mbar_wait(&s_empty[slot], ((g / kFuseRing) + 1) & 1);  // the walkers took use g/kFuseRing - 1
+      // pre-state of (request q, block b of the group): walker warp q/32, lane q%32, unit b/2, half b&1
+      uint64_t* ring = reinterpret_cast<uint64_t*>(s_ring[slot]);
+#pragma unroll
+      for (uint32_t k = 0; k < BPL; ++k)
+        if (ok[k]) ring[(((q[k] >> 5) * 4 + (b >> 1)) * 32 + (q[k] & 31)) * 2 + (b & 1)] = pre[k];
+      mbar_arrive(&s_full[slot]);
+    }
+    return;
+  }
+
+  // ---------------- walker warps: one lane per request, groups of 8 links as in chain_finalize_kernel.  A group's
+  // pre-states are read from the ring right after its wait: the hashers set the pace here (the walk alone takes
+  // less than half the time of the tile's prompt stream), and chain_finalize's one-group-early register copy
+  // does not fit in 64 registers beside the rest.
+  const uint32_t r = r_tile + warp * 32 + lane;
+  const bool valid = r < R;
+  const uint32_t n = s_n[warp * 32 + lane];
+  uint64_t h = valid ? h0[r] : 0;
+  const uint32_t MP2 = MP / 2;
+  ulonglong2* out = reinterpret_cast<ulonglong2*>(chain) + (uint64_t)(valid ? r : 0) * MP2;
+  uint32_t ng_full = valid ? n / 8 : 0;  // groups in which every lane of the warp has 8 blocks
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) ng_full = min(ng_full, __shfl_xor_sync(0xFFFFFFFFu, ng_full, d));
+
+  // group g's pre-states into registers, then the slot goes back to the hashers
+  ulonglong2 in[4], res[4];
+  auto take = [&](uint32_t g) {
+    const uint32_t slot = g % kFuseRing;
+    mbar_wait(&s_full[slot], (g / kFuseRing) & 1);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) in[k] = lds16(&s_ring[slot][warp][k][lane]);
+    mbar_arrive(&s_empty[slot]);
+  };
+
+  uint32_t g = 0;
+#pragma unroll 1
+  for (; g < ng_full; ++g) {
+    take(g);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      h = chain_step(in[k].x, h);
+      res[k].x = h;
+      h = chain_step(in[k].y, h);
+      res[k].y = h;
+    }
+    ulonglong2* o = out + g * 4;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) st_row16(o + k, res[k]);  // (ng_full > 0: every lane is valid)
+  }
+  // ragged groups up to the tile's longest request: some lane's chain ends inside, or has ended (zeros stored)
+#pragma unroll 1
+  for (; g < ng; ++g) {
+    take(g);
+    ulonglong2* o = out + g * 4;
+    const uint32_t i0 = g * 8;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      ulonglong2 v;
+      uint64_t t = chain_step(in[k].x, h);
+      const bool v0 = i0 + 2 * k < n;
+      h = v0 ? t : h;
+      v.x = v0 ? t : 0;
+      t = chain_step(in[k].y, h);
+      const bool v1 = i0 + 2 * k + 1 < n;
+      h = v1 ? t : h;
+      v.y = v1 ? t : 0;
+      if (valid) st_row16(o + k, v);
+    }
+  }
+  if (valid) {
+    const ulonglong2 z = make_ulonglong2(0, 0);
+    for (uint32_t u = g * 4; u < MP2; ++u) st_row16(out + u, z);
+  }
+}
+
 // Fully serial path for block sizes that are not a multiple of 32.
 __global__ void __launch_bounds__(128) hash_generic_kernel(const uint8_t* __restrict__ prompts,
                                                           const uint64_t* __restrict__ offsets,
@@ -377,6 +608,38 @@ cudaError_t launch_chain_finalize(const uint64_t* pre, const uint32_t* nblocks, 
   const uint32_t grid = (groups + kChainWarps - 1) / kChainWarps;
   if (compact) chain_finalize_kernel<3, 8><<<grid, kChainWarps * 32, 0, s>>>(pre, nblocks, h0, R, MP, chain);
   else chain_finalize_kernel<4, 1><<<grid, kChainWarps * 32, 0, s>>>(pre, nblocks, h0, R, MP, chain);
+  return cudaGetLastError();
+}
+
+template <int STRIPES>
+static void launch_hash_chain_tile(uint32_t walk, uint32_t grid, cudaStream_t s, const uint8_t* prompts,
+                                   const uint64_t* offsets, const uint64_t* h0, uint32_t R, uint32_t M, uint32_t MP,
+                                   uint64_t* chain, uint32_t* nblocks, uint32_t* zero_word) {
+  constexpr uint32_t threads = kFuseWarps * 32;
+  if (walk == 4)
+    hash_chain_kernel<STRIPES, 4><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+  else if (walk == 2)
+    hash_chain_kernel<STRIPES, 2><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+  else
+    hash_chain_kernel<STRIPES, 1><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+}
+
+cudaError_t launch_hash_chain(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
+                              uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain, uint32_t* nblocks, int sm_count,
+                              cudaStream_t s, uint32_t* zero_word) {
+  if (R == 0) return cudaSuccess;
+  // the smallest tile whose grid still fits one CTA per SM; 128 requests per CTA beyond that
+  uint32_t walk = 1;
+  while (walk < 4 && (R + 32 * walk - 1) / (32 * walk) > (uint32_t)sm_count) walk *= 2;
+  const uint32_t grid = (R + 32 * walk - 1) / (32 * walk);
+  if (B == 64)
+    launch_hash_chain_tile<2>(walk, grid, s, prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+  else if (B == 32)
+    launch_hash_chain_tile<1>(walk, grid, s, prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+  else if (B == 128)
+    launch_hash_chain_tile<4>(walk, grid, s, prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+  else
+    return cudaErrorInvalidValue;
   return cudaGetLastError();
 }
 

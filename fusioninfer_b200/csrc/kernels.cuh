@@ -182,6 +182,12 @@ cudaError_t launch_hash_blocks(const uint8_t* prompts, const uint64_t* offsets, 
 // compact: the 64-register / 24 KB shape whose 128 CTAs all fit on a 16-SM partition (pipelined path)
 cudaError_t launch_chain_finalize(const uint64_t* pre, const uint32_t* nblocks, const uint64_t* h0,
                                   uint32_t R, uint32_t MP, uint64_t* chain, bool compact, cudaStream_t s);
+// hash_blocks + chain_finalize fused (block_bytes 32, 64 or 128 only: hash_chain_fused(B)); no pre-state buffer.
+// sm_count sets the tile: 32, 64 or 128 requests per CTA, the smallest whose grid fits one CTA per SM
+inline bool hash_chain_fused(uint32_t B) { return B == 32 || B == 64 || B == 128; }
+cudaError_t launch_hash_chain(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
+                              uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain, uint32_t* nblocks,
+                              int sm_count, cudaStream_t s, uint32_t* zero_word = nullptr);
 cudaError_t launch_hash_generic(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
                                 uint32_t R, uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain,
                                 uint32_t* nblocks, cudaStream_t s);

@@ -1,0 +1,154 @@
+// hashchain.cu — the fused hash_chain kernel against hash_blocks + chain_finalize, back to back: bit-exact
+// chains and block counts on ragged, unaligned and truncated prompts (every block size the fused kernel takes,
+// odd batch sizes), then CUDA-event times at the cfg 3 shape (16 384 requests x 4 096-token prompts, 64-byte
+// blocks, 256 blocks) and the cfg 2 shape (4 096 requests x 2 048-token prompts).  Prints one line per case.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I fusioninfer_b200/csrc -o tools/microbench/hashchain tools/microbench/hashchain.cu
+#include <cstdio>
+#include <cstdlib>
+#include <cstring>
+#include <random>
+#include <vector>
+
+#include "hash_kernels.cu"
+
+#define CK(x)                                                                              \
+  do {                                                                                     \
+    cudaError_t e_ = (x);                                                                  \
+    if (e_ != cudaSuccess) {                                                               \
+      std::fprintf(stderr, "%s:%d %s: %s\n", __FILE__, __LINE__, #x, cudaGetErrorString(e_)); \
+      std::exit(1);                                                                        \
+    }                                                                                      \
+  } while (0)
+
+static int g_sms = 132;
+
+struct Batch {
+  uint32_t R, B, M, MP;
+  uint8_t* prompts;
+  uint64_t *offsets, *h0, *pre, *chain_a, *chain_b;
+  uint32_t *nb_a, *nb_b;
+};
+
+// ragged: lengths uniform in [0, (M + 3) * B + B - 1] and random byte gaps between prompts (unaligned starts)
+static Batch make_batch(uint32_t R, uint32_t B, uint32_t M, bool ragged, uint64_t seed) {
+  Batch b{R, B, M, (M + 7) & ~7u};
+  std::mt19937_64 rng(seed);
+  std::vector<uint64_t> off(R + 1);
+  uint64_t at = 0;
+  for (uint32_t r = 0; r < R; ++r) {
+    if (ragged) at += rng() % 24;
+    off[r] = at;
+    at += ragged ? rng() % ((uint64_t)(M + 4) * B) : (uint64_t)M * B;
+  }
+  off[R] = at;
+  std::vector<uint8_t> bytes(at + 64);
+  for (auto& x : bytes) x = (uint8_t)rng();
+  std::vector<uint64_t> h0(R);
+  for (auto& x : h0) x = rng();
+  const uint32_t Rp = (R + 31) & ~31u;
+  CK(cudaMalloc(&b.prompts, bytes.size()));
+  CK(cudaMalloc(&b.offsets, (R + 1) * sizeof(uint64_t)));
+  CK(cudaMalloc(&b.h0, R * sizeof(uint64_t)));
+  CK(cudaMalloc(&b.pre, (size_t)Rp * b.MP * sizeof(uint64_t)));
+  CK(cudaMalloc(&b.chain_a, (size_t)R * b.MP * sizeof(uint64_t)));
+  CK(cudaMalloc(&b.chain_b, (size_t)R * b.MP * sizeof(uint64_t)));
+  CK(cudaMalloc(&b.nb_a, R * sizeof(uint32_t)));
+  CK(cudaMalloc(&b.nb_b, R * sizeof(uint32_t)));
+  CK(cudaMemcpy(b.prompts, bytes.data(), bytes.size(), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(b.offsets, off.data(), off.size() * sizeof(uint64_t), cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(b.h0, h0.data(), h0.size() * sizeof(uint64_t), cudaMemcpyHostToDevice));
+  CK(cudaMemset(b.chain_a, 0xA5, (size_t)R * b.MP * sizeof(uint64_t)));
+  CK(cudaMemset(b.chain_b, 0x5A, (size_t)R * b.MP * sizeof(uint64_t)));
+  return b;
+}
+static void free_batch(Batch& b) {
+  cudaFree(b.prompts), cudaFree(b.offsets), cudaFree(b.h0), cudaFree(b.pre);
+  cudaFree(b.chain_a), cudaFree(b.chain_b), cudaFree(b.nb_a), cudaFree(b.nb_b);
+}
+static void run_pair(Batch& b) {
+  CK(fi::launch_hash_blocks(b.prompts, b.offsets, b.R, b.B, b.M, b.MP, b.pre, b.nb_a, 0, 0));
+  CK(fi::launch_chain_finalize(b.pre, b.nb_a, b.h0, b.R, b.MP, b.chain_a, false, 0));
+}
+static void run_fused(Batch& b) {
+  CK(fi::launch_hash_chain(b.prompts, b.offsets, b.h0, b.R, b.B, b.M, b.MP, b.chain_b, b.nb_b, g_sms, 0));
+}
+static bool same(const Batch& b) {
+  std::vector<uint64_t> ca((size_t)b.R * b.MP), cb(ca.size());
+  std::vector<uint32_t> na(b.R), nb(b.R);
+  CK(cudaMemcpy(ca.data(), b.chain_a, ca.size() * 8, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(cb.data(), b.chain_b, cb.size() * 8, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(na.data(), b.nb_a, na.size() * 4, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(nb.data(), b.nb_b, nb.size() * 4, cudaMemcpyDeviceToHost));
+  return ca == cb && na == nb;
+}
+
+static bool time_shape(const char* name, uint32_t R, uint32_t M) {
+  Batch b = make_batch(R, 64, M, false, 3);
+  cudaEvent_t e0, e1, p0, p1;
+  CK(cudaEventCreate(&e0));
+  CK(cudaEventCreate(&e1));
+  CK(cudaEventCreate(&p0));
+  CK(cudaEventCreate(&p1));
+  for (int w = 0; w < 5; ++w) run_pair(b), run_fused(b);
+  CK(cudaDeviceSynchronize());
+  const int iters = 50;
+  for (int rep = 0; rep < 3; ++rep) {
+    float ms_hash = 0, ms_chain = 0, ms_pair = 0, ms_fused = 0;
+    for (int it = 0; it < iters; ++it) {
+      float t;
+      CK(cudaEventRecord(e0));
+      CK(fi::launch_hash_blocks(b.prompts, b.offsets, b.R, b.B, b.M, b.MP, b.pre, b.nb_a, 0, 0));
+      CK(cudaEventRecord(p0));
+      CK(fi::launch_chain_finalize(b.pre, b.nb_a, b.h0, b.R, b.MP, b.chain_a, false, 0));
+      CK(cudaEventRecord(e1));
+      CK(cudaEventSynchronize(e1));
+      CK(cudaEventElapsedTime(&t, e0, p0));
+      ms_hash += t;
+      CK(cudaEventElapsedTime(&t, p0, e1));
+      ms_chain += t;
+      CK(cudaEventElapsedTime(&t, e0, e1));
+      ms_pair += t;
+      CK(cudaEventRecord(p0));
+      run_fused(b);
+      CK(cudaEventRecord(p1));
+      CK(cudaEventSynchronize(p1));
+      CK(cudaEventElapsedTime(&t, p0, p1));
+      ms_fused += t;
+    }
+    std::printf("%s rep %d: hash_blocks %.1f us + chain_finalize %.1f us = %.1f us | hash_chain %.1f us\n", name, rep,
+                1e3 * ms_hash / iters, 1e3 * ms_chain / iters, 1e3 * ms_pair / iters, 1e3 * ms_fused / iters);
+  }
+  const bool ok = same(b);
+  std::printf("%s outputs %s\n", name, ok ? "identical" : "DIFFER");
+  free_batch(b);
+  return ok;
+}
+
+int main() {
+  int fails = 0;
+  CK(cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0));
+  // correctness: every fused block size, ragged + unaligned + truncated, batch sizes with a partial last tile
+  const uint32_t Rs[] = {1, 31, 129, 1000};
+  const uint32_t Bs[] = {32, 64, 128};
+  const uint32_t Ms[] = {5, 100, 256};
+  for (uint32_t R : Rs)
+    for (uint32_t B : Bs)
+      for (uint32_t M : Ms)
+        for (int ragged = 0; ragged < 2; ++ragged) {
+          Batch b = make_batch(R, B, M, ragged, R * 7919ull + B * 31 + M + ragged);
+          run_pair(b);
+          run_fused(b);
+          CK(cudaDeviceSynchronize());
+          const bool ok = same(b);
+          if (!ok) {
+            ++fails;
+            std::printf("MISMATCH R=%u B=%u M=%u ragged=%d\n", R, B, M, ragged);
+          }
+          free_batch(b);
+        }
+  std::printf("correctness: %d mismatching case(s) of %zu\n", fails, sizeof(Rs) / 4 * sizeof(Bs) / 4 * sizeof(Ms) / 4 * 2);
+
+  // timing at cfg 3 (16 384 x 256 blocks: 128 requests per CTA) and cfg 2 (4 096 x 128 blocks: 32 per CTA)
+  bool ok = time_shape("cfg3", 16384, 256) && time_shape("cfg2", 4096, 128);
+  return (fails || !ok) ? 1 : 0;
+}
