@@ -244,6 +244,9 @@ struct fi_epp {
   int cur_buf = 0;
   uint64_t n_sets = 0, n_clears = 0;
   std::unordered_set<PairKey, PairHash> cleared;
+  // fi_epp_index_remove_endpoints: [0] pairs removed, then (u32) the local endpoints whose device LRU is reset.
+  // Allocated at the first call.
+  unsigned long long* d_rm = nullptr;
   LruArena lru_arena;  // backing store of the LRUs (one huge-page mapping)
   std::vector<LruSet> lrus;
   std::unique_ptr<WorkerPool> pool;  // host LRU workers (fi_epp_index_add_chains), created on first use
@@ -1749,6 +1752,7 @@ void fi_epp_destroy(fi_epp* h) {
   cudaFree(h->d_probed);
   cudaFree(h->d_work);
   cudaFree(h->d_ctr);
+  cudaFree(h->d_rm);
   cudaFree(h->d_eps);
   cudaFree(h->d_sc);
   cudaFree(h->d_elig);
@@ -2054,6 +2058,71 @@ int fi_epp_index_apply(fi_epp* h, const fi_index_op* ops, uint64_t n) {
     }
     return flush_ops(h);
   });
+}
+
+// Upstream indexer.RemovePod for a list of endpoints: one sweep over the index rows clears their bits whatever put
+// them there (LRU Adds or direct SETs), keys nobody holds any more are retired (tombstones, like a CLEAR), and the
+// endpoints' LRUs start empty.  Ordered like fi_epp_index_apply: behind the ops staged so far and the picks called
+// so far, ahead of every later pick.
+int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t n, uint64_t* pairs_removed) {
+  if (!h || (!endpoints && n)) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  if (pairs_removed) *pairs_removed = 0;
+  for (uint32_t i = 0; i < n; ++i)
+    if (endpoints[i] >= h->cfg.num_endpoints) return fail(h, FI_ERR_INVALID, "endpoint out of range");
+  if (h->world > 1) return fail(h, FI_ERR_STATE, "sharded pool: fi_epp_index_remove_endpoints needs a single-rank handle");
+  const uint32_t lo = h->cfg.endpoint_begin, EL = h->cfg.endpoint_count;
+  RemoveSet rs{};
+  std::vector<uint32_t> local;  // distinct local endpoints, for the device LRU
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t e = endpoints[i] - lo;
+    if (e >= EL || (rs.row[e >> 5] >> (e & 31)) & 1u) continue;
+    rs.row[e >> 5] |= 1u << (e & 31);
+    local.push_back(e);
+  }
+  if (local.empty()) return FI_OK;
+  for (uint32_t w = 0; w < h->W; ++w)
+    if (rs.row[w]) {
+      rs.word[rs.m] = w;
+      rs.bits[rs.m] = rs.row[w];
+      ++rs.m;
+    }
+  int rc = flush_ops(h);  // staged SET / CLEAR groups and host-LRU deltas go first
+  if (rc != FI_OK) return rc;
+  rc = check_counters(h);
+  if (rc != FI_OK) return rc;
+  if (!h->d_rm) FI_CUDA(cudaMalloc(&h->d_rm, sizeof(unsigned long long) + (size_t)EL * sizeof(uint32_t)));
+  uint32_t* d_eps = reinterpret_cast<uint32_t*>(h->d_rm + 1);
+  // picks called before this one must not see the removal
+  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
+  FI_CUDA(cudaMemsetAsync(h->d_rm, 0, sizeof(unsigned long long), h->s_index));
+  {
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_index_remove_sweep(h->ix, h->d_ctr, rs, remove_whole_rows(rs, h->W), h->rank, h->d_rm, h->sm_count, h->s_index));
+  }
+  if (h->lru_mode == 1 && h->dlru_ready) {
+    // (pageable source: the copy has taken the data when cudaMemcpyAsync returns)
+    FI_CUDA(cudaMemcpyAsync(d_eps, local.data(), local.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+    h->stats.h2d_bytes += local.size() * sizeof(uint32_t);
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_lru_reset(h->dlru, d_eps, (uint32_t)local.size(), h->s_index));
+  }
+  for (uint32_t e : local)
+    if (e < h->lrus.size()) h->lrus[e].clear();
+  // the sweep's tombstones reach the rebuild decision of the next index update
+  FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
+  h->ctr_pending = true;
+  FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
+  h->gen_index++;
+  if (pairs_removed) {
+    unsigned long long c = 0;
+    FI_CUDA(cudaMemcpyAsync(&c, h->d_rm, sizeof(c), cudaMemcpyDeviceToHost, h->s_index));
+    FI_CUDA(cudaStreamSynchronize(h->s_index));
+    *pairs_removed = c;
+  }
+  return FI_OK;
 }
 
 int fi_epp_index_add_chain(fi_epp* h, uint32_t endpoint, const uint64_t* hashes, uint32_t n) {

@@ -105,6 +105,7 @@ void* fihc_lru_new(uint32_t cap) { return new fi::LruSet(cap); }
 void fihc_lru_free(void* l) { delete (fi::LruSet*)l; }
 uint32_t fihc_lru_size(void* l) { return ((fi::LruSet*)l)->size(); }
 int fihc_lru_contains(void* l, uint64_t k) { return ((fi::LruSet*)l)->contains(k) ? 1 : 0; }
+void fihc_lru_clear(void* l) { ((fi::LruSet*)l)->clear(); }
 void fihc_lru_touch(void* l, const uint64_t* keys, uint32_t n, uint8_t* inserted, uint8_t* did_evict, uint64_t* evicted) {
   fi::LruSet* s = (fi::LruSet*)l;
   for (uint32_t i = 0; i < n; ++i) {

@@ -174,15 +174,20 @@ __device__ uint32_t table_find_slot(const IndexView& ix, uint64_t h) {
 }
 
 // rank `rbit`'s row of the key at (slot, node) has emptied: drop its directory bit; if no rank holds the key
-// any more retire the key and its node
-__device__ __forceinline__ void rank_vanished(const IndexView& ix, IndexCounters* ctr, uint32_t slot, uint32_t node,
-                                              uint32_t rbit) {
+// any more retire the key and its node (true: the caller counts the tombstone)
+__device__ __forceinline__ bool rank_vanished_retires(const IndexView& ix, uint32_t slot, uint32_t node, uint32_t rbit) {
   const uint32_t oldm = atomicAnd(ix.rmask + node, ~rbit);
   if ((oldm & rbit) && (oldm & ~rbit) == 0u && slot != SLOT_MISS) {
     ix.keys[slot] = KEY_TOMB;
     ix.klog[node] = 0;
-    atomicAdd(&ctr->tombstones, 1ull);
+    return true;
   }
+  return false;
+}
+
+__device__ __forceinline__ void rank_vanished(const IndexView& ix, IndexCounters* ctr, uint32_t slot, uint32_t node,
+                                              uint32_t rbit) {
+  if (rank_vanished_retires(ix, slot, node, rbit)) atomicAdd(&ctr->tombstones, 1ull);
 }
 
 template <bool REMOTE>
@@ -263,6 +268,120 @@ __global__ void __launch_bounds__(256) index_rebuild_kernel(IndexView from, Inde
   }
 }
 
+// ---- removal of whole endpoints (fi_epp_index_remove_endpoints) ------------------------------------------------
+// One pass over the live nodes [0, min(used, C)) and the two special nodes C, C+1 — the table is not walked.  Index
+// kernels run one at a time on the index stream and picks only read, so the thread that owns a row word stores it
+// plainly; cnt takes an atomicSub because the words of a node may belong to different threads, and the thread that
+// takes it to 0 retires the key exactly like a CLEAR does.
+
+// sweep item t -> node: t < n the regular nodes, then C and C+1
+__device__ __forceinline__ uint32_t sweep_node(const IndexView& ix, uint64_t t, uint64_t n) {
+  return (uint32_t)(t < n ? t : ix.C + (t - n));
+}
+
+// true: the key was retired (removing every endpoint retires every key: the tombstones are counted per CTA, not
+// with one atomic on the same counter each)
+__device__ __forceinline__ bool remove_from_node(const IndexView& ix, uint32_t node, uint32_t gone, uint32_t rbit) {
+  if (atomicSub(ix.cnt + node, gone) != gone) return false;
+  const uint32_t slot = node < ix.C ? table_find_slot(ix, ix.klog[node]) : SLOT_MISS;
+  return rank_vanished_retires(ix, slot, node, rbit);
+}
+
+__device__ __forceinline__ void sweep_total(uint32_t pairs, uint32_t tombs, unsigned long long* removed, IndexCounters* ctr) {
+  __shared__ unsigned long long s_pairs;
+  __shared__ uint32_t s_tombs;
+  if (threadIdx.x == 0) s_pairs = s_tombs = 0;
+  __syncthreads();
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    pairs += __shfl_xor_sync(0xFFFFFFFFu, pairs, d);
+    tombs += __shfl_xor_sync(0xFFFFFFFFu, tombs, d);
+  }
+  if ((threadIdx.x & 31) == 0) {
+    if (pairs) atomicAdd(&s_pairs, (unsigned long long)pairs);
+    if (tombs) atomicAdd(&s_tombs, tombs);
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    if (s_pairs) atomicAdd(removed, s_pairs);
+    if (s_tombs) atomicAdd(&ctr->tombstones, (unsigned long long)s_tombs);
+  }
+}
+
+// Per-word shape: a thread owns kSweepNodes nodes per pass and reads only the m listed words of each — removing one
+// endpoint costs one 32-byte sector per node, not the whole row.  The loads of all its nodes are issued before any
+// result is used.
+constexpr int kSweepNodes = 4;
+__global__ void __launch_bounds__(256) index_remove_words_kernel(IndexView ix, IndexCounters* ctr, const __grid_constant__ RemoveSet rs,
+                                                                 uint32_t rbit, unsigned long long* removed) {
+  const uint64_t used = *reinterpret_cast<volatile unsigned long long*>(&ctr->used);
+  const uint64_t n = used < ix.C ? used : ix.C;
+  const uint64_t nodes = n + 2, stride = (uint64_t)gridDim.x * blockDim.x;
+  uint32_t mine = 0, tombs = 0;
+  for (uint64_t t0 = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; t0 < nodes; t0 += stride * kSweepNodes) {
+    uint32_t node[kSweepNodes], gone[kSweepNodes];
+#pragma unroll
+    for (int u = 0; u < kSweepNodes; ++u) {
+      const uint64_t t = t0 + u * stride;
+      node[u] = t < nodes ? sweep_node(ix, t, n) : NODE_INVALID;
+      gone[u] = 0;
+    }
+    for (uint32_t k = 0; k < rs.m; ++k) {
+      const uint32_t w = rs.word[k], mk = rs.bits[k];
+      uint32_t old[kSweepNodes];
+#pragma unroll
+      for (int u = 0; u < kSweepNodes; ++u) old[u] = node[u] != NODE_INVALID ? ix.rows[((uint64_t)node[u] << ix.logW) + w] : 0u;
+#pragma unroll
+      for (int u = 0; u < kSweepNodes; ++u) {
+        const uint32_t hit = old[u] & mk;
+        if (hit) {
+          ix.rows[((uint64_t)node[u] << ix.logW) + w] = old[u] & ~mk;
+          gone[u] += __popc(hit);
+        }
+      }
+    }
+#pragma unroll
+    for (int u = 0; u < kSweepNodes; ++u) {
+      if (gone[u]) {
+        mine += gone[u];
+        tombs += remove_from_node(ix, node[u], gone[u], rbit);
+      }
+    }
+  }
+  sweep_total(mine, tombs, removed, ctr);
+}
+
+// Whole-row shape: a thread owns one 16-byte chunk of a row, the W/4 chunks of a node are consecutive lanes of one
+// warp (coalesced), and their counts are summed with shuffles so that one lane per node updates cnt.
+__global__ void __launch_bounds__(256) index_remove_rows_kernel(IndexView ix, IndexCounters* ctr, const __grid_constant__ RemoveSet rs,
+                                                                uint32_t rbit, unsigned long long* removed) {
+  const uint64_t used = *reinterpret_cast<volatile unsigned long long*>(&ctr->used);
+  const uint64_t n = used < ix.C ? used : ix.C;
+  const uint32_t lchunks = ix.logW - 2, chunks = 1u << lchunks;  // W >= 4 (remove_whole_rows)
+  const uint64_t items = (n + 2) << lchunks, stride = (uint64_t)gridDim.x * blockDim.x;
+  uint32_t mine = 0, tombs = 0;
+  // every lane of a warp runs the same number of passes (shuffles inside)
+  for (uint64_t i0 = blockIdx.x * (uint64_t)blockDim.x; i0 < items; i0 += stride) {
+    const uint64_t i = i0 + threadIdx.x;
+    const uint32_t c = (uint32_t)(i & (chunks - 1));
+    uint32_t node = NODE_INVALID, gone = 0;
+    if (i < items) {
+      node = sweep_node(ix, i >> lchunks, n);
+      uint4* p = reinterpret_cast<uint4*>(ix.rows + ((uint64_t)node << ix.logW)) + c;
+      const uint4 old = *p;
+      const uint4 mk = make_uint4(rs.row[4 * c], rs.row[4 * c + 1], rs.row[4 * c + 2], rs.row[4 * c + 3]);
+      gone = __popc(old.x & mk.x) + __popc(old.y & mk.y) + __popc(old.z & mk.z) + __popc(old.w & mk.w);
+      if (gone) *p = make_uint4(old.x & ~mk.x, old.y & ~mk.y, old.z & ~mk.z, old.w & ~mk.w);
+    }
+    mine += gone;
+    uint32_t node_gone = gone;
+    for (uint32_t d = 1; d < chunks; d <<= 1) node_gone += __shfl_xor_sync(0xFFFFFFFFu, node_gone, d);
+    if (c == 0 && node_gone) tombs += remove_from_node(ix, node, node_gone, rbit);
+  }
+  sweep_total(mine, tombs, removed, ctr);
+}
+static_assert(MAX_ROW_WORDS / 4 <= 32, "the 16-byte chunks of a row must fit in one warp");
+
 // membership query (tests / diagnostics): out[i] = 1 iff (endpoint, hash) is present
 __global__ void __launch_bounds__(256) index_contains_kernel(IndexView ix, const fi_index_op* __restrict__ q, uint64_t n,
                                                              uint32_t ep_begin, uint32_t ep_count,
@@ -325,6 +444,18 @@ cudaError_t launch_index_remote_vanish(IndexView ix, IndexCounters* ctr, const u
 
 cudaError_t launch_index_rebuild(IndexView from, IndexView to, IndexCounters* ctr, cudaStream_t s) {
   index_rebuild_kernel<<<grid_for(from.C), 256, 0, s>>>(from, to, ctr);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_index_remove_sweep(IndexView ix, IndexCounters* ctr, const RemoveSet& rs, bool whole_rows, uint32_t rank,
+                                      unsigned long long* removed, int sm_count, cudaStream_t s) {
+  if (rs.m == 0) return cudaSuccess;
+  // the node count is read on the device (ctr->used): one wave of resident CTAs strides over whatever it is
+  auto kernel = whole_rows ? index_remove_rows_kernel : index_remove_words_kernel;
+  int per_sm = 0;
+  const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256, 0);
+  if (e != cudaSuccess) return e;
+  kernel<<<(unsigned)(sm_count * (per_sm > 0 ? per_sm : 1)), 256, 0, s>>>(ix, ctr, rs, 1u << rank, removed);
   return cudaGetLastError();
 }
 

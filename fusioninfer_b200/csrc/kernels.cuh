@@ -63,6 +63,16 @@ struct GossipLog {
   uint64_t cap;
 };
 
+// Removal set of fi_epp_index_remove_endpoints, passed as a kernel parameter: the row words that hold a removed
+// local endpoint (word[k], its bits[k], k < m) and the same as a whole-row mask (row[w], w < W).
+constexpr uint32_t MAX_ROW_WORDS = 128;  // 4096 local endpoints (validate_config)
+struct RemoveSet {
+  uint32_t m;
+  uint32_t word[MAX_ROW_WORDS];
+  uint32_t bits[MAX_ROW_WORDS];
+  uint32_t row[MAX_ROW_WORDS];
+};
+
 struct ProfileDev {
   uint32_t n_scorers;
   uint32_t n_filters;                    // by-label filters, ANDed (fi_profile: role_mask first, then more_filters)
@@ -206,6 +216,28 @@ cudaError_t launch_index_remote_appear(IndexView ix, IndexCounters* ctr, const u
 cudaError_t launch_index_remote_vanish(IndexView ix, IndexCounters* ctr, const uint64_t* hashes, uint64_t n,
                                        uint32_t rank, cudaStream_t s);
 cudaError_t launch_index_rebuild(IndexView from, IndexView to, IndexCounters* ctr, cudaStream_t s);
+// clear the removal set's bits from every live row (and the two special nodes), retire the keys nobody holds any
+// more, add the number of cleared bits to *removed.  whole_rows: 16-byte whole-row loads instead of one load per
+// listed word (remove_whole_rows decides)
+cudaError_t launch_index_remove_sweep(IndexView ix, IndexCounters* ctr, const RemoveSet& rs, bool whole_rows, uint32_t rank,
+                                      unsigned long long* removed, int sm_count, cudaStream_t s);
+// Every 32-byte sector of a row holds a listed word: then both sweep shapes move the same bytes and the whole-row
+// one issues a quarter of the loads.  Rows narrower than 16 bytes always take the per-word shape.
+inline bool remove_whole_rows(const RemoveSet& rs, uint32_t W) {
+  if (W < 4) return false;
+  const uint32_t sector_words = 8;
+  const uint32_t sectors = (W + sector_words - 1) / sector_words;
+  uint32_t hit = 0;
+  bool seen[MAX_ROW_WORDS / 8 + 1] = {};
+  for (uint32_t k = 0; k < rs.m; ++k) {
+    const uint32_t s = rs.word[k] / sector_words;
+    if (!seen[s]) {
+      seen[s] = true;
+      ++hit;
+    }
+  }
+  return hit == sectors;
+}
 cudaError_t launch_index_contains(IndexView ix, const fi_index_op* q, uint64_t n, uint32_t ep_begin,
                                   uint32_t ep_count, uint8_t* out, cudaStream_t s);
 

@@ -146,6 +146,15 @@ class alignas(128) LruSet {
     return map_[find_slot(key)].idx != kNone;
   }
 
+  // Forget every entry.  The node and map memory stay with the set: the arena is a bump allocator and never
+  // takes memory back.
+  void clear() {
+    if (!nodes_) return;
+    for (uint64_t i = 0; i <= mask_; ++i) map_[i] = Slot{0, kNone, 0};
+    size_ = 0;
+    head_ = tail_ = kNone;
+  }
+
  private:
   static constexpr uint32_t kNone = 0xFFFFFFFFu;
   struct Node {

@@ -59,6 +59,8 @@ cudaError_t launch_lru_append(const DevLru& lru, const LruBatch& b, fi_index_op*
                               uint64_t clears_cap, uint32_t ep_begin, cudaStream_t s);
 cudaError_t launch_lru_evict(const DevLru& lru, fi_index_op* clears, unsigned long long* n_clears, uint64_t clears_cap,
                              uint32_t ep_begin, cudaStream_t s);
+// empty the LRUs of the n local endpoints eps[0..n) (device array; n <= 65535)
+cudaError_t launch_lru_reset(const DevLru& lru, const uint32_t* eps, uint32_t n, cudaStream_t s);
 // diagnostics: the live keys of local endpoint e, least recently used first
 cudaError_t launch_lru_dump(const DevLru& lru, uint32_t e, uint64_t* out, uint32_t* n_out, cudaStream_t s);
 

@@ -441,6 +441,19 @@ __global__ void __launch_bounds__(kWideCta) lru_maintain_kernel(DevLru lru, cons
   if (threadIdx.x == 0 && atomicAdd(lru.used + e, 0u) != s_tot) atomicExch(lru.error, 6u);
 }
 
+// ---- reset: the listed endpoints' LRUs become empty (fi_epp_index_remove_endpoints) -----------------------------
+// The table is zeroed (both special slots too) and head = tail = count = used = 0.  The log keeps its records: a
+// record is live only while the table points at it, so none of them is.  hold / dcount / ovf are scratch of a
+// running sub-batch and are rewritten before they are read.
+__global__ void __launch_bounds__(256) lru_reset_kernel(DevLru lru, const uint32_t* __restrict__ eps) {
+  const uint32_t e = eps[blockIdx.y];
+  uint4* tab = reinterpret_cast<uint4*>(lru.slots + (uint64_t)e * (lru.TS + 2));
+  static_assert(sizeof(LruSlot) == sizeof(uint4), "one 16-byte store per slot");
+  const uint4 z = make_uint4(0, 0, 0, 0);
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < lru.TS + 2; i += gridDim.x * blockDim.x) tab[i] = z;
+  if (blockIdx.x == 0 && threadIdx.x == 0) lru.head[e] = lru.tail[e] = lru.count[e] = lru.used[e] = 0;
+}
+
 // diagnostics (tests): the live keys of endpoint e, oldest first
 __global__ void __launch_bounds__(256) lru_dump_kernel(DevLru lru, uint32_t e, uint64_t* out, uint32_t* n_out) {
   const LruSlot* tab = lru.slots + (uint64_t)e * (lru.TS + 2);
@@ -498,6 +511,12 @@ cudaError_t launch_lru_append(const DevLru& lru, const LruBatch& b, fi_index_op*
 cudaError_t launch_lru_evict(const DevLru& lru, fi_index_op* clears, unsigned long long* n_clears, uint64_t clears_cap,
                              uint32_t ep_begin, cudaStream_t s) {
   lru_evict_kernel<<<lru.EL, kWideCta, 0, s>>>(lru, clears, n_clears, clears_cap, ep_begin);
+  return cudaGetLastError();
+}
+cudaError_t launch_lru_reset(const DevLru& lru, const uint32_t* eps, uint32_t n, cudaStream_t s) {
+  if (n == 0) return cudaSuccess;
+  const uint32_t blocks = (lru.TS + 2 + 255) / 256;  // at most 64 CTAs per endpoint, each striding over its table
+  lru_reset_kernel<<<dim3(blocks < 64 ? blocks : 64, n), 256, 0, s>>>(lru, eps);
   return cudaGetLastError();
 }
 cudaError_t launch_lru_dump(const DevLru& lru, uint32_t e, uint64_t* out, uint32_t* n_out, cudaStream_t s) {

@@ -165,6 +165,16 @@ class EndpointPicker:
         ops = np.ascontiguousarray(ops, dtype=OP_DTYPE)
         self._check(self._lib.fi_epp_index_apply(self._h, _ptr(ops), len(ops)), "fi_epp_index_apply")
 
+    def remove_endpoints(self, endpoints, count: bool = False) -> Optional[int]:
+        """upstream indexer.RemovePod: drop every cached prefix of the listed endpoints from the index and empty their
+        LRUs (pod gone, restarted, or its index about to be given to a new pod).  Ordered like index_apply.
+        count=True blocks until the removal is applied and returns how many (endpoint, hash) pairs it removed."""
+        eps = np.ascontiguousarray(np.atleast_1d(np.asarray(endpoints, dtype=np.uint32)))
+        out = C.c_uint64(0)
+        self._check(self._lib.fi_epp_index_remove_endpoints(self._h, _ptr(eps), len(eps), C.byref(out) if count else None),
+                    "fi_epp_index_remove_endpoints")
+        return out.value if count else None
+
     def index_add_chain(self, endpoint: int, hashes: np.ndarray):
         hashes = np.ascontiguousarray(hashes, dtype=np.uint64)
         self._check(

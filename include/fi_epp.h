@@ -260,6 +260,17 @@ int fi_epp_endpoints_lora_update(fi_epp* h, const fi_endpoint_lora* states, uint
  * number of times in the same order, each with its own ops (possibly none). */
 int fi_epp_index_apply(fi_epp* h, const fi_index_op* ops, uint64_t n);
 
+/* upstream indexer.RemovePod: forget everything the index and the LRU hold for the listed endpoints (pod deleted,
+ * restarted with an empty KV cache, or its index about to be reused for a new pod).  Every (endpoint, hash) pair
+ * leaves the index, whether an Add or a direct SET put it there; keys no endpoint holds any more leave with it; the
+ * endpoints' LRUs become empty (a later Add inserts anew).  Endpoint state (fi_epp_endpoints_update) is untouched.
+ * Duplicates and endpoints that hold nothing are no-ops.  Asynchronous and ordered like fi_epp_index_apply: ops
+ * submitted before the call are applied first, picks called before it (in-flight fi_epp_pick_submit batches
+ * included) do not see the removal, every later pick does.  pairs_removed != NULL: block until applied and write
+ * how many (endpoint, hash) pairs left the index.  FI_ERR_INVALID if an endpoint is >= num_endpoints (nothing is
+ * applied); FI_ERR_STATE on a sharded pool. */
+int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t n, uint64_t* pairs_removed);
+
 /* Upstream indexer.Add(hashes, pod): touch each hash in `endpoint`'s LRU
  * (capacity lru_capacity), emit SET for new entries and CLEAR for evicted
  * ones.  Requires lru_capacity > 0.  Single-rank handles only (FI_ERR_STATE on a sharded pool). */
