@@ -745,46 +745,54 @@ __global__ void __launch_bounds__(1024) prepare_endpoints_kernel(const EndpointD
   }
 }
 
+// One instantiation per kernel variant: the shared-memory opt-in (cudaFuncSetAttribute) applies to one function
+// only, and occupancy differs between variants, so each variant keeps its own cache, per device.
+template <int LPR, int VEC, bool LPM, bool LORA>
+cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_t s) {
+  const auto kern = match_pick_kernel<LPR, VEC, LPM, LORA>;
+  const size_t smem = (size_t)kWarps * p.MP * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
+  // occupancy is a property of (kernel, smem): query once per distinct smem size
+  static size_t cached_smem_dev[64];
+  static int cached_per_sm_dev[64];
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  if (e != cudaSuccess) return e;
+  dev &= 63;
+  size_t& cached_smem = cached_smem_dev[dev];
+  int& cached_per_sm = cached_per_sm_dev[dev];
+  if (cached_smem != smem + 1) {  // +1: zero-initialised statics mean "not cached"
+    if (smem > 48 * 1024) {
+      e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+      if (e != cudaSuccess) return e;
+    }
+    int per_sm = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kWarps * 32, smem);
+    if (e != cudaSuccess) return e;
+    cached_per_sm = per_sm < 1 ? 1 : per_sm;
+    cached_smem = smem + 1;
+  }
+  uint32_t grid = (p.R + kWarps - 1) / kWarps;
+  uint32_t per_sm_now = (uint32_t)cached_per_sm;
+  if (p.max_ctas_per_sm && p.max_ctas_per_sm < per_sm_now) per_sm_now = p.max_ctas_per_sm;
+  const uint32_t cap = (uint32_t)sm_count * per_sm_now;
+  if (grid > cap) grid = cap;
+  if (grid == 0) grid = 1;
+  if (p.zero_work_counter) {
+    e = cudaMemsetAsync(p.work_counter, 0, sizeof(uint32_t), s);
+    if (e != cudaSuccess) return e;
+  }
+  kern<<<grid, kWarps * 32, smem, s>>>(p);
+  return cudaGetLastError();
+}
+
 template <int LPR, int VEC>
 cudaError_t launch_match_t(const MatchParams& p, int sm_count, cudaStream_t s) {
-  const size_t smem = (size_t)kWarps * p.MP * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
-  auto go = [&](auto kern) -> cudaError_t {
-    // occupancy is a property of (kernel, smem): query once per distinct smem size
-    static size_t cached_smem_dev[64];
-    static int cached_per_sm_dev[64];
-    int dev = 0;
-    cudaError_t e = cudaGetDevice(&dev);
-    if (e != cudaSuccess) return e;
-    dev &= 63;
-    size_t& cached_smem = cached_smem_dev[dev];
-    int& cached_per_sm = cached_per_sm_dev[dev];
-    if (cached_smem != smem + 1) {  // +1: zero-initialised statics mean "not cached"
-      if (smem > 48 * 1024) {
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return e;
-      }
-      int per_sm = 0;
-      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kWarps * 32, smem);
-      if (e != cudaSuccess) return e;
-      cached_per_sm = per_sm < 1 ? 1 : per_sm;
-      cached_smem = smem + 1;
-    }
-    uint32_t grid = (p.R + kWarps - 1) / kWarps;
-    uint32_t per_sm_now = (uint32_t)cached_per_sm;
-    if (p.max_ctas_per_sm && p.max_ctas_per_sm < per_sm_now) per_sm_now = p.max_ctas_per_sm;
-    const uint32_t cap = (uint32_t)sm_count * per_sm_now;
-    if (grid > cap) grid = cap;
-    if (grid == 0) grid = 1;
-    if (p.zero_work_counter) {
-      e = cudaMemsetAsync(p.work_counter, 0, sizeof(uint32_t), s);
-      if (e != cudaSuccess) return e;
-    }
-    kern<<<grid, kWarps * 32, smem, s>>>(p);
-    return cudaGetLastError();
-  };
   const bool lpm = p.lpm == FI_MATCH_LPM;
-  if (p.st.has_lora) return lpm ? go(match_pick_kernel<LPR, VEC, true, true>) : go(match_pick_kernel<LPR, VEC, false, true>);
-  return lpm ? go(match_pick_kernel<LPR, VEC, true, false>) : go(match_pick_kernel<LPR, VEC, false, false>);
+  if (p.st.has_lora)
+    return lpm ? launch_match_variant<LPR, VEC, true, true>(p, sm_count, s)
+               : launch_match_variant<LPR, VEC, false, true>(p, sm_count, s);
+  return lpm ? launch_match_variant<LPR, VEC, true, false>(p, sm_count, s)
+             : launch_match_variant<LPR, VEC, false, false>(p, sm_count, s);
 }
 
 }  // namespace

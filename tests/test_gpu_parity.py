@@ -712,10 +712,12 @@ def _check_lru_state(gpu, ref, E):
         want = np.array(list(ref[e].d.keys()), dtype=np.uint64)
         assert np.array_equal(got, want), f"endpoint {e}: {len(got)} vs {len(want)} entries"
     # membership: every key ever seen, at every endpoint
-    seen = sorted({k for l in ref for k in l.d} | getattr(_check_lru_state, "extra", set()))
-    q = [(k, e, 0) for k in seen for e in range(E)]
-    have = gpu.index_contains(H.ops_array(q))
-    want = np.array([k in ref[e].d for k in seen for e in range(E)], dtype=bool)
+    seen = np.array(sorted({k for l in ref for k in l.d} | getattr(_check_lru_state, "extra", set())), dtype=np.uint64)
+    q = np.zeros(len(seen) * E, dtype=H.OP_DTYPE)  # every (key, endpoint) pair, key-major
+    q["hash"] = np.repeat(seen, E)
+    q["endpoint"] = np.tile(np.arange(E, dtype=np.uint32), len(seen))
+    have = gpu.index_contains(q)
+    want = np.stack([np.isin(seen, np.array(list(ref[e].d), dtype=np.uint64)) for e in range(E)], axis=1).ravel()
     assert np.array_equal(have.astype(bool), want)
 
 
@@ -724,7 +726,17 @@ def test_device_lru_order_and_membership_random_batches():
     re-touched within and across batches, hot endpoints that force several sub-batches, enough churn for the
     log compaction / table rebuild to run many times; recency order (fi_epp_lru_dump) and index membership
     are compared after every batch."""
-    E, cap, M = 6, 90, 24
+    _device_lru_random_batches(cap=90, M=24)
+
+
+@pytest.mark.parametrize("cap,M", [(1023, 1023), (1100, 1023)])
+def test_device_lru_random_batches_long_chains(cap, M):
+    """The same with chains of up to 1023 blocks: a single chain can fill (cap = M) or nearly fill an LRU."""
+    _device_lru_random_batches(cap, M)
+
+
+def _device_lru_random_batches(cap, M):
+    E = 6
     gpu = _device_lru_handle(E, cap, M)
     ref = [_PyLru(cap) for _ in range(E)]
     rng = np.random.default_rng(2024)
@@ -769,7 +781,17 @@ def test_device_lru_order_and_membership_random_batches():
 def test_device_lru_edge_cases():
     """capacity hit exactly; a chain as long as the capacity; the hashes 0 and ~0 (the tables' own markers);
     single-chain calls interleaved with batches; empty calls."""
-    E, cap, M = 3, 16, 16
+    _device_lru_edge_cases(cap=16, M=16)
+
+
+@pytest.mark.parametrize("cap,M", [(1023, 1023), (1100, 1023)])
+def test_device_lru_edge_cases_long_chains(cap, M):
+    """The same with 1023-key chains: one chain fills the LRU exactly (cap = M) or nearly (M < cap)."""
+    _device_lru_edge_cases(cap, M)
+
+
+def _device_lru_edge_cases(cap, M):
+    E = 3
     gpu = _device_lru_handle(E, cap, M)
     ref = [_PyLru(cap) for _ in range(E)]
     ever = set()
@@ -785,14 +807,14 @@ def test_device_lru_edge_cases():
         _check_lru_state.extra = ever
         _check_lru_state(gpu, ref, E)
 
-    a = np.arange(1, 17, dtype=np.uint64) * np.uint64(0x9E3779B97F4A7C15)
-    add([0], [a], [16])                      # fills endpoint 0 exactly
-    add([0], [a[::-1].copy()], [16])         # same keys, reversed recency: no eviction
+    a = np.arange(1, M + 1, dtype=np.uint64) * np.uint64(0x9E3779B97F4A7C15)
+    add([0], [a], [M])                       # fills endpoint 0 exactly (M = cap)
+    add([0], [a[::-1].copy()], [M])          # same keys, reversed recency: no eviction
     b = a + np.uint64(7)
-    add([0, 0], [b, a], [16, 16])            # a chain of `capacity` new keys evicts everything, then back again
-    special = np.array([0, 0xFFFFFFFFFFFFFFFF, 5, 0, 9, 0xFFFFFFFFFFFFFFFF] + [11] * 10, dtype=np.uint64)
+    add([0, 0], [b, a], [M, M])              # a chain of `capacity` new keys evicts everything, then back again
+    special = np.array([0, 0xFFFFFFFFFFFFFFFF, 5, 0, 9, 0xFFFFFFFFFFFFFFFF] + [11] * (M - 6), dtype=np.uint64)
     add([1, 2], [special, special], [6, 4])  # the hashes 0 and ~0 are ordinary members
-    for i in range(20):                      # push them out again, one new key per call (single-chain entry point)
+    for i in range(cap + 4):                 # push them out again, one new key per call (single-chain entry point)
         k = np.array([1000 + i], dtype=np.uint64)
         gpu.index_add_chain(1, k)
         ref[1].add_chain(k)
@@ -807,12 +829,21 @@ def test_device_lru_edge_cases():
 
 def test_device_lru_from_device_chains():
     """fi_epp_index_add_chains_device: the chains stay in device memory (chains_out of the device pick); same
-    picks as the oracle over several churn steps."""
+    chains and picks as the oracle over several churn steps."""
+    _device_lru_from_device_chains(max_blocks=32, T=512, cap=300, slots=1 << 17)
+
+
+def test_device_lru_from_device_chains_long_prompts():
+    """The same at max_blocks = 1023: chains_out's pitch (1023) is not the device buffers' (1024)."""
+    _device_lru_from_device_chains(max_blocks=1023, T=16 * 1024, cap=3000, slots=1 << 20)
+
+
+def _device_lru_from_device_chains(max_blocks, T, cap, slots):
     import torch
 
-    wl = H.small_workload(E=40, R=256, T=512, max_blocks=32, lru_capacity=0)
+    wl = H.small_workload(E=40, R=256, T=T, max_blocks=max_blocks, lru_capacity=0)
     prof = [{"name": "d", "scorers": [(P, 100), (K, 9), (Q, 5)]}]
-    cfg = H.config_for(wl, profiles=prof, lru_capacity=300, index_slots=1 << 17)
+    cfg = H.config_for(wl, profiles=prof, lru_capacity=cap, index_slots=slots, max_prompt_bytes=wl.R * wl.T * 4)
     gpu, cpu = _pair(cfg)
     st = wl.endpoint_states()
     gpu.update_endpoints(st)
@@ -831,23 +862,33 @@ def test_device_lru_from_device_chains():
         got = d_out.cpu().numpy().view(H.PICK_DTYPE).reshape(wl.R, 1)
         want, wch = cpu.pick_batch(tok, offs, wl.h0, want_chains=True)
         assert H.picks_equal(got, want), f"step {step}\n" + H.describe_diff(got, want)
+        assert np.array_equal(d_ch.cpu().numpy().view(np.uint64).reshape(wl.R, wl.max_blocks), wch), f"step {step}"
         gpu.index_add_chains_device(got[:, 0]["endpoint"], d_ch.data_ptr(), wl.max_blocks, got[:, 0]["n_blocks"], stream=stream)
         cpu.index_add_chains(want[:, 0]["endpoint"], wch, want[:, 0]["n_blocks"])
     assert gpu.index_stats().tombstones > 0
     gpu.close()
 
 
-@pytest.mark.parametrize("partition", [None, 0, 40])
-def test_pipelined_back_to_back_batches(partition):
+@pytest.mark.parametrize("partition,max_blocks", [
+    pytest.param(None, 128, id="None"), pytest.param(0, 128, id="0"), pytest.param(40, 128, id="40"),
+    pytest.param(None, 1023, id="None-1023"), pytest.param(40, 1023, id="40-1023"),
+    pytest.param(16, 1023, id="16-1023"),
+])
+def test_pipelined_back_to_back_batches(partition, max_blocks):
     """Twelve batches of different sizes submitted back to back with nothing in between (so that the pipeline really
     has its two — partitioned GPU: three — batches in flight and reuses every slot buffer several times), one wait
     at the end, every output equal to the oracle's; then the same again after a stream-ordered pick.  With a 40-SM
     walker partition, R = 512 exceeds the 4 hashing CTAs per SM of the other partition, so hash_blocks' CTAs each
-    take several requests."""
+    take several requests.  max_blocks = 1023: prompts past the cap with a partial last block, chain pitch 1024; on a
+    partitioned GPU hash_blocks and the chain walk run at that pitch (16 SMs: the compact walker shape, 40: the full
+    one)."""
     import torch
 
-    wl = H.small_workload(E=200, R=512, T=2048, max_blocks=128)
-    cfg = H.config_for(wl, profiles=WEIGHTED)
+    if max_blocks == 128:
+        wl = H.small_workload(E=200, R=512, T=2048, max_blocks=128)
+    else:
+        wl = H.small_workload(E=200, R=512, T=16 * (max_blocks + 1) + 5, max_blocks=max_blocks, groups_per_endpoint=2)
+    cfg = H.config_for(wl, profiles=WEIGHTED, max_prompt_bytes=wl.R * wl.T * 4)
     gpu, cpu = _pair(cfg)
     if partition is not None:
         gpu.set_option("pipe_partition", partition)
