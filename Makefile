@@ -12,7 +12,9 @@ CU_SRCS := $(CSRC)/hash_kernels.cu $(CSRC)/index_kernels.cu $(CSRC)/lru_kernels.
 CU_OBJS := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(CU_SRCS))
 HDRS := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/fi_epp.h
 
-all: $(LIB) $(HOSTCHECK) oracle
+RANKED_ORACLE := $(OBJDIR)/libepp_ranked_oracle.so
+
+all: $(LIB) $(HOSTCHECK) oracle $(RANKED_ORACLE)
 
 $(OBJDIR)/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -33,6 +35,11 @@ $(HOSTCHECK): $(CSRC)/hostcheck.cpp $(CSRC)/xxh64.cuh $(CSRC)/bitslice.cuh $(CSR
 
 oracle:
 	$(MAKE) -C oracle
+
+# the CPU oracle plus its ranked pick (tests/ranked_oracle.cpp), test infrastructure only
+$(RANKED_ORACLE): tests/ranked_oracle.cpp oracle/epp_oracle.cpp include/fi_epp.h
+	@mkdir -p $(OBJDIR)
+	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ tests/ranked_oracle.cpp
 
 clean:
 	rm -rf $(OBJDIR) $(LIB) $(HOSTCHECK)

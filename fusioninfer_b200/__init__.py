@@ -14,6 +14,7 @@ from .picker import (  # noqa: F401
     FiEppError,
     PinnedBuffer,
     config_from_yaml,
+    config_picker_endpoints,
     default_config,
     make_config,
     model_seed,
@@ -24,6 +25,7 @@ __all__ = [
     "FiEppError",
     "PinnedBuffer",
     "config_from_yaml",
+    "config_picker_endpoints",
     "default_config",
     "make_config",
     "model_seed",

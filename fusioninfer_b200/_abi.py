@@ -18,6 +18,7 @@ FI_EPP_MAX_FILTERS = 4
 FI_EPP_MAX_LABELS = 24
 FI_ROLE_FIRST_FREE = 8
 FI_EPP_MAX_BLOCKS = 1023
+FI_EPP_MAX_RANKED = 16
 FI_NO_ENDPOINT = 0xFFFFFFFF
 FI_EPP_UNIQUE_ID_BYTES = 128
 
@@ -205,6 +206,7 @@ SYMBOLS = [
     ("fi_epp_status_string", C.c_char_p, [C.c_int]),
     ("fi_epp_config_default", C.c_int, [C.POINTER(fi_epp_config)]),
     ("fi_epp_config_from_yaml", C.c_int, [C.c_char_p, C.c_size_t, C.POINTER(fi_epp_config), C.c_char_p, C.c_size_t]),
+    ("fi_epp_config_picker_endpoints", C.c_int, [C.c_char_p, C.c_size_t, _P, C.c_char_p, C.c_size_t]),
     ("fi_epp_create", C.c_int, [C.POINTER(fi_epp_config), C.POINTER(_P)]),
     ("fi_epp_destroy", None, [_P]),
     ("fi_epp_last_error", C.c_char_p, [_P]),
@@ -228,6 +230,9 @@ SYMBOLS = [
     ("fi_epp_pick_batch_device", C.c_int, [_P, _P, _P, _P, C.c_uint32, C.c_uint64, _P, _P, _P]),
     ("fi_epp_pick_batch_lora", C.c_int, [_P, _P, _P, _P, _P, C.c_uint32, _P, _P]),
     ("fi_epp_pick_batch_device_lora", C.c_int, [_P, _P, _P, _P, _P, C.c_uint32, C.c_uint64, _P, _P, _P]),
+    ("fi_epp_pick_batch_ranked", C.c_int, [_P, _P, _P, _P, _P, C.c_uint32, C.c_uint32, _P, _P]),
+    ("fi_epp_pick_batch_device_ranked", C.c_int,
+     [_P, _P, _P, _P, _P, C.c_uint32, C.c_uint64, C.c_uint32, _P, _P, _P]),
     ("fi_epp_pinned_alloc", _P, [C.c_size_t]),
     ("fi_epp_pinned_free", None, [_P]),
     ("fi_epp_comm_unique_id", C.c_int, [_P]),

@@ -200,6 +200,9 @@ struct fi_epp {
   uint64_t* d_chain = nullptr;
   uint32_t* d_nblocks = nullptr;
   fi_pick* d_picks = nullptr;   // [R][P] final
+  fi_pick* d_ranked = nullptr;  // [R][P][k] of fi_epp_pick_batch_ranked: allocated by the first such call, grown with k
+  fi_pick* h_ranked = nullptr;  // pinned mirror
+  size_t ranked_cap = 0;        // picks both hold
   fi_pick* d_local = nullptr;   // [R][P] this rank's picks (sharded)
   fi_pick* d_gather = nullptr;  // [world][R][P]
   // peer-memory exchange (sharded mode; kernels.cuh PeerXchg)
@@ -1170,9 +1173,10 @@ void fill_match_params(fi_epp* h, MatchParams& mp, const uint64_t* chain, const 
   mp.lane_zero = 0;
 }
 
-// the whole pick on device buffers; result in d_out ([R][P])
+// the whole pick on device buffers; result in d_out ([R][P], or [R][P][ranked_k] for the ranked pick, ranked_k > 0:
+// single rank only)
 int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0,
-                  const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed) {
+                  const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed, uint32_t ranked_k) {
   const bool sharded = h->world > 1;
   if (sharded && (h->n_sets || h->n_clears))
     return fail(h, FI_ERR_STATE, "sharded pool: index updates are collective (fi_epp_index_apply / fi_epp_index_add_chains)");
@@ -1198,6 +1202,7 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
   }
   MatchParams mp{};
   fill_match_params(h, mp, h->d_chain, h->d_nblocks, d_offsets, d_h0, d_adapters, R, sharded ? h->d_local : d_out, !sharded);
+  mp.k = ranked_k;
 
   const uint32_t S = h->feed_slices;
   if (feed && !sharded && h->fast_hash && S > 1 && R >= 64 * S && feed->offsets[R] >= (8ull << 20)) {
@@ -1226,7 +1231,7 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
       ms.h0 = mp.h0 + r0;
       ms.r_base = r0;
       ms.R = Rk;
-      ms.out = mp.out + (size_t)r0 * h->P;
+      ms.out = mp.out + (size_t)r0 * h->P * (ranked_k ? ranked_k : 1);
       ms.work_counter = h->d_work + k;
       LaunchScope ls(h, h->s_main, K_MATCH);
       FI_CUDA(launch_match_pick(ms, h->sm_count, h->s_main));
@@ -1327,8 +1332,8 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
 }
 
 int run_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0,
-             const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed = nullptr) {
-  int rc = run_pick_impl(h, d_prompts, d_offsets, d_h0, d_adapters, R, d_out, feed);
+             const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed = nullptr, uint32_t ranked_k = 0) {
+  int rc = run_pick_impl(h, d_prompts, d_offsets, d_h0, d_adapters, R, d_out, feed, ranked_k);
   if (rc != FI_OK) return rc;
   h->ev_pick = h->ev_pick_own;
   FI_CUDA(cudaEventRecord(h->ev_pick, h->s_main));  // index updates submitted later wait for this pick
@@ -1737,6 +1742,7 @@ void fi_epp_destroy(fi_epp* h) {
   cudaFree(h->d_chain);
   cudaFree(h->d_nblocks);
   cudaFree(h->d_picks);
+  cudaFree(h->d_ranked);
   cudaFree(h->d_local);
   cudaFree(h->d_gather);
   cudaFree(h->d_glog_n);
@@ -1778,6 +1784,7 @@ void fi_epp_destroy(fi_epp* h) {
     if (h->ev_buf[b]) cudaEventDestroy(h->ev_buf[b]);
   }
   if (h->h_picks) cudaFreeHost(h->h_picks);
+  if (h->h_ranked) cudaFreeHost(h->h_ranked);
   if (h->h_offsets) cudaFreeHost(h->h_offsets);
   if (h->h_h0) cudaFreeHost(h->h_h0);
   if (h->h_nblocks) cudaFreeHost(h->h_nblocks);
@@ -2569,6 +2576,86 @@ int fi_epp_pick_batch_device_lora(fi_epp* h, const void* d_prompts, const void* 
   FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_user, 0));
   int rc = run_pick(h, (const uint8_t*)d_prompts, (const uint64_t*)d_offsets, (const uint64_t*)d_h0,
                     (const uint64_t*)d_adapters, R, (fi_pick*)d_out);
+  if (rc != FI_OK) return rc;
+  if (d_chains_out) {
+    rc = copy_chains_out(h, (uint64_t*)d_chains_out, R, cudaMemcpyDeviceToDevice, h->s_main);
+    if (rc != FI_OK) return rc;
+  }
+  FI_CUDA(cudaEventRecord(h->ev_done, h->s_main));
+  FI_CUDA(cudaStreamWaitEvent(us, h->ev_done, 0));
+  return FI_OK;
+}
+
+// ---- ranked picks (docs/SPEC.md S.6a): run_pick with k > 0, which selects the RANKED match-kernel variant --------
+int fi_epp_pick_batch_ranked(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
+                             const uint64_t* adapters, uint32_t R, uint32_t k, fi_pick* out, uint64_t* chains_out) {
+  if (!h || !offsets || (!h0 && R) || !out || (!prompts && R && offsets[R])) return FI_ERR_INVALID;
+  if (k == 0 || k > FI_EPP_MAX_RANKED) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  if (h->world > 1) return fail(h, FI_ERR_STATE, "ranked picks need a single-rank pool");
+  if (R == 0) return FI_OK;
+  uint64_t total = 0;
+  int rc = check_batch(h, offsets, R, &total);
+  if (rc != FI_OK) return rc;
+  // the k-wide result buffers exist only on handles that rank; sized for max_batch so that R does not regrow them
+  const size_t need = (size_t)h->cfg.max_batch * h->P * k;
+  if (need > h->ranked_cap) {
+    FI_CUDA(cudaStreamSynchronize(h->s_main));
+    cudaFree(h->d_ranked);
+    if (h->h_ranked) cudaFreeHost(h->h_ranked);
+    h->d_ranked = nullptr;
+    h->h_ranked = nullptr;
+    h->ranked_cap = 0;
+    if (cudaMalloc(&h->d_ranked, need * sizeof(fi_pick)) != cudaSuccess ||
+        cudaMallocHost(&h->h_ranked, need * sizeof(fi_pick)) != cudaSuccess) {
+      cudaGetLastError();
+      cudaFree(h->d_ranked);
+      if (h->h_ranked) cudaFreeHost(h->h_ranked);
+      h->d_ranked = nullptr;
+      h->h_ranked = nullptr;
+      return fail(h, FI_ERR_NOMEM, "cannot allocate the ranked pick buffers");
+    }
+    h->ranked_cap = need;
+  }
+  rc = stage_inputs(h, prompts, offsets, h0, R, total, /*copy_prompts=*/false);  // run_pick feeds the prompts
+  if (rc != FI_OK) return rc;
+  if (adapters) {
+    std::memcpy(h->h_adapters, adapters, (size_t)R * sizeof(uint64_t));
+    FI_CUDA(cudaMemcpyAsync(h->d_adapters, h->h_adapters, (size_t)R * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main));
+    h->stats.h2d_bytes += (size_t)R * sizeof(uint64_t);
+  }
+  const HostFeed feed{prompts, offsets};
+  rc = run_pick(h, h->d_prompts, h->d_offsets, h->d_h0, adapters ? h->d_adapters : nullptr, R, h->d_ranked, &feed, k);
+  if (rc != FI_OK) return rc;
+  const size_t pb = (size_t)R * h->P * k * sizeof(fi_pick);
+  FI_CUDA(cudaMemcpyAsync(h->h_ranked, h->d_ranked, pb, cudaMemcpyDeviceToHost, h->s_main));
+  h->stats.d2h_bytes += pb;
+  if (chains_out) {
+    rc = copy_chains_out(h, chains_out, R, cudaMemcpyDeviceToHost, h->s_main);
+    if (rc != FI_OK) return rc;
+  }
+  FI_CUDA(cudaStreamSynchronize(h->s_main));
+  std::memcpy(out, h->h_ranked, pb);
+  return FI_OK;
+}
+
+int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                                    const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, uint32_t k,
+                                    void* d_out, void* d_chains_out, void* stream) {
+  if (!h || !d_offsets || (!d_h0 && R) || !d_out) return FI_ERR_INVALID;
+  if (k == 0 || k > FI_EPP_MAX_RANKED) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  if (h->world > 1) return fail(h, FI_ERR_STATE, "ranked picks need a single-rank pool");
+  if (R == 0) return FI_OK;
+  if (R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
+  (void)total_prompt_bytes;  // inputs stay where they are: no staging copy, no capacity limit
+  cudaStream_t us = (cudaStream_t)stream;
+  FI_CUDA(cudaEventRecord(h->ev_user, us));
+  FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_user, 0));
+  int rc = run_pick(h, (const uint8_t*)d_prompts, (const uint64_t*)d_offsets, (const uint64_t*)d_h0,
+                    (const uint64_t*)d_adapters, R, (fi_pick*)d_out, nullptr, k);
   if (rc != FI_OK) return rc;
   if (d_chains_out) {
     rc = copy_chains_out(h, (uint64_t*)d_chains_out, R, cudaMemcpyDeviceToDevice, h->s_main);

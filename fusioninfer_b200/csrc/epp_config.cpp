@@ -280,11 +280,22 @@ static uint32_t label_bit(fi_epp_config& cfg, const std::string& label, const st
   return bit;
 }
 
-extern "C" int fi_epp_config_from_yaml(const char* yaml, size_t len, fi_epp_config* cfg, char* err, size_t err_len) {
-  if (!yaml || !cfg) {
-    set_err(err, err_len, "null argument");
-    return FI_ERR_INVALID;
-  }
+// maxNumOfEndpoints of a max-score-picker: how many endpoints upstream's picker returns, best first (default 1)
+static uint32_t picker_max_endpoints(const Plugin& p) {
+  const Node* n = p.params ? p.params->get("maxNumOfEndpoints") : nullptr;
+  if (!n) return 1;
+  long long v = 0;
+  if (n->kind != Node::SCALAR || !to_i64(n->scalar, &v) || v < 1 || v > (long long)FI_EPP_MAX_RANKED)
+    throw ParseError{"max-score-picker " + p.name + ": maxNumOfEndpoints must be an integer in [1, " +
+                     std::to_string(FI_EPP_MAX_RANKED) + "]"};
+  return (uint32_t)v;
+}
+
+// The loader behind fi_epp_config_from_yaml and fi_epp_config_picker_endpoints.  picker_endpoints != NULL: also
+// read each profile's max-score-picker maxNumOfEndpoints into picker_endpoints[profile] (1 when absent), and reject
+// a value that is not an integer in [1, FI_EPP_MAX_RANKED].  With NULL that parameter is not looked at, so
+// fi_epp_config_from_yaml accepts every document it accepted before the ranked pick existed.
+static int load_config(const char* yaml, size_t len, fi_epp_config* cfg, uint32_t* picker_endpoints, char* err, size_t err_len) {
   try {
     std::vector<Line> lines = split_lines(yaml, len);
     if (lines.empty()) throw ParseError{"empty document"};
@@ -413,6 +424,7 @@ extern "C" int fi_epp_config_from_yaml(const char* yaml, size_t len, fi_epp_conf
           prof.scorers[prof.n_scorers].weight = (int32_t)weight;
           ++prof.n_scorers;
         } else if (p->type == "max-score-picker") {
+          if (picker_endpoints && !has_picker) picker_endpoints[out.n_profiles] = picker_max_endpoints(*p);
           has_picker = true;
         } else if (p->type == "by-label") {
           // strategy.go:135-144 shows the schema: `label` + `validValues`.  Every (label, value) pair stands for
@@ -460,4 +472,26 @@ extern "C" int fi_epp_config_from_yaml(const char* yaml, size_t len, fi_epp_conf
     set_err(err, err_len, e.what());
     return FI_ERR_CONFIG;
   }
+}
+
+extern "C" int fi_epp_config_from_yaml(const char* yaml, size_t len, fi_epp_config* cfg, char* err, size_t err_len) {
+  if (!yaml || !cfg) {
+    set_err(err, err_len, "null argument");
+    return FI_ERR_INVALID;
+  }
+  return load_config(yaml, len, cfg, nullptr, err, err_len);
+}
+
+extern "C" int fi_epp_config_picker_endpoints(const char* yaml, size_t len, uint32_t out[FI_EPP_MAX_PROFILES], char* err,
+                                              size_t err_len) {
+  if (!yaml || !out) {
+    set_err(err, err_len, "null argument");
+    return FI_ERR_INVALID;
+  }
+  uint32_t k[FI_EPP_MAX_PROFILES] = {};  // profiles the document does not have stay 0
+  fi_epp_config scratch{};
+  const int rc = load_config(yaml, len, &scratch, k, err, err_len);
+  if (rc != FI_OK) return rc;
+  std::memcpy(out, k, sizeof(k));
+  return FI_OK;
 }

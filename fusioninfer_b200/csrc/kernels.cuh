@@ -160,12 +160,13 @@ struct MatchParams {
   // pd-profile-handler
   uint32_t apply_pd, pd_decode, pd_prefill;
   double pd_threshold;
-  fi_pick* out;                       // [R][P]
+  fi_pick* out;                       // [R][P], or [R][P][k] when k > 0
   unsigned long long* probed_blocks;  // optional Σ N_probe
   uint32_t* work_counter;             // dynamic request queue of the launch
   uint32_t zero_work_counter;         // launcher zeroes it first (0: the caller already did)
   uint32_t max_ctas_per_sm;           // 0: as many as fit; else a cap (pipelined API: leave room for hash_blocks)
   uint32_t lane_zero;                 // always 0: makes the ticket address formally lane-dependent (match_kernels.cu take_ticket)
+  uint32_t k;                         // 0: one pick per profile, out [R][P]; else the ranked pick, out [R][P][k] (S.6a)
   PeerXchg px;                        // sharded mode, peer-memory exchange (px.enabled)
 };
 

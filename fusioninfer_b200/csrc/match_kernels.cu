@@ -19,7 +19,7 @@
 //      share the per-batch "zero-match best" precomputed by prepare_endpoints —
 //      valid because every scorer weight is >= 0, so a total is monotone in the
 //      match count;
-//   5. warp-shuffle argmax; equal totals are resolved by the request's tie rotation (tiebreak.cuh — upstream's
+//   5. warp-shuffle argmax (the RANKED variant: k selection rounds, ranked_profile); equal totals are resolved by the request's tie rotation (tiebreak.cuh — upstream's
 //      MaxScorePicker shuffles, Appendix A.5), then the pd-profile-handler threshold rule (Appendix A.6,
 //      /root/reference/pkg/router/strategy.go:129-133).
 //
@@ -244,11 +244,96 @@ __device__ __forceinline__ uint32_t take_ticket(uint32_t* counter, uint32_t opaq
   return t;
 }
 
+// docs/SPEC.md S.6a, the ranked pick of one profile (RANKED variant of match_pick_kernel): out[(r*P + pi)*k + j] for
+// j < k.  Every eligible endpoint is scored, the way the LoRA branch does: after the merge every lane group holds
+// the full counters, so group g takes bits [g*32/G, (g+1)*32/G) of its lanes' words (the per-batch zero-match best
+// does not apply; lora_score only when the configuration has a LoRA scorer).  k rounds then select in the single
+// pick's order — better(): total desc, then the tie rotation, a strict total order because tie keys are unique.
+// Each lane keeps its best endpoint among those ranked after the previous round's winner; a warp butterfly picks
+// the round's winner and only the lane that owned it rescans its endpoints, bounded by the winner's (score, key).
+// No "taken" mask: a round is one butterfly plus one lane's rescan.  Once every lane is out of candidates the
+// rounds write the padding entry (FI_NO_ENDPOINT, match 0, score 0).
+template <int VEC, int G>
+__device__ __forceinline__ void ranked_profile(const MatchParams& p, uint32_t pi, const BitCounter (&cnt)[VEC],
+                                               const TieRot& tr, uint32_t n, uint32_t r, int lane, int t, int g,
+                                               uint32_t& dec_e, uint32_t& dec_m) {
+  const ProfileDev& pr = p.st.prof[pi];
+  const double* sc_p = p.st.sc + (uint64_t)pi * FI_EPP_MAX_SCORERS * p.st.Epad;
+  const bool lora = p.st.has_lora != 0;
+  const uint64_t adapter = (lora && p.adapters) ? p.adapters[r] : 0;
+  constexpr uint32_t BPG = 32 / G;
+  const uint32_t gmask_bits = (BPG >= 32 ? 0xFFFFFFFFu : ((1u << BPG) - 1u)) << (g * BPG);
+  // this lane's best endpoint ranked strictly after (ts, tk); ts < 0: no bound (totals are >= 0)
+  auto scan = [&](double ts, uint32_t tk) {
+    Best b;
+    b.score = -1.0;
+    b.e = FI_NO_ENDPOINT;
+    b.m = 0;
+    b.k = 0xFFFFFFFFu;
+#pragma unroll
+    for (int x = 0; x < VEC; ++x) {
+      const uint32_t wi = t * VEC + x;
+      uint32_t cand = p.st.elig[(uint64_t)pi * p.ix.W + wi] & gmask_bits;
+      while (cand) {
+        const uint32_t bit = __ffs(cand) - 1;
+        cand &= cand - 1;
+        const uint32_t e = wi * 32 + bit;
+        const uint32_t m = bc_get(cnt[x], bit);
+        const double s = total_score(pr, sc_p, p.st.Epad, e, m, n, lora ? lora_score(p.st.lora[e], adapter) : 0.0);
+        const uint32_t k = tr.key(e);
+        if (ts >= 0.0 && !(ts > s || (ts == s && tk < k))) continue;  // ranked before or at the bound
+        if (better(s, k, b)) {
+          b.score = s;
+          b.e = e;
+          b.m = m;
+          b.k = k;
+        }
+      }
+    }
+    return b;
+  };
+  Best b = scan(-1.0, 0u);
+  const uint32_t K = p.k;
+  fi_pick* out = p.out + ((uint64_t)r * p.st.n_profiles + pi) * K;
+  for (uint32_t j = 0; j < K; ++j) {
+    Best w = b;
+#pragma unroll
+    for (int d = 16; d > 0; d >>= 1) {
+      const double os = __shfl_xor_sync(FULL, w.score, d);
+      const uint32_t oe = __shfl_xor_sync(FULL, w.e, d);
+      const uint32_t om = __shfl_xor_sync(FULL, w.m, d);
+      const uint32_t ok = __shfl_xor_sync(FULL, w.k, d);
+      if (better(os, ok, w)) {
+        w.score = os;
+        w.e = oe;
+        w.m = om;
+        w.k = ok;
+      }
+    }
+    const bool none = w.e == FI_NO_ENDPOINT;  // warp-uniform
+    if (j == 0 && pi == p.pd_decode) {
+      dec_e = w.e;
+      dec_m = w.m;
+    }
+    if (lane == 0) {
+      fi_pick pk;
+      pk.endpoint = none ? FI_NO_ENDPOINT : w.e + p.ep_begin;
+      pk.match_blocks = none ? 0 : (uint16_t)w.m;
+      pk.n_blocks = (uint16_t)n;
+      pk.score = none ? 0.0 : w.score;
+      out[j] = pk;
+    }
+    if (!none && b.e == w.e) b = scan(w.score, w.k);  // endpoints belong to one lane each: only the winner's rescans
+  }
+}
+
 // LPR lanes read one row (VEC words each, LPR*VEC = words per row); a load
 // instruction therefore covers G = 32/LPR rows.  E = 1024 → LPR 16, VEC 2: a 128-byte
 // row is 16 × 8-byte loads and one instruction brings in 2 rows; 16 rows in flight.
-template <int LPR, int VEC, bool LPM, bool LORA>
-__global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 ? FI_MATCH_MIN_BLOCKS : FI_MATCH_MIN_BLOCKS + 1))
+// (The RANKED variant keeps the counters live through its selection rounds: it asks for two CTAs per SM, the
+// register budget of the four-word shape, instead of spilling under the three-CTA budget of the two-word one.)
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED>
+__global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MIN_BLOCKS : FI_MATCH_MIN_BLOCKS + 1))
     match_pick_kernel(const MatchParams p) {
   constexpr int G = 32 / LPR;                 // rows per load instruction
 #ifndef FI_MATCH_BATCH
@@ -431,6 +516,10 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 ? FI_MATCH_MIN_BLOCKS :
 #pragma unroll
     for (int pi = 0; pi < (int)FI_EPP_MAX_PROFILES; ++pi) {
       if (pi < (int)P) {
+        if constexpr (RANKED) {
+          ranked_profile<VEC, G>(p, (uint32_t)pi, cnt, tr, n, r, lane, t, g, dec_e, dec_m);
+          continue;
+        }
         const ProfileDev& pr = p.st.prof[pi];
         const double* sc_p = p.st.sc + (uint64_t)pi * FI_EPP_MAX_SCORERS * p.st.Epad;
         Best b;
@@ -554,7 +643,11 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 ? FI_MATCH_MIN_BLOCKS :
           pk.match_blocks = 0;
           pk.n_blocks = (uint16_t)n;
           pk.score = 0.0;
-          p.out[(uint64_t)r * P + p.pd_prefill] = pk;
+          if constexpr (RANKED) {  // the prefill profile's whole list
+            for (uint32_t j = 0; j < p.k; ++j) p.out[((uint64_t)r * P + p.pd_prefill) * p.k + j] = pk;
+          } else {
+            p.out[(uint64_t)r * P + p.pd_prefill] = pk;
+          }
         }
       }
       if (p.probed_blocks) atomicAdd(p.probed_blocks, (unsigned long long)(matched_rows + (real_miss ? 1 : 0)));
@@ -747,9 +840,9 @@ __global__ void __launch_bounds__(1024) prepare_endpoints_kernel(const EndpointD
 
 // One instantiation per kernel variant: the shared-memory opt-in (cudaFuncSetAttribute) applies to one function
 // only, and occupancy differs between variants, so each variant keeps its own cache, per device.
-template <int LPR, int VEC, bool LPM, bool LORA>
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED>
 cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_t s) {
-  const auto kern = match_pick_kernel<LPR, VEC, LPM, LORA>;
+  const auto kern = match_pick_kernel<LPR, VEC, LPM, LORA, RANKED>;
   const size_t smem = (size_t)kWarps * p.MP * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
   // occupancy is a property of (kernel, smem): query once per distinct smem size
   static size_t cached_smem_dev[64];
@@ -788,11 +881,14 @@ cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_
 template <int LPR, int VEC>
 cudaError_t launch_match_t(const MatchParams& p, int sm_count, cudaStream_t s) {
   const bool lpm = p.lpm == FI_MATCH_LPM;
+  if (p.k)  // ranked pick: the LoRA scorer is handled at run time inside the variant
+    return lpm ? launch_match_variant<LPR, VEC, true, false, true>(p, sm_count, s)
+               : launch_match_variant<LPR, VEC, false, false, true>(p, sm_count, s);
   if (p.st.has_lora)
-    return lpm ? launch_match_variant<LPR, VEC, true, true>(p, sm_count, s)
-               : launch_match_variant<LPR, VEC, false, true>(p, sm_count, s);
-  return lpm ? launch_match_variant<LPR, VEC, true, false>(p, sm_count, s)
-             : launch_match_variant<LPR, VEC, false, false>(p, sm_count, s);
+    return lpm ? launch_match_variant<LPR, VEC, true, true, false>(p, sm_count, s)
+               : launch_match_variant<LPR, VEC, false, true, false>(p, sm_count, s);
+  return lpm ? launch_match_variant<LPR, VEC, true, false, false>(p, sm_count, s)
+             : launch_match_variant<LPR, VEC, false, false, false>(p, sm_count, s);
 }
 
 }  // namespace

@@ -46,6 +46,18 @@ def config_from_yaml(yaml_text: str, base: Optional[abi.fi_epp_config] = None) -
     return cfg
 
 
+def config_picker_endpoints(yaml_text: str) -> list[int]:
+    """maxNumOfEndpoints of the max-score-picker each profile of the document references, in profile order (1 when
+    absent): how many ranked endpoints (pick_batch_ranked) each profile hands the proxy."""
+    raw = yaml_text.encode()
+    out = (C.c_uint32 * abi.FI_EPP_MAX_PROFILES)()
+    err = C.create_string_buffer(512)
+    rc = abi.load().fi_epp_config_picker_endpoints(raw, len(raw), out, err, len(err))
+    if rc != abi.FI_OK:
+        raise FiEppError(rc, "fi_epp_config_picker_endpoints", err.value.decode())
+    return [int(v) for v in out if v]
+
+
 def make_config(
     *,
     num_endpoints: int,
@@ -272,6 +284,18 @@ class EndpointPicker:
         self._check(rc, "fi_epp_pick_batch")
         return (picks, chains) if want_chains else picks
 
+    def pick_batch_ranked(self, prompts, offsets, h0, k: int, want_chains: bool = False, adapters=None):
+        """The best k endpoints of every profile, best first (docs/SPEC.md S.6a).  -> picks [R, n_profiles, k]
+        (PICK_DTYPE)[, chains]; entry 0 is pick_batch's pick, a short list ends in FI_NO_ENDPOINT entries."""
+        prompts, offsets, h0, R = self._inputs(prompts, offsets, h0)
+        picks = np.zeros((R, self.n_profiles, max(int(k), 1)), dtype=PICK_DTYPE)
+        chains = np.zeros((R, self.max_blocks), dtype=np.uint64) if want_chains else None
+        ad = None if adapters is None else np.ascontiguousarray(np.broadcast_to(np.asarray(adapters, dtype=np.uint64), (R,)))
+        rc = self._lib.fi_epp_pick_batch_ranked(self._h, _ptr(prompts), _ptr(offsets), _ptr(h0), _ptr(ad), R, int(k),
+                                                _ptr(picks), _ptr(chains))
+        self._check(rc, "fi_epp_pick_batch_ranked")
+        return (picks, chains) if want_chains else picks
+
     def pick_batch_raw(self, prompts_ptr: int, offsets_ptr: int, h0_ptr: int, R: int, out_ptr: int, chains_ptr: int = 0):
         """Host-pointer variant without numpy marshalling (pinned buffers from pinned_alloc)."""
         self._check(
@@ -287,6 +311,17 @@ class EndpointPicker:
                 self._h, d_prompts, d_offsets, d_h0, R, total_bytes, d_out, d_chains or None, stream or None
             ),
             "fi_epp_pick_batch_device",
+        )
+
+    def pick_batch_device_ranked(self, d_prompts: int, d_offsets: int, d_h0: int, R: int, total_bytes: int, k: int,
+                                 d_out: int, d_chains: int = 0, stream: int = 0, d_adapters: int = 0):
+        """pick_batch_ranked on device buffers: d_out holds R * n_profiles * k picks."""
+        self._check(
+            self._lib.fi_epp_pick_batch_device_ranked(
+                self._h, d_prompts, d_offsets, d_h0, d_adapters or None, R, total_bytes, int(k), d_out, d_chains or None,
+                stream or None
+            ),
+            "fi_epp_pick_batch_device_ranked",
         )
 
     def pick_submit(self, d_prompts: int, d_offsets: int, d_h0: int, R: int, total_bytes: int, d_out: int, stream: int = 0):

@@ -233,6 +233,15 @@ int fi_epp_config_default(fi_epp_config* cfg);
  * On FI_ERR_CONFIG a message is written to err (NUL-terminated, truncated). */
 int fi_epp_config_from_yaml(const char* yaml, size_t len, fi_epp_config* cfg, char* err, size_t err_len);
 
+/* Widest ranked pick (fi_epp_pick_batch_ranked): a max-score-picker may ask for this many endpoints per profile. */
+#define FI_EPP_MAX_RANKED 16u
+/* maxNumOfEndpoints of the max-score-picker each profile references, in the profile order
+ * fi_epp_config_from_yaml produces (1 when absent); entries past the document's profiles are 0.  FI_ERR_CONFIG for
+ * a value that is not an integer in [1, FI_EPP_MAX_RANKED], and for everything fi_epp_config_from_yaml rejects
+ * (which itself does not look at maxNumOfEndpoints). */
+int fi_epp_config_picker_endpoints(const char* yaml, size_t len, uint32_t out[FI_EPP_MAX_PROFILES], char* err,
+                                   size_t err_len);
+
 int fi_epp_create(const fi_epp_config* cfg, fi_epp** out);
 void fi_epp_destroy(fi_epp* h);
 const char* fi_epp_last_error(const fi_epp* h);
@@ -340,6 +349,24 @@ int fi_epp_pick_batch_lora(fi_epp* h, const uint8_t* prompts, const uint64_t* of
 int fi_epp_pick_batch_device_lora(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
                                   const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, void* d_out,
                                   void* d_chains_out, void* stream);
+
+/* Ranked picks: upstream max-score-picker with maxNumOfEndpoints = k.  For each request and profile the profile's
+ * eligible endpoints ordered by total descending, then by the request's tie rotation ("Ties" above) — the order
+ * whose first entry is the pick of fi_epp_pick_batch, bit for bit.  Each entry carries the endpoint's own
+ * match_blocks and fp64 total; fewer than k eligible endpoints: the tail is FI_NO_ENDPOINT, match 0, score 0.  With
+ * pd_enabled the threshold test uses the decode profile's entry 0, and a skipped prefill profile's whole list is
+ * FI_NO_ENDPOINT.  A profile's top k_p is the first k_p entries of its top k, so one call with k = max_p k_p (see
+ * fi_epp_config_picker_endpoints) serves profiles with different limits.
+ * out: R*n_profiles*k picks, out[(r*n_profiles + p)*k + j] = rank j of profile p.  1 <= k <= FI_EPP_MAX_RANKED
+ * (else FI_ERR_INVALID); adapters may be NULL (as fi_epp_pick_batch_lora); FI_ERR_STATE on a sharded pool.
+ * Otherwise they behave like fi_epp_pick_batch_lora / fi_epp_pick_batch_device_lora: the same staging, chains_out,
+ * ordering against index updates, removals and pipelined submits, and fi_epp_index_add_chains_device(.., NULL, ..)
+ * afterwards adds this call's chains. */
+int fi_epp_pick_batch_ranked(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
+                             const uint64_t* adapters, uint32_t R, uint32_t k, fi_pick* out, uint64_t* chains_out);
+int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                                    const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, uint32_t k,
+                                    void* d_out, void* d_chains_out, void* stream);
 
 /* Pipelined device path.  fi_epp_pick_submit enqueues one batch exactly like fi_epp_pick_batch_device (inputs
  * ready in `stream` order at the call) but does NOT order `stream` behind the result: batch k+1's block
