@@ -5,7 +5,6 @@
 // ordered before the next pick), the host LRU, the per-batch score tables, and the
 // optional NCCL communicator for endpoint-range sharded pools.  No CPU fallback:
 // creation fails without a CUDA device.
-#include <cuda.h>  // types and prototypes of the green-context API only: reached through cudaGetDriverEntryPoint, libcuda is not linked
 #include <cuda_runtime.h>
 #include <unistd.h>
 #include <dlfcn.h>
@@ -153,43 +152,9 @@ struct fi_epp {
   uint64_t* d_chain2 = nullptr;
   uint32_t* d_nblocks2 = nullptr;
   cudaEvent_t ev_in = nullptr, ev_a[2] = {}, ev_b[2] = {};
-  cudaEvent_t ev_pick = nullptr;   // completion of the most recent pick of any kind: ev_pick_own, or (partitioned
-                                   // pipeline) the slot event of the batch submitted last — a handle, not a second record
-  cudaEvent_t ev_pick_own = nullptr;
+  cudaEvent_t ev_pick = nullptr;   // completion of the most recent pick of any kind (recorded on s_main)
   cudaEvent_t ev_plain = nullptr;  // completion of the most recent stream-ordered (not pipelined) pick
   uint64_t pipe_seq = 0;          // batches submitted
-  // per-SM caps of the pipelined path's two co-running kernels (0 = uncapped); FI_EPP_PIPE_HASH_CTAS /
-  // FI_EPP_PIPE_MATCH_CTAS, option "pipe_hash_ctas" / "pipe_match_ctas".  The hash cap applies where stage A is
-  // hash_blocks (the partitioned pipeline, block sizes hash_chain does not take): hash_chain CTAs (32 to 128
-  // requests each) fill a whole SM, whatever the cap.
-  uint32_t pipe_hash_ctas = 0;
-  uint32_t pipe_match_ctas = 0;
-  // SM-partitioned pipeline (green contexts, CUDA 12.4+): the chain walk is serial latency that fills a few % of
-  // the warp slots but cannot share schedulers with a busy kernel, so without a partition nothing overlaps it.
-  // With the GPU split into a partition for the walker and one for hash_blocks / match_pick, batch k is matched
-  // while batch k+1's chains are walked and batch k+2 is hashed: three batches in flight.
-  // FI_EPP_PIPE_PARTITION=<SMs> / option "pipe_partition": SMs asked for the walker partition (0 = off: two
-  // batches in flight on the whole GPU).  Off by default: on an H100 (132 SMs) hash_blocks dominates the step
-  // and loses more on the smaller partition than the overlapped walk saves.  Measured at cfg 3 on one H100 SXM
-  // (700 W), us per step: off 219.7; 24 -> 261.5, 32 -> 255.1, 40 -> 259.1, 48 -> 256.7, 56 -> 261.5; with the
-  // L1-allocating prompt loads of hash_kernels.cu: off 201.0-201.5, 40 -> 243.9-245.6.
-  int part_want = 0;
-  int part_compact = -1;        // walker shape on the partition: -1 = the 64-register shape only where the 78-register one does
-                                // not fit (fewer than 24 SMs); FI_EPP_WALK_COMPACT=0/1 forces it
-  int part_state = 0;           // 0: not tried, 1: active, -1: unavailable (fallback to the unpartitioned pipeline)
-  bool part_active = false;     // the partitioned pipeline has batches in flight / owns the slot events
-  // how often ev_index / ev_plain / ev_lru have been re-recorded, and the values the partitioned pipeline's streams
-  // already waited for: a submit makes ~16 runtime calls instead of ~23 (eight processes on a 16-core host are
-  // launch-bound otherwise)
-  uint64_t gen_index = 0, gen_plain = 0, gen_lru = 0;
-  uint64_t seen_index = ~0ull, seen_plain = ~0ull, seen_lru = ~0ull;
-  uint64_t part_seq = 0;        // batches submitted to it since it last became active
-  int part_walk_sms = 0, part_main_sms = 0;
-  CUgreenCtx gctx_walk = nullptr, gctx_main = nullptr;
-  cudaStream_t s_pw = nullptr, s_pa = nullptr, s_pb = nullptr;  // walker | hashing, matching (big partition)
-  uint64_t* d_pre2 = nullptr;
-  uint32_t* d_nblocks3 = nullptr;
-  cudaEvent_t ev_h[2] = {}, ev_b3[3] = {}, ev_up = nullptr;
   cudaEvent_t ev_index = nullptr, ev_user = nullptr, ev_done = nullptr, ev_ctr = nullptr;
 
   // request buffers (device)
@@ -495,7 +460,6 @@ int check_counters(fi_epp* h) {
     int rc = rebuild_index(h);
     if (rc != FI_OK) return rc;
     FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
-  h->gen_index++;
   }
   return FI_OK;
 }
@@ -543,7 +507,6 @@ int flush_ops(fi_epp* h) {
   FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
   h->ctr_pending = true;
   FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
-  h->gen_index++;
   h->n_sets = h->n_clears = 0;
   h->cleared.clear();
   h->cur_buf ^= 1;
@@ -595,7 +558,6 @@ int gossip_round(fi_epp* h) {
     h->ctr_pending = true;
   }
   FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
-  h->gen_index++;
   return FI_OK;
 }
 
@@ -731,7 +693,6 @@ int alloc_dev_lru(fi_epp* h) {
   FI_CUDA(cudaMemsetAsync(h->d_lru_state, 0, state_words * sizeof(uint32_t), h->s_index));
   FI_CUDA(cudaMemsetAsync(h->d_lru_ctr, 0, 8 * sizeof(unsigned long long), h->s_index));
   FI_CUDA(cudaEventRecord(h->ev_lru, h->s_index));
-  h->gen_lru++;
   d.head = h->d_lru_state;
   d.tail = d.head + EL;
   d.count = d.tail + EL;
@@ -943,9 +904,7 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
   if (rc != FI_OK) return rc;
   FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));  // covers the status copy too
   FI_CUDA(cudaEventRecord(h->ev_lru, h->s_index));
-  h->gen_lru++;
   FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
-  h->gen_index++;
   if (h->verbose) {
     const auto t1 = std::chrono::steady_clock::now();
     std::fprintf(stderr, "[fi_epp] device LRU%s: %u requests (%zu kept), %zu sub-batch(es), %zu deferred, host side %.3f ms\n",
@@ -996,10 +955,10 @@ int run_hash(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, con
     uint64_t* pre = h->d_pre + (size_t)r0 * h->MP;  // tiled by groups of 32 requests: r0 % 32 == 0
     {
       LaunchScope ls(h, s, K_HASH);
-      FI_CUDA(launch_hash_blocks(d_prompts, d_offsets + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, pre, nb, 0, s));
+      FI_CUDA(launch_hash_blocks(d_prompts, d_offsets + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, pre, nb, s));
     }
     LaunchScope ls(h, s, K_CHAIN);
-    FI_CUDA(launch_chain_finalize(pre, nb, d_h0 + r0, R, h->MP, chain, false, s));
+    FI_CUDA(launch_chain_finalize(pre, nb, d_h0 + r0, R, h->MP, chain, s));
   } else {
     LaunchScope ls(h, s, K_HASH);
     FI_CUDA(launch_hash_generic(d_prompts, d_offsets + r0, d_h0 + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP,
@@ -1169,7 +1128,6 @@ void fill_match_params(fi_epp* h, MatchParams& mp, const uint64_t* chain, const 
   mp.out = out;
   mp.probed_blocks = h->profiling ? h->d_probed : nullptr;
   mp.work_counter = h->d_work;
-  mp.zero_work_counter = 1;
   mp.lane_zero = 0;
 }
 
@@ -1195,11 +1153,8 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
   if (rc != FI_OK) return rc;
   rc = upload_lora(h);
   if (rc != FI_OK) return rc;
-  if (h->pipe_seq) {  // a plain pick after pipelined submits: their stages share d_pre / d_chain with ours
+  if (h->pipe_seq)  // a plain pick after pipelined submits: their stages share d_pre / d_chain with ours
     FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[(h->pipe_seq - 1) & 1], 0));
-    FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_pick, 0));  // (their matches may run on the partition's stream)
-    h->part_active = false;
-  }
   MatchParams mp{};
   fill_match_params(h, mp, h->d_chain, h->d_nblocks, d_offsets, d_h0, d_adapters, R, sharded ? h->d_local : d_out, !sharded);
   mp.k = ranked_k;
@@ -1335,191 +1290,9 @@ int run_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, con
              const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed = nullptr, uint32_t ranked_k = 0) {
   int rc = run_pick_impl(h, d_prompts, d_offsets, d_h0, d_adapters, R, d_out, feed, ranked_k);
   if (rc != FI_OK) return rc;
-  h->ev_pick = h->ev_pick_own;
   FI_CUDA(cudaEventRecord(h->ev_pick, h->s_main));  // index updates submitted later wait for this pick
   FI_CUDA(cudaEventRecord(h->ev_plain, h->s_main));
-  h->gen_plain++;
   h->last_plain_R = R;
-  return FI_OK;
-}
-
-// ---- SM partition of the pipelined path (green contexts through the driver entry points) ------------------
-struct GreenApi {
-  CUresult (*DeviceGet)(CUdevice*, int) = nullptr;
-  CUresult (*DeviceGetDevResource)(CUdevice, CUdevResource*, CUdevResourceType) = nullptr;
-  CUresult (*DevSmResourceSplitByCount)(CUdevResource*, unsigned int*, const CUdevResource*, CUdevResource*, unsigned int,
-                                        unsigned int) = nullptr;
-  CUresult (*DevResourceGenerateDesc)(CUdevResourceDesc*, CUdevResource*, unsigned int) = nullptr;
-  CUresult (*GreenCtxCreate)(CUgreenCtx*, CUdevResourceDesc, CUdevice, unsigned int) = nullptr;
-  CUresult (*GreenCtxDestroy)(CUgreenCtx) = nullptr;
-  CUresult (*GreenCtxStreamCreate)(CUstream*, CUgreenCtx, unsigned int, int) = nullptr;
-  bool loaded = false, ok = false;
-};
-GreenApi g_green;
-
-bool load_green_api() {
-  if (g_green.loaded) return g_green.ok;
-  g_green.loaded = true;
-  auto get = [](const char* name, void** fn) {
-    cudaDriverEntryPointQueryResult qr;
-    return cudaGetDriverEntryPoint(name, fn, cudaEnableDefault, &qr) == cudaSuccess && qr == cudaDriverEntryPointSuccess && *fn;
-  };
-  g_green.ok = get("cuDeviceGet", (void**)&g_green.DeviceGet) &&
-               get("cuDeviceGetDevResource", (void**)&g_green.DeviceGetDevResource) &&
-               get("cuDevSmResourceSplitByCount", (void**)&g_green.DevSmResourceSplitByCount) &&
-               get("cuDevResourceGenerateDesc", (void**)&g_green.DevResourceGenerateDesc) &&
-               get("cuGreenCtxCreate", (void**)&g_green.GreenCtxCreate) &&
-               get("cuGreenCtxDestroy", (void**)&g_green.GreenCtxDestroy) &&
-               get("cuGreenCtxStreamCreate", (void**)&g_green.GreenCtxStreamCreate);
-  cudaGetLastError();
-  return g_green.ok;
-}
-
-void destroy_partition(fi_epp* h) {
-  if (g_green.ok) {
-    if (h->gctx_walk) g_green.GreenCtxDestroy(h->gctx_walk);
-    if (h->gctx_main) g_green.GreenCtxDestroy(h->gctx_main);
-  }
-  h->gctx_walk = h->gctx_main = nullptr;
-}
-
-// Try to split the GPU; on any failure the pipelined path keeps running unpartitioned.
-void setup_partition(fi_epp* h) {
-  if (h->part_state != 0) return;
-  h->part_state = -1;
-  if (h->part_want <= 0 || h->world > 1 || !load_green_api()) return;
-  CUdevice dev;
-  CUdevResource all{}, grp{}, rem{};
-  unsigned int nb = 1;
-  if (g_green.DeviceGet(&dev, h->cfg.device) != CUDA_SUCCESS) return;
-  if (g_green.DeviceGetDevResource(dev, &all, CU_DEV_RESOURCE_TYPE_SM) != CUDA_SUCCESS) return;
-  if (g_green.DevSmResourceSplitByCount(&grp, &nb, &all, &rem, 0, (unsigned)h->part_want) != CUDA_SUCCESS || nb != 1) return;
-  if (grp.sm.smCount < 8 || rem.sm.smCount < 64) return;
-  CUdevResourceDesc dw = nullptr, dm = nullptr;
-  if (g_green.DevResourceGenerateDesc(&dw, &grp, 1) != CUDA_SUCCESS) return;
-  if (g_green.DevResourceGenerateDesc(&dm, &rem, 1) != CUDA_SUCCESS) return;
-  if (g_green.GreenCtxCreate(&h->gctx_walk, dw, dev, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS) return;
-  if (g_green.GreenCtxCreate(&h->gctx_main, dm, dev, CU_GREEN_CTX_DEFAULT_STREAM) != CUDA_SUCCESS) {
-    destroy_partition(h);
-    return;
-  }
-  // hash_blocks(k+2) and match_pick(k) become runnable at the same moment (both wait for match_pick(k-1)) and share
-  // the big partition; with one hashing CTA per request, which of them gets its CTAs resident first can decide the
-  // step.  Stream priorities make the block scheduler prefer one of them whenever SMs free up
-  // (FI_EPP_PIPE_PRIO=match | hash | none; none by default).
-  int prio_lo = 0, prio_hi = 0;
-  cudaDeviceGetStreamPriorityRange(&prio_lo, &prio_hi);  // lo = least (numerically greatest), hi = greatest priority
-  int pa = 0, pb = 0;
-  const char* pe = std::getenv("FI_EPP_PIPE_PRIO");
-  const std::string prio = pe ? pe : "none";
-  if (prio == "match") {
-    pa = prio_lo;
-    pb = prio_hi;
-  } else if (prio == "hash") {
-    pa = prio_hi;
-    pb = prio_lo;
-  }
-  CUstream sw = nullptr, sa = nullptr, sb = nullptr;
-  if (g_green.GreenCtxStreamCreate(&sw, h->gctx_walk, CU_STREAM_NON_BLOCKING, 0) != CUDA_SUCCESS ||
-      g_green.GreenCtxStreamCreate(&sa, h->gctx_main, CU_STREAM_NON_BLOCKING, pa) != CUDA_SUCCESS ||
-      g_green.GreenCtxStreamCreate(&sb, h->gctx_main, CU_STREAM_NON_BLOCKING, pb) != CUDA_SUCCESS) {
-    destroy_partition(h);
-    return;
-  }
-  h->s_pw = (cudaStream_t)sw;
-  h->s_pa = (cudaStream_t)sa;
-  h->s_pb = (cudaStream_t)sb;
-  bool ok = cudaMalloc(&h->d_pre2, (size_t)h->chain_rows * h->MP * sizeof(uint64_t)) == cudaSuccess &&
-            cudaMalloc(&h->d_nblocks3, (size_t)h->cfg.max_batch * sizeof(uint32_t)) == cudaSuccess;
-  for (cudaEvent_t* e : {&h->ev_h[0], &h->ev_h[1], &h->ev_b3[0], &h->ev_b3[1], &h->ev_b3[2], &h->ev_up})
-    ok = ok && cudaEventCreateWithFlags(e, cudaEventDisableTiming) == cudaSuccess;
-  if (!ok) {
-    cudaGetLastError();
-    return;
-  }
-  h->part_walk_sms = (int)grp.sm.smCount;
-  h->part_main_sms = (int)rem.sm.smCount;
-  h->part_state = 1;
-  if (h->verbose)
-    std::fprintf(stderr, "[fi_epp] pipelined path: SM partition %d (chain walk) + %d (hashing, matching), three batches in flight\n",
-                 h->part_walk_sms, h->part_main_sms);
-}
-
-// Pipelined device path on the partitioned GPU: hash(k) and match(k) on the big partition's two streams,
-// chain(k) on the walker partition.  Buffers: pre[2] and chain[2] by batch parity, nblocks[3] by k mod 3 (hash(k+2)
-// writes its block counts while match(k) still reads its own).
-int submit_pick_partitioned(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0, uint32_t R,
-                            fi_pick* d_out, cudaStream_t us) {
-  const uint64_t k = h->pipe_seq;
-  const uint32_t s2 = (uint32_t)(k & 1), s3 = (uint32_t)(k % 3);
-  uint64_t* pre = s2 ? h->d_pre2 : h->d_pre;
-  uint64_t* chain = s2 ? h->d_chain2 : h->d_chain;
-  uint32_t* nb = s3 == 0 ? h->d_nblocks : (s3 == 1 ? h->d_nblocks2 : h->d_nblocks3);
-  // ---- hash(k): inputs ready in the caller's stream order; pre[s2] free once chain(k-2) has read it, nb[s3] once
-  // match(k-3) has; d_pre / d_chain are shared with stream-ordered picks and with the device LRU's reads
-  FI_CUDA(cudaEventRecord(h->ev_in, us));
-  FI_CUDA(cudaStreamWaitEvent(h->s_pa, h->ev_in, 0));
-  if (h->seen_plain != h->gen_plain) {
-    FI_CUDA(cudaStreamWaitEvent(h->s_pa, h->ev_plain, 0));
-    h->seen_plain = h->gen_plain;
-  }
-  if (h->ev_lru && h->seen_lru != h->gen_lru) {
-    FI_CUDA(cudaStreamWaitEvent(h->s_pa, h->ev_lru, 0));
-    h->seen_lru = h->gen_lru;
-  }
-  if (h->part_seq >= 2) FI_CUDA(cudaStreamWaitEvent(h->s_pa, h->ev_a[s2], 0));
-  if (h->part_seq >= 3) FI_CUDA(cudaStreamWaitEvent(h->s_pa, h->ev_b3[s3], 0));
-  {
-    LaunchScope ls(h, h->s_pa, K_HASH);
-    // (the kernel also zeroes the request-queue counter of this batch's match_pick: one runtime call less per batch)
-    // hash_blocks runs as 4 persistent CTAs per SM here (FI_EPP_PIPE_HASH_CTAS / option "pipe_hash_ctas" overrides;
-    // a large value = one CTA per request).  With one CTA per request the step depends on which of the two kernels
-    // gets its CTAs resident first: hash_blocks' 16 384 short CTAs and match_pick's long ones (80 registers x 256
-    // threads x 3 per SM) can lock each other out of the SMs.  Four hashing CTAs (32 K registers) always leave room
-    // for one matching CTA next to them.
-    const uint32_t hash_ctas = h->pipe_hash_ctas ? h->pipe_hash_ctas : 4u;
-    FI_CUDA(launch_hash_blocks(d_prompts, d_offsets, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, pre, nb,
-                               hash_ctas * (uint32_t)h->part_main_sms, h->s_pa, h->d_work + 8 + s3));
-  }
-  FI_CUDA(cudaEventRecord(h->ev_h[s2], h->s_pa));
-  // ---- chain(k) on its own SMs: chain[s2] free once match(k-2) has read it
-  FI_CUDA(cudaStreamWaitEvent(h->s_pw, h->ev_h[s2], 0));
-  if (h->part_seq >= 2) FI_CUDA(cudaStreamWaitEvent(h->s_pw, h->ev_b3[(k + 1) % 3], 0));  // (k - 2) mod 3
-  {
-    LaunchScope ls(h, h->s_pw, K_CHAIN);
-    const bool compact = h->part_compact < 0 ? h->part_walk_sms < 24 : h->part_compact != 0;
-    FI_CUDA(launch_chain_finalize(pre, nb, d_h0, R, h->MP, chain, compact, h->s_pw));
-  }
-  FI_CUDA(cudaEventRecord(h->ev_a[s2], h->s_pw));
-  // ---- match(k): every submitted index op and pod-state update is visible
-  if (h->eps_dirty || h->lora_dirty) {
-    int rc = upload_endpoints(h);  // (on s_main)
-    if (rc != FI_OK) return rc;
-    rc = upload_lora(h);
-    if (rc != FI_OK) return rc;
-    FI_CUDA(cudaEventRecord(h->ev_up, h->s_main));
-    FI_CUDA(cudaStreamWaitEvent(h->s_pb, h->ev_up, 0));
-  }
-  if (h->seen_index != h->gen_index) {
-    FI_CUDA(cudaStreamWaitEvent(h->s_pb, h->ev_index, 0));
-    h->seen_index = h->gen_index;
-  }
-  FI_CUDA(cudaStreamWaitEvent(h->s_pb, h->ev_a[s2], 0));
-  MatchParams mp{};
-  fill_match_params(h, mp, chain, nb, d_offsets, d_h0, nullptr, R, d_out, true);
-  mp.work_counter = h->d_work + 8 + s3;
-  mp.max_ctas_per_sm = h->pipe_match_ctas;
-  mp.zero_work_counter = 0;  // hash_blocks of this batch did
-  {
-    LaunchScope ls(h, h->s_pb, K_MATCH);
-    FI_CUDA(launch_match_pick(mp, h->part_main_sms, h->s_pb));
-  }
-  FI_CUDA(cudaEventRecord(h->ev_b3[s3], h->s_pb));
-  h->ev_pick = h->ev_b3[s3];
-  h->pipe_seq++;
-  h->part_seq++;
-  h->stats.pick_calls++;
-  h->stats.requests += R;
   return FI_OK;
 }
 
@@ -1533,19 +1306,6 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
   if (!h->d_chain2) {
     FI_CUDA(cudaMalloc(&h->d_chain2, (size_t)h->cfg.max_batch * h->MP * sizeof(uint64_t)));
     FI_CUDA(cudaMalloc(&h->d_nblocks2, (size_t)h->cfg.max_batch * sizeof(uint32_t)));
-  }
-  setup_partition(h);
-  if (h->part_state == 1 && h->trace_call < 0) {
-    if (!h->part_active) {
-      // switching from the two-stream pipeline (or first use): everything in flight there is ordered before us
-      // through ev_plain / ev_pick; the slot events of the partitioned pipeline start fresh
-      FI_CUDA(cudaStreamWaitEvent(h->s_pa, h->ev_pick, 0));
-      FI_CUDA(cudaStreamWaitEvent(h->s_pw, h->ev_pick, 0));
-      h->part_active = true;
-      h->part_seq = 0;
-      h->seen_index = h->seen_plain = h->seen_lru = ~0ull;
-    }
-    return submit_pick_partitioned(h, d_prompts, d_offsets, d_h0, R, d_out, us);
   }
   // FI_EPP_TRACE=<call>: timeline of three consecutive pipelined batches (printed by fi_epp_pick_wait)
   if (!h->profiling && h->trace_call >= 0 && (long)h->stats.pick_calls >= h->trace_call &&
@@ -1581,19 +1341,16 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
                               h->sm_count, h->s_a));
   } else {
     {
+      // this batch's block hashing runs beside the previous batch's match_pick
       LaunchScope ls(h, h->s_a, K_HASH);
-      // The SM split of the pipeline: this batch's block hashing runs BESIDE the previous batch's match_pick —
-      // hash_blocks as at most pipe_hash_ctas CTAs per SM, match_pick as at most pipe_match_ctas (its three CTAs of
-      // 79 registers would leave no room) — instead of one after the other.
-      FI_CUDA(launch_hash_blocks(d_prompts, d_offsets, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, h->d_pre, nb,
-                                 h->pipe_hash_ctas * (uint32_t)h->sm_count, h->s_a));
+      FI_CUDA(launch_hash_blocks(d_prompts, d_offsets, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, h->d_pre, nb, h->s_a));
     }
     // The chain walk is serial latency — a warp per scheduler that wants an issue slot every few cycles — and
     // slows several-fold next to a busy kernel that competes for the same schedulers, so it waits for the
     // previous batch's match to drain; what overlaps is this batch's block hashing with that match.
     if (h->pipe_seq >= 1) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot ^ 1u], 0));
     LaunchScope ls(h, h->s_a, K_CHAIN);
-    FI_CUDA(launch_chain_finalize(h->d_pre, nb, d_h0, R, h->MP, chain, false, h->s_a));
+    FI_CUDA(launch_chain_finalize(h->d_pre, nb, d_h0, R, h->MP, chain, h->s_a));
   }
   FI_CUDA(cudaEventRecord(h->ev_a[slot], h->s_a));
   // ---- stage B
@@ -1606,13 +1363,11 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
   MatchParams mp{};
   fill_match_params(h, mp, chain, nb, d_offsets, d_h0, nullptr, R, d_out, true);
   mp.work_counter = h->d_work + 8 + slot;
-  mp.max_ctas_per_sm = h->pipe_match_ctas;
   {
     LaunchScope ls(h, h->s_main, K_MATCH);
     FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main));
   }
   FI_CUDA(cudaEventRecord(h->ev_b[slot], h->s_main));
-  h->ev_pick = h->ev_pick_own;
   FI_CUDA(cudaEventRecord(h->ev_pick, h->s_main));
   h->pipe_seq++;
   h->stats.pick_calls++;
@@ -1793,17 +1548,10 @@ void fi_epp_destroy(fi_epp* h) {
     if (e) cudaEventDestroy(e);
   for (int k = 0; k < fi_epp::kMaxFeedSlices; ++k)
     if (h->ev_copy[k]) cudaEventDestroy(h->ev_copy[k]);
-  for (cudaEvent_t e : {h->ev_in, h->ev_a[0], h->ev_a[1], h->ev_b[0], h->ev_b[1], h->ev_pick_own, h->ev_plain})
+  for (cudaEvent_t e : {h->ev_in, h->ev_a[0], h->ev_a[1], h->ev_b[0], h->ev_b[1], h->ev_pick, h->ev_plain})
     if (e) cudaEventDestroy(e);
   cudaFree(h->d_chain2);
   cudaFree(h->d_nblocks2);
-  cudaFree(h->d_pre2);
-  cudaFree(h->d_nblocks3);
-  for (cudaEvent_t e : {h->ev_h[0], h->ev_h[1], h->ev_b3[0], h->ev_b3[1], h->ev_b3[2], h->ev_up})
-    if (e) cudaEventDestroy(e);
-  for (cudaStream_t st : {h->s_pw, h->s_pa, h->s_pb})
-    if (st) cudaStreamDestroy(st);
-  destroy_partition(h);
   for (cudaStream_t s : {h->s_main, h->s_index, h->s_copy, h->s_a})
     if (s) cudaStreamDestroy(s);
   delete h;
@@ -1855,12 +1603,6 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
   h->fast_hash = (cfg->block_bytes % 32) == 0;
   if (const char* e = std::getenv("FI_EPP_TRACE")) h->trace_call = std::strtol(e, nullptr, 10);
   h->verbose = std::getenv("FI_EPP_VERBOSE") != nullptr;
-  if (const char* e = std::getenv("FI_EPP_PIPE_PARTITION")) {
-    h->part_want = (int)std::strtol(e, nullptr, 10);
-  }
-  if (const char* e = std::getenv("FI_EPP_WALK_COMPACT")) h->part_compact = std::strtol(e, nullptr, 10) != 0 ? 1 : 0;
-  if (const char* e = std::getenv("FI_EPP_PIPE_HASH_CTAS")) h->pipe_hash_ctas = (uint32_t)std::strtol(e, nullptr, 10);
-  if (const char* e = std::getenv("FI_EPP_PIPE_MATCH_CTAS")) h->pipe_match_ctas = (uint32_t)std::strtol(e, nullptr, 10);
   if (h->cfg.max_prompt_bytes == 0)
     h->cfg.max_prompt_bytes = (uint64_t)cfg->max_batch * cfg->block_bytes * cfg->max_blocks;
   if (h->cfg.index_slots == 0) {
@@ -1875,9 +1617,8 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
   FI_TRY(cudaStreamCreateWithFlags(&h->s_index, cudaStreamNonBlocking));
   FI_TRY(cudaStreamCreateWithFlags(&h->s_copy, cudaStreamNonBlocking));
   FI_TRY(cudaStreamCreateWithFlags(&h->s_a, cudaStreamNonBlocking));
-  for (cudaEvent_t* e : {&h->ev_in, &h->ev_a[0], &h->ev_a[1], &h->ev_b[0], &h->ev_b[1], &h->ev_pick_own, &h->ev_plain})
+  for (cudaEvent_t* e : {&h->ev_in, &h->ev_a[0], &h->ev_a[1], &h->ev_b[0], &h->ev_b[1], &h->ev_pick, &h->ev_plain})
     FI_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-  h->ev_pick = h->ev_pick_own;
   for (int k = 0; k < fi_epp::kMaxFeedSlices; ++k) FI_TRY(cudaEventCreateWithFlags(&h->ev_copy[k], cudaEventDisableTiming));
   if (const char* e = std::getenv("FI_EPP_FEED_SLICES")) {
     const long v = std::strtol(e, nullptr, 10);
@@ -2122,7 +1863,6 @@ int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t
   FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
   h->ctr_pending = true;
   FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
-  h->gen_index++;
   if (pairs_removed) {
     unsigned long long c = 0;
     FI_CUDA(cudaMemcpyAsync(&c, h->d_rm, sizeof(c), cudaMemcpyDeviceToHost, h->s_index));
@@ -2683,14 +2423,10 @@ int fi_epp_pick_submit(fi_epp* h, const void* d_prompts, const void* d_offsets, 
                      (cudaStream_t)stream);
 }
 
-// out[0] = 1 if the pipelined path (fi_epp_pick_submit) runs on a partitioned GPU, out[1] / out[2] = SMs of the chain-walk
-// partition / of the hashing + matching partition (0 when unpartitioned or not yet used).
+// The pipelined path always runs on the whole GPU: out = {0, 0, 0} (include/fi_epp.h).
 int fi_epp_pipeline_info(fi_epp* h, int32_t out[3]) {
   if (!h || !out) return FI_ERR_INVALID;
-  std::lock_guard<std::mutex> lk(h->mu);
-  out[0] = h->part_state == 1 ? 1 : 0;
-  out[1] = h->part_state == 1 ? h->part_walk_sms : 0;
-  out[2] = h->part_state == 1 ? h->part_main_sms : 0;
+  out[0] = out[1] = out[2] = 0;
   return FI_OK;
 }
 
@@ -2794,31 +2530,10 @@ int fi_epp_set_option(fi_epp* h, const char* name, int64_t value) {
     h->feed_slices = (uint32_t)value;
     return FI_OK;
   }
-  if (n == "pipe_hash_ctas" || n == "pipe_match_ctas") {
-    if (value < 0 || value > 4096) return fail(h, FI_ERR_INVALID, n + ": 0..4096");
-    (n == "pipe_hash_ctas" ? h->pipe_hash_ctas : h->pipe_match_ctas) = (uint32_t)value;
-    return FI_OK;
-  }
   if (n == "device_lru") {
     if (value != 0 && value != 1) return fail(h, FI_ERR_INVALID, "device_lru: 0 or 1");
     if (h->lru_mode >= 0 && h->lru_mode != (int)value) return fail(h, FI_ERR_STATE, "device_lru: the handle's LRU is already in use");
     h->lru_want = (int)value;
-    return FI_OK;
-  }
-  if (n == "pipe_partition") {
-    if (value < 0 || value > 64) return fail(h, FI_ERR_INVALID, "pipe_partition: 0 (off) or the walker partition's SM count");
-    if (h->part_state == 1 && value == 0) {
-      // back to the unpartitioned pipeline (contexts are released with the handle); nothing of the partitioned
-      // one may still be in flight: the two share the pre-state / chain buffers
-      cudaSetDevice(h->cfg.device);
-      for (cudaStream_t st : {h->s_pa, h->s_pw, h->s_pb})
-        if (st) cudaStreamSynchronize(st);
-      h->part_state = -1;
-      h->part_active = false;
-    } else if (h->part_state != 1) {
-      h->part_want = (int)value;
-      h->part_state = 0;
-    }
     return FI_OK;
   }
   if (n == "lru_table_slots") {

@@ -62,58 +62,54 @@ __device__ __forceinline__ void xacc2_stripe(XAcc2& a, const Stripe& q) {
 
 template <int STRIPES>
 __global__ void __launch_bounds__(256, STRIPES <= 2 ? 8 : 5) hash_blocks_kernel(const uint8_t* __restrict__ prompts,
-                                                          const uint64_t* __restrict__ offsets, uint32_t R, uint32_t M,
+                                                          const uint64_t* __restrict__ offsets, uint32_t M,
                                                           uint32_t MP, uint64_t* __restrict__ pre,
-                                                          uint32_t* __restrict__ nblocks, uint32_t* __restrict__ zero_word) {
+                                                          uint32_t* __restrict__ nblocks) {
   constexpr uint32_t B = STRIPES * 32;
   const uint32_t MP2 = MP / 2;
   const uint64_t pol = make_evict_first_policy();
-  if (zero_word && blockIdx.x == 0 && threadIdx.x == 0) *zero_word = 0;
-  // one request per CTA pass; the grid is R CTAs, or capped when the kernel has to share the SMs with the
-  // previous batch's match_pick (pipelined API)
-  for (uint32_t r = blockIdx.x; r < R; r += gridDim.x) {
-    const uint64_t off = offsets[r];
-    const uint64_t len = offsets[r + 1] - off;
-    const uint64_t nb64 = len / B;
-    const uint32_t n = nb64 > M ? M : (uint32_t)nb64;
-    if (threadIdx.x == 0) nblocks[r] = n;
-    const uint8_t* base = prompts + off;
-    const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(base) & 15);
-    if (mis == 0) {
-      for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
-        const uint4* p = reinterpret_cast<const uint4*>(base + (uint64_t)i * B);
-        uint4 q[2 * STRIPES];
+  const uint32_t r = blockIdx.x;  // one request per CTA
+  const uint64_t off = offsets[r];
+  const uint64_t len = offsets[r + 1] - off;
+  const uint64_t nb64 = len / B;
+  const uint32_t n = nb64 > M ? M : (uint32_t)nb64;
+  if (threadIdx.x == 0) nblocks[r] = n;
+  const uint8_t* base = prompts + off;
+  const uint32_t mis = (uint32_t)(reinterpret_cast<uintptr_t>(base) & 15);
+  if (mis == 0) {
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+      const uint4* p = reinterpret_cast<const uint4*>(base + (uint64_t)i * B);
+      uint4 q[2 * STRIPES];
 #pragma unroll
-        for (int s = 0; s < 2 * STRIPES; ++s) q[s] = ld_stream_v4(p + s, pol);
-        XAcc2 a = xacc2_init();
+      for (int s = 0; s < 2 * STRIPES; ++s) q[s] = ld_stream_v4(p + s, pol);
+      XAcc2 a = xacc2_init();
 #pragma unroll
-        for (int s = 0; s < STRIPES; ++s)
-          xacc2_stripe(a, Stripe{{q[2 * s].x, q[2 * s].y, q[2 * s].z, q[2 * s].w, q[2 * s + 1].x, q[2 * s + 1].y,
-                                  q[2 * s + 1].z, q[2 * s + 1].w}});
-        pre[pre_index(r, i, MP2)] = xacc2_finish(a, (uint64_t)B + 8);
+      for (int s = 0; s < STRIPES; ++s)
+        xacc2_stripe(a, Stripe{{q[2 * s].x, q[2 * s].y, q[2 * s].z, q[2 * s].w, q[2 * s + 1].x, q[2 * s + 1].y,
+                                q[2 * s + 1].z, q[2 * s + 1].w}});
+      pre[pre_index(r, i, MP2)] = xacc2_finish(a, (uint64_t)B + 8);
+    }
+  } else {
+    // arbitrary byte alignment: aligned 64-bit windows + funnel shift
+    for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+      const uintptr_t addr = reinterpret_cast<uintptr_t>(base + (uint64_t)i * B);
+      const uint64_t* wp = reinterpret_cast<const uint64_t*>(addr & ~(uintptr_t)7);
+      const uint32_t sh = (uint32_t)(addr & 7) * 8;
+      uint64_t w[4 * STRIPES + 1];
+#pragma unroll
+      for (int k = 0; k < 4 * STRIPES; ++k) w[k] = __ldg(wp + k);
+      w[4 * STRIPES] = sh ? __ldg(wp + 4 * STRIPES) : 0;
+      if (sh) {
+#pragma unroll
+        for (int k = 0; k < 4 * STRIPES; ++k) w[k] = (w[k] >> sh) | (w[k + 1] << (64 - sh));
       }
-    } else {
-      // arbitrary byte alignment: aligned 64-bit windows + funnel shift
-      for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
-        const uintptr_t addr = reinterpret_cast<uintptr_t>(base + (uint64_t)i * B);
-        const uint64_t* wp = reinterpret_cast<const uint64_t*>(addr & ~(uintptr_t)7);
-        const uint32_t sh = (uint32_t)(addr & 7) * 8;
-        uint64_t w[4 * STRIPES + 1];
+      XAcc2 a = xacc2_init();
 #pragma unroll
-        for (int k = 0; k < 4 * STRIPES; ++k) w[k] = __ldg(wp + k);
-        w[4 * STRIPES] = sh ? __ldg(wp + 4 * STRIPES) : 0;
-        if (sh) {
-#pragma unroll
-          for (int k = 0; k < 4 * STRIPES; ++k) w[k] = (w[k] >> sh) | (w[k + 1] << (64 - sh));
-        }
-        XAcc2 a = xacc2_init();
-#pragma unroll
-        for (int s = 0; s < STRIPES; ++s)
-          xacc2_stripe(a, Stripe{{(uint32_t)w[4 * s], (uint32_t)(w[4 * s] >> 32), (uint32_t)w[4 * s + 1],
-                                  (uint32_t)(w[4 * s + 1] >> 32), (uint32_t)w[4 * s + 2], (uint32_t)(w[4 * s + 2] >> 32),
-                                  (uint32_t)w[4 * s + 3], (uint32_t)(w[4 * s + 3] >> 32)}});
-        pre[pre_index(r, i, MP2)] = xacc2_finish(a, (uint64_t)B + 8);
-      }
+      for (int s = 0; s < STRIPES; ++s)
+        xacc2_stripe(a, Stripe{{(uint32_t)w[4 * s], (uint32_t)(w[4 * s] >> 32), (uint32_t)w[4 * s + 1],
+                                (uint32_t)(w[4 * s + 1] >> 32), (uint32_t)w[4 * s + 2], (uint32_t)(w[4 * s + 2] >> 32),
+                                (uint32_t)w[4 * s + 3], (uint32_t)(w[4 * s + 3] >> 32)}});
+      pre[pre_index(r, i, MP2)] = xacc2_finish(a, (uint64_t)B + 8);
     }
   }
 }
@@ -173,10 +169,8 @@ __global__ void __launch_bounds__(256) hash_blocks_any_kernel(const uint8_t* __r
 //   * the loop is unrolled by two groups with the register roles swapped, so no buffer is ever copied;
 //   * the buffers are padded to whole groups (MP % 8 == 0): no per-unit predicates.
 // Entries [n, MP) of every row are zeroed.
-// kRing ring slots, prefetch distance kRing - 1 groups.  Two shapes: RING = 4 with the whole register file (one warp
-// per scheduler when the 128 CTAs of a 16 384-request batch spread over the whole GPU: nothing else hides the
-// pre-state loads), and RING = 3 capped at 64 registers / 24 KB so that all 128 CTAs fit on a walker partition of
-// 16 SMs (eight warps per scheduler hide each other's latency there).
+// kRing ring slots, prefetch distance kRing - 1 groups, and the whole register file: there is one warp per scheduler
+// when the 128 CTAs of a 16 384-request batch spread over the whole GPU, so nothing else hides the pre-state loads.
 
 __device__ __forceinline__ void cp_async16_cg(void* smem, const void* gmem) {
   const unsigned sa = (unsigned)__cvta_generic_to_shared(smem);
@@ -199,12 +193,14 @@ __device__ __forceinline__ ulonglong2 lds16(const ulonglong2* p) {
 
 // Four warps (128 requests) per CTA, one per SM sub-partition.
 constexpr int kChainWarps = 4;
+constexpr int kRing = 4;
 
-template <int kRing, int MINB>
-__global__ void __launch_bounds__(kChainWarps * 32, MINB) chain_finalize_kernel(const uint64_t* __restrict__ pre,
-                                                                          const uint32_t* __restrict__ nblocks,
-                                                                          const uint64_t* __restrict__ h0, uint32_t R,
-                                                                          uint32_t MP, uint64_t* __restrict__ chain) {
+// (the minimum of 1 CTA per SM is the register allocation the walker was measured with: 68 registers; without the
+// bound ptxas allocates 66 and schedules the loop differently)
+__global__ void __launch_bounds__(kChainWarps * 32, 1) chain_finalize_kernel(const uint64_t* __restrict__ pre,
+                                                                       const uint32_t* __restrict__ nblocks,
+                                                                       const uint64_t* __restrict__ h0, uint32_t R,
+                                                                       uint32_t MP, uint64_t* __restrict__ chain) {
   constexpr int kAhead = kRing - 1;
   __shared__ __align__(16) ulonglong2 s_ring[kChainWarps][kRing][4][32];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -388,8 +384,7 @@ __global__ void __launch_bounds__(kFuseWarps * 32, 1) hash_chain_kernel(const ui
                                                                    const uint64_t* __restrict__ h0, uint32_t R,
                                                                    uint32_t M, uint32_t MP,
                                                                    uint64_t* __restrict__ chain,
-                                                                   uint32_t* __restrict__ nblocks,
-                                                                   uint32_t* __restrict__ zero_word) {
+                                                                   uint32_t* __restrict__ nblocks) {
   constexpr uint32_t B = STRIPES * 32;
   // A hashing warp's job: 8 blocks of 4 * BPL requests, BPL blocks per lane (two blocks' loads in flight per
   // thread, one at 128-byte blocks).  Lanes 8j .. 8j+7 read one request's 8 blocks: 512 contiguous bytes.
@@ -406,7 +401,6 @@ __global__ void __launch_bounds__(kFuseWarps * 32, 1) hash_chain_kernel(const ui
 
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t r_tile = blockIdx.x * kFuseReq;
-  if (zero_word && blockIdx.x == 0 && tid == 0) *zero_word = 0;
   if (tid == 0) {
     s_groups = 0;
     for (uint32_t s = 0; s < kFuseRing; ++s) {
@@ -582,62 +576,57 @@ __global__ void __launch_bounds__(128) hash_generic_kernel(const uint8_t* __rest
 }  // namespace
 
 cudaError_t launch_hash_blocks(const uint8_t* prompts, const uint64_t* offsets, uint32_t R, uint32_t B, uint32_t M,
-                               uint32_t MP, uint64_t* pre, uint32_t* nblocks, uint32_t grid_cap, cudaStream_t s,
-                               uint32_t* zero_word) {
+                               uint32_t MP, uint64_t* pre, uint32_t* nblocks, cudaStream_t s) {
   if (R == 0) return cudaSuccess;
   uint32_t threads = (M + 31) / 32 * 32;
   if (threads > 256) threads = 256;
-  const uint32_t grid = (grid_cap && grid_cap < R) ? grid_cap : R;
   if (B == 64)
-    hash_blocks_kernel<2><<<grid, threads, 0, s>>>(prompts, offsets, R, M, MP, pre, nblocks, zero_word);
+    hash_blocks_kernel<2><<<R, threads, 0, s>>>(prompts, offsets, M, MP, pre, nblocks);
   else if (B == 32)
-    hash_blocks_kernel<1><<<grid, threads, 0, s>>>(prompts, offsets, R, M, MP, pre, nblocks, zero_word);
+    hash_blocks_kernel<1><<<R, threads, 0, s>>>(prompts, offsets, M, MP, pre, nblocks);
   else if (B == 128)
-    hash_blocks_kernel<4><<<grid, threads, 0, s>>>(prompts, offsets, R, M, MP, pre, nblocks, zero_word);
-  else {
+    hash_blocks_kernel<4><<<R, threads, 0, s>>>(prompts, offsets, M, MP, pre, nblocks);
+  else
     hash_blocks_any_kernel<<<R, threads, 0, s>>>(prompts, offsets, B, M, MP, pre, nblocks);
-    if (zero_word) cudaMemsetAsync(zero_word, 0, sizeof(uint32_t), s);
-  }
   return cudaGetLastError();
 }
 
 cudaError_t launch_chain_finalize(const uint64_t* pre, const uint32_t* nblocks, const uint64_t* h0, uint32_t R,
-                                  uint32_t MP, uint64_t* chain, bool compact, cudaStream_t s) {
+                                  uint32_t MP, uint64_t* chain, cudaStream_t s) {
   if (R == 0) return cudaSuccess;
   const uint32_t groups = (R + 31) / 32;
   const uint32_t grid = (groups + kChainWarps - 1) / kChainWarps;
-  if (compact) chain_finalize_kernel<3, 8><<<grid, kChainWarps * 32, 0, s>>>(pre, nblocks, h0, R, MP, chain);
-  else chain_finalize_kernel<4, 1><<<grid, kChainWarps * 32, 0, s>>>(pre, nblocks, h0, R, MP, chain);
+  chain_finalize_kernel<<<grid, kChainWarps * 32, 0, s>>>(pre, nblocks, h0, R, MP, chain);
   return cudaGetLastError();
 }
 
 template <int STRIPES>
 static void launch_hash_chain_tile(uint32_t walk, uint32_t grid, cudaStream_t s, const uint8_t* prompts,
                                    const uint64_t* offsets, const uint64_t* h0, uint32_t R, uint32_t M, uint32_t MP,
-                                   uint64_t* chain, uint32_t* nblocks, uint32_t* zero_word) {
+                                   uint64_t* chain, uint32_t* nblocks) {
   constexpr uint32_t threads = kFuseWarps * 32;
   if (walk == 4)
-    hash_chain_kernel<STRIPES, 4><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+    hash_chain_kernel<STRIPES, 4><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks);
   else if (walk == 2)
-    hash_chain_kernel<STRIPES, 2><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+    hash_chain_kernel<STRIPES, 2><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks);
   else
-    hash_chain_kernel<STRIPES, 1><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+    hash_chain_kernel<STRIPES, 1><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks);
 }
 
 cudaError_t launch_hash_chain(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
                               uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain, uint32_t* nblocks, int sm_count,
-                              cudaStream_t s, uint32_t* zero_word) {
+                              cudaStream_t s) {
   if (R == 0) return cudaSuccess;
   // the smallest tile whose grid still fits one CTA per SM; 128 requests per CTA beyond that
   uint32_t walk = 1;
   while (walk < 4 && (R + 32 * walk - 1) / (32 * walk) > (uint32_t)sm_count) walk *= 2;
   const uint32_t grid = (R + 32 * walk - 1) / (32 * walk);
   if (B == 64)
-    launch_hash_chain_tile<2>(walk, grid, s, prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+    launch_hash_chain_tile<2>(walk, grid, s, prompts, offsets, h0, R, M, MP, chain, nblocks);
   else if (B == 32)
-    launch_hash_chain_tile<1>(walk, grid, s, prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+    launch_hash_chain_tile<1>(walk, grid, s, prompts, offsets, h0, R, M, MP, chain, nblocks);
   else if (B == 128)
-    launch_hash_chain_tile<4>(walk, grid, s, prompts, offsets, h0, R, M, MP, chain, nblocks, zero_word);
+    launch_hash_chain_tile<4>(walk, grid, s, prompts, offsets, h0, R, M, MP, chain, nblocks);
   else
     return cudaErrorInvalidValue;
   return cudaGetLastError();

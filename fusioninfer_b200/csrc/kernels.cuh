@@ -162,9 +162,7 @@ struct MatchParams {
   double pd_threshold;
   fi_pick* out;                       // [R][P], or [R][P][k] when k > 0
   unsigned long long* probed_blocks;  // optional Σ N_probe
-  uint32_t* work_counter;             // dynamic request queue of the launch
-  uint32_t zero_work_counter;         // launcher zeroes it first (0: the caller already did)
-  uint32_t max_ctas_per_sm;           // 0: as many as fit; else a cap (pipelined API: leave room for hash_blocks)
+  uint32_t* work_counter;             // dynamic request queue of the launch (the launcher zeroes it first)
   uint32_t lane_zero;                 // always 0: makes the ticket address formally lane-dependent (match_kernels.cu take_ticket)
   uint32_t k;                         // 0: one pick per profile, out [R][P]; else the ranked pick, out [R][P][k] (S.6a)
   PeerXchg px;                        // sharded mode, peer-memory exchange (px.enabled)
@@ -185,20 +183,16 @@ struct MergeParams {
 };
 
 // ---- launchers (each returns the cudaGetLastError() of its launch) -----------
-// grid_cap: 0 = one CTA per request; else at most that many CTAs (the pipelined API shares the SMs with match_pick)
-// zero_word: optional device word the kernel clears (the pipelined path's request-queue counter of the batch)
 cudaError_t launch_hash_blocks(const uint8_t* prompts, const uint64_t* offsets, uint32_t R, uint32_t B,
-                               uint32_t M, uint32_t MP, uint64_t* pre, uint32_t* nblocks, uint32_t grid_cap,
-                               cudaStream_t s, uint32_t* zero_word = nullptr);
-// compact: the 64-register / 24 KB shape whose 128 CTAs all fit on a 16-SM partition (pipelined path)
+                               uint32_t M, uint32_t MP, uint64_t* pre, uint32_t* nblocks, cudaStream_t s);
 cudaError_t launch_chain_finalize(const uint64_t* pre, const uint32_t* nblocks, const uint64_t* h0,
-                                  uint32_t R, uint32_t MP, uint64_t* chain, bool compact, cudaStream_t s);
+                                  uint32_t R, uint32_t MP, uint64_t* chain, cudaStream_t s);
 // hash_blocks + chain_finalize fused (block_bytes 32, 64 or 128 only: hash_chain_fused(B)); no pre-state buffer.
 // sm_count sets the tile: 32, 64 or 128 requests per CTA, the smallest whose grid fits one CTA per SM
 inline bool hash_chain_fused(uint32_t B) { return B == 32 || B == 64 || B == 128; }
 cudaError_t launch_hash_chain(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
                               uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain, uint32_t* nblocks,
-                              int sm_count, cudaStream_t s, uint32_t* zero_word = nullptr);
+                              int sm_count, cudaStream_t s);
 cudaError_t launch_hash_generic(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
                                 uint32_t R, uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain,
                                 uint32_t* nblocks, cudaStream_t s);

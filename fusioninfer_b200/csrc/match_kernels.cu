@@ -32,7 +32,6 @@
 // the rank's (score, endpoint) pick, stored straight into every rank's memory (PeerXchg) and reduced by
 // merge_picks_kernel.
 #include <climits>
-#include <cstdlib>
 
 #include "bitslice.cuh"
 #include "index_device.cuh"
@@ -865,15 +864,11 @@ cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_
     cached_smem = smem + 1;
   }
   uint32_t grid = (p.R + kWarps - 1) / kWarps;
-  uint32_t per_sm_now = (uint32_t)cached_per_sm;
-  if (p.max_ctas_per_sm && p.max_ctas_per_sm < per_sm_now) per_sm_now = p.max_ctas_per_sm;
-  const uint32_t cap = (uint32_t)sm_count * per_sm_now;
+  const uint32_t cap = (uint32_t)sm_count * (uint32_t)cached_per_sm;
   if (grid > cap) grid = cap;
   if (grid == 0) grid = 1;
-  if (p.zero_work_counter) {
-    e = cudaMemsetAsync(p.work_counter, 0, sizeof(uint32_t), s);
-    if (e != cudaSuccess) return e;
-  }
+  e = cudaMemsetAsync(p.work_counter, 0, sizeof(uint32_t), s);
+  if (e != cudaSuccess) return e;
   kern<<<grid, kWarps * 32, smem, s>>>(p);
   return cudaGetLastError();
 }
@@ -897,16 +892,15 @@ cudaError_t launch_match_pick(const MatchParams& p, int sm_count, cudaStream_t s
   if (p.R == 0) return cudaSuccess;
   // Words per row = LPR * VEC.  Two words per lane (half the counter registers of VEC = 4 -> three CTAs
   // = 24 warps per SM instead of 16): the kernel is bound by per-warp instruction latency and wants warps, not
-  // wide loads (E = 1024, cfg 3 on one H100 SXM, 700 W: match_pick 74.5 us with two words per lane vs 98.1-98.4 us with four, two runs each; FI_EPP_MATCH_VEC=4 selects the four-word shape
-  // there for comparison).
-  static const int vec = [] { const char* e = std::getenv("FI_EPP_MATCH_VEC"); return e ? std::atoi(e) : 2; }();
+  // wide loads (E = 1024, cfg 3 on one H100 SXM, 700 W: match_pick 74.5 us with two words per lane vs 98.1-98.4 us
+  // with four, two runs each).
   switch (p.ix.W) {
     case 1: return launch_match_t<1, 1>(p, sm_count, s);
     case 2: return launch_match_t<1, 2>(p, sm_count, s);
     case 4: return launch_match_t<2, 2>(p, sm_count, s);
     case 8: return launch_match_t<4, 2>(p, sm_count, s);
     case 16: return launch_match_t<8, 2>(p, sm_count, s);
-    case 32: return vec == 4 ? launch_match_t<8, 4>(p, sm_count, s) : launch_match_t<16, 2>(p, sm_count, s);
+    case 32: return launch_match_t<16, 2>(p, sm_count, s);
     case 64: return launch_match_t<32, 2>(p, sm_count, s);
     case 128: return launch_match_t<32, 4>(p, sm_count, s);
     default: return cudaErrorInvalidValue;

@@ -222,7 +222,8 @@ class EndpointPicker:
         return out[: n.value].copy()
 
     def pipeline_info(self) -> dict:
-        """How pick_submit runs: partitioned GPU (three batches in flight) or not (two)."""
+        """How pick_submit runs.  It always runs on the whole GPU with two batches in flight, so this returns
+        partitioned False and 0 for walk_sms and main_sms."""
         out = (C.c_int32 * 3)()
         self._check(self._lib.fi_epp_pipeline_info(self._h, out), "fi_epp_pipeline_info")
         return {"partitioned": bool(out[0]), "walk_sms": int(out[1]), "main_sms": int(out[2])}

@@ -378,10 +378,8 @@ int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void
 int fi_epp_pick_submit(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
                        uint64_t total_prompt_bytes, void* d_out, void* stream);
 int fi_epp_pick_wait(fi_epp* h, void* stream);
-/* How the pipelined path runs: out[0] = 1 if the GPU is partitioned (green contexts: the chain walk of batch k+1 on
- * its own out[1] SMs while batch k is matched and batch k+2 hashed on the other out[2] — three batches in flight),
- * 0 if not (driver without green contexts, option "pipe_partition" = 0, sharded pool): two batches in flight on
- * the whole GPU.  Valid after the first fi_epp_pick_submit. */
+/* How the pipelined path runs: out[0] = 1 if the GPU is partitioned between its stages, out[1] / out[2] = SMs of the
+ * partitions.  The pipelined path always runs on the whole GPU with two batches in flight, so out is {0, 0, 0}. */
 int fi_epp_pipeline_info(fi_epp* h, int32_t out[3]);
 
 void* fi_epp_pinned_alloc(size_t bytes);
@@ -410,10 +408,6 @@ int fi_epp_comm_exchange(fi_epp* h);
  *   "lru_table_slots"  slots per endpoint table of the device LRU (0 = sized by free HBM, 4..32 x lru_capacity)
  *   "feed_slices"  slices of a host-buffer pick's prompt copy, 1..16 (default 8)
  *   "lru_threads"  host worker threads of fi_epp_index_add_chains (takes effect at the next call)
- *   "pipe_partition"  SMs of the chain-walk partition of the pipelined path (default 0 = no partition)
- *   "pipe_hash_ctas", "pipe_match_ctas"  CTAs per SM of the two kernels the pipelined path runs side by side (0 = default:
- *                  partitioned GPU 4 hashing CTAs per SM, otherwise one CTA per request; match_pick as many as fit)
- *                  (fi_epp_pick_submit: batch k+1's block hashing next to batch k's match; 0 = uncapped)
  * FI_ERR_INVALID for an unknown name or a value out of range. */
 int fi_epp_set_option(fi_epp* h, const char* name, int64_t value);
 

@@ -7,7 +7,7 @@ tolerance 0: both sides do the same IEEE-754 round-to-nearest mul/add/div sequen
 import numpy as np
 import pytest
 
-from fusioninfer_b200 import EndpointPicker, make_config, synth
+from fusioninfer_b200 import EndpointPicker, FiEppError, make_config, synth
 from fusioninfer_b200 import _abi as abi
 from oracle import epp_oracle as eo
 from tests import helpers as H
@@ -501,11 +501,8 @@ def test_pick_parity_after_churn_and_rebuild():
     gpu.close()
 
 
-@pytest.mark.parametrize("partition", [None, 0, 16, 40])
-def test_pipelined_submit_equals_oracle_with_index_updates_in_between(partition):
-    """fi_epp_pick_submit keeps two batches in flight (batch k+1 is hashed while batch k is matched) — three on a
-    partitioned GPU (option pipe_partition = SMs of the chain walk's own partition: 16 runs the compact walker shape,
-    40 the full one; None = the default, unpartitioned, like 0).  Seven
+def test_pipelined_submit_equals_oracle_with_index_updates_in_between():
+    """fi_epp_pick_submit keeps two batches in flight (batch k+1 is hashed while batch k is matched).  Seven
     different batches of different sizes are submitted back to back, index updates and a pod-state refresh
     are interleaved (each batch must see the index and the pod states as of ITS submit call), stream-ordered
     picks are mixed in; after one fi_epp_pick_wait every output equals the oracle's."""
@@ -516,8 +513,6 @@ def test_pipelined_submit_equals_oracle_with_index_updates_in_between(partition)
     pd = dict(pd, threshold=900.0)
     cfg = H.config_for(wl, profiles=profiles, pd=pd)
     gpu, cpu = _pair(cfg)
-    if partition is not None:
-        gpu.set_option("pipe_partition", partition)
     st = wl.endpoint_states()
     gpu.update_endpoints(st)
     cpu.update_endpoints(st)
@@ -869,29 +864,25 @@ def _device_lru_from_device_chains(max_blocks, T, cap, slots):
     gpu.close()
 
 
-@pytest.mark.parametrize("partition,max_blocks", [
-    pytest.param(None, 128, id="None"), pytest.param(0, 128, id="0"), pytest.param(40, 128, id="40"),
-    pytest.param(None, 1023, id="None-1023"), pytest.param(40, 1023, id="40-1023"),
-    pytest.param(16, 1023, id="16-1023"),
+@pytest.mark.parametrize("block_tokens,max_blocks", [
+    pytest.param(16, 128, id="64B-128"), pytest.param(16, 1023, id="64B-1023"),
+    pytest.param(24, 128, id="96B-128"), pytest.param(24, 1023, id="96B-1023"),
 ])
-def test_pipelined_back_to_back_batches(partition, max_blocks):
+def test_pipelined_back_to_back_batches(block_tokens, max_blocks):
     """Twelve batches of different sizes submitted back to back with nothing in between (so that the pipeline really
-    has its two — partitioned GPU: three — batches in flight and reuses every slot buffer several times), one wait
-    at the end, every output equal to the oracle's; then the same again after a stream-ordered pick.  With a 40-SM
-    walker partition, R = 512 exceeds the 4 hashing CTAs per SM of the other partition, so hash_blocks' CTAs each
-    take several requests.  max_blocks = 1023: prompts past the cap with a partial last block, chain pitch 1024; on a
-    partitioned GPU hash_blocks and the chain walk run at that pitch (16 SMs: the compact walker shape, 40: the full
-    one)."""
+    has its two batches in flight and reuses every slot buffer several times), one wait at the end, every output
+    equal to the oracle's; then the same again after a stream-ordered pick.  64-byte blocks run stage A as one
+    hash_chain launch, 96-byte blocks as hash_blocks + chain_finalize.  max_blocks = 1023: prompts past the cap with
+    a partial last block, chain pitch 1024."""
     import torch
 
     if max_blocks == 128:
-        wl = H.small_workload(E=200, R=512, T=2048, max_blocks=128)
+        wl = H.small_workload(E=200, R=512, T=128 * block_tokens, max_blocks=128, block_tokens=block_tokens)
     else:
-        wl = H.small_workload(E=200, R=512, T=16 * (max_blocks + 1) + 5, max_blocks=max_blocks, groups_per_endpoint=2)
+        wl = H.small_workload(E=200, R=512, T=block_tokens * (max_blocks + 1) + 5, max_blocks=max_blocks,
+                              groups_per_endpoint=2, block_tokens=block_tokens)
     cfg = H.config_for(wl, profiles=WEIGHTED, max_prompt_bytes=wl.R * wl.T * 4)
     gpu, cpu = _pair(cfg)
-    if partition is not None:
-        gpu.set_option("pipe_partition", partition)
     _load(wl, gpu, cpu)
     s = torch.cuda.current_stream().cuda_stream
     sizes = [512, 37, 512, 1, 300, 512, 512, 64, 511, 512, 200, 512]
@@ -920,12 +911,19 @@ def test_pipelined_back_to_back_batches(partition, max_blocks):
         if rnd == 0:  # a stream-ordered pick between the two pipelined rounds
             tok, offs = wl.prompts(batch=99)
             assert H.picks_equal(gpu.pick_batch(tok, offs, wl.h0), cpu.pick_batch(tok, offs, wl.h0))
-    info = gpu.pipeline_info()
-    if partition in (None, 0):
-        assert not info["partitioned"]
-    else:
-        assert info["partitioned"] and info["walk_sms"] == partition, info
-        assert 4 * info["main_sms"] < max(sizes), info
+    assert not gpu.pipeline_info()["partitioned"]
+    gpu.close()
+
+
+@pytest.mark.parametrize("name", ["pipe_partition", "pipe_hash_ctas", "pipe_match_ctas"])
+def test_removed_pipeline_options_are_unknown(name):
+    """The SM partition of the pipelined path and its per-SM CTA caps are gone: their option names are unknown."""
+    wl = H.small_workload(E=8, R=4)
+    gpu = EndpointPicker(H.config_for(wl))
+    with pytest.raises(FiEppError) as ei:
+        gpu.set_option(name, 0)
+    assert ei.value.status == abi.FI_ERR_INVALID
+    assert "unknown option" in str(ei.value)
     gpu.close()
 
 

@@ -66,8 +66,8 @@ static void free_batch(Batch& b) {
   cudaFree(b.chain_a), cudaFree(b.chain_b), cudaFree(b.nb_a), cudaFree(b.nb_b);
 }
 static void run_pair(Batch& b) {
-  CK(fi::launch_hash_blocks(b.prompts, b.offsets, b.R, b.B, b.M, b.MP, b.pre, b.nb_a, 0, 0));
-  CK(fi::launch_chain_finalize(b.pre, b.nb_a, b.h0, b.R, b.MP, b.chain_a, false, 0));
+  CK(fi::launch_hash_blocks(b.prompts, b.offsets, b.R, b.B, b.M, b.MP, b.pre, b.nb_a, 0));
+  CK(fi::launch_chain_finalize(b.pre, b.nb_a, b.h0, b.R, b.MP, b.chain_a, 0));
 }
 static void run_fused(Batch& b) {
   CK(fi::launch_hash_chain(b.prompts, b.offsets, b.h0, b.R, b.B, b.M, b.MP, b.chain_b, b.nb_b, g_sms, 0));
@@ -97,9 +97,9 @@ static bool time_shape(const char* name, uint32_t R, uint32_t M) {
     for (int it = 0; it < iters; ++it) {
       float t;
       CK(cudaEventRecord(e0));
-      CK(fi::launch_hash_blocks(b.prompts, b.offsets, b.R, b.B, b.M, b.MP, b.pre, b.nb_a, 0, 0));
+      CK(fi::launch_hash_blocks(b.prompts, b.offsets, b.R, b.B, b.M, b.MP, b.pre, b.nb_a, 0));
       CK(cudaEventRecord(p0));
-      CK(fi::launch_chain_finalize(b.pre, b.nb_a, b.h0, b.R, b.MP, b.chain_a, false, 0));
+      CK(fi::launch_chain_finalize(b.pre, b.nb_a, b.h0, b.R, b.MP, b.chain_a, 0));
       CK(cudaEventRecord(e1));
       CK(cudaEventSynchronize(e1));
       CK(cudaEventElapsedTime(&t, e0, p0));
