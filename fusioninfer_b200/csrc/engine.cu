@@ -94,7 +94,7 @@ struct PairHash {
 
 constexpr uint64_t kOpChunk = 1ull << 20;  // ops per pinned staging buffer
 
-enum KernelKind { K_HASH = 0, K_CHAIN = 1, K_MATCH = 2, K_INDEX = 3, K_OTHER = 4, K_KINDS = 5 };
+enum KernelKind { K_HASH = 0, K_MATCH = 1, K_INDEX = 2, K_OTHER = 3, K_KINDS = 4 };
 
 uint32_t pow2_ceil32(uint32_t v) {
   uint32_t p = 1;
@@ -147,7 +147,7 @@ struct fi_epp {
   uint32_t feed_slices = 8;  // FI_EPP_FEED_SLICES (1: one copy, then the whole batch)
   // Pipelined device path (fi_epp_pick_submit / fi_epp_pick_wait): stage A (block hashing + chain walk) of
   // batch k+1 runs on s_a while stage B (match + pick) of batch k runs on s_main; the chain / block-count
-  // buffers are double-buffered (slot = batch parity), the pre-states are not (stage A is serial on s_a).
+  // buffers are double-buffered (slot = batch parity).
   cudaStream_t s_a = nullptr;
   uint64_t* d_chain2 = nullptr;
   uint32_t* d_nblocks2 = nullptr;
@@ -161,7 +161,6 @@ struct fi_epp {
   uint8_t* d_prompts = nullptr;
   uint64_t* d_offsets = nullptr;
   uint64_t* d_h0 = nullptr;
-  uint64_t* d_pre = nullptr;
   uint64_t* d_chain = nullptr;
   uint32_t* d_nblocks = nullptr;
   fi_pick* d_picks = nullptr;   // [R][P] final
@@ -179,7 +178,7 @@ struct fi_epp {
   // less than receiving 2 KiB of chain over NVLink; not measured on H100s, bench.py --gpus N times both); FI_EPP_SHARD_HASH=
   // split / option "shard_hash" = 1: every rank hashes R/world requests and the chains are all-gathered
   bool split_hash = false;
-  uint32_t chain_rows = 0;  // rows allocated in d_chain / d_pre / d_nblocks (max_batch padded for the gather)
+  uint32_t chain_rows = 0;  // rows allocated in d_chain / d_nblocks (max_batch padded for the gather)
   // sharded mode: directory gossip (index_kernels.cu): this rank's transition log of the current round and the
   // buffers the ranks' logs are gathered into
   unsigned long long* d_glog_n = nullptr;  // [2] appear / vanish counts
@@ -339,7 +338,6 @@ void drain_profile(fi_epp* h) {
     if (cudaEventSynchronize(e.b) == cudaSuccess && cudaEventElapsedTime(&ms, e.a, e.b) == cudaSuccess) {
       switch (e.kind) {
         case K_HASH: h->stats.ms_hash_blocks += ms; h->stats.n_hash_blocks++; break;
-        case K_CHAIN: h->stats.ms_chain_probe += ms; h->stats.n_chain_probe++; break;
         case K_MATCH: h->stats.ms_match_pick += ms; h->stats.n_match_pick++; break;
         case K_INDEX: h->stats.ms_index_apply += ms; h->stats.n_index_apply++; break;
         default: h->stats.ms_other += ms; h->stats.n_other++; break;
@@ -947,20 +945,11 @@ int run_hash(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, con
              uint32_t R, cudaStream_t s) {
   uint64_t* chain = h->d_chain + (size_t)r0 * h->MP;
   uint32_t* nb = h->d_nblocks + r0;
-  if (hash_chain_fused(h->cfg.block_bytes)) {  // block hashing and chain walk in one kernel, no pre-states in HBM
-    LaunchScope ls(h, s, K_HASH);
+  LaunchScope ls(h, s, K_HASH);
+  if (h->fast_hash) {  // block hashing and chain walk in one kernel, no pre-states in HBM
     FI_CUDA(launch_hash_chain(d_prompts, d_offsets + r0, d_h0 + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP,
                               chain, nb, h->sm_count, s));
-  } else if (h->fast_hash) {
-    uint64_t* pre = h->d_pre + (size_t)r0 * h->MP;  // tiled by groups of 32 requests: r0 % 32 == 0
-    {
-      LaunchScope ls(h, s, K_HASH);
-      FI_CUDA(launch_hash_blocks(d_prompts, d_offsets + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, pre, nb, s));
-    }
-    LaunchScope ls(h, s, K_CHAIN);
-    FI_CUDA(launch_chain_finalize(pre, nb, d_h0 + r0, R, h->MP, chain, s));
   } else {
-    LaunchScope ls(h, s, K_HASH);
     FI_CUDA(launch_hash_generic(d_prompts, d_offsets + r0, d_h0 + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP,
                                 chain, nb, s));
   }
@@ -1082,7 +1071,7 @@ int setup_peer_exchange(fi_epp* h) {
 // FI_EPP_TRACE=<call index>: print that call's kernel timeline (start/end relative to the call's start)
 void dump_trace(fi_epp* h, uint32_t R) {
   if (!h->tracing) return;
-  static const char* names[] = {"hash_blocks", "chain_finalize", "match_pick", "index", "other"};
+  static const char* names[] = {"hash_chain", "match_pick", "index", "other"};
   cudaStreamSynchronize(h->s_main);
   std::fprintf(stderr, "[fi_epp trace] rank %u call %ld: R=%u\n", h->rank, h->trace_call, R);
   for (auto& e : h->pending_ev) {
@@ -1153,7 +1142,7 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
   if (rc != FI_OK) return rc;
   rc = upload_lora(h);
   if (rc != FI_OK) return rc;
-  if (h->pipe_seq)  // a plain pick after pipelined submits: their stages share d_pre / d_chain with ours
+  if (h->pipe_seq)  // a plain pick after pipelined submits: their stage A shares d_chain (slot 0) with ours
     FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[(h->pipe_seq - 1) & 1], 0));
   MatchParams mp{};
   fill_match_params(h, mp, h->d_chain, h->d_nblocks, d_offsets, d_h0, d_adapters, R, sharded ? h->d_local : d_out, !sharded);
@@ -1325,32 +1314,20 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
   uint64_t* chain = slot ? h->d_chain2 : h->d_chain;
   uint32_t* nb = slot ? h->d_nblocks2 : h->d_nblocks;
   // ---- stage A: inputs are ready in the caller's stream order; the slot's buffers are free once the
-  // match of two batches ago is done; d_pre and slot 0's d_chain / d_nblocks are free once the previous plain pick
+  // match of two batches ago is done; slot 0's d_chain / d_nblocks are free once the previous plain pick
   // (if any) is done
   FI_CUDA(cudaEventRecord(h->ev_in, us));
   FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_in, 0));
   if (h->pipe_seq >= 2) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot], 0));
   FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_plain, 0));
   if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_lru, 0));  // a device-LRU Add may still be reading d_chain
-  if (hash_chain_fused(h->cfg.block_bytes)) {
+  {
     // Block hashing and chain walk in one kernel (hash_kernels.cu hash_chain).  It does not wait for the previous
     // batch's match_pick: its CTAs fill whole SMs, so they take the SMs that match's CTAs leave as its queue drains
     // (DESIGN.md §4.0: 180.0 us per step this way, 190.8 us waiting for the match).
     LaunchScope ls(h, h->s_a, K_HASH);
     FI_CUDA(launch_hash_chain(d_prompts, d_offsets, d_h0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, chain, nb,
                               h->sm_count, h->s_a));
-  } else {
-    {
-      // this batch's block hashing runs beside the previous batch's match_pick
-      LaunchScope ls(h, h->s_a, K_HASH);
-      FI_CUDA(launch_hash_blocks(d_prompts, d_offsets, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, h->d_pre, nb, h->s_a));
-    }
-    // The chain walk is serial latency — a warp per scheduler that wants an issue slot every few cycles — and
-    // slows several-fold next to a busy kernel that competes for the same schedulers, so it waits for the
-    // previous batch's match to drain; what overlaps is this batch's block hashing with that match.
-    if (h->pipe_seq >= 1) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot ^ 1u], 0));
-    LaunchScope ls(h, h->s_a, K_CHAIN);
-    FI_CUDA(launch_chain_finalize(h->d_pre, nb, d_h0, R, h->MP, chain, h->s_a));
   }
   FI_CUDA(cudaEventRecord(h->ev_a[slot], h->s_a));
   // ---- stage B
@@ -1493,7 +1470,6 @@ void fi_epp_destroy(fi_epp* h) {
   cudaFree(h->d_prompts);
   cudaFree(h->d_offsets);
   cudaFree(h->d_h0);
-  cudaFree(h->d_pre);
   cudaFree(h->d_chain);
   cudaFree(h->d_nblocks);
   cudaFree(h->d_picks);
@@ -1628,15 +1604,15 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
     FI_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
   FI_TRY(cudaEventRecord(h->ev_index, h->s_index));
   const uint64_t R = cfg->max_batch;
-  // rows of the per-request buffers: whole groups of 32 requests (the pre-states are tiled), and — for a shard
-  // of a bigger pool — room for the in-place all-gather of `world` equal slices of 32-aligned length
+  // rows of the per-request buffers: whole groups of 32 requests (the sliced host feed and the split-hash gather
+  // cut the batch on 32-request boundaries), and — for a shard of a bigger pool — room for the in-place all-gather
+  // of `world` equal slices of 32-aligned length
   h->chain_rows = (uint32_t)((R + 31) / 32 * 32);
   if (cfg->endpoint_count < cfg->num_endpoints) h->chain_rows += 32 * (FI_MAX_RANKS + 1);
   if (const char* e = std::getenv("FI_EPP_SHARD_HASH")) h->split_hash = std::strcmp(e, "split") == 0;
   FI_TRY(cudaMalloc(&h->d_prompts, h->cfg.max_prompt_bytes + 64));
   FI_TRY(cudaMalloc(&h->d_offsets, (R + 1) * sizeof(uint64_t)));
   FI_TRY(cudaMalloc(&h->d_h0, R * sizeof(uint64_t)));
-  FI_TRY(cudaMalloc(&h->d_pre, (size_t)h->chain_rows * h->MP * sizeof(uint64_t)));
   FI_TRY(cudaMalloc(&h->d_chain, (size_t)h->chain_rows * h->MP * sizeof(uint64_t)));
   FI_TRY(cudaMalloc(&h->d_nblocks, (size_t)h->chain_rows * sizeof(uint32_t)));
   FI_TRY(cudaMalloc(&h->d_picks, R * h->P * sizeof(fi_pick)));
@@ -2237,7 +2213,7 @@ int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets
   if (rc != FI_OK) return rc;
   rc = stage_inputs(h, prompts, offsets, h0, R, total);
   if (rc != FI_OK) return rc;
-  if (h->pipe_seq)  // a pipelined batch's stage A (on s_a) shares d_chain (slot 0) and d_pre with us
+  if (h->pipe_seq)  // a pipelined batch's stage A (on s_a) shares d_chain (slot 0) with us
     FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[(h->pipe_seq - 1) & 1], 0));
   if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_lru, 0));  // a device-LRU Add may still be reading d_chain
   h->last_plain_R = 0;  // d_chain no longer holds a pick batch's chains

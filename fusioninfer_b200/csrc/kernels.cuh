@@ -2,8 +2,6 @@
 //
 // HBM layout (DESIGN.md "Data layout"):
 //   prompts   concatenated prompt bytes, request r = [offsets[r], offsets[r+1])
-//   pre       tiled u64     block pre-states (hash_blocks → chain_finalize): 16-byte unit u of
-//                           request r at ((r/32)*MP/2 + u)*32 + r%32 — coalesced for the chain walker
 //   chain     [R][MP] u64   chained block hashes h_1..h_n (SURVEY.md Appendix A.1)
 //   index     keys    [C]     u64 table, buckets of 4 keys = one 32 B sector; 0 = empty, ~0 = tombstone
 //             node_of [C]     u32 node of the key in that slot
@@ -183,13 +181,8 @@ struct MergeParams {
 };
 
 // ---- launchers (each returns the cudaGetLastError() of its launch) -----------
-cudaError_t launch_hash_blocks(const uint8_t* prompts, const uint64_t* offsets, uint32_t R, uint32_t B,
-                               uint32_t M, uint32_t MP, uint64_t* pre, uint32_t* nblocks, cudaStream_t s);
-cudaError_t launch_chain_finalize(const uint64_t* pre, const uint32_t* nblocks, const uint64_t* h0,
-                                  uint32_t R, uint32_t MP, uint64_t* chain, cudaStream_t s);
-// hash_blocks + chain_finalize fused (block_bytes 32, 64 or 128 only: hash_chain_fused(B)); no pre-state buffer.
+// block hashing and chain walk in one kernel, for block_bytes % 32 == 0 (cudaErrorInvalidValue otherwise).
 // sm_count sets the tile: 32, 64 or 128 requests per CTA, the smallest whose grid fits one CTA per SM
-inline bool hash_chain_fused(uint32_t B) { return B == 32 || B == 64 || B == 128; }
 cudaError_t launch_hash_chain(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
                               uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain, uint32_t* nblocks,
                               int sm_count, cudaStream_t s);

@@ -211,7 +211,8 @@ typedef struct fi_epp_stats {
   uint64_t requests;
   uint64_t h2d_bytes;
   uint64_t d2h_bytes;
-  /* per-kernel device time, accumulated only while profiling is on */
+  /* per-kernel device time, accumulated only while profiling is on.  Block hashing and the chain walk (one
+   * kernel) are reported entirely under *_hash_blocks; the *_chain_probe fields stay 0. */
   double ms_hash_blocks, ms_chain_probe, ms_match_pick, ms_index_apply, ms_other;
   uint64_t n_hash_blocks, n_chain_probe, n_match_pick, n_index_apply, n_other;
   uint64_t probed_blocks; /* sum over requests of N_probe (SURVEY.md §8d), profiling only */

@@ -228,13 +228,13 @@ def _hash_walk(R, sms):
 
 
 @pytest.mark.parametrize("M", [5, 24, 1023])
-@pytest.mark.parametrize("B", [32, 64, 128, 96, 160])
+@pytest.mark.parametrize("B", [32, 64, 128, 96, 160, 256])
 def test_hash_parity_every_tile_shape(B, M):
     """Batches of 1 .. 128 * SMs + 45 requests: the smallest batch of each tile shape (WALK = 1, 2, 4), partial last
     tiles, and a grid larger than the SM count.  Ragged lengths and unaligned starts; about one request in 32 is
-    longer than the cap (it sets its tile's group count and wraps the ring), the rest are short.  B = 96 and 160
-    take hash_blocks_any and the separate chain walk.  Chains, block counts and the zero tail beyond n are
-    compared with the oracle."""
+    longer than the cap (it sets its tile's group count and wraps the ring), the rest are short.  B = 96, 160 and
+    256 take hash_chain<0, WALK>, which reads the stripe count at run time.  Chains, block counts and the zero tail
+    beyond n are compared with the oracle."""
     import torch
 
     sms = torch.cuda.get_device_properties(0).multi_processor_count

@@ -871,9 +871,9 @@ def _device_lru_from_device_chains(max_blocks, T, cap, slots):
 def test_pipelined_back_to_back_batches(block_tokens, max_blocks):
     """Twelve batches of different sizes submitted back to back with nothing in between (so that the pipeline really
     has its two batches in flight and reuses every slot buffer several times), one wait at the end, every output
-    equal to the oracle's; then the same again after a stream-ordered pick.  64-byte blocks run stage A as one
-    hash_chain launch, 96-byte blocks as hash_blocks + chain_finalize.  max_blocks = 1023: prompts past the cap with
-    a partial last block, chain pitch 1024."""
+    equal to the oracle's; then the same again after a stream-ordered pick.  Stage A is one hash_chain launch:
+    hash_chain<2, WALK> at 64-byte blocks, the run-time stripe count hash_chain<0, WALK> at 96-byte blocks.
+    max_blocks = 1023: prompts past the cap with a partial last block, chain pitch 1024."""
     import torch
 
     if max_blocks == 128:

@@ -1,7 +1,8 @@
-// hashchain.cu — the fused hash_chain kernel against hash_blocks + chain_finalize, back to back: bit-exact
-// chains and block counts on ragged, unaligned and truncated prompts (every block size the fused kernel takes,
-// odd batch sizes), then CUDA-event times at the cfg 3 shape (16 384 requests x 4 096-token prompts, 64-byte
-// blocks, 256 blocks) and the cfg 2 shape (4 096 requests x 2 048-token prompts).  Prints one line per case.
+// hashchain.cu — the hash_chain kernel against hash_generic, the fully serial kernel that hashes every block as one
+// XXH64 message (no pre-state split): bit-exact chains and block counts on ragged, unaligned and truncated prompts
+// (block sizes 32, 64, 96, 128, 160 and 256, odd batch sizes), then CUDA-event times of hash_chain at the cfg 3
+// shape (16 384 requests x 4 096-token prompts, 64-byte blocks, 256 blocks), the cfg 2 shape (4 096 requests x
+// 2 048-token prompts) and the cfg 3 shape at 96- and 160-byte blocks.  Prints one line per case.
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I fusioninfer_b200/csrc -o tools/microbench/hashchain tools/microbench/hashchain.cu
 #include <cstdio>
 #include <cstdlib>
@@ -25,11 +26,11 @@ static int g_sms = 132;
 struct Batch {
   uint32_t R, B, M, MP;
   uint8_t* prompts;
-  uint64_t *offsets, *h0, *pre, *chain_a, *chain_b;
+  uint64_t *offsets, *h0, *chain_a, *chain_b;
   uint32_t *nb_a, *nb_b;
 };
 
-// ragged: lengths uniform in [0, (M + 3) * B + B - 1] and random byte gaps between prompts (unaligned starts)
+// ragged: lengths uniform in [0, (M + 4) * B - 1] and random byte gaps between prompts (unaligned starts)
 static Batch make_batch(uint32_t R, uint32_t B, uint32_t M, bool ragged, uint64_t seed) {
   Batch b{R, B, M, (M + 7) & ~7u};
   std::mt19937_64 rng(seed);
@@ -45,11 +46,9 @@ static Batch make_batch(uint32_t R, uint32_t B, uint32_t M, bool ragged, uint64_
   for (auto& x : bytes) x = (uint8_t)rng();
   std::vector<uint64_t> h0(R);
   for (auto& x : h0) x = rng();
-  const uint32_t Rp = (R + 31) & ~31u;
   CK(cudaMalloc(&b.prompts, bytes.size()));
   CK(cudaMalloc(&b.offsets, (R + 1) * sizeof(uint64_t)));
   CK(cudaMalloc(&b.h0, R * sizeof(uint64_t)));
-  CK(cudaMalloc(&b.pre, (size_t)Rp * b.MP * sizeof(uint64_t)));
   CK(cudaMalloc(&b.chain_a, (size_t)R * b.MP * sizeof(uint64_t)));
   CK(cudaMalloc(&b.chain_b, (size_t)R * b.MP * sizeof(uint64_t)));
   CK(cudaMalloc(&b.nb_a, R * sizeof(uint32_t)));
@@ -62,14 +61,13 @@ static Batch make_batch(uint32_t R, uint32_t B, uint32_t M, bool ragged, uint64_
   return b;
 }
 static void free_batch(Batch& b) {
-  cudaFree(b.prompts), cudaFree(b.offsets), cudaFree(b.h0), cudaFree(b.pre);
+  cudaFree(b.prompts), cudaFree(b.offsets), cudaFree(b.h0);
   cudaFree(b.chain_a), cudaFree(b.chain_b), cudaFree(b.nb_a), cudaFree(b.nb_b);
 }
-static void run_pair(Batch& b) {
-  CK(fi::launch_hash_blocks(b.prompts, b.offsets, b.R, b.B, b.M, b.MP, b.pre, b.nb_a, 0));
-  CK(fi::launch_chain_finalize(b.pre, b.nb_a, b.h0, b.R, b.MP, b.chain_a, 0));
+static void run_generic(Batch& b) {
+  CK(fi::launch_hash_generic(b.prompts, b.offsets, b.h0, b.R, b.B, b.M, b.MP, b.chain_a, b.nb_a, 0));
 }
-static void run_fused(Batch& b) {
+static void run_chain(Batch& b) {
   CK(fi::launch_hash_chain(b.prompts, b.offsets, b.h0, b.R, b.B, b.M, b.MP, b.chain_b, b.nb_b, g_sms, 0));
 }
 static bool same(const Batch& b) {
@@ -82,44 +80,34 @@ static bool same(const Batch& b) {
   return ca == cb && na == nb;
 }
 
-static bool time_shape(const char* name, uint32_t R, uint32_t M) {
-  Batch b = make_batch(R, 64, M, false, 3);
-  cudaEvent_t e0, e1, p0, p1;
+// hash_chain alone, 3 x 50 launches; the outputs of the last one against hash_generic
+static bool time_shape(const char* name, uint32_t R, uint32_t B, uint32_t M) {
+  Batch b = make_batch(R, B, M, false, 3);
+  cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
-  CK(cudaEventCreate(&p0));
-  CK(cudaEventCreate(&p1));
-  for (int w = 0; w < 5; ++w) run_pair(b), run_fused(b);
+  for (int w = 0; w < 5; ++w) run_chain(b);
   CK(cudaDeviceSynchronize());
   const int iters = 50;
   for (int rep = 0; rep < 3; ++rep) {
-    float ms_hash = 0, ms_chain = 0, ms_pair = 0, ms_fused = 0;
+    float ms = 0;
     for (int it = 0; it < iters; ++it) {
       float t;
       CK(cudaEventRecord(e0));
-      CK(fi::launch_hash_blocks(b.prompts, b.offsets, b.R, b.B, b.M, b.MP, b.pre, b.nb_a, 0));
-      CK(cudaEventRecord(p0));
-      CK(fi::launch_chain_finalize(b.pre, b.nb_a, b.h0, b.R, b.MP, b.chain_a, 0));
+      run_chain(b);
       CK(cudaEventRecord(e1));
       CK(cudaEventSynchronize(e1));
-      CK(cudaEventElapsedTime(&t, e0, p0));
-      ms_hash += t;
-      CK(cudaEventElapsedTime(&t, p0, e1));
-      ms_chain += t;
       CK(cudaEventElapsedTime(&t, e0, e1));
-      ms_pair += t;
-      CK(cudaEventRecord(p0));
-      run_fused(b);
-      CK(cudaEventRecord(p1));
-      CK(cudaEventSynchronize(p1));
-      CK(cudaEventElapsedTime(&t, p0, p1));
-      ms_fused += t;
+      ms += t;
     }
-    std::printf("%s rep %d: hash_blocks %.1f us + chain_finalize %.1f us = %.1f us | hash_chain %.1f us\n", name, rep,
-                1e3 * ms_hash / iters, 1e3 * ms_chain / iters, 1e3 * ms_pair / iters, 1e3 * ms_fused / iters);
+    std::printf("%s (B=%u, %u blocks) rep %d: hash_chain %.1f us\n", name, B, M, rep, 1e3 * ms / iters);
   }
+  run_generic(b);
+  CK(cudaDeviceSynchronize());
   const bool ok = same(b);
   std::printf("%s outputs %s\n", name, ok ? "identical" : "DIFFER");
+  CK(cudaEventDestroy(e0));
+  CK(cudaEventDestroy(e1));
   free_batch(b);
   return ok;
 }
@@ -127,17 +115,18 @@ static bool time_shape(const char* name, uint32_t R, uint32_t M) {
 int main() {
   int fails = 0;
   CK(cudaDeviceGetAttribute(&g_sms, cudaDevAttrMultiProcessorCount, 0));
-  // correctness: every fused block size, ragged + unaligned + truncated, batch sizes with a partial last tile
+  // correctness: compiled-in (32, 64, 128) and run-time (96, 160, 256) stripe counts, ragged + unaligned +
+  // truncated, batch sizes with a partial last tile
   const uint32_t Rs[] = {1, 31, 129, 1000};
-  const uint32_t Bs[] = {32, 64, 128};
+  const uint32_t Bs[] = {32, 64, 96, 128, 160, 256};
   const uint32_t Ms[] = {5, 100, 256};
   for (uint32_t R : Rs)
     for (uint32_t B : Bs)
       for (uint32_t M : Ms)
         for (int ragged = 0; ragged < 2; ++ragged) {
           Batch b = make_batch(R, B, M, ragged, R * 7919ull + B * 31 + M + ragged);
-          run_pair(b);
-          run_fused(b);
+          run_generic(b);
+          run_chain(b);
           CK(cudaDeviceSynchronize());
           const bool ok = same(b);
           if (!ok) {
@@ -148,7 +137,11 @@ int main() {
         }
   std::printf("correctness: %d mismatching case(s) of %zu\n", fails, sizeof(Rs) / 4 * sizeof(Bs) / 4 * sizeof(Ms) / 4 * 2);
 
-  // timing at cfg 3 (16 384 x 256 blocks: 128 requests per CTA) and cfg 2 (4 096 x 128 blocks: 32 per CTA)
-  bool ok = time_shape("cfg3", 16384, 256) && time_shape("cfg2", 4096, 128);
+  // timing at cfg 3 (16 384 x 256 blocks: 128 requests per CTA), cfg 2 (4 096 x 128 blocks: 32 per CTA), and the
+  // cfg 3 prompts (16 KiB each) cut into 96- and 160-byte blocks
+  bool ok = time_shape("cfg3", 16384, 64, 256);
+  ok = time_shape("cfg2", 4096, 64, 128) && ok;
+  ok = time_shape("cfg3-96B", 16384, 96, 16384 / 96) && ok;
+  ok = time_shape("cfg3-160B", 16384, 160, 16384 / 160) && ok;
   return (fails || !ok) ? 1 : 0;
 }
