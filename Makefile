@@ -13,8 +13,9 @@ CU_OBJS := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(CU_SRCS))
 HDRS := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/fi_epp.h
 
 RANKED_ORACLE := $(OBJDIR)/libepp_ranked_oracle.so
+SUBSET_ORACLE := $(OBJDIR)/libepp_subset_oracle.so
 
-all: $(LIB) $(HOSTCHECK) oracle $(RANKED_ORACLE)
+all: $(LIB) $(HOSTCHECK) oracle $(RANKED_ORACLE) $(SUBSET_ORACLE)
 
 $(OBJDIR)/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -40,6 +41,11 @@ oracle:
 $(RANKED_ORACLE): tests/ranked_oracle.cpp oracle/epp_oracle.cpp include/fi_epp.h
 	@mkdir -p $(OBJDIR)
 	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ tests/ranked_oracle.cpp
+
+# the CPU oracle plus its subset pick (tests/subset_oracle.cpp), test infrastructure only
+$(SUBSET_ORACLE): tests/subset_oracle.cpp oracle/epp_oracle.cpp include/fi_epp.h
+	@mkdir -p $(OBJDIR)
+	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ tests/subset_oracle.cpp
 
 clean:
 	rm -rf $(OBJDIR) $(LIB) $(HOSTCHECK)

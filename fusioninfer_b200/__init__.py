@@ -18,6 +18,7 @@ from .picker import (  # noqa: F401
     default_config,
     make_config,
     model_seed,
+    subset_bitsets,
 )
 
 __all__ = [
@@ -29,6 +30,7 @@ __all__ = [
     "default_config",
     "make_config",
     "model_seed",
+    "subset_bitsets",
     "PICK_DTYPE",
     "OP_DTYPE",
     "ENDPOINT_DTYPE",

@@ -167,6 +167,8 @@ struct fi_epp {
   fi_pick* d_ranked = nullptr;  // [R][P][k] of fi_epp_pick_batch_ranked: allocated by the first such call, grown with k
   fi_pick* h_ranked = nullptr;  // pinned mirror
   size_t ranked_cap = 0;        // picks both hold
+  uint32_t* d_subsets = nullptr;  // [max_batch][ceil(E/32)] staging of fi_epp_pick_batch_subset: allocated by its first call
+  uint32_t* h_subsets = nullptr;  // pinned
   fi_pick* d_local = nullptr;   // [R][P] this rank's picks (sharded)
   fi_pick* d_gather = nullptr;  // [world][R][P]
   // peer-memory exchange (sharded mode; kernels.cuh PeerXchg)
@@ -1121,9 +1123,10 @@ void fill_match_params(fi_epp* h, MatchParams& mp, const uint64_t* chain, const 
 }
 
 // the whole pick on device buffers; result in d_out ([R][P], or [R][P][ranked_k] for the ranked pick, ranked_k > 0:
-// single rank only)
+// single rank only).  d_subsets: the ranked pick's per-request candidate bitsets ([R][ceil(E/32)], S.5a), or null
 int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0,
-                  const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed, uint32_t ranked_k) {
+                  const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed, uint32_t ranked_k,
+                  const uint32_t* d_subsets) {
   const bool sharded = h->world > 1;
   if (sharded && (h->n_sets || h->n_clears))
     return fail(h, FI_ERR_STATE, "sharded pool: index updates are collective (fi_epp_index_apply / fi_epp_index_add_chains)");
@@ -1147,6 +1150,11 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
   MatchParams mp{};
   fill_match_params(h, mp, h->d_chain, h->d_nblocks, d_offsets, d_h0, d_adapters, R, sharded ? h->d_local : d_out, !sharded);
   mp.k = ranked_k;
+  if (d_subsets) {
+    mp.subsets = d_subsets;
+    mp.sub_pitch = (h->cfg.num_endpoints + 31) / 32;
+    mp.eps = h->d_eps;
+  }
 
   const uint32_t S = h->feed_slices;
   if (feed && !sharded && h->fast_hash && S > 1 && R >= 64 * S && feed->offsets[R] >= (8ull << 20)) {
@@ -1172,6 +1180,7 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
       ms.nblocks = mp.nblocks + r0;
       ms.offsets = mp.offsets ? mp.offsets + r0 : nullptr;
       ms.adapters = mp.adapters ? mp.adapters + r0 : nullptr;
+      ms.subsets = mp.subsets ? mp.subsets + (size_t)r0 * mp.sub_pitch : nullptr;
       ms.h0 = mp.h0 + r0;
       ms.r_base = r0;
       ms.R = Rk;
@@ -1276,8 +1285,9 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
 }
 
 int run_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0,
-             const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed = nullptr, uint32_t ranked_k = 0) {
-  int rc = run_pick_impl(h, d_prompts, d_offsets, d_h0, d_adapters, R, d_out, feed, ranked_k);
+             const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed = nullptr, uint32_t ranked_k = 0,
+             const uint32_t* d_subsets = nullptr) {
+  int rc = run_pick_impl(h, d_prompts, d_offsets, d_h0, d_adapters, R, d_out, feed, ranked_k, d_subsets);
   if (rc != FI_OK) return rc;
   FI_CUDA(cudaEventRecord(h->ev_pick, h->s_main));  // index updates submitted later wait for this pick
   FI_CUDA(cudaEventRecord(h->ev_plain, h->s_main));
@@ -1474,6 +1484,7 @@ void fi_epp_destroy(fi_epp* h) {
   cudaFree(h->d_nblocks);
   cudaFree(h->d_picks);
   cudaFree(h->d_ranked);
+  cudaFree(h->d_subsets);
   cudaFree(h->d_local);
   cudaFree(h->d_gather);
   cudaFree(h->d_glog_n);
@@ -1516,6 +1527,7 @@ void fi_epp_destroy(fi_epp* h) {
   }
   if (h->h_picks) cudaFreeHost(h->h_picks);
   if (h->h_ranked) cudaFreeHost(h->h_ranked);
+  if (h->h_subsets) cudaFreeHost(h->h_subsets);
   if (h->h_offsets) cudaFreeHost(h->h_offsets);
   if (h->h_h0) cudaFreeHost(h->h_h0);
   if (h->h_nblocks) cudaFreeHost(h->h_nblocks);
@@ -2303,13 +2315,26 @@ int fi_epp_pick_batch_device_lora(fi_epp* h, const void* d_prompts, const void* 
 }
 
 // ---- ranked picks (docs/SPEC.md S.6a): run_pick with k > 0, which selects the RANKED match-kernel variant --------
-int fi_epp_pick_batch_ranked(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
-                             const uint64_t* adapters, uint32_t R, uint32_t k, fi_pick* out, uint64_t* chains_out) {
+// Subset picks (S.5a) are ranked picks with per-request candidate bitsets, which select its SUBSET twin.  The bitsets
+// are pool-wide, so a handle over part of the pool cannot apply them (FI_ERR_STATE, like a sharded pool).
+static int check_subset_handle(fi_epp* h) {
+  if (h->world > 1 || h->cfg.endpoint_begin != 0 || h->cfg.endpoint_count != h->cfg.num_endpoints)
+    return fail(h, FI_ERR_STATE, "subset picks need a single handle over the whole pool");
+  return FI_OK;
+}
+
+static int pick_ranked_host(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
+                            const uint64_t* adapters, const uint32_t* subsets, uint32_t R, uint32_t k, fi_pick* out,
+                            uint64_t* chains_out) {
   if (!h || !offsets || (!h0 && R) || !out || (!prompts && R && offsets[R])) return FI_ERR_INVALID;
   if (k == 0 || k > FI_EPP_MAX_RANKED) return FI_ERR_INVALID;
   std::lock_guard<std::mutex> lk(h->mu);
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   if (h->world > 1) return fail(h, FI_ERR_STATE, "ranked picks need a single-rank pool");
+  if (subsets) {
+    const int rs = check_subset_handle(h);
+    if (rs != FI_OK) return rs;
+  }
   if (R == 0) return FI_OK;
   uint64_t total = 0;
   int rc = check_batch(h, offsets, R, &total);
@@ -2341,8 +2366,28 @@ int fi_epp_pick_batch_ranked(fi_epp* h, const uint8_t* prompts, const uint64_t* 
     FI_CUDA(cudaMemcpyAsync(h->d_adapters, h->h_adapters, (size_t)R * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main));
     h->stats.h2d_bytes += (size_t)R * sizeof(uint64_t);
   }
+  if (subsets) {
+    // the bitset staging exists only on handles that restrict picks; sized for max_batch
+    const size_t pitch = (h->cfg.num_endpoints + 31) / 32;
+    if (!h->d_subsets) {
+      if (cudaMalloc(&h->d_subsets, (size_t)h->cfg.max_batch * pitch * sizeof(uint32_t)) != cudaSuccess ||
+          cudaMallocHost(&h->h_subsets, (size_t)h->cfg.max_batch * pitch * sizeof(uint32_t)) != cudaSuccess) {
+        cudaGetLastError();
+        cudaFree(h->d_subsets);
+        if (h->h_subsets) cudaFreeHost(h->h_subsets);
+        h->d_subsets = nullptr;
+        h->h_subsets = nullptr;
+        return fail(h, FI_ERR_NOMEM, "cannot allocate the subset staging buffers");
+      }
+    }
+    const size_t sb = (size_t)R * pitch * sizeof(uint32_t);
+    std::memcpy(h->h_subsets, subsets, sb);
+    FI_CUDA(cudaMemcpyAsync(h->d_subsets, h->h_subsets, sb, cudaMemcpyHostToDevice, h->s_main));
+    h->stats.h2d_bytes += sb;
+  }
   const HostFeed feed{prompts, offsets};
-  rc = run_pick(h, h->d_prompts, h->d_offsets, h->d_h0, adapters ? h->d_adapters : nullptr, R, h->d_ranked, &feed, k);
+  rc = run_pick(h, h->d_prompts, h->d_offsets, h->d_h0, adapters ? h->d_adapters : nullptr, R, h->d_ranked, &feed, k,
+                subsets ? h->d_subsets : nullptr);
   if (rc != FI_OK) return rc;
   const size_t pb = (size_t)R * h->P * k * sizeof(fi_pick);
   FI_CUDA(cudaMemcpyAsync(h->h_ranked, h->d_ranked, pb, cudaMemcpyDeviceToHost, h->s_main));
@@ -2356,14 +2401,18 @@ int fi_epp_pick_batch_ranked(fi_epp* h, const uint8_t* prompts, const uint64_t* 
   return FI_OK;
 }
 
-int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
-                                    const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, uint32_t k,
-                                    void* d_out, void* d_chains_out, void* stream) {
+static int pick_ranked_device(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                              const void* d_adapters, const void* d_subsets, uint32_t R, uint64_t total_prompt_bytes,
+                              uint32_t k, void* d_out, void* d_chains_out, void* stream) {
   if (!h || !d_offsets || (!d_h0 && R) || !d_out) return FI_ERR_INVALID;
   if (k == 0 || k > FI_EPP_MAX_RANKED) return FI_ERR_INVALID;
   std::lock_guard<std::mutex> lk(h->mu);
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   if (h->world > 1) return fail(h, FI_ERR_STATE, "ranked picks need a single-rank pool");
+  if (d_subsets) {
+    const int rs = check_subset_handle(h);
+    if (rs != FI_OK) return rs;
+  }
   if (R == 0) return FI_OK;
   if (R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
   (void)total_prompt_bytes;  // inputs stay where they are: no staging copy, no capacity limit
@@ -2371,7 +2420,7 @@ int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void
   FI_CUDA(cudaEventRecord(h->ev_user, us));
   FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_user, 0));
   int rc = run_pick(h, (const uint8_t*)d_prompts, (const uint64_t*)d_offsets, (const uint64_t*)d_h0,
-                    (const uint64_t*)d_adapters, R, (fi_pick*)d_out, nullptr, k);
+                    (const uint64_t*)d_adapters, R, (fi_pick*)d_out, nullptr, k, (const uint32_t*)d_subsets);
   if (rc != FI_OK) return rc;
   if (d_chains_out) {
     rc = copy_chains_out(h, (uint64_t*)d_chains_out, R, cudaMemcpyDeviceToDevice, h->s_main);
@@ -2380,6 +2429,32 @@ int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void
   FI_CUDA(cudaEventRecord(h->ev_done, h->s_main));
   FI_CUDA(cudaStreamWaitEvent(us, h->ev_done, 0));
   return FI_OK;
+}
+
+int fi_epp_pick_batch_ranked(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
+                             const uint64_t* adapters, uint32_t R, uint32_t k, fi_pick* out, uint64_t* chains_out) {
+  return pick_ranked_host(h, prompts, offsets, h0, adapters, nullptr, R, k, out, chains_out);
+}
+
+int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                                    const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, uint32_t k,
+                                    void* d_out, void* d_chains_out, void* stream) {
+  return pick_ranked_device(h, d_prompts, d_offsets, d_h0, d_adapters, nullptr, R, total_prompt_bytes, k, d_out,
+                            d_chains_out, stream);
+}
+
+int fi_epp_pick_batch_subset(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
+                             const uint64_t* adapters, const uint32_t* subsets, uint32_t R, uint32_t k, fi_pick* out,
+                             uint64_t* chains_out) {
+  return pick_ranked_host(h, prompts, offsets, h0, adapters, subsets, R, k, out, chains_out);
+}
+
+int fi_epp_pick_batch_device_subset(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                                    const void* d_adapters, const void* d_subsets, uint32_t R,
+                                    uint64_t total_prompt_bytes, uint32_t k, void* d_out, void* d_chains_out,
+                                    void* stream) {
+  return pick_ranked_device(h, d_prompts, d_offsets, d_h0, d_adapters, d_subsets, R, total_prompt_bytes, k, d_out,
+                            d_chains_out, stream);
 }
 
 int fi_epp_pick_submit(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,

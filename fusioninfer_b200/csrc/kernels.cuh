@@ -164,6 +164,10 @@ struct MatchParams {
   uint32_t lane_zero;                 // always 0: makes the ticket address formally lane-dependent (match_kernels.cu take_ticket)
   uint32_t k;                         // 0: one pick per profile, out [R][P]; else the ranked pick, out [R][P][k] (S.6a)
   PeerXchg px;                        // sharded mode, peer-memory exchange (px.enabled)
+  // subset picks (docs/SPEC.md S.5a), ranked launches only; appended so that the other fields keep their offsets
+  const uint32_t* subsets;  // [R][sub_pitch] candidate bitset of each request over the pool, or null (unrestricted)
+  uint32_t sub_pitch;       // words per subset row: ceil(E_global / 32); words past it read as 0
+  const EndpointDev* eps;   // [E_global] raw endpoint state: the per-request queue min / max of a subset pick
 };
 
 struct MergeParams {

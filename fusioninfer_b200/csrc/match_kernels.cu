@@ -19,7 +19,8 @@
 //      share the per-batch "zero-match best" precomputed by prepare_endpoints —
 //      valid because every scorer weight is >= 0, so a total is monotone in the
 //      match count;
-//   5. warp-shuffle argmax (the RANKED variant: k selection rounds, ranked_profile); equal totals are resolved by the request's tie rotation (tiebreak.cuh — upstream's
+//   5. warp-shuffle argmax (the RANKED variant: k selection rounds, ranked_profile; its SUBSET twin scores only each
+//      request's candidate subset, S.5a); equal totals are resolved by the request's tie rotation (tiebreak.cuh — upstream's
 //      MaxScorePicker shuffles, Appendix A.5), then the pd-profile-handler threshold rule (Appendix A.6,
 //      /root/reference/pkg/router/strategy.go:129-133).
 //
@@ -93,8 +94,11 @@ __device__ __forceinline__ double lora_score(const LoraDev& l, uint64_t adapter)
   return waiting ? 0.6 : 0.0;
 }
 
+// REQ_QUEUE (subset picks, S.5a): the queue scorer's value is q_v, normalised over the request's own eligible set,
+// instead of the per-batch table entry
+template <bool REQ_QUEUE = false>
 __device__ __forceinline__ double total_score(const ProfileDev& pr, const double* __restrict__ sc_p, uint32_t Epad,
-                                              uint32_t e, uint32_t m, uint32_t n, double lora_v = 0.0) {
+                                              uint32_t e, uint32_t m, uint32_t n, double lora_v = 0.0, double q_v = 0.0) {
   double total = 0.0;
 #pragma unroll
   for (int s = 0; s < (int)FI_EPP_MAX_SCORERS; ++s) {
@@ -104,6 +108,8 @@ __device__ __forceinline__ double total_score(const ProfileDev& pr, const double
         v = n ? __ddiv_rn((double)m, (double)n) : 0.0;
       else if (pr.kind[s] == FI_SCORER_LORA)
         v = lora_v;
+      else if (REQ_QUEUE && pr.kind[s] == FI_SCORER_QUEUE)
+        v = q_v;
       else
         v = sc_p[(uint64_t)s * Epad + e];
       total = __dadd_rn(total, __dmul_rn(v, pr.weight[s]));
@@ -252,16 +258,47 @@ __device__ __forceinline__ uint32_t take_ticket(uint32_t* counter, uint32_t opaq
 // the round's winner and only the lane that owned it rescans its endpoints, bounded by the winner's (score, key).
 // No "taken" mask: a round is one butterfly plus one lane's rescan.  Once every lane is out of candidates the
 // rounds write the padding entry (FI_NO_ENDPOINT, match 0, score 0).
-template <int VEC, int G>
+// SUBSET (S.5a): sub[x] is the request's candidate word t*VEC + x.  The eligible words become elig & sub, and the
+// queue scorer is normalised by the min / max queue depth over those endpoints (a warp reduction over the raw
+// endpoint state), in prepare_endpoints' arithmetic; the per-batch queue column does not apply.
+template <int VEC, int G, bool SUBSET>
 __device__ __forceinline__ void ranked_profile(const MatchParams& p, uint32_t pi, const BitCounter (&cnt)[VEC],
-                                               const TieRot& tr, uint32_t n, uint32_t r, int lane, int t, int g,
-                                               uint32_t& dec_e, uint32_t& dec_m) {
+                                               const uint32_t (&sub)[VEC], const TieRot& tr, uint32_t n, uint32_t r,
+                                               int lane, int t, int g, uint32_t& dec_e, uint32_t& dec_m) {
   const ProfileDev& pr = p.st.prof[pi];
   const double* sc_p = p.st.sc + (uint64_t)pi * FI_EPP_MAX_SCORERS * p.st.Epad;
   const bool lora = p.st.has_lora != 0;
   const uint64_t adapter = (lora && p.adapters) ? p.adapters[r] : 0;
   constexpr uint32_t BPG = 32 / G;
   const uint32_t gmask_bits = (BPG >= 32 ? 0xFFFFFFFFu : ((1u << BPG) - 1u)) << (g * BPG);
+  bool has_q = false;  // SUBSET: the profile has a queue scorer
+  int minq = 0, maxq = 0;
+  if constexpr (SUBSET) {
+#pragma unroll
+    for (int s = 0; s < (int)FI_EPP_MAX_SCORERS; ++s) has_q |= s < (int)pr.n_scorers && pr.kind[s] == FI_SCORER_QUEUE;
+    if (has_q) {  // warp-uniform
+      int mn = INT_MAX, mx = INT_MIN;
+#pragma unroll
+      for (int x = 0; x < VEC; ++x) {
+        const uint32_t wi = t * VEC + x;
+        uint32_t cand = p.st.elig[(uint64_t)pi * p.ix.W + wi] & sub[x] & gmask_bits;
+        while (cand) {
+          const uint32_t bit = __ffs(cand) - 1;
+          cand &= cand - 1;
+          const int q = __ldg(&p.eps[p.ep_begin + wi * 32 + bit].queue_depth);
+          mn = min(mn, q);
+          mx = max(mx, q);
+        }
+      }
+#pragma unroll
+      for (int d = 16; d > 0; d >>= 1) {
+        mn = min(mn, __shfl_xor_sync(FULL, mn, d));
+        mx = max(mx, __shfl_xor_sync(FULL, mx, d));
+      }
+      minq = mn;
+      maxq = mx;
+    }
+  }
   // this lane's best endpoint ranked strictly after (ts, tk); ts < 0: no bound (totals are >= 0)
   auto scan = [&](double ts, uint32_t tk) {
     Best b;
@@ -273,12 +310,22 @@ __device__ __forceinline__ void ranked_profile(const MatchParams& p, uint32_t pi
     for (int x = 0; x < VEC; ++x) {
       const uint32_t wi = t * VEC + x;
       uint32_t cand = p.st.elig[(uint64_t)pi * p.ix.W + wi] & gmask_bits;
+      if constexpr (SUBSET) cand &= sub[x];
       while (cand) {
         const uint32_t bit = __ffs(cand) - 1;
         cand &= cand - 1;
         const uint32_t e = wi * 32 + bit;
         const uint32_t m = bc_get(cnt[x], bit);
-        const double s = total_score(pr, sc_p, p.st.Epad, e, m, n, lora ? lora_score(p.st.lora[e], adapter) : 0.0);
+        double qv = 0.0;
+        if constexpr (SUBSET) {
+          if (has_q) {
+            const int q = __ldg(&p.eps[p.ep_begin + e].queue_depth);
+            qv = (maxq == minq) ? 1.0
+                                : __ddiv_rn((double)((long long)maxq - (long long)q), (double)((long long)maxq - (long long)minq));
+            qv = qv < 0.0 ? 0.0 : (qv > 1.0 ? 1.0 : qv);
+          }
+        }
+        const double s = total_score<SUBSET>(pr, sc_p, p.st.Epad, e, m, n, lora ? lora_score(p.st.lora[e], adapter) : 0.0, qv);
         const uint32_t k = tr.key(e);
         if (ts >= 0.0 && !(ts > s || (ts == s && tk < k))) continue;  // ranked before or at the bound
         if (better(s, k, b)) {
@@ -331,7 +378,10 @@ __device__ __forceinline__ void ranked_profile(const MatchParams& p, uint32_t pi
 // row is 16 × 8-byte loads and one instruction brings in 2 rows; 16 rows in flight.
 // (The RANKED variant keeps the counters live through its selection rounds: it asks for two CTAs per SM, the
 // register budget of the four-word shape, instead of spilling under the three-CTA budget of the two-word one.)
-template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED>
+// SUBSET (with RANKED only): every request carries a candidate bitset (docs/SPEC.md S.5a).  Steps 1-3 do not look
+// at it — the walk and the counts stay pool-wide — and its words are loaded when the request starts, so they
+// arrive under the walk; only the scoring of ranked_profile uses them.
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false>
 __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MIN_BLOCKS : FI_MATCH_MIN_BLOCKS + 1))
     match_pick_kernel(const MatchParams p) {
   constexpr int G = 32 / LPR;                 // rows per load instruction
@@ -379,6 +429,15 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
     if (r >= p.R) break;
     if (lane == 0) r_next = take_ticket(p.work_counter, threadIdx.x & p.lane_zero);
     const uint32_t n = p.nblocks[r];
+    uint32_t sub[VEC];  // SUBSET: this lane's words of the request's candidate bitset
+#pragma unroll
+    for (int x = 0; x < VEC; ++x) {
+      sub[x] = 0u;
+      if constexpr (SUBSET) {
+        const uint32_t wi = t * VEC + x;
+        if (wi < p.sub_pitch) sub[x] = __ldg(p.subsets + (uint64_t)r * p.sub_pitch + wi);
+      }
+    }
     uint64_t* s_chain = s_chain_base + (size_t)buf * p.MP;
 #ifdef FI_MATCH_TIMING
     const long long tm0 = clock64();
@@ -516,7 +575,7 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
     for (int pi = 0; pi < (int)FI_EPP_MAX_PROFILES; ++pi) {
       if (pi < (int)P) {
         if constexpr (RANKED) {
-          ranked_profile<VEC, G>(p, (uint32_t)pi, cnt, tr, n, r, lane, t, g, dec_e, dec_m);
+          ranked_profile<VEC, G, SUBSET>(p, (uint32_t)pi, cnt, sub, tr, n, r, lane, t, g, dec_e, dec_m);
           continue;
         }
         const ProfileDev& pr = p.st.prof[pi];
@@ -839,9 +898,9 @@ __global__ void __launch_bounds__(1024) prepare_endpoints_kernel(const EndpointD
 
 // One instantiation per kernel variant: the shared-memory opt-in (cudaFuncSetAttribute) applies to one function
 // only, and occupancy differs between variants, so each variant keeps its own cache, per device.
-template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED>
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false>
 cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_t s) {
-  const auto kern = match_pick_kernel<LPR, VEC, LPM, LORA, RANKED>;
+  const auto kern = match_pick_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET>;
   const size_t smem = (size_t)kWarps * p.MP * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
   // occupancy is a property of (kernel, smem): query once per distinct smem size
   static size_t cached_smem_dev[64];
@@ -876,6 +935,9 @@ cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_
 template <int LPR, int VEC>
 cudaError_t launch_match_t(const MatchParams& p, int sm_count, cudaStream_t s) {
   const bool lpm = p.lpm == FI_MATCH_LPM;
+  if (p.k && p.subsets)  // ranked pick over per-request candidate subsets
+    return lpm ? launch_match_variant<LPR, VEC, true, false, true, true>(p, sm_count, s)
+               : launch_match_variant<LPR, VEC, false, false, true, true>(p, sm_count, s);
   if (p.k)  // ranked pick: the LoRA scorer is handled at run time inside the variant
     return lpm ? launch_match_variant<LPR, VEC, true, false, true>(p, sm_count, s)
                : launch_match_variant<LPR, VEC, false, false, true>(p, sm_count, s);

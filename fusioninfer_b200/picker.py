@@ -58,6 +58,22 @@ def config_picker_endpoints(yaml_text: str) -> list[int]:
     return [int(v) for v in out if v]
 
 
+def subset_bitsets(subsets: Sequence[Optional[Sequence[int]]], num_endpoints: int) -> np.ndarray:
+    """Per-request candidate subsets -> the [R, ceil(num_endpoints / 32)] uint32 rows of pick_batch_subset.
+    None means no hint (every bit set); an empty list is an all-zero row (no candidate: FI_NO_ENDPOINT).
+    Endpoints outside [0, num_endpoints) are dropped, as the data plane's addresses outside the pool are."""
+    words = (int(num_endpoints) + 31) // 32
+    out = np.zeros((len(subsets), words), dtype=np.uint32)
+    for r, s in enumerate(subsets):
+        if s is None:
+            out[r] = 0xFFFFFFFF
+            continue
+        e = np.asarray(s, dtype=np.int64).ravel()
+        e = e[(e >= 0) & (e < num_endpoints)]
+        np.bitwise_or.at(out[r], e >> 5, (np.uint32(1) << (e & 31).astype(np.uint32)))
+    return out
+
+
 def make_config(
     *,
     num_endpoints: int,
@@ -297,6 +313,24 @@ class EndpointPicker:
         self._check(rc, "fi_epp_pick_batch_ranked")
         return (picks, chains) if want_chains else picks
 
+    def pick_batch_subset(self, prompts, offsets, h0, subsets, k: int = 1, adapters=None, want_chains: bool = False):
+        """The ranked pick restricted to each request's candidate subset (docs/SPEC.md S.5a).  subsets: the
+        [R, ceil(E / 32)] uint32 bitsets of subset_bitsets, or None (unrestricted: the same bytes as
+        pick_batch_ranked).  -> picks [R, n_profiles, k] (PICK_DTYPE)[, chains]"""
+        prompts, offsets, h0, R = self._inputs(prompts, offsets, h0)
+        picks = np.zeros((R, self.n_profiles, max(int(k), 1)), dtype=PICK_DTYPE)
+        chains = np.zeros((R, self.max_blocks), dtype=np.uint64) if want_chains else None
+        ad = None if adapters is None else np.ascontiguousarray(np.broadcast_to(np.asarray(adapters, dtype=np.uint64), (R,)))
+        sub = None
+        if subsets is not None:
+            sub = np.ascontiguousarray(subsets, dtype=np.uint32)
+            if sub.shape != (R, (int(self.cfg.num_endpoints) + 31) // 32):
+                raise ValueError(f"subsets must be [R, ceil(E / 32)] uint32 words, got {sub.shape}")
+        rc = self._lib.fi_epp_pick_batch_subset(self._h, _ptr(prompts), _ptr(offsets), _ptr(h0), _ptr(ad), _ptr(sub), R,
+                                                int(k), _ptr(picks), _ptr(chains))
+        self._check(rc, "fi_epp_pick_batch_subset")
+        return (picks, chains) if want_chains else picks
+
     def pick_batch_raw(self, prompts_ptr: int, offsets_ptr: int, h0_ptr: int, R: int, out_ptr: int, chains_ptr: int = 0):
         """Host-pointer variant without numpy marshalling (pinned buffers from pinned_alloc)."""
         self._check(
@@ -323,6 +357,18 @@ class EndpointPicker:
                 stream or None
             ),
             "fi_epp_pick_batch_device_ranked",
+        )
+
+    def pick_batch_device_subset(self, d_prompts: int, d_offsets: int, d_h0: int, R: int, total_bytes: int, k: int,
+                                 d_out: int, d_subsets: int = 0, d_chains: int = 0, stream: int = 0, d_adapters: int = 0):
+        """pick_batch_subset on device buffers: d_subsets holds R rows of ceil(E / 32) uint32 words (0: unrestricted),
+        d_out R * n_profiles * k picks."""
+        self._check(
+            self._lib.fi_epp_pick_batch_device_subset(
+                self._h, d_prompts, d_offsets, d_h0, d_adapters or None, d_subsets or None, R, total_bytes, int(k), d_out,
+                d_chains or None, stream or None
+            ),
+            "fi_epp_pick_batch_device_subset",
         )
 
     def pick_submit(self, d_prompts: int, d_offsets: int, d_h0: int, R: int, total_bytes: int, d_out: int, stream: int = 0):

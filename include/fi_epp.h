@@ -369,6 +369,27 @@ int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void
                                     const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, uint32_t k,
                                     void* d_out, void* d_chains_out, void* stream);
 
+/* Subset picks: the ranked pick with a per-request candidate subset (the data plane's destination-endpoint subset
+ * hint, docs/SPEC.md S.5a).  subsets: R rows of ceil(num_endpoints / 32) uint32 words; bit e%32 of word e/32 of
+ * row r set means endpoint e is a candidate for request r.  A request without a hint has every bit set; an empty
+ * hint is an all-zero row; bits at or above num_endpoints are ignored.  Only eligible candidates are ranked, and
+ * the queue scorer's min / max are taken over each request's eligible candidates.  The prefix walk stays pool-wide
+ * (it stops at the first block no endpoint of the pool holds), and so does the tie rotation.  A request and
+ * profile without an eligible candidate gets FI_NO_ENDPOINT (match 0, score 0) in every entry.
+ * subsets == NULL: every request is unrestricted, and the result is byte-identical to fi_epp_pick_batch_ranked.
+ * k and out as fi_epp_pick_batch_ranked (k = 1 is the single pick over the subset, [R][P] layout).  Everything else
+ * as the ranked calls: arguments, errors, staging, chains_out, ordering against index updates, removals and
+ * pipelined submits, fi_epp_index_add_chains_device(.., NULL, ..) afterwards.  Non-NULL subsets on a handle that
+ * covers only part of the pool (endpoint_begin / endpoint_count) or on a sharded pool: FI_ERR_STATE.  The host call
+ * stages the bitsets in a buffer allocated by its first call with subsets (max_batch rows). */
+int fi_epp_pick_batch_subset(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
+                             const uint64_t* adapters, const uint32_t* subsets, uint32_t R, uint32_t k,
+                             fi_pick* out, uint64_t* chains_out);
+int fi_epp_pick_batch_device_subset(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                                    const void* d_adapters, const void* d_subsets, uint32_t R,
+                                    uint64_t total_prompt_bytes, uint32_t k, void* d_out, void* d_chains_out,
+                                    void* stream);
+
 /* Pipelined device path.  fi_epp_pick_submit enqueues one batch exactly like fi_epp_pick_batch_device (inputs
  * ready in `stream` order at the call) but does NOT order `stream` behind the result: batch k+1's block
  * hashing and chain walk run while batch k is still being matched (two batches in flight, internal
