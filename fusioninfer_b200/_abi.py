@@ -241,6 +241,10 @@ SYMBOLS = [
     ("fi_epp_comm_unique_id", C.c_int, [_P]),
     ("fi_epp_pick_submit", C.c_int, [_P, _P, _P, _P, C.c_uint32, C.c_uint64, _P, _P]),
     ("fi_epp_pick_wait", C.c_int, [_P, _P]),
+    ("fi_epp_pick_submit_ex", C.c_int,
+     [_P, _P, _P, _P, _P, _P, C.c_uint32, C.c_uint64, C.c_uint32, _P, _P, _P, C.POINTER(C.c_uint64)]),
+    ("fi_epp_pick_wait_batch", C.c_int, [_P, C.c_uint64, _P]),
+    ("fi_epp_index_add_submitted", C.c_int, [_P, C.c_uint64, _P, _P, C.c_uint32]),
     ("fi_epp_comm_init", C.c_int, [_P, _P, C.c_uint32, C.c_uint32]),
     ("fi_epp_comm_exchange", C.c_int, [_P]),
     ("fi_epp_set_profiling", C.c_int, [_P, C.c_int]),

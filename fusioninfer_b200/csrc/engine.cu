@@ -155,6 +155,14 @@ struct fi_epp {
   cudaEvent_t ev_pick = nullptr;   // completion of the most recent pick of any kind (recorded on s_main)
   cudaEvent_t ev_plain = nullptr;  // completion of the most recent stream-ordered (not pipelined) pick
   uint64_t pipe_seq = 0;          // batches submitted
+  // Tickets (fi_epp_pick_submit_ex / fi_epp_pick_wait_batch / fi_epp_index_add_submitted): every submit, pipelined or
+  // not, takes the next number; ev_ticket[t % kTicketRing] is recorded on s_main when batch t is complete.
+  static constexpr int kTicketRing = 8;
+  cudaEvent_t ev_ticket[kTicketRing] = {};
+  uint64_t tickets = 0;
+  uint64_t slot_ticket[2] = {~0ull, ~0ull};  // ticket whose chains slot s still holds (~0: none)
+  uint32_t slot_R[2] = {0, 0};
+  cudaEvent_t ev_slot_read[2] = {};          // the last copy of slot s's chains for fi_epp_index_add_submitted
   cudaEvent_t ev_index = nullptr, ev_user = nullptr, ev_done = nullptr, ev_ctr = nullptr;
 
   // request buffers (device)
@@ -204,6 +212,9 @@ struct fi_epp {
   IndexCounters* d_ctr = nullptr;
   IndexCounters* h_ctr = nullptr;  // pinned
   bool ctr_pending = false;
+  // the last counters read (`used`) and how many new keys the updates queued since then can add at most (one per
+  // SET or LRU touch): check_counters_lagged decides from these when the pending counters are not in yet
+  uint64_t ctr_used_known = 0, ctr_unchecked = 0;
   uint64_t rebuilds = 0, ops_applied = 0;
   fi_index_op* h_sets[2] = {nullptr, nullptr};
   fi_index_op* h_clears[2] = {nullptr, nullptr};
@@ -235,7 +246,18 @@ struct fi_epp {
   struct LruHostStat {
     uint32_t error, any_ovf;  // (any_ovf: the touch kernel's overflow flag of the running sub-batch)
     unsigned long long n_sets, n_maintained, n_clears_cur, n_clears, n_doomed;
+    uint32_t planned_ovf;     // the touch kernel's overflow flag after a fi_epp_index_add_submitted call (must stay 0)
   };
+  // fi_epp_index_add_submitted: double-buffered plan and chain staging (Add j uses padd[j & 1]; ev_done: consumed)
+  struct PipeAdd {
+    uint32_t* d_plan = nullptr;
+    uint32_t* h_plan = nullptr;  // pinned
+    size_t cap = 0;              // in u32 words
+    uint64_t* d_chains = nullptr;  // [max_batch][MP]
+    cudaEvent_t ev_done = nullptr;
+  };
+  PipeAdd padd[2];
+  uint64_t padd_seq = 0;
   uint64_t lru_deferred = 0, lru_sub_batches = 0;  // host-side totals
   LruHostStat* h_lru_stat = nullptr;         // pinned copy, refreshed after every call
   uint32_t* d_lru_plan = nullptr;            // the planner's arrays of the current call
@@ -448,8 +470,12 @@ int check_counters(fi_epp* h) {
   if (!h->ctr_pending) return FI_OK;
   FI_CUDA(cudaEventSynchronize(h->ev_ctr));
   h->ctr_pending = false;
+  h->ctr_used_known = h->h_ctr->used;
+  h->ctr_unchecked = 0;
   if (h->h_lru_stat && h->h_lru_stat->error)
     return fail(h, FI_ERR_STATE, "device LRU: invariant " + std::to_string(h->h_lru_stat->error) + " broken");
+  if (h->h_lru_stat && h->h_lru_stat->planned_ovf)
+    return fail(h, FI_ERR_STATE, "device LRU: a table overflowed in a sub-batch planned not to (broken invariant)");
   if (h->h_ctr->overflow) return fail(h, FI_ERR_CAPACITY, "index full: raise index_slots");
   const uint64_t used = h->h_ctr->used, tomb = h->h_ctr->tombstones;
   if (used * 10 > h->ix.C * 7) {
@@ -462,6 +488,19 @@ int check_counters(fi_epp* h) {
     FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
   }
   return FI_OK;
+}
+
+// check_counters without its host wait where the wait cannot change anything (the pipelined calls): the counters of
+// the previous update are not in yet, but the last ones read leave room below the rebuild threshold for every key the
+// unchecked updates and `extra` more touches can add (at most one each), so they cannot ask for a rebuild (or report
+// a full index) yet.  Counters that are in are checked as always, and so are the device LRU's error flags.
+int check_counters_lagged(fi_epp* h, uint64_t extra) {
+  if (h->ctr_pending && h->world == 1) {
+    const cudaError_t q = cudaEventQuery(h->ev_ctr);
+    if (q == cudaErrorNotReady && (h->ctr_used_known + h->ctr_unchecked + extra) * 10 <= h->ix.C * 7) return FI_OK;
+    if (q != cudaSuccess && q != cudaErrorNotReady) FI_CUDA(q);
+  }
+  return check_counters(h);
 }
 
 GossipLog gossip_log(fi_epp* h) {
@@ -502,6 +541,7 @@ int flush_ops(fi_epp* h) {
                                h->rank, gl, h->s_index));
   }
   h->ops_applied += h->n_sets + h->n_clears;
+  h->ctr_unchecked += h->n_sets;
   FI_CUDA(cudaEventRecord(h->ev_buf[b], h->s_index));
   FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
   FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
@@ -716,6 +756,81 @@ int lru_refresh_stat(fi_epp* h) {
   return FI_OK;
 }
 
+// One sub-batch of a planned Add (the lru_plan.h arrays staged at `dp`): the view the LRU kernels take, and the
+// kernels themselves.  Both Add paths (lru_device_add, lru_add_submitted) enqueue a sub-batch through these two.
+LruBatch lru_sub_batch(fi_epp* h, const uint32_t* dp, const LruPlan& pl, size_t sb, const uint64_t* chains, uint32_t pitch,
+                       const uint32_t** inc) {
+  const size_t K = pl.req_id.size(), nsub = pl.subs.size(), EL = h->cfg.endpoint_count;
+  const LruSubBatch& sbt = pl.subs[sb];
+  LruBatch b{};
+  b.req_id = dp + sbt.k_begin;
+  b.req_ep = dp + K + sbt.k_begin;
+  b.req_n = dp + 2 * K + sbt.k_begin;
+  b.req_off = dp + 3 * K + sbt.k_begin;
+  b.ep_list = dp + 4 * K + sbt.k_begin;
+  b.ep_start = dp + 5 * K + sb * (EL + 1);
+  *inc = dp + 5 * K + nsub * (EL + 1) + sb * EL;
+  b.chains = chains;
+  b.pitch = pitch;
+  b.K = sbt.k_end - sbt.k_begin;
+  b.slot_of = h->d_lru_slot_of;
+  b.wcount = h->d_lru_wcount;
+  b.base = h->d_lru_base;
+  b.sets = h->d_lru_sets;
+  return b;
+}
+
+// maintain (log compaction / table rebuild) and touch of one sub-batch
+int lru_enqueue_touch(fi_epp* h, const LruBatch& b, const uint32_t* inc) {
+  {
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_lru_maintain(h->dlru, inc, false, h->s_index));
+  }
+  LaunchScope ls(h, h->s_index, K_INDEX);
+  FI_CUDA(launch_lru_touch(h->dlru, b, h->s_index));
+  return FI_OK;
+}
+
+// the rest of one sub-batch after its touch: winners, log records, index SETs, evictions, index CLEARs (clear_ovf:
+// then the overflow flags of the touch are reset); the index counters are copied back for the next rebuild decision
+int lru_enqueue_apply(fi_epp* h, const LruBatch& b, uint64_t touches, const GossipLog& glog, bool clear_ovf) {
+  const uint32_t EL = h->cfg.endpoint_count, lo = h->cfg.endpoint_begin;
+  FI_CUDA(cudaMemsetAsync(h->d_lru_ctr + 2, 0, sizeof(unsigned long long), h->s_index));
+  {
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_lru_count(h->dlru, b, h->s_index));
+  }
+  {
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_lru_scan(h->dlru, b, h->s_index));
+  }
+  {
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_lru_append(h->dlru, b, h->d_lru_clears, h->d_lru_ctr + 2, 2 * h->lru_touch_cap, lo, h->s_index));
+  }
+  {
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_index_set(h->ix, h->d_ctr, h->d_lru_sets, touches, lo, EL, h->rank, glog, h->s_index));
+  }
+  {
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_lru_evict(h->dlru, h->d_lru_clears, h->d_lru_ctr + 2, 2 * h->lru_touch_cap, lo, h->s_index));
+  }
+  {
+    // CLEARs of a sub-batch: at most one per doomed key (<= touches) and one per eviction (<= keys it added)
+    const uint64_t cap = std::min<uint64_t>(2 * h->lru_touch_cap, 2 * touches);
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_index_clear_counted(h->ix, h->d_ctr, h->d_lru_clears, cap, h->d_lru_ctr + 2, lo, EL, h->rank, glog,
+                                       h->s_index));
+  }
+  if (clear_ovf) FI_CUDA(cudaMemsetAsync(h->dlru.ovf, 0, ((size_t)EL + 1) * sizeof(uint32_t), h->s_index));  // ovf[] and any_ovf
+  FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
+  h->ctr_pending = true;
+  h->ctr_unchecked += touches;
+  return FI_OK;
+}
+
 // indexer.Add(chains[r], endpoints[r]) for r = 0..R-1 through the device LRU.  `chains` is a host pointer
 // (copied to the device first) or, with on_device, memory the index stream can read.  The first pass is
 // OPTIMISTIC: sub-batches are cut only by the scratch arrays' size, and an endpoint whose table cannot take the
@@ -818,29 +933,10 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
       if (rc != FI_OK) return rc;
     }
     const LruSubBatch& sbt = pl.subs[sb];
-    LruBatch b{};
-    b.req_id = dp + sbt.k_begin;
-    b.req_ep = dp + K + sbt.k_begin;
-    b.req_n = dp + 2 * K + sbt.k_begin;
-    b.req_off = dp + 3 * K + sbt.k_begin;
-    b.ep_list = dp + 4 * K + sbt.k_begin;
-    b.ep_start = dp + 5 * K + sb * ((size_t)EL + 1);
-    const uint32_t* inc = dp + 5 * K + nsub * ((size_t)EL + 1) + sb * (size_t)EL;
-    b.chains = d_chains;
-    b.pitch = pitch;
-    b.K = sbt.k_end - sbt.k_begin;
-    b.slot_of = h->d_lru_slot_of;
-    b.wcount = h->d_lru_wcount;
-    b.base = h->d_lru_base;
-    b.sets = h->d_lru_sets;
-    {
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_lru_maintain(h->dlru, inc, false, h->s_index));
-    }
-    {
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_lru_touch(h->dlru, b, h->s_index));
-    }
+    const uint32_t* inc = nullptr;
+    const LruBatch b = lru_sub_batch(h, dp, pl, sb, d_chains, pitch, &inc);
+    rc = lru_enqueue_touch(h, b, inc);
+    if (rc != FI_OK) return rc;
     // did some endpoint's table refuse keys?  (one host round trip per sub-batch; everything after it is queued
     // without waiting)
     FI_CUDA(cudaMemcpyAsync(&h->h_lru_stat->any_ovf, h->dlru.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index));
@@ -863,38 +959,8 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
           ++n_deferred;
         }
     }
-    FI_CUDA(cudaMemsetAsync(h->d_lru_ctr + 2, 0, sizeof(unsigned long long), h->s_index));
-    {
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_lru_count(h->dlru, b, h->s_index));
-    }
-    {
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_lru_scan(h->dlru, b, h->s_index));
-    }
-    {
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_lru_append(h->dlru, b, h->d_lru_clears, h->d_lru_ctr + 2, 2 * h->lru_touch_cap, lo, h->s_index));
-    }
-    {
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_index_set(h->ix, h->d_ctr, h->d_lru_sets, sbt.touches, lo, EL, h->rank, glog, h->s_index));
-    }
-    {
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_lru_evict(h->dlru, h->d_lru_clears, h->d_lru_ctr + 2, 2 * h->lru_touch_cap, lo, h->s_index));
-    }
-    {
-      // CLEARs of a sub-batch: at most one per doomed key (<= touches) and one per eviction (<= keys it added)
-      const uint64_t cap = std::min<uint64_t>(2 * h->lru_touch_cap, 2 * sbt.touches);
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_index_clear_counted(h->ix, h->d_ctr, h->d_lru_clears, cap, h->d_lru_ctr + 2, lo, EL, h->rank, glog,
-                                         h->s_index));
-    }
-    if (any_ovf) FI_CUDA(cudaMemsetAsync(h->dlru.ovf, 0, ((size_t)EL + 1) * sizeof(uint32_t), h->s_index));  // ovf[] and any_ovf
-    FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
-    FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
-    h->ctr_pending = true;
+    rc = lru_enqueue_apply(h, b, sbt.touches, glog, any_ovf);
+    if (rc != FI_OK) return rc;
     if (sharded) {  // the other ranks replay this sub-batch's transitions into their directories (and we theirs)
       rc = gossip_round(h);
       if (rc != FI_OK) return rc;
@@ -917,6 +983,99 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
     for (uint32_t r = 0; r < R; ++r) ep2[r] = (n_deferred && deferred[r]) ? endpoints[r] : FI_NO_ENDPOINT;
     return lru_device_add(h, ep2.data(), d_chains, true, pitch, nblocks, R, true);
   }
+  return FI_OK;
+}
+
+// the index-stream part of lru_add_submitted: plan upload, sub-batches, status copies
+int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, size_t words, fi_epp::PipeAdd& pa) {
+  // like every index update, ordered behind the picks submitted so far (a pick sees the index as of its call)
+  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_slot_read[slot], 0));
+  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
+  FI_CUDA(cudaMemcpyAsync(pa.d_plan, pa.h_plan, words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+  h->stats.h2d_bytes += words * sizeof(uint32_t);
+  const GossipLog glog = gossip_log(h);
+  h->lru_sub_batches += pl.subs.size();
+  for (size_t sb = 0; sb < pl.subs.size(); ++sb) {
+    const uint64_t touches = pl.subs[sb].touches;
+    int rc = check_counters_lagged(h, touches);  // may rebuild the index (on s_index, before this sub-batch)
+    if (rc != FI_OK) return rc;
+    const uint32_t* inc = nullptr;
+    const LruBatch b = lru_sub_batch(h, pa.d_plan, pl, sb, pa.d_chains, h->MP, &inc);
+    rc = lru_enqueue_touch(h, b, inc);
+    if (rc != FI_OK) return rc;
+    rc = lru_enqueue_apply(h, b, touches, glog, false);
+    if (rc != FI_OK) return rc;
+  }
+  int rc = lru_refresh_stat(h);
+  if (rc != FI_OK) return rc;
+  FI_CUDA(cudaMemcpyAsync(&h->h_lru_stat->planned_ovf, h->dlru.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));  // covers the status copies too
+  FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
+  return FI_OK;
+}
+
+// fi_epp_index_add_submitted: indexer.Add(chain_r, endpoints[r]) for the batch whose chains pipeline slot `slot`
+// holds.  Unlike lru_device_add, which waits on the host for the device in every sub-batch:
+//  - sub-batches are cut with lru_touch_bound (lru_plan.h), so no table can overflow: there is no optimistic pass,
+//    no overflow readback and no deferral (the touch kernel's flag is still copied back and reported as a broken
+//    invariant by the next counters check);
+//  - the plan and chain staging are double-buffered: the call waits at most for the Add before the previous one;
+//  - the index counters may lag (check_counters_lagged) — while the lag rule holds; when it does not (an index near
+//    its rebuild threshold), the call waits for the previous update's counters as lru_device_add does;
+//  - the chains are first copied out of the slot on s_copy, as soon as the batch's hashing is done, so that the submit
+//    that reuses the slot waits for that copy only and not for this Add, which runs behind the picks in flight.
+int lru_add_submitted(fi_epp* h, uint32_t slot, const uint32_t* endpoints, const uint32_t* nblocks, uint32_t R) {
+  int rc = ensure_dev_lru(h);
+  if (rc != FI_OK) return rc;
+  const uint32_t EL = h->cfg.endpoint_count, lo = h->cfg.endpoint_begin;
+  for (uint32_t r = 0; r < R; ++r)
+    if (nblocks[r] > h->cfg.lru_capacity && endpoints[r] - lo < EL)
+      return fail(h, FI_ERR_INVALID, "device LRU: a chain longer than lru_capacity");
+  rc = flush_ops(h);  // ops staged through fi_epp_index_apply come first
+  if (rc != FI_OK) return rc;
+  LruPlan& pl = h->lru_plan;
+  lru_plan_batch(endpoints, nblocks, R, lo, EL, lru_touch_bound(h->dlru.TS, h->dlru.capacity), h->lru_touch_cap,
+                 h->cfg.max_batch, &pl);
+  if (pl.subs.empty()) return FI_OK;
+  const size_t K = pl.req_id.size(), nsub = pl.subs.size();
+  const size_t words = 5 * K + nsub * ((size_t)2 * EL + 1);
+  fi_epp::PipeAdd& pa = h->padd[h->padd_seq & 1];
+  if (pa.ev_done) FI_CUDA(cudaEventSynchronize(pa.ev_done));  // the Add before the previous one is done with it
+  if (!pa.ev_done) {
+    FI_CUDA(cudaEventCreateWithFlags(&pa.ev_done, cudaEventDisableTiming));
+    FI_CUDA(cudaMalloc(&pa.d_chains, (size_t)h->cfg.max_batch * h->MP * sizeof(uint64_t)));
+  }
+  if (words > pa.cap) {
+    cudaFree(pa.d_plan);
+    if (pa.h_plan) cudaFreeHost(pa.h_plan);
+    pa.d_plan = nullptr;
+    pa.h_plan = nullptr;
+    pa.cap = 0;
+    const size_t cap = words + words / 2 + 1024;
+    FI_CUDA(cudaMalloc(&pa.d_plan, cap * sizeof(uint32_t)));
+    FI_CUDA(cudaMallocHost(&pa.h_plan, cap * sizeof(uint32_t)));
+    pa.cap = cap;
+  }
+  uint32_t* hp = pa.h_plan;
+  std::memcpy(hp, pl.req_id.data(), K * 4);
+  std::memcpy(hp + K, pl.req_ep.data(), K * 4);
+  std::memcpy(hp + 2 * K, pl.req_n.data(), K * 4);
+  std::memcpy(hp + 3 * K, pl.req_off.data(), K * 4);
+  std::memcpy(hp + 4 * K, pl.ep_list.data(), K * 4);
+  std::memcpy(hp + 5 * K, pl.ep_start.data(), pl.ep_start.size() * 4);
+  std::memcpy(hp + 5 * K + nsub * ((size_t)EL + 1), pl.inc.data(), pl.inc.size() * 4);
+  const uint64_t* slot_chain = slot ? h->d_chain2 : h->d_chain;
+  FI_CUDA(cudaStreamWaitEvent(h->s_copy, h->ev_a[slot], 0));  // the batch's chains are written
+  FI_CUDA(cudaMemcpyAsync(pa.d_chains, slot_chain, (size_t)R * h->MP * sizeof(uint64_t), cudaMemcpyDeviceToDevice, h->s_copy));
+  FI_CUDA(cudaEventRecord(h->ev_slot_read[slot], h->s_copy));
+  // From here on work that reads pa's buffers is queued: whatever happens, pa.ev_done marks its end (the s_index wait
+  // on the chain copy makes it cover that copy too), and the next call takes the other buffers.
+  rc = lru_add_submitted_enqueue(h, slot, pl, words, pa);
+  cudaError_t e = cudaStreamWaitEvent(h->s_index, h->ev_slot_read[slot], 0);
+  if (e == cudaSuccess) e = cudaEventRecord(pa.ev_done, h->s_index);
+  h->padd_seq++;
+  if (rc != FI_OK) return rc;
+  if (e != cudaSuccess) return fail(h, FI_ERR_CUDA, cudaGetErrorString(e));
   return FI_OK;
 }
 
@@ -1147,6 +1306,9 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
   if (rc != FI_OK) return rc;
   if (h->pipe_seq)  // a plain pick after pipelined submits: their stage A shares d_chain (slot 0) with ours
     FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[(h->pipe_seq - 1) & 1], 0));
+  if (h->padd_seq)  // fi_epp_index_add_submitted may still be copying slot 0's chains
+    FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_slot_read[0], 0));
+  h->slot_ticket[0] = h->slot_ticket[1] = ~0ull;  // the submitted batches' chains are no longer available
   MatchParams mp{};
   fill_match_params(h, mp, h->d_chain, h->d_nblocks, d_offsets, d_h0, d_adapters, R, sharded ? h->d_local : d_out, !sharded);
   mp.k = ranked_k;
@@ -1295,12 +1457,23 @@ int run_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, con
   return FI_OK;
 }
 
-// Pipelined device path: enqueue one batch.  Stage A on s_a, stage B on s_main (see fi_epp::s_a).
+// the next ticket: recorded on s_main behind everything queued there so far (the batch just enqueued)
+int issue_ticket(fi_epp* h, uint64_t* t) {
+  FI_CUDA(cudaEventRecord(h->ev_ticket[h->tickets % fi_epp::kTicketRing], h->s_main));
+  *t = h->tickets++;
+  return FI_OK;
+}
+
+// Pipelined device path: enqueue one batch.  Stage A on s_a, stage B on s_main (see fi_epp::s_a).  d_adapters,
+// ranked_k, d_subsets and d_chains_out as run_pick / copy_chains_out (fi_epp_pick_submit passes none of them);
+// lagged: the index counters may lag (check_counters_lagged, fi_epp_pick_submit_ex).
 int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0, uint32_t R,
-                fi_pick* d_out, cudaStream_t us) {
+                fi_pick* d_out, cudaStream_t us, uint64_t* ticket, const uint64_t* d_adapters = nullptr,
+                uint32_t ranked_k = 0, const uint32_t* d_subsets = nullptr, uint64_t* d_chains_out = nullptr,
+                bool lagged = false) {
   int rc = flush_ops(h);
   if (rc != FI_OK) return rc;
-  rc = check_counters(h);
+  rc = lagged ? check_counters_lagged(h, 0) : check_counters(h);
   if (rc != FI_OK) return rc;
   if (!h->d_chain2) {
     FI_CUDA(cudaMalloc(&h->d_chain2, (size_t)h->cfg.max_batch * h->MP * sizeof(uint64_t)));
@@ -1331,6 +1504,7 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
   if (h->pipe_seq >= 2) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot], 0));
   FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_plain, 0));
   if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_lru, 0));  // a device-LRU Add may still be reading d_chain
+  if (h->padd_seq) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_slot_read[slot], 0));  // (fi_epp_index_add_submitted)
   {
     // Block hashing and chain walk in one kernel (hash_kernels.cu hash_chain).  It does not wait for the previous
     // batch's match_pick: its CTAs fill whole SMs, so they take the SMs that match's CTAs leave as its queue drains
@@ -1348,14 +1522,29 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
   if (rc != FI_OK) return rc;
   FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[slot], 0));
   MatchParams mp{};
-  fill_match_params(h, mp, chain, nb, d_offsets, d_h0, nullptr, R, d_out, true);
+  fill_match_params(h, mp, chain, nb, d_offsets, d_h0, d_adapters, R, d_out, true);
   mp.work_counter = h->d_work + 8 + slot;
+  mp.k = ranked_k;
+  if (d_subsets) {
+    mp.subsets = d_subsets;
+    mp.sub_pitch = (h->cfg.num_endpoints + 31) / 32;
+    mp.eps = h->d_eps;
+  }
   {
     LaunchScope ls(h, h->s_main, K_MATCH);
     FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main));
   }
+  if (d_chains_out) {
+    const size_t row = (size_t)h->cfg.max_blocks * sizeof(uint64_t);
+    FI_CUDA(cudaMemcpy2DAsync(d_chains_out, row, chain, (size_t)h->MP * sizeof(uint64_t), row, R, cudaMemcpyDeviceToDevice,
+                              h->s_main));
+  }
   FI_CUDA(cudaEventRecord(h->ev_b[slot], h->s_main));
   FI_CUDA(cudaEventRecord(h->ev_pick, h->s_main));
+  rc = issue_ticket(h, ticket);
+  if (rc != FI_OK) return rc;
+  h->slot_ticket[slot] = *ticket;
+  h->slot_R[slot] = R;
   h->pipe_seq++;
   h->stats.pick_calls++;
   h->stats.requests += R;
@@ -1536,8 +1725,17 @@ void fi_epp_destroy(fi_epp* h) {
     if (e) cudaEventDestroy(e);
   for (int k = 0; k < fi_epp::kMaxFeedSlices; ++k)
     if (h->ev_copy[k]) cudaEventDestroy(h->ev_copy[k]);
-  for (cudaEvent_t e : {h->ev_in, h->ev_a[0], h->ev_a[1], h->ev_b[0], h->ev_b[1], h->ev_pick, h->ev_plain})
+  for (cudaEvent_t e : {h->ev_in, h->ev_a[0], h->ev_a[1], h->ev_b[0], h->ev_b[1], h->ev_pick, h->ev_plain,
+                        h->ev_slot_read[0], h->ev_slot_read[1]})
     if (e) cudaEventDestroy(e);
+  for (int k = 0; k < fi_epp::kTicketRing; ++k)
+    if (h->ev_ticket[k]) cudaEventDestroy(h->ev_ticket[k]);
+  for (fi_epp::PipeAdd& pa : h->padd) {
+    cudaFree(pa.d_plan);
+    if (pa.h_plan) cudaFreeHost(pa.h_plan);
+    cudaFree(pa.d_chains);
+    if (pa.ev_done) cudaEventDestroy(pa.ev_done);
+  }
   cudaFree(h->d_chain2);
   cudaFree(h->d_nblocks2);
   for (cudaStream_t s : {h->s_main, h->s_index, h->s_copy, h->s_a})
@@ -1605,8 +1803,10 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
   FI_TRY(cudaStreamCreateWithFlags(&h->s_index, cudaStreamNonBlocking));
   FI_TRY(cudaStreamCreateWithFlags(&h->s_copy, cudaStreamNonBlocking));
   FI_TRY(cudaStreamCreateWithFlags(&h->s_a, cudaStreamNonBlocking));
-  for (cudaEvent_t* e : {&h->ev_in, &h->ev_a[0], &h->ev_a[1], &h->ev_b[0], &h->ev_b[1], &h->ev_pick, &h->ev_plain})
+  for (cudaEvent_t* e : {&h->ev_in, &h->ev_a[0], &h->ev_a[1], &h->ev_b[0], &h->ev_b[1], &h->ev_pick, &h->ev_plain,
+                         &h->ev_slot_read[0], &h->ev_slot_read[1]})
     FI_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
+  for (int k = 0; k < fi_epp::kTicketRing; ++k) FI_TRY(cudaEventCreateWithFlags(&h->ev_ticket[k], cudaEventDisableTiming));
   for (int k = 0; k < fi_epp::kMaxFeedSlices; ++k) FI_TRY(cudaEventCreateWithFlags(&h->ev_copy[k], cudaEventDisableTiming));
   if (const char* e = std::getenv("FI_EPP_FEED_SLICES")) {
     const long v = std::strtol(e, nullptr, 10);
@@ -2228,7 +2428,9 @@ int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets
   if (h->pipe_seq)  // a pipelined batch's stage A (on s_a) shares d_chain (slot 0) with us
     FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[(h->pipe_seq - 1) & 1], 0));
   if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_lru, 0));  // a device-LRU Add may still be reading d_chain
+  if (h->padd_seq) FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_slot_read[0], 0));
   h->last_plain_R = 0;  // d_chain no longer holds a pick batch's chains
+  h->slot_ticket[0] = h->slot_ticket[1] = ~0ull;
   rc = run_hash(h, h->d_prompts, h->d_offsets, h->d_h0, 0, R, h->s_main);
   if (rc != FI_OK) return rc;
   if (chains_out) {
@@ -2465,13 +2667,63 @@ int fi_epp_pick_submit(fi_epp* h, const void* d_prompts, const void* d_offsets, 
     std::lock_guard<std::mutex> lk(h->mu);
     plain = h->world > 1 || !h->fast_hash;  // sharded pools and odd block sizes: the stream-ordered path
   }
-  if (plain) return fi_epp_pick_batch_device(h, d_prompts, d_offsets, d_h0, R, total_prompt_bytes, d_out, nullptr, stream);
+  uint64_t t = 0;
+  if (plain) {
+    const int rc = fi_epp_pick_batch_device(h, d_prompts, d_offsets, d_h0, R, total_prompt_bytes, d_out, nullptr, stream);
+    if (rc != FI_OK || R == 0) return rc;
+    std::lock_guard<std::mutex> lk(h->mu);
+    return issue_ticket(h, &t);  // the batch's number, as fi_epp_pick_submit_ex would have given it
+  }
   std::lock_guard<std::mutex> lk(h->mu);
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   if (R == 0) return FI_OK;
   if (R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
   return submit_pick(h, (const uint8_t*)d_prompts, (const uint64_t*)d_offsets, (const uint64_t*)d_h0, R, (fi_pick*)d_out,
-                     (cudaStream_t)stream);
+                     (cudaStream_t)stream, &t);
+}
+
+// Pipelined submit of any pick variant (docs/SPEC.md S.9): the arguments, checks and output of the stream-ordered
+// counterpart (fi_epp_pick_batch_device_lora for k == 0, fi_epp_pick_batch_device_subset otherwise), with the staging
+// of fi_epp_pick_submit.  Handles that fi_epp_pick_submit serves stream-ordered run the counterpart itself.
+int fi_epp_pick_submit_ex(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, const void* d_adapters,
+                          const void* d_subsets, uint32_t R, uint64_t total_prompt_bytes, uint32_t k, void* d_out,
+                          void* d_chains_out, void* stream, uint64_t* ticket) {
+  if (!h || !d_offsets || (!d_h0 && R) || (!d_out && (R || k))) return FI_ERR_INVALID;
+  if (k > FI_EPP_MAX_RANKED || (k == 0 && d_subsets)) return FI_ERR_INVALID;
+  bool plain;
+  {
+    std::lock_guard<std::mutex> lk(h->mu);
+    plain = h->world > 1 || !h->fast_hash;
+  }
+  uint64_t t = 0;
+  if (plain) {
+    const int rc = k ? pick_ranked_device(h, d_prompts, d_offsets, d_h0, d_adapters, d_subsets, R, total_prompt_bytes, k,
+                                          d_out, d_chains_out, stream)
+                     : fi_epp_pick_batch_device_lora(h, d_prompts, d_offsets, d_h0, d_adapters, R, total_prompt_bytes,
+                                                     d_out, d_chains_out, stream);
+    if (rc != FI_OK) return rc;
+    std::lock_guard<std::mutex> lk(h->mu);
+    const int rt = issue_ticket(h, &t);
+    if (rt == FI_OK && ticket) *ticket = t;
+    return rt;
+  }
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  if (d_subsets) {
+    const int rs = check_subset_handle(h);
+    if (rs != FI_OK) return rs;
+  }
+  int rc = FI_OK;
+  if (R == 0) {
+    rc = issue_ticket(h, &t);  // an empty batch: complete once everything before it is
+  } else {
+    if (R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
+    rc = submit_pick(h, (const uint8_t*)d_prompts, (const uint64_t*)d_offsets, (const uint64_t*)d_h0, R, (fi_pick*)d_out,
+                     (cudaStream_t)stream, &t, (const uint64_t*)d_adapters, k, (const uint32_t*)d_subsets,
+                     (uint64_t*)d_chains_out, /*lagged=*/true);
+  }
+  if (rc == FI_OK && ticket) *ticket = t;
+  return rc;
 }
 
 // The pipelined path always runs on the whole GPU: out = {0, 0, 0} (include/fi_epp.h).
@@ -2491,6 +2743,49 @@ int fi_epp_pick_wait(fi_epp* h, void* stream) {
     dump_trace(h, 0);
   }
   return FI_OK;
+}
+
+int fi_epp_pick_wait_batch(fi_epp* h, uint64_t ticket, void* stream) {
+  if (!h) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  if (ticket >= h->tickets) return fail(h, FI_ERR_INVALID, "ticket never issued");
+  // s_main completes the batches in order: a ticket older than the ring is done by the oldest one it still tracks
+  const uint64_t oldest = h->tickets - std::min<uint64_t>(h->tickets, fi_epp::kTicketRing);
+  const uint64_t t = std::max(ticket, oldest);
+  FI_CUDA(cudaStreamWaitEvent((cudaStream_t)stream, h->ev_ticket[t % fi_epp::kTicketRing], 0));
+  if (!h->profiling && !h->pending_ev.empty() && h->ev_trace0) {
+    h->tracing = true;
+    dump_trace(h, 0);
+  }
+  return FI_OK;
+}
+
+// PreRequest for a submitted batch (docs/SPEC.md S.9): fi_epp_index_add_chains_device(.., NULL, ..) with the chains
+// of batch `ticket`, read from its pipeline slot, through the non-stalling device-LRU path (lru_add_submitted).
+int fi_epp_index_add_submitted(fi_epp* h, uint64_t ticket, const uint32_t* endpoints, const uint32_t* nblocks,
+                               uint32_t R) {
+  if (!h || ((!endpoints || !nblocks) && R)) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  if (ticket >= h->tickets) return fail(h, FI_ERR_INVALID, "ticket never issued");
+  if (!h->cfg.lru_capacity) return fail(h, FI_ERR_STATE, "lru_capacity is 0: no LRU");
+  if (h->world > 1) return fail(h, FI_ERR_STATE, "sharded pool: use the collective fi_epp_index_add_chains");
+  int slot = -1;
+  for (int s = 0; s < 2; ++s)
+    if (h->slot_ticket[s] == ticket) slot = s;
+  if (slot < 0)
+    return fail(h, FI_ERR_STATE, "the chains of that batch are gone (two later submits, a stream-ordered pick or hash "
+                                 "since, or a batch that was not pipelined)");
+  if (R > h->slot_R[slot]) return fail(h, FI_ERR_STATE, "R larger than the submitted batch");
+  for (uint32_t r = 0; r < R; ++r) {
+    if (endpoints[r] != FI_NO_ENDPOINT && endpoints[r] >= h->cfg.num_endpoints) return fail(h, FI_ERR_INVALID, "endpoint out of range");
+    if (nblocks[r] > h->cfg.max_blocks) return fail(h, FI_ERR_INVALID, "nblocks[r] larger than max_blocks");
+  }
+  int rc = choose_lru_mode(h);
+  if (rc != FI_OK) return rc;
+  if (h->lru_mode != 1) return fail(h, FI_ERR_STATE, "fi_epp_index_add_submitted needs the device LRU");
+  return lru_add_submitted(h, (uint32_t)slot, endpoints, nblocks, R);
 }
 
 int fi_epp_comm_unique_id(uint8_t out[FI_EPP_UNIQUE_ID_BYTES]) {

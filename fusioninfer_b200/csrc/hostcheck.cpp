@@ -4,6 +4,7 @@
 #include <cstdint>
 #include <cstring>
 #include <algorithm>
+#include <set>
 #include <unordered_map>
 #include <unordered_set>
 #include <vector>
@@ -241,6 +242,65 @@ int fihc_lru_plan_check(uint32_t E, uint32_t cap, const uint32_t* endpoints, con
     for (uint32_t e = 0; e < E; ++e)
       if (order[e] != seq_order[e]) return 1;
   }
+  return 0;
+}
+
+// lru_touch_bound (lru_plan.h): the per-endpoint touches a sub-batch of fi_epp_index_add_submitted may carry
+uint32_t fihc_lru_touch_bound(uint32_t TS, uint32_t C) { return fi::lru_touch_bound(TS, C); }
+
+// The device LRU's table occupancy under plans cut with lru_touch_bound: per endpoint, `used` (regular slots taken:
+// entries + tombstones) follows lru_maintain_kernel's rule before every sub-batch (kept if (used + min(add, C)) * 10
+// <= 6 TS, else rebuilt to the live entries), then every key the sub-batch touches that is not an entry takes a slot,
+// and the LRU keeps the C most recent keys (what falls out becomes a tombstone: used stays).  The touch kernel reserves
+// a slot before it looks further, so up to `add` reservations can be outstanding at once: it cannot fail iff
+// used_before + add <= TS * 85 / 100.  Returns 0 if that holds for every endpoint and sub-batch, else 1; *max_pct =
+// the highest used_before + add seen, in percent of TS; *subs = sub-batches in total.
+int fihc_lru_bound_check(uint32_t E, uint32_t cap, uint32_t TS, const uint32_t* endpoints, const uint64_t* chains,
+                         uint32_t pitch, const uint32_t* nblocks, uint32_t R, uint32_t batches, uint64_t cap_touches,
+                         uint32_t cap_requests, double* max_pct, uint32_t* subs) {
+  const uint64_t limit = (uint64_t)TS * 85 / 100;
+  const uint32_t bound = fi::lru_touch_bound(TS, cap);
+  std::vector<fi::LruSet> lru(E, fi::LruSet(cap));
+  std::vector<uint64_t> used(E, 0);
+  fi::LruPlan pl;
+  uint64_t peak = 0, nsubs = 0;
+  for (uint32_t b = 0; b < batches; ++b) {
+    const uint32_t* ep = endpoints + (size_t)b * R;
+    const uint64_t* ch = chains + (size_t)b * R * pitch;
+    const uint32_t* nb = nblocks + (size_t)b * R;
+    fi::lru_plan_batch(ep, nb, R, 0, E, bound, cap_touches, cap_requests, &pl);
+    nsubs += pl.subs.size();
+    for (size_t sb = 0; sb < pl.subs.size(); ++sb) {
+      const uint32_t* inc = pl.inc.data() + sb * (size_t)E;
+      const fi::LruSubBatch& s = pl.subs[sb];
+      for (uint32_t e = 0; e < E; ++e) {
+        const uint64_t add = inc[e];
+        if (!add) continue;
+        const uint64_t addc = std::min<uint64_t>(add, cap);
+        if ((used[e] + addc) * 10 > (uint64_t)TS * 6) used[e] = lru[e].size();
+        peak = std::max(peak, used[e] + add);
+        if (used[e] + add > limit) return 1;
+      }
+      std::set<std::pair<uint32_t, uint64_t>> fresh;  // (endpoint, key) pairs new to their endpoint in this sub-batch
+      for (uint32_t k = s.k_begin; k < s.k_end; ++k) {
+        const uint32_t e = pl.req_ep[k];
+        const uint64_t* c = ch + (size_t)pl.req_id[k] * pitch;
+        for (uint32_t i = 0; i < pl.req_n[k]; ++i)
+          if (!lru[e].contains(c[i]) && fresh.insert({e, c[i]}).second) used[e]++;
+      }
+      for (uint32_t k = s.k_begin; k < s.k_end; ++k) {
+        const uint32_t e = pl.req_ep[k];
+        const uint64_t* c = ch + (size_t)pl.req_id[k] * pitch;
+        for (uint32_t i = 0; i < pl.req_n[k]; ++i) {
+          uint64_t ev = 0;
+          bool did = false;
+          lru[e].touch(c[i], &ev, &did);
+        }
+      }
+    }
+  }
+  if (max_pct) *max_pct = 100.0 * (double)peak / TS;
+  if (subs) *subs = (uint32_t)nsubs;
   return 0;
 }
 

@@ -15,10 +15,27 @@
 //   ep_start[e] .. ep_start[e+1]  range of ep_list holding the k's of local endpoint e, ascending
 //   inc[e]       touches endpoint e receives in the sub-batch (upper bound of its new log records)
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <vector>
 
 namespace fi {
+
+// Touches one endpoint may receive in a sub-batch so that the touch kernel can never find its table full: the bound
+// fi_epp_index_add_submitted plans with (it has no overflow readback).  Per endpoint, with `add` touches in the
+// sub-batch (so at most `add` new keys, and at most `add` slot reservations outstanding at any time), table size TS,
+// capacity C and used = regular slots taken (entries + tombstones), lru_maintain_kernel (lru_kernels.cu) leaves
+//   either the table as it is, only if (used + min(add, C)) * 10 <= 6 TS, i.e. used <= calm - min(add, C),
+//   or a table rebuilt from the live entries: used = count <= C (evict ran at the end of the previous sub-batch),
+// and a new key is inserted only while used < limit = TS * 85 / 100 (integer division, as alloc_dev_lru computes it;
+// calm = TS * 6 / 10 likewise).  The touch kernel cannot overflow iff used + add <= limit:
+//   add <= C:  calm <= limit, and C + add <= 2 C <= limit (TS >= 4 C): always;
+//   add > C:   add <= limit - calm + C (table kept) and add <= limit - C (table rebuilt).
+// The bound is the smaller of the two, >= 2 C since TS >= 4 C, so every chain (at most C blocks) fits.
+inline uint32_t lru_touch_bound(uint32_t TS, uint32_t C) {
+  const uint64_t limit = (uint64_t)TS * 85 / 100, calm = (uint64_t)TS * 6 / 10;
+  return (uint32_t)std::min<uint64_t>(limit - calm + C, limit - C);
+}
 
 struct LruSubBatch {
   uint32_t k_begin = 0, k_end = 0;  // range of the kept-request arrays

@@ -382,6 +382,33 @@ class EndpointPicker:
         """Make `stream` wait (device-side) for every batch submitted so far."""
         self._check(self._lib.fi_epp_pick_wait(self._h, stream or None), "fi_epp_pick_wait")
 
+    def pick_submit_ex(self, d_prompts: int, d_offsets: int, d_h0: int, R: int, total_bytes: int, d_out: int, k: int = 0,
+                       d_adapters: int = 0, d_subsets: int = 0, d_chains: int = 0, stream: int = 0) -> int:
+        """Pipelined submit of any pick variant (docs/SPEC.md S.9): k = 0 the single pick ([R, n_profiles] picks, like
+        pick_batch_device with adapters), k >= 1 the ranked / subset pick ([R, n_profiles, k]).  d_chains (optional):
+        R * max_blocks hashes.  -> the batch's ticket, for pick_wait_batch and index_add_submitted."""
+        t = C.c_uint64(0)
+        self._check(
+            self._lib.fi_epp_pick_submit_ex(self._h, d_prompts, d_offsets, d_h0, d_adapters or None, d_subsets or None, R,
+                                            total_bytes, int(k), d_out, d_chains or None, stream or None, C.byref(t)),
+            "fi_epp_pick_submit_ex",
+        )
+        return t.value
+
+    def pick_wait_batch(self, ticket: int, stream: int = 0):
+        """Make `stream` wait (device-side) for batch `ticket` and the ones before it, not for later ones."""
+        self._check(self._lib.fi_epp_pick_wait_batch(self._h, int(ticket), stream or None), "fi_epp_pick_wait_batch")
+
+    def index_add_submitted(self, ticket: int, endpoints: np.ndarray, nblocks: np.ndarray):
+        """upstream PreRequest for a submitted batch: indexer.Add of its chains (kept by the handle) to the picked
+        endpoints, without the overflow readback of index_add_chains_device; it waits on the host for the previous
+        update's index counters only when the index is too close to its rebuild threshold to let them lag (docs/SPEC.md
+        S.9, DESIGN.md §4.0).  Ordered like index_apply."""
+        endpoints = np.ascontiguousarray(endpoints, dtype=np.uint32)
+        nblocks = np.ascontiguousarray(nblocks, dtype=np.uint32)
+        self._check(self._lib.fi_epp_index_add_submitted(self._h, int(ticket), _ptr(endpoints), _ptr(nblocks), len(endpoints)),
+                    "fi_epp_index_add_submitted")
+
     # -- multi-GPU -------------------------------------------------------------
     @staticmethod
     def comm_unique_id() -> bytes:

@@ -400,6 +400,36 @@ int fi_epp_pick_batch_device_subset(fi_epp* h, const void* d_prompts, const void
 int fi_epp_pick_submit(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
                        uint64_t total_prompt_bytes, void* d_out, void* stream);
 int fi_epp_pick_wait(fi_epp* h, void* stream);
+
+/* Pipelined calls for a serving loop (docs/SPEC.md S.9): submit(k+1) -> wait_batch(k) -> read picks ->
+ * add_submitted(k).
+ * fi_epp_pick_submit_ex: pipelined submit of any pick variant, byte-identical to its stream-ordered counterpart on the
+ * index as of the call.  k == 0: [R][n_profiles] picks like fi_epp_pick_batch_device_lora (d_adapters may be NULL;
+ * d_subsets must be NULL, else FI_ERR_INVALID).  1 <= k <= FI_EPP_MAX_RANKED: [R][n_profiles][k] like
+ * fi_epp_pick_batch_device_subset (d_subsets NULL = the ranked call).  Argument checks and errors are the
+ * counterpart's.  d_chains_out (optional): R * max_blocks hashes, as the counterparts' chains_out.  *ticket (may be
+ * NULL): the batch's sequence number, monotonic per handle and shared with fi_epp_pick_submit (one per batch of
+ * R > 0 there).  Handles that fi_epp_pick_submit serves stream-ordered (sharded, block_bytes % 32 != 0) run the
+ * counterpart, which returns FI_ERR_STATE for ranked and subset picks on a sharded pool. */
+int fi_epp_pick_submit_ex(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                          const void* d_adapters, const void* d_subsets, uint32_t R, uint64_t total_prompt_bytes,
+                          uint32_t k, void* d_out, void* d_chains_out, void* stream, uint64_t* ticket);
+/* `stream` waits (on the device; the host does not block) for batch `ticket` and the batches before it, not for
+ * later ones (a ticket more than 8 submits old waits for the oldest of the last 8).  FI_ERR_INVALID for a ticket
+ * never issued. */
+int fi_epp_pick_wait_batch(fi_epp* h, uint64_t ticket, void* stream);
+/* PreRequest for a submitted batch: indexer.Add(chain_r, endpoints[r]) for r < R (<= the batch's R), the chains read
+ * from the handle's own buffer for that batch; equal to fi_epp_index_add_chains with those chains.  Ordered like every
+ * index update: picks submitted before the call do not see it, every pick submitted after it does.  It skips the host
+ * waits of fi_epp_index_add_chains_device (overflow readback, previous staging) and waits for the previous update's
+ * index counters only when the last counters read leave too little room below the rebuild threshold for the keys the
+ * pending updates may add; at index loads near that threshold it therefore waits like the stream-ordered Add
+ * (DESIGN.md §4.0).  A batch's chains stay available until the
+ * next-but-one submit or any stream-ordered pick or hash call; after that, for batches that were not pipelined
+ * (sharded handles, block_bytes % 32 != 0), with the host LRU or with lru_capacity == 0: FI_ERR_STATE.  FI_ERR_INVALID
+ * for a ticket never issued, an endpoint >= num_endpoints or nblocks[r] > max_blocks. */
+int fi_epp_index_add_submitted(fi_epp* h, uint64_t ticket, const uint32_t* endpoints, const uint32_t* nblocks,
+                               uint32_t R);
 /* How the pipelined path runs: out[0] = 1 if the GPU is partitioned between its stages, out[1] / out[2] = SMs of the
  * partitions.  The pipelined path always runs on the whole GPU with two batches in flight, so out is {0, 0, 0}. */
 int fi_epp_pipeline_info(fi_epp* h, int32_t out[3]);
