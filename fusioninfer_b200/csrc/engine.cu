@@ -1507,8 +1507,9 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
   if (h->padd_seq) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_slot_read[slot], 0));  // (fi_epp_index_add_submitted)
   {
     // Block hashing and chain walk in one kernel (hash_kernels.cu hash_chain).  It does not wait for the previous
-    // batch's match_pick: its CTAs fill whole SMs, so they take the SMs that match's CTAs leave as its queue drains
-    // (DESIGN.md §4.0: 180.0 us per step this way, 190.8 us waiting for the match).
+    // batch's match_pick: a full batch runs half-SM CTAs, and one starts on an SM as soon as two of match's three
+    // CTAs there have run out of queue (DESIGN.md §4.0; giving match fewer CTAs per SM so that the two kernels share
+    // every SM for the whole step was measured slower: §7).
     LaunchScope ls(h, h->s_a, K_HASH);
     FI_CUDA(launch_hash_chain(d_prompts, d_offsets, d_h0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, chain, nb,
                               h->sm_count, h->s_a));

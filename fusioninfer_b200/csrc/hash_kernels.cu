@@ -59,20 +59,23 @@ __device__ __forceinline__ ulonglong2 lds16(const ulonglong2* p) {
 }
 
 // ---- hash_chain: block hashing and chain walk in one kernel --------------------------------------------------
-// One CTA owns a tile of 32 * WALK requests and runs on an SM of its own (1 024 threads at 64 registers fill the
-// register file).  Warps WALK-31 hash the tile's blocks column chunk by column chunk: group g = blocks [8g, 8g+8) of
+// One CTA of WARPS warps owns a tile of 32 * WALK requests.  WARPS = 32 runs on an SM of its own (1 024 threads at 64
+// registers fill the register file); WARPS = 16 is the half-SM tile, two CTAs per SM.  Warps WALK .. WARPS-1 hash the
+// tile's blocks column chunk by column chunk: group g = blocks [8g, 8g+8) of
 // all the tile's requests is one slot of a shared-memory ring of 8-byte pre-states, laid out [walker warp][16-byte
 // unit][lane] (conflict-free for the walker).  Warps 0 .. WALK-1, on different SM sub-partitions, walk the chains of
 // 32 requests each in groups of 8 links, taking the pre-states from the ring as they land.  The walk (~43 us at
 // cfg 3) then runs under the tile's prompt stream (~120 us) instead of after it, and the pre-states never go to
-// HBM.  WALK = 4 (128 requests per CTA) when the batch has at least ~4 requests per 128 per SM; smaller batches take
-// smaller tiles so that they still spread over every SM (launch_hash_chain).
+// HBM.  Batches of up to 64 requests per SM take whole-SM tiles of 32 or 64 requests so that they still spread over
+// every SM; larger ones take half-SM tiles of 64 requests (2 walkers + 14 hashers, the same 28 : 4 warps per SM as a
+// whole-SM tile of 128 would have).  A half-SM CTA starts as soon as half an SM's registers are free, which matters
+// when the previous batch's match_pick is draining off the SMs (pipelined submits), and 16 384 requests make 256
+// CTAs over 264 slots where 128-request tiles left 4 of 132 SMs idle (launch_hash_chain; DESIGN.md §4.0).
 // STRIPES = block_bytes / 32 for 32-, 64- and 128-byte blocks; STRIPES = 0 reads it from block_bytes at run time
 // (every other multiple of 32).  Only the hashing lanes depend on it: the ring, the handshake and the walkers do not.
 // Handshake per slot: mbarrier `full` (every hashing lane that filled part of the slot arrives; the walkers wait)
 // and `empty` (every walker lane arrives once it has the slot in registers; the hashers wait before they refill it).
-constexpr int kFuseWarps = 32;           // warps 0 .. WALK-1 walk, the rest hash
-constexpr int kFuseRingBytes = 32768;    // ring of 8 KiB (WALK = 4) to 2 KiB (WALK = 1) slots
+constexpr int kFuseRingBytesPerWarp = 1024;  // ring of 32 KiB per full-SM CTA, 16 KiB per half-SM CTA, in slots of 2 KiB per walker
 
 __device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
   asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;\n" ::"r"((unsigned)__cvta_generic_to_shared(bar)), "r"(count)
@@ -127,8 +130,8 @@ __device__ __forceinline__ uint64_t pre_unaligned(const uint8_t* blk, uint32_t B
   return xacc2_finish(a, (uint64_t)B + 8);
 }
 
-template <int STRIPES, int WALK>
-__global__ void __launch_bounds__(kFuseWarps * 32, 1) hash_chain_kernel(const uint8_t* __restrict__ prompts,
+template <int STRIPES, int WALK, int WARPS>
+__global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(const uint8_t* __restrict__ prompts,
                                                                    const uint64_t* __restrict__ offsets,
                                                                    const uint64_t* __restrict__ h0, uint32_t R,
                                                                    uint32_t M, uint32_t MP,
@@ -141,8 +144,8 @@ __global__ void __launch_bounds__(kFuseWarps * 32, 1) hash_chain_kernel(const ui
   // read one request's 8 blocks: 512 contiguous bytes at 64-byte blocks.
   constexpr uint32_t BPL = STRIPES == 4 || STRIPES == 0 ? 1 : 2;
   constexpr uint32_t kFuseReq = 32 * WALK;  // requests per CTA
-  constexpr uint32_t kFuseHashWarps = kFuseWarps - WALK;
-  constexpr uint32_t kFuseRing = kFuseRingBytes / (WALK * 4 * 32 * 16);
+  constexpr uint32_t kFuseHashWarps = WARPS - WALK;
+  constexpr uint32_t kFuseRing = WARPS * kFuseRingBytesPerWarp / (WALK * 4 * 32 * 16);
   constexpr uint32_t kJobs = kFuseReq / (4 * BPL);  // jobs per group
   __shared__ __align__(16) ulonglong2 s_ring[kFuseRing][WALK][4][32];
   __shared__ uint64_t s_full[kFuseRing], s_empty[kFuseRing];
@@ -331,38 +334,45 @@ __global__ void __launch_bounds__(128) hash_generic_kernel(const uint8_t* __rest
 
 }  // namespace
 
+// One tile shape: WALK = 1 or 2 on a whole SM, or the half-SM tile (16 warps, WALK = 2).
 template <int STRIPES>
-static void launch_hash_chain_tile(uint32_t walk, uint32_t grid, cudaStream_t s, const uint8_t* prompts,
+static void launch_hash_chain_tile(uint32_t walk, uint32_t warps, uint32_t grid, cudaStream_t s, const uint8_t* prompts,
                                    const uint64_t* offsets, const uint64_t* h0, uint32_t R, uint32_t B, uint32_t M,
                                    uint32_t MP, uint64_t* chain, uint32_t* nblocks) {
-  constexpr uint32_t threads = kFuseWarps * 32;
-  if (walk == 4)
-    hash_chain_kernel<STRIPES, 4><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B);
+  if (warps == 16)
+    hash_chain_kernel<STRIPES, 2, 16><<<grid, 512, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B);
   else if (walk == 2)
-    hash_chain_kernel<STRIPES, 2><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B);
+    hash_chain_kernel<STRIPES, 2, 32><<<grid, 1024, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B);
   else
-    hash_chain_kernel<STRIPES, 1><<<grid, threads, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B);
+    hash_chain_kernel<STRIPES, 1, 32><<<grid, 1024, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B);
+}
+
+cudaError_t launch_hash_chain_shape(uint32_t walk, uint32_t warps, const uint8_t* prompts, const uint64_t* offsets,
+                                    const uint64_t* h0, uint32_t R, uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain,
+                                    uint32_t* nblocks, cudaStream_t s) {
+  if (R == 0) return cudaSuccess;
+  if (!((warps == 32 && (walk == 1 || walk == 2)) || (warps == 16 && walk == 2))) return cudaErrorInvalidValue;
+  const uint32_t grid = (R + 32 * walk - 1) / (32 * walk);
+  if (B == 64)
+    launch_hash_chain_tile<2>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
+  else if (B == 32)
+    launch_hash_chain_tile<1>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
+  else if (B == 128)
+    launch_hash_chain_tile<4>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
+  else if (B % 32 == 0)
+    launch_hash_chain_tile<0>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
+  else
+    return cudaErrorInvalidValue;
+  return cudaGetLastError();
 }
 
 cudaError_t launch_hash_chain(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
                               uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain, uint32_t* nblocks, int sm_count,
                               cudaStream_t s) {
-  if (R == 0) return cudaSuccess;
-  // the smallest tile whose grid still fits one CTA per SM; 128 requests per CTA beyond that
-  uint32_t walk = 1;
-  while (walk < 4 && (R + 32 * walk - 1) / (32 * walk) > (uint32_t)sm_count) walk *= 2;
-  const uint32_t grid = (R + 32 * walk - 1) / (32 * walk);
-  if (B == 64)
-    launch_hash_chain_tile<2>(walk, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
-  else if (B == 32)
-    launch_hash_chain_tile<1>(walk, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
-  else if (B == 128)
-    launch_hash_chain_tile<4>(walk, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
-  else if (B % 32 == 0)
-    launch_hash_chain_tile<0>(walk, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
-  else
-    return cudaErrorInvalidValue;
-  return cudaGetLastError();
+  // the smallest whole-SM tile whose grid still fits one CTA per SM; half-SM tiles beyond that
+  const uint32_t walk = (R + 31) / 32 > (uint32_t)sm_count ? 2 : 1;
+  const uint32_t warps = (R + 63) / 64 > (uint32_t)sm_count ? 16 : 32;
+  return launch_hash_chain_shape(walk, warps, prompts, offsets, h0, R, B, M, MP, chain, nblocks, s);
 }
 
 cudaError_t launch_hash_generic(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,

@@ -186,10 +186,15 @@ struct MergeParams {
 
 // ---- launchers (each returns the cudaGetLastError() of its launch) -----------
 // block hashing and chain walk in one kernel, for block_bytes % 32 == 0 (cudaErrorInvalidValue otherwise).
-// sm_count sets the tile: 32, 64 or 128 requests per CTA, the smallest whose grid fits one CTA per SM
+// sm_count sets the tile: 32 or 64 requests per whole-SM CTA, the smallest whose grid fits one CTA per SM, and
+// half-SM CTAs of 64 requests for larger batches
 cudaError_t launch_hash_chain(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
                               uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain, uint32_t* nblocks,
                               int sm_count, cudaStream_t s);
+// the same with the tile shape given: walk = 1 or 2 with warps = 32 (whole SM), walk = 2 with warps = 16 (half SM)
+cudaError_t launch_hash_chain_shape(uint32_t walk, uint32_t warps, const uint8_t* prompts, const uint64_t* offsets,
+                                    const uint64_t* h0, uint32_t R, uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain,
+                                    uint32_t* nblocks, cudaStream_t s);
 cudaError_t launch_hash_generic(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
                                 uint32_t R, uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain,
                                 uint32_t* nblocks, cudaStream_t s);

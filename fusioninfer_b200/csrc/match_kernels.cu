@@ -163,7 +163,7 @@ __device__ __forceinline__ void load_row_words(const uint32_t* __restrict__ p, b
 
 // Nodes of ALL blocks of a request, before any row is read.  A cached prefix was inserted in chain order, so its
 // nodes are consecutive (index_device.cuh): after ONE table lookup for block `pos` every later block i checks
-// "my node = that node + (i - pos)" — coalesced reads of klog, all chunks of the request in flight at once.  The
+// "my node = that node + (i - pos)" — coalesced reads of klog, kSpecChunks chunks of 32 blocks in flight at once.  The
 // table is probed again only where that fails: normally at the first block the index does not hold, which ends
 // the walk (both match modes stop at the first block no pod holds).  A prefix whose nodes are scattered (an index
 // built out of chain order) gets kSpecTries such rounds, then its remaining blocks probe the table in parallel,
@@ -174,7 +174,11 @@ __device__ __forceinline__ void load_row_words(const uint32_t* __restrict__ p, b
 // round trips per 32 blocks, and the last fully cached prompt keeps the other warps waiting.  With the nodes
 // known up front the rows of a request are independent loads.)
 constexpr int kSpecTries = 4;
-constexpr int kSpecChunks = 8;  // chunks of 32 blocks verified per round (256 blocks; longer chains loop)
+// Chunks of 32 blocks verified per round; a round is issued only when every block of the one before it verified.  Two
+// (64 blocks): at cfg 3 the walk ends at block 103 on average, and checking all 256 blocks of a chain at once read
+// about 1 KB of klog per request that no one used.  cfg 3 on one H100 80GB HBM3 (700 W), us per pipelined step,
+// three runs each in one call: 8 chunks 171.7-172.0, 3 chunks 168.1-168.2, 2 chunks 168.4-168.5, 1 chunk 169.4-169.5.
+constexpr int kSpecChunks = 2;
 
 __device__ __forceinline__ uint32_t resolve_request_nodes(const IndexView& ix, const uint64_t* __restrict__ s_chain,
                                                           uint32_t* __restrict__ s_node, uint32_t n, int lane, bool have_first,

@@ -1,6 +1,6 @@
 // hashchain.cu — the hash_chain kernel against hash_generic, the fully serial kernel that hashes every block as one
 // XXH64 message (no pre-state split): bit-exact chains and block counts on ragged, unaligned and truncated prompts
-// (block sizes 32, 64, 96, 128, 160 and 256, odd batch sizes), then CUDA-event times of hash_chain at the cfg 3
+// (block sizes 32, 64, 96, 128, 160 and 256, odd batch sizes, every tile shape), then CUDA-event times of hash_chain at the cfg 3
 // shape (16 384 requests x 4 096-token prompts, 64-byte blocks, 256 blocks), the cfg 2 shape (4 096 requests x
 // 2 048-token prompts) and the cfg 3 shape at 96- and 160-byte blocks.  Prints one line per case.
 //   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -I fusioninfer_b200/csrc -o tools/microbench/hashchain tools/microbench/hashchain.cu
@@ -67,8 +67,12 @@ static void free_batch(Batch& b) {
 static void run_generic(Batch& b) {
   CK(fi::launch_hash_generic(b.prompts, b.offsets, b.h0, b.R, b.B, b.M, b.MP, b.chain_a, b.nb_a, 0));
 }
-static void run_chain(Batch& b) {
-  CK(fi::launch_hash_chain(b.prompts, b.offsets, b.h0, b.R, b.B, b.M, b.MP, b.chain_b, b.nb_b, g_sms, 0));
+// walk = 0: the shape launch_hash_chain picks for the batch
+static void run_chain(Batch& b, uint32_t walk = 0, uint32_t warps = 0) {
+  if (walk)
+    CK(fi::launch_hash_chain_shape(walk, warps, b.prompts, b.offsets, b.h0, b.R, b.B, b.M, b.MP, b.chain_b, b.nb_b, 0));
+  else
+    CK(fi::launch_hash_chain(b.prompts, b.offsets, b.h0, b.R, b.B, b.M, b.MP, b.chain_b, b.nb_b, g_sms, 0));
 }
 static bool same(const Batch& b) {
   std::vector<uint64_t> ca((size_t)b.R * b.MP), cb(ca.size());
@@ -81,12 +85,12 @@ static bool same(const Batch& b) {
 }
 
 // hash_chain alone, 3 x 50 launches; the outputs of the last one against hash_generic
-static bool time_shape(const char* name, uint32_t R, uint32_t B, uint32_t M) {
+static bool time_shape(const char* name, uint32_t R, uint32_t B, uint32_t M, uint32_t walk = 0, uint32_t warps = 0) {
   Batch b = make_batch(R, B, M, false, 3);
   cudaEvent_t e0, e1;
   CK(cudaEventCreate(&e0));
   CK(cudaEventCreate(&e1));
-  for (int w = 0; w < 5; ++w) run_chain(b);
+  for (int w = 0; w < 5; ++w) run_chain(b, walk, warps);
   CK(cudaDeviceSynchronize());
   const int iters = 50;
   for (int rep = 0; rep < 3; ++rep) {
@@ -94,7 +98,7 @@ static bool time_shape(const char* name, uint32_t R, uint32_t B, uint32_t M) {
     for (int it = 0; it < iters; ++it) {
       float t;
       CK(cudaEventRecord(e0));
-      run_chain(b);
+      run_chain(b, walk, warps);
       CK(cudaEventRecord(e1));
       CK(cudaEventSynchronize(e1));
       CK(cudaEventElapsedTime(&t, e0, e1));
@@ -126,21 +130,27 @@ int main() {
         for (int ragged = 0; ragged < 2; ++ragged) {
           Batch b = make_batch(R, B, M, ragged, R * 7919ull + B * 31 + M + ragged);
           run_generic(b);
-          run_chain(b);
-          CK(cudaDeviceSynchronize());
-          const bool ok = same(b);
-          if (!ok) {
-            ++fails;
-            std::printf("MISMATCH R=%u B=%u M=%u ragged=%d\n", R, B, M, ragged);
+          const uint32_t shapes[3][2] = {{1, 32}, {2, 32}, {2, 16}};  // whole-SM WALK = 1, 2 and the half-SM tile
+          for (auto& sh : shapes) {
+            CK(cudaMemset(b.chain_b, 0x5A, (size_t)b.R * b.MP * sizeof(uint64_t)));
+            run_chain(b, sh[0], sh[1]);
+            CK(cudaDeviceSynchronize());
+            if (!same(b)) {
+              ++fails;
+              std::printf("MISMATCH R=%u B=%u M=%u ragged=%d walk=%u warps=%u\n", R, B, M, ragged, sh[0], sh[1]);
+            }
           }
           free_batch(b);
         }
-  std::printf("correctness: %d mismatching case(s) of %zu\n", fails, sizeof(Rs) / 4 * sizeof(Bs) / 4 * sizeof(Ms) / 4 * 2);
+  std::printf("correctness: %d mismatching case(s) of %zu\n", fails, sizeof(Rs) / 4 * sizeof(Bs) / 4 * sizeof(Ms) / 4 * 2 * 3);
 
-  // timing at cfg 3 (16 384 x 256 blocks: 128 requests per CTA), cfg 2 (4 096 x 128 blocks: 32 per CTA), and the
-  // cfg 3 prompts (16 KiB each) cut into 96- and 160-byte blocks
+  // timing at cfg 3 (16 384 x 256 blocks: half-SM tiles of 64 requests, against whole-SM tiles of 64), cfg 2
+  // (4 096 x 128 blocks: 32 per whole-SM CTA, against half-SM tiles), and the cfg 3 prompts (16 KiB each) cut into
+  // 96- and 160-byte blocks
   bool ok = time_shape("cfg3", 16384, 64, 256);
+  ok = time_shape("cfg3 whole-SM WALK=2", 16384, 64, 256, 2, 32) && ok;
   ok = time_shape("cfg2", 4096, 64, 128) && ok;
+  ok = time_shape("cfg2 half-SM", 4096, 64, 128, 2, 16) && ok;
   ok = time_shape("cfg3-96B", 16384, 96, 16384 / 96) && ok;
   ok = time_shape("cfg3-160B", 16384, 160, 16384 / 160) && ok;
   return (fails || !ok) ? 1 : 0;
