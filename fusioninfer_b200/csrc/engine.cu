@@ -126,6 +126,19 @@ unsigned usable_cores() {
   return n ? n : 1u;
 }
 
+// A device staging buffer and its pinned host mirror (h stays null for a device-only buffer), grown by grow_staging
+template <typename T>
+struct Staging {
+  T* d = nullptr;
+  T* h = nullptr;
+  size_t cap = 0;  // elements
+  void release() {
+    cudaFree(d);
+    if (h) cudaFreeHost(h);
+    *this = Staging{};
+  }
+};
+
 }  // namespace
 
 struct fi_epp {
@@ -172,11 +185,8 @@ struct fi_epp {
   uint64_t* d_chain = nullptr;
   uint32_t* d_nblocks = nullptr;
   fi_pick* d_picks = nullptr;   // [R][P] final
-  fi_pick* d_ranked = nullptr;  // [R][P][k] of fi_epp_pick_batch_ranked: allocated by the first such call, grown with k
-  fi_pick* h_ranked = nullptr;  // pinned mirror
-  size_t ranked_cap = 0;        // picks both hold
-  uint32_t* d_subsets = nullptr;  // [max_batch][ceil(E/32)] staging of fi_epp_pick_batch_subset: allocated by its first call
-  uint32_t* h_subsets = nullptr;  // pinned
+  Staging<fi_pick> ranked;      // [R][P][k] of the host ranked pick: allocated by the first such call, grown with k
+  Staging<uint32_t> subsets;    // [max_batch][ceil(E/32)] staging of fi_epp_pick_batch_subset: allocated by its first call
   fi_pick* d_local = nullptr;   // [R][P] this rank's picks (sharded)
   fi_pick* d_gather = nullptr;  // [world][R][P]
   // peer-memory exchange (sharded mode; kernels.cuh PeerXchg)
@@ -250,9 +260,7 @@ struct fi_epp {
   };
   // fi_epp_index_add_submitted: double-buffered plan and chain staging (Add j uses padd[j & 1]; ev_done: consumed)
   struct PipeAdd {
-    uint32_t* d_plan = nullptr;
-    uint32_t* h_plan = nullptr;  // pinned
-    size_t cap = 0;              // in u32 words
+    Staging<uint32_t> plan;        // the packed plan (lru_plan.h)
     uint64_t* d_chains = nullptr;  // [max_batch][MP]
     cudaEvent_t ev_done = nullptr;
   };
@@ -260,14 +268,11 @@ struct fi_epp {
   uint64_t padd_seq = 0;
   uint64_t lru_deferred = 0, lru_sub_batches = 0;  // host-side totals
   LruHostStat* h_lru_stat = nullptr;         // pinned copy, refreshed after every call
-  uint32_t* d_lru_plan = nullptr;            // the planner's arrays of the current call
-  uint32_t* h_lru_plan = nullptr;            // pinned staging of the same
-  size_t lru_plan_cap = 0;                   // in u32 words
+  Staging<uint32_t> lru_plan_buf;            // the packed plan of the current call (lru_plan.h)
   uint32_t *d_lru_slot_of = nullptr, *d_lru_wcount = nullptr, *d_lru_base = nullptr;
   fi_index_op *d_lru_sets = nullptr, *d_lru_clears = nullptr;
   uint64_t lru_touch_cap = 0;                // touches per sub-batch the scratch arrays hold
-  uint64_t* d_lru_chains = nullptr;          // staging of host chains
-  size_t lru_chains_cap = 0;                 // in u64 words
+  Staging<uint64_t> lru_chains;              // staging of host chains (device only)
   cudaEvent_t ev_lru = nullptr;              // the previous call's staging has been consumed
   cudaEvent_t ev_lru_ovf = nullptr;          // the touch kernel's overflow flag has reached the host
   uint32_t last_plain_R = 0;                 // rows of d_chain the most recent stream-ordered pick wrote
@@ -321,6 +326,22 @@ namespace {
 int fail(fi_epp* h, int code, const std::string& m) {
   h->err = m;
   return code;
+}
+
+// Make `s` hold at least n elements: a smaller one is replaced by `alloc` (>= n) elements, its pinned mirror too if
+// `pinned`.  On failure nothing of it stays allocated (cap 0) and the call fails with FI_ERR_NOMEM.
+template <typename T>
+int grow_staging(fi_epp* h, Staging<T>& s, size_t n, size_t alloc, bool pinned) {
+  if (n <= s.cap) return FI_OK;
+  s.release();
+  if (cudaMalloc(&s.d, alloc * sizeof(T)) != cudaSuccess ||
+      (pinned && cudaMallocHost(&s.h, alloc * sizeof(T)) != cudaSuccess)) {
+    cudaGetLastError();
+    s.release();
+    return fail(h, FI_ERR_NOMEM, "cannot allocate a staging buffer of " + std::to_string(alloc * sizeof(T)) + " bytes");
+  }
+  s.cap = alloc;
+  return FI_OK;
 }
 
 cudaEvent_t get_event(fi_epp* h) {
@@ -756,23 +777,22 @@ int lru_refresh_stat(fi_epp* h) {
   return FI_OK;
 }
 
-// One sub-batch of a planned Add (the lru_plan.h arrays staged at `dp`): the view the LRU kernels take, and the
+// One sub-batch of a planned Add (the plan packed at `dp` by lru_plan_pack): the view the LRU kernels take, and the
 // kernels themselves.  Both Add paths (lru_device_add, lru_add_submitted) enqueue a sub-batch through these two.
 LruBatch lru_sub_batch(fi_epp* h, const uint32_t* dp, const LruPlan& pl, size_t sb, const uint64_t* chains, uint32_t pitch,
                        const uint32_t** inc) {
-  const size_t K = pl.req_id.size(), nsub = pl.subs.size(), EL = h->cfg.endpoint_count;
-  const LruSubBatch& sbt = pl.subs[sb];
+  const LruPlanOffsets o = lru_plan_offsets(pl, h->cfg.endpoint_count, sb);
   LruBatch b{};
-  b.req_id = dp + sbt.k_begin;
-  b.req_ep = dp + K + sbt.k_begin;
-  b.req_n = dp + 2 * K + sbt.k_begin;
-  b.req_off = dp + 3 * K + sbt.k_begin;
-  b.ep_list = dp + 4 * K + sbt.k_begin;
-  b.ep_start = dp + 5 * K + sb * (EL + 1);
-  *inc = dp + 5 * K + nsub * (EL + 1) + sb * EL;
+  b.req_id = dp + o.req_id;
+  b.req_ep = dp + o.req_ep;
+  b.req_n = dp + o.req_n;
+  b.req_off = dp + o.req_off;
+  b.ep_list = dp + o.ep_list;
+  b.ep_start = dp + o.ep_start;
+  *inc = dp + o.inc;
   b.chains = chains;
   b.pitch = pitch;
-  b.K = sbt.k_end - sbt.k_begin;
+  b.K = pl.subs[sb].k_end - pl.subs[sb].k_begin;
   b.slot_of = h->d_lru_slot_of;
   b.wcount = h->d_lru_wcount;
   b.base = h->d_lru_base;
@@ -864,60 +884,37 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
     if (rc != FI_OK) return rc;
   }
   const GossipLog glog = gossip_log(h);
-  // staging: req_id | req_ep | req_n | req_off | ep_list | ep_start[nsub][EL+1] | inc[nsub][EL]
-  const size_t words = 5 * K + nsub * ((size_t)2 * EL + 1);
+  const size_t words = lru_plan_words(pl, EL);
   FI_CUDA(cudaEventSynchronize(h->ev_lru));  // the previous call's staging (and chain copy) has been consumed
-  if (words > h->lru_plan_cap) {
-    cudaFree(h->d_lru_plan);
-    if (h->h_lru_plan) cudaFreeHost(h->h_lru_plan);
-    h->d_lru_plan = nullptr;
-    h->h_lru_plan = nullptr;
-    h->lru_plan_cap = 0;
-    const size_t cap = words + words / 2 + 1024;
-    FI_CUDA(cudaMalloc(&h->d_lru_plan, cap * sizeof(uint32_t)));
-    FI_CUDA(cudaMallocHost(&h->h_lru_plan, cap * sizeof(uint32_t)));
-    h->lru_plan_cap = cap;
-  }
-  uint32_t* hp = h->h_lru_plan;
-  if (words) {
-  std::memcpy(hp, pl.req_id.data(), K * 4);
-  std::memcpy(hp + K, pl.req_ep.data(), K * 4);
-  std::memcpy(hp + 2 * K, pl.req_n.data(), K * 4);
-  std::memcpy(hp + 3 * K, pl.req_off.data(), K * 4);
-  std::memcpy(hp + 4 * K, pl.ep_list.data(), K * 4);
-  std::memcpy(hp + 5 * K, pl.ep_start.data(), pl.ep_start.size() * 4);
-  std::memcpy(hp + 5 * K + nsub * ((size_t)EL + 1), pl.inc.data(), pl.inc.size() * 4);
-  }
+  rc = grow_staging(h, h->lru_plan_buf, words, words + words / 2 + 1024, true);  // room to spare: plans vary in size
+  if (rc != FI_OK) return rc;
+  lru_plan_pack(pl, h->lru_plan_buf.h);
   // the LRU kernels run on the index stream; like every index update they are ordered behind the picks
   // submitted so far (a pick sees the index as of its call)
   FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
-  if (words) FI_CUDA(cudaMemcpyAsync(h->d_lru_plan, hp, words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+  if (words)
+    FI_CUDA(cudaMemcpyAsync(h->lru_plan_buf.d, h->lru_plan_buf.h, words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
   h->stats.h2d_bytes += words * sizeof(uint32_t);
   const uint64_t* d_chains = chains;
   if (!on_device && K) {
     const size_t cw = (size_t)R * pitch;
-    if (cw > h->lru_chains_cap) {
-      cudaFree(h->d_lru_chains);
-      h->d_lru_chains = nullptr;
-      h->lru_chains_cap = 0;
-      FI_CUDA(cudaMalloc(&h->d_lru_chains, cw * sizeof(uint64_t)));
-      h->lru_chains_cap = cw;
-    }
+    rc = grow_staging(h, h->lru_chains, cw, cw, false);
+    if (rc != FI_OK) return rc;
+    d_chains = h->lru_chains.d;
     // only the rows the plan kept are needed; whole-range copy when most are (one DMA), row copies otherwise
     if (K * 2 >= R) {
-      FI_CUDA(cudaMemcpyAsync(h->d_lru_chains, chains, cw * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_index));
+      FI_CUDA(cudaMemcpyAsync(h->lru_chains.d, chains, cw * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_index));
       h->stats.h2d_bytes += cw * sizeof(uint64_t);
     } else {
       for (size_t k = 0; k < K; ++k) {
         const size_t r = pl.req_id[k];
-        FI_CUDA(cudaMemcpyAsync(h->d_lru_chains + r * pitch, chains + r * pitch, (size_t)pl.req_n[k] * sizeof(uint64_t),
+        FI_CUDA(cudaMemcpyAsync(h->lru_chains.d + r * pitch, chains + r * pitch, (size_t)pl.req_n[k] * sizeof(uint64_t),
                                 cudaMemcpyHostToDevice, h->s_index));
         h->stats.h2d_bytes += (size_t)pl.req_n[k] * sizeof(uint64_t);
       }
     }
-    d_chains = h->d_lru_chains;
   }
-  const uint32_t* dp = h->d_lru_plan;
+  const uint32_t* dp = h->lru_plan_buf.d;
   h->lru_sub_batches += nsub;
   std::vector<uint8_t> deferred;  // per request of this call: its endpoint overflowed in the optimistic pass
   std::vector<uint32_t> ovf_host;
@@ -991,7 +988,7 @@ int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, size_
   // like every index update, ordered behind the picks submitted so far (a pick sees the index as of its call)
   FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_slot_read[slot], 0));
   FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
-  FI_CUDA(cudaMemcpyAsync(pa.d_plan, pa.h_plan, words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+  FI_CUDA(cudaMemcpyAsync(pa.plan.d, pa.plan.h, words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
   h->stats.h2d_bytes += words * sizeof(uint32_t);
   const GossipLog glog = gossip_log(h);
   h->lru_sub_batches += pl.subs.size();
@@ -1000,7 +997,7 @@ int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, size_
     int rc = check_counters_lagged(h, touches);  // may rebuild the index (on s_index, before this sub-batch)
     if (rc != FI_OK) return rc;
     const uint32_t* inc = nullptr;
-    const LruBatch b = lru_sub_batch(h, pa.d_plan, pl, sb, pa.d_chains, h->MP, &inc);
+    const LruBatch b = lru_sub_batch(h, pa.plan.d, pl, sb, pa.d_chains, h->MP, &inc);
     rc = lru_enqueue_touch(h, b, inc);
     if (rc != FI_OK) return rc;
     rc = lru_enqueue_apply(h, b, touches, glog, false);
@@ -1037,33 +1034,16 @@ int lru_add_submitted(fi_epp* h, uint32_t slot, const uint32_t* endpoints, const
   lru_plan_batch(endpoints, nblocks, R, lo, EL, lru_touch_bound(h->dlru.TS, h->dlru.capacity), h->lru_touch_cap,
                  h->cfg.max_batch, &pl);
   if (pl.subs.empty()) return FI_OK;
-  const size_t K = pl.req_id.size(), nsub = pl.subs.size();
-  const size_t words = 5 * K + nsub * ((size_t)2 * EL + 1);
+  const size_t words = lru_plan_words(pl, EL);
   fi_epp::PipeAdd& pa = h->padd[h->padd_seq & 1];
   if (pa.ev_done) FI_CUDA(cudaEventSynchronize(pa.ev_done));  // the Add before the previous one is done with it
   if (!pa.ev_done) {
     FI_CUDA(cudaEventCreateWithFlags(&pa.ev_done, cudaEventDisableTiming));
     FI_CUDA(cudaMalloc(&pa.d_chains, (size_t)h->cfg.max_batch * h->MP * sizeof(uint64_t)));
   }
-  if (words > pa.cap) {
-    cudaFree(pa.d_plan);
-    if (pa.h_plan) cudaFreeHost(pa.h_plan);
-    pa.d_plan = nullptr;
-    pa.h_plan = nullptr;
-    pa.cap = 0;
-    const size_t cap = words + words / 2 + 1024;
-    FI_CUDA(cudaMalloc(&pa.d_plan, cap * sizeof(uint32_t)));
-    FI_CUDA(cudaMallocHost(&pa.h_plan, cap * sizeof(uint32_t)));
-    pa.cap = cap;
-  }
-  uint32_t* hp = pa.h_plan;
-  std::memcpy(hp, pl.req_id.data(), K * 4);
-  std::memcpy(hp + K, pl.req_ep.data(), K * 4);
-  std::memcpy(hp + 2 * K, pl.req_n.data(), K * 4);
-  std::memcpy(hp + 3 * K, pl.req_off.data(), K * 4);
-  std::memcpy(hp + 4 * K, pl.ep_list.data(), K * 4);
-  std::memcpy(hp + 5 * K, pl.ep_start.data(), pl.ep_start.size() * 4);
-  std::memcpy(hp + 5 * K + nsub * ((size_t)EL + 1), pl.inc.data(), pl.inc.size() * 4);
+  rc = grow_staging(h, pa.plan, words, words + words / 2 + 1024, true);  // as lru_device_add's
+  if (rc != FI_OK) return rc;
+  lru_plan_pack(pl, pa.plan.h);
   const uint64_t* slot_chain = slot ? h->d_chain2 : h->d_chain;
   FI_CUDA(cudaStreamWaitEvent(h->s_copy, h->ev_a[slot], 0));  // the batch's chains are written
   FI_CUDA(cudaMemcpyAsync(pa.d_chains, slot_chain, (size_t)R * h->MP * sizeof(uint64_t), cudaMemcpyDeviceToDevice, h->s_copy));
@@ -1076,28 +1056,6 @@ int lru_add_submitted(fi_epp* h, uint32_t slot, const uint32_t* endpoints, const
   h->padd_seq++;
   if (rc != FI_OK) return rc;
   if (e != cudaSuccess) return fail(h, FI_ERR_CUDA, cudaGetErrorString(e));
-  return FI_OK;
-}
-
-int upload_endpoints(fi_epp* h) {
-  if (!h->eps_dirty) return FI_OK;
-  FI_CUDA(cudaMemcpyAsync(h->d_eps, h->eps.data(), h->eps.size() * sizeof(EndpointDev), cudaMemcpyHostToDevice, h->s_main));
-  h->stats.h2d_bytes += h->eps.size() * sizeof(EndpointDev);
-  {
-    LaunchScope ls(h, h->s_main, K_OTHER);
-    FI_CUDA(launch_prepare_endpoints(h->d_eps, h->cfg.num_endpoints, h->cfg.endpoint_begin, h->cfg.endpoint_count, h->st,
-                                     h->d_sc, h->d_elig, h->d_zero, h->d_ztie, h->s_main));
-  }
-  // eps is pageable host memory: the copy above has been staged by the time the call returns
-  h->eps_dirty = false;
-  return FI_OK;
-}
-
-int upload_lora(fi_epp* h) {
-  if (!h->lora_dirty) return FI_OK;
-  FI_CUDA(cudaMemcpyAsync(h->d_lora, h->lora.data(), h->lora.size() * sizeof(LoraDev), cudaMemcpyHostToDevice, h->s_main));
-  h->stats.h2d_bytes += h->lora.size() * sizeof(LoraDev);
-  h->lora_dirty = false;
   return FI_OK;
 }
 
@@ -1249,43 +1207,112 @@ void dump_trace(fi_epp* h, uint32_t R) {
   h->tracing = false;
 }
 
-// host prompts still to be copied (fi_epp_pick_batch): run_pick copies them, in slices when it can
-struct HostFeed {
-  const uint8_t* prompts;   // host
-  const uint64_t* offsets;  // host, [R+1]
+// One pick call of any variant: the single pick (k == 0), the ranked pick (k > 0, docs/SPEC.md S.6a) and the subset
+// pick (subsets, S.5a), each with or without LoRA adapters.  Host or device pointers, by entry point.
+struct PickCall {
+  const uint8_t* prompts;
+  const uint64_t* offsets;   // [R + 1]
+  const uint64_t* h0;        // [R]
+  const uint64_t* adapters;  // [R] adapter ids, or null
+  const uint32_t* subsets;   // [R][ceil(E/32)] candidate bitsets, or null
+  uint32_t R;
+  uint32_t k;                // 0: out is [R][P]; else [R][P][k]
+  fi_pick* out;
+  uint64_t* chains_out;      // [R][max_blocks], or null
 };
 
-void fill_match_params(fi_epp* h, MatchParams& mp, const uint64_t* chain, const uint32_t* nb, const uint64_t* d_offsets,
-                       const uint64_t* d_h0, const uint64_t* d_adapters, uint32_t R, fi_pick* out, bool local_pd) {
+// the same from the untyped pointers the device entry points take
+PickCall device_call(const void* p, const void* o, const void* h0, const void* a, const void* s, uint32_t R, uint32_t k,
+                     void* out, void* ch) {
+  return {(const uint8_t*)p, (const uint64_t*)o, (const uint64_t*)h0, (const uint64_t*)a, (const uint32_t*)s, R, k,
+          (fi_pick*)out, (uint64_t*)ch};
+}
+
+// chains_out[R][max_blocks] = the chains at `chain` (pitch MP), on stream s; nothing if chains_out is null
+int copy_chains_out(fi_epp* h, const uint64_t* chain, uint64_t* chains_out, uint32_t R, cudaMemcpyKind kind, cudaStream_t s) {
+  if (!chains_out) return FI_OK;
+  const size_t row = (size_t)h->cfg.max_blocks * sizeof(uint64_t);
+  FI_CUDA(cudaMemcpy2DAsync(chains_out, row, chain, (size_t)h->MP * sizeof(uint64_t), row, R, kind, s));
+  if (kind == cudaMemcpyDeviceToHost) h->stats.d2h_bytes += row * R;
+  return FI_OK;
+}
+
+// Stage B's prelude, the same for the stream-ordered pick and the pipelined submit: s_main waits for every index update
+// submitted so far, the endpoint and adapter tables go up if they changed, and `mp` describes the match of call `c`
+// (device pointers) over the chains at chain / nb.  Sharded: the rank's picks go to d_local, and the merge applies P/D.
+int prepare_match(fi_epp* h, const PickCall& c, const uint64_t* chain, const uint32_t* nb, MatchParams& mp) {
+  FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_index, 0));  // every submitted op is visible
+  if (h->eps_dirty) {
+    FI_CUDA(cudaMemcpyAsync(h->d_eps, h->eps.data(), h->eps.size() * sizeof(EndpointDev), cudaMemcpyHostToDevice, h->s_main));
+    h->stats.h2d_bytes += h->eps.size() * sizeof(EndpointDev);
+    LaunchScope ls(h, h->s_main, K_OTHER);
+    FI_CUDA(launch_prepare_endpoints(h->d_eps, h->cfg.num_endpoints, h->cfg.endpoint_begin, h->cfg.endpoint_count, h->st,
+                                     h->d_sc, h->d_elig, h->d_zero, h->d_ztie, h->s_main));
+    h->eps_dirty = false;  // (eps is pageable host memory: the copy has been staged by the time it returns)
+  }
+  if (h->lora_dirty) {
+    FI_CUDA(cudaMemcpyAsync(h->d_lora, h->lora.data(), h->lora.size() * sizeof(LoraDev), cudaMemcpyHostToDevice, h->s_main));
+    h->stats.h2d_bytes += h->lora.size() * sizeof(LoraDev);
+    h->lora_dirty = false;
+  }
+  const bool sharded = h->world > 1;
+  mp = MatchParams{};
   mp.chain = chain;
   mp.nblocks = nb;
-  mp.offsets = d_offsets;
-  mp.adapters = d_adapters;
-  mp.R = R;
+  mp.offsets = c.offsets;
+  mp.adapters = c.adapters;
+  mp.R = c.R;
   mp.MP = h->MP;
   mp.ix = h->ix;
   mp.st = h->st;
   mp.ep_begin = h->cfg.endpoint_begin;
   mp.ep_count = h->cfg.endpoint_count;
   mp.E_global = h->cfg.num_endpoints;
-  mp.r_base = 0;
-  mp.h0 = d_h0;
+  mp.h0 = c.h0;
   mp.lpm = h->cfg.match_mode;
-  mp.apply_pd = (h->cfg.pd_enabled && local_pd) ? 1 : 0;
+  mp.apply_pd = (h->cfg.pd_enabled && !sharded) ? 1 : 0;
   mp.pd_decode = h->cfg.pd_decode_profile;
   mp.pd_prefill = h->cfg.pd_prefill_profile;
   mp.pd_threshold = h->cfg.pd_threshold;
-  mp.out = out;
+  mp.out = sharded ? h->d_local : c.out;
   mp.probed_blocks = h->profiling ? h->d_probed : nullptr;
   mp.work_counter = h->d_work;
-  mp.lane_zero = 0;
+  mp.k = c.k;
+  if (c.subsets) {
+    mp.subsets = c.subsets;
+    mp.sub_pitch = (h->cfg.num_endpoints + 31) / 32;
+    mp.eps = h->d_eps;
+  }
+  return FI_OK;
 }
 
-// the whole pick on device buffers; result in d_out ([R][P], or [R][P][ranked_k] for the ranked pick, ranked_k > 0:
-// single rank only).  d_subsets: the ranked pick's per-request candidate bitsets ([R][ceil(E/32)], S.5a), or null
-int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0,
-                  const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed, uint32_t ranked_k,
-                  const uint32_t* d_subsets) {
+// Pipeline slot 0's chain buffer, d_chain / d_nblocks (slot 1, d_chain2 / d_nblocks2, serves odd-numbered submits only).
+//   Writers: the stream-ordered pick (run_pick_impl) and fi_epp_hash_batch, on s_main;
+//            stage A of an even-numbered pipelined submit (submit_pick), on s_a.
+//   Readers: the match and chain copy-out of the pick or submit that wrote it, on s_main (ev_plain, ev_b[0]);
+//            fi_epp_index_add_chains_device(.., NULL, ..), a device-LRU Add on s_index (ev_lru);
+//            fi_epp_index_add_submitted's copy of a submitted batch's chains, on s_copy (ev_slot_read[0]).
+// A stream-ordered writer calls claim_chain_slot0 before it writes: its stream waits for the last submit's stage A and
+// for the readers on other streams (wait_slot_readers), and no submitted batch's chains can be taken any more.  Stage A
+// of a submit waits for the same readers of its own slot, for the match of the batch two back and the last
+// stream-ordered pick (submit_pick).
+int wait_slot_readers(fi_epp* h, uint32_t slot, cudaStream_t s) {
+  if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(s, h->ev_lru, 0));
+  if (h->padd_seq) FI_CUDA(cudaStreamWaitEvent(s, h->ev_slot_read[slot], 0));
+  return FI_OK;
+}
+
+int claim_chain_slot0(fi_epp* h, cudaStream_t s) {
+  if (h->pipe_seq) FI_CUDA(cudaStreamWaitEvent(s, h->ev_a[(h->pipe_seq - 1) & 1], 0));
+  const int rc = wait_slot_readers(h, 0, s);
+  if (rc == FI_OK) h->slot_ticket[0] = h->slot_ticket[1] = ~0ull;
+  return rc;
+}
+
+// the whole pick of call `c` on device buffers (out: single rank only for k > 0); feed: the same call on host buffers,
+// whose prompts are still to be copied to c.prompts (in slices when it can), or null
+int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
+  const uint32_t R = c.R;
   const bool sharded = h->world > 1;
   if (sharded && (h->n_sets || h->n_clears))
     return fail(h, FI_ERR_STATE, "sharded pool: index updates are collective (fi_epp_index_apply / fi_epp_index_add_chains)");
@@ -1299,30 +1326,17 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
     FI_CUDA(cudaStreamSynchronize(h->s_main));
     FI_CUDA(cudaEventRecord(h->ev_trace0, h->s_main));
   }
-  FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_index, 0));  // every submitted op is visible
-  rc = upload_endpoints(h);
+  MatchParams mp;
+  rc = prepare_match(h, c, h->d_chain, h->d_nblocks, mp);
   if (rc != FI_OK) return rc;
-  rc = upload_lora(h);
+  rc = claim_chain_slot0(h, h->s_main);
   if (rc != FI_OK) return rc;
-  if (h->pipe_seq)  // a plain pick after pipelined submits: their stage A shares d_chain (slot 0) with ours
-    FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[(h->pipe_seq - 1) & 1], 0));
-  if (h->padd_seq)  // fi_epp_index_add_submitted may still be copying slot 0's chains
-    FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_slot_read[0], 0));
-  h->slot_ticket[0] = h->slot_ticket[1] = ~0ull;  // the submitted batches' chains are no longer available
-  MatchParams mp{};
-  fill_match_params(h, mp, h->d_chain, h->d_nblocks, d_offsets, d_h0, d_adapters, R, sharded ? h->d_local : d_out, !sharded);
-  mp.k = ranked_k;
-  if (d_subsets) {
-    mp.subsets = d_subsets;
-    mp.sub_pitch = (h->cfg.num_endpoints + 31) / 32;
-    mp.eps = h->d_eps;
-  }
 
   const uint32_t S = h->feed_slices;
   if (feed && !sharded && h->fast_hash && S > 1 && R >= 64 * S && feed->offsets[R] >= (8ull << 20)) {
     // Sliced feed.  (On DEVICE-resident inputs slicing the step is slower — DESIGN.md "What did not
     // work" — but here the copy engine is the bottleneck and the kernels of slice k hide under copy k+1.)
-    uint8_t* dp = const_cast<uint8_t*>(d_prompts);
+    uint8_t* dp = const_cast<uint8_t*>(c.prompts);
     const uint32_t per = (((R + S - 1) / S) + 31) & ~31u;
     uint32_t used = 0;
     for (uint32_t k = 0; k * per < R; ++k, ++used) {
@@ -1335,7 +1349,7 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
     for (uint32_t k = 0; k < used; ++k) {
       const uint32_t r0 = k * per, Rk = std::min(per, R - r0);
       FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_copy[k], 0));
-      rc = run_hash(h, d_prompts, d_offsets, d_h0, r0, Rk, h->s_main);
+      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, Rk, h->s_main);
       if (rc != FI_OK) return rc;
       MatchParams ms = mp;
       ms.chain = mp.chain + (size_t)r0 * h->MP;
@@ -1346,33 +1360,25 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
       ms.h0 = mp.h0 + r0;
       ms.r_base = r0;
       ms.R = Rk;
-      ms.out = mp.out + (size_t)r0 * h->P * (ranked_k ? ranked_k : 1);
+      ms.out = mp.out + (size_t)r0 * h->P * std::max(c.k, 1u);
       ms.work_counter = h->d_work + k;
       LaunchScope ls(h, h->s_main, K_MATCH);
       FI_CUDA(launch_match_pick(ms, h->sm_count, h->s_main));
     }
-    dump_trace(h, R);
-    h->stats.pick_calls++;
-    h->stats.requests += R;
     return FI_OK;
   }
   if (feed && feed->offsets[R]) {  // one copy, then the whole batch
-    FI_CUDA(cudaMemcpyAsync(const_cast<uint8_t*>(d_prompts), feed->prompts, feed->offsets[R], cudaMemcpyHostToDevice, h->s_main));
+    FI_CUDA(cudaMemcpyAsync(const_cast<uint8_t*>(c.prompts), feed->prompts, feed->offsets[R], cudaMemcpyHostToDevice, h->s_main));
     h->stats.h2d_bytes += feed->offsets[R];
   }
   if (!sharded) {
     // (A sub-batch pipeline over several streams was tried and measured slower on device-resident
     // inputs — DESIGN.md "What did not work": the chain walk costs a flat serial latency at any batch
     // size and small slices pay launch/ramp overheads.)
-    rc = run_hash(h, d_prompts, d_offsets, d_h0, 0, R, h->s_main);
+    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main);
     if (rc != FI_OK) return rc;
-    {
-      LaunchScope ls(h, h->s_main, K_MATCH);
-      FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main));
-    }
-    dump_trace(h, R);
-    h->stats.pick_calls++;
-    h->stats.requests += R;
+    LaunchScope ls(h, h->s_main, K_MATCH);
+    FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main));
     return FI_OK;
   }
 
@@ -1384,7 +1390,7 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
     const uint32_t per = (((R + h->world - 1) / h->world) + 31) & ~31u;  // ≤ chain_rows / world
     const uint32_t r0 = std::min(R, h->rank * per), r1 = std::min(R, r0 + per);
     if (r1 > r0) {
-      rc = run_hash(h, d_prompts, d_offsets, d_h0, r0, r1 - r0, h->s_main);
+      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, r1 - r0, h->s_main);
       if (rc != FI_OK) return rc;
     }
     rc = nccl_allgather(h, h->d_chain + (size_t)h->rank * per * h->MP, h->d_chain, (size_t)per * h->MP * sizeof(uint64_t));
@@ -1393,7 +1399,7 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
     if (rc != FI_OK) return rc;
     h->stats.n_other += 2;  // two collectives of the step (not kernels of this library)
   } else {
-    rc = run_hash(h, d_prompts, d_offsets, d_h0, 0, R, h->s_main);
+    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main);
     if (rc != FI_OK) return rc;
   }
   const bool p2p = h->px.enabled != 0;
@@ -1426,34 +1432,32 @@ int run_pick_impl(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets
   mg.R = R;
   mg.P = h->P;
   mg.nblocks = h->d_nblocks;
-  mg.offsets = d_offsets;
+  mg.offsets = c.offsets;
   mg.chain = h->d_chain;
-  mg.h0 = d_h0;
+  mg.h0 = c.h0;
   mg.MP = h->MP;
   mg.E_global = h->cfg.num_endpoints;
   mg.apply_pd = h->cfg.pd_enabled;
   mg.pd_decode = h->cfg.pd_decode_profile;
   mg.pd_prefill = h->cfg.pd_prefill_profile;
   mg.pd_threshold = h->cfg.pd_threshold;
-  mg.out = d_out;
+  mg.out = c.out;
   {
     LaunchScope ls(h, h->s_main, K_OTHER);
     FI_CUDA(launch_merge_picks(mg, h->s_main));
   }
-  dump_trace(h, R);
-  h->stats.pick_calls++;
-  h->stats.requests += R;
   return FI_OK;
 }
 
-int run_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0,
-             const uint64_t* d_adapters, uint32_t R, fi_pick* d_out, const HostFeed* feed = nullptr, uint32_t ranked_k = 0,
-             const uint32_t* d_subsets = nullptr) {
-  int rc = run_pick_impl(h, d_prompts, d_offsets, d_h0, d_adapters, R, d_out, feed, ranked_k, d_subsets);
+int run_pick(fi_epp* h, const PickCall& c, const PickCall* feed) {
+  int rc = run_pick_impl(h, c, feed);
   if (rc != FI_OK) return rc;
+  dump_trace(h, c.R);
+  h->stats.pick_calls++;
+  h->stats.requests += c.R;
   FI_CUDA(cudaEventRecord(h->ev_pick, h->s_main));  // index updates submitted later wait for this pick
   FI_CUDA(cudaEventRecord(h->ev_plain, h->s_main));
-  h->last_plain_R = R;
+  h->last_plain_R = c.R;
   return FI_OK;
 }
 
@@ -1464,13 +1468,10 @@ int issue_ticket(fi_epp* h, uint64_t* t) {
   return FI_OK;
 }
 
-// Pipelined device path: enqueue one batch.  Stage A on s_a, stage B on s_main (see fi_epp::s_a).  d_adapters,
-// ranked_k, d_subsets and d_chains_out as run_pick / copy_chains_out (fi_epp_pick_submit passes none of them);
-// lagged: the index counters may lag (check_counters_lagged, fi_epp_pick_submit_ex).
-int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0, uint32_t R,
-                fi_pick* d_out, cudaStream_t us, uint64_t* ticket, const uint64_t* d_adapters = nullptr,
-                uint32_t ranked_k = 0, const uint32_t* d_subsets = nullptr, uint64_t* d_chains_out = nullptr,
-                bool lagged = false) {
+// Pipelined device path: enqueue one batch, call `c` on device buffers.  Stage A on s_a, stage B on s_main (see
+// fi_epp::s_a).  lagged: the index counters may lag (check_counters_lagged, fi_epp_pick_submit_ex).
+int submit_pick(fi_epp* h, const PickCall& c, cudaStream_t us, uint64_t* ticket, bool lagged) {
+  const uint32_t R = c.R;
   int rc = flush_ops(h);
   if (rc != FI_OK) return rc;
   rc = lagged ? check_counters_lagged(h, 0) : check_counters(h);
@@ -1498,48 +1499,35 @@ int submit_pick(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, 
   uint32_t* nb = slot ? h->d_nblocks2 : h->d_nblocks;
   // ---- stage A: inputs are ready in the caller's stream order; the slot's buffers are free once the
   // match of two batches ago is done; slot 0's d_chain / d_nblocks are free once the previous plain pick
-  // (if any) is done
+  // (if any) is done; and the readers on other streams (claim_chain_slot0)
   FI_CUDA(cudaEventRecord(h->ev_in, us));
   FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_in, 0));
   if (h->pipe_seq >= 2) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot], 0));
   FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_plain, 0));
-  if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_lru, 0));  // a device-LRU Add may still be reading d_chain
-  if (h->padd_seq) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_slot_read[slot], 0));  // (fi_epp_index_add_submitted)
+  rc = wait_slot_readers(h, slot, h->s_a);
+  if (rc != FI_OK) return rc;
   {
     // Block hashing and chain walk in one kernel (hash_kernels.cu hash_chain).  It does not wait for the previous
     // batch's match_pick: a full batch runs half-SM CTAs, and one starts on an SM as soon as two of match's three
     // CTAs there have run out of queue (DESIGN.md §4.0; giving match fewer CTAs per SM so that the two kernels share
     // every SM for the whole step was measured slower: §7).
     LaunchScope ls(h, h->s_a, K_HASH);
-    FI_CUDA(launch_hash_chain(d_prompts, d_offsets, d_h0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, chain, nb,
+    FI_CUDA(launch_hash_chain(c.prompts, c.offsets, c.h0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, chain, nb,
                               h->sm_count, h->s_a));
   }
   FI_CUDA(cudaEventRecord(h->ev_a[slot], h->s_a));
   // ---- stage B
-  FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_index, 0));  // every submitted op is visible
-  rc = upload_endpoints(h);
-  if (rc != FI_OK) return rc;
-  rc = upload_lora(h);
+  MatchParams mp;
+  rc = prepare_match(h, c, chain, nb, mp);
   if (rc != FI_OK) return rc;
   FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[slot], 0));
-  MatchParams mp{};
-  fill_match_params(h, mp, chain, nb, d_offsets, d_h0, d_adapters, R, d_out, true);
   mp.work_counter = h->d_work + 8 + slot;
-  mp.k = ranked_k;
-  if (d_subsets) {
-    mp.subsets = d_subsets;
-    mp.sub_pitch = (h->cfg.num_endpoints + 31) / 32;
-    mp.eps = h->d_eps;
-  }
   {
     LaunchScope ls(h, h->s_main, K_MATCH);
     FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main));
   }
-  if (d_chains_out) {
-    const size_t row = (size_t)h->cfg.max_blocks * sizeof(uint64_t);
-    FI_CUDA(cudaMemcpy2DAsync(d_chains_out, row, chain, (size_t)h->MP * sizeof(uint64_t), row, R, cudaMemcpyDeviceToDevice,
-                              h->s_main));
-  }
+  rc = copy_chains_out(h, chain, c.chains_out, R, cudaMemcpyDeviceToDevice, h->s_main);
+  if (rc != FI_OK) return rc;
   FI_CUDA(cudaEventRecord(h->ev_b[slot], h->s_main));
   FI_CUDA(cudaEventRecord(h->ev_pick, h->s_main));
   rc = issue_ticket(h, ticket);
@@ -1673,8 +1661,8 @@ void fi_epp_destroy(fi_epp* h) {
   cudaFree(h->d_chain);
   cudaFree(h->d_nblocks);
   cudaFree(h->d_picks);
-  cudaFree(h->d_ranked);
-  cudaFree(h->d_subsets);
+  h->ranked.release();
+  h->subsets.release();
   cudaFree(h->d_local);
   cudaFree(h->d_gather);
   cudaFree(h->d_glog_n);
@@ -1703,9 +1691,8 @@ void fi_epp_destroy(fi_epp* h) {
   h->lrus.clear();
   h->lru_arena.release();
   free_dev_lru(h);
-  cudaFree(h->d_lru_plan);
-  if (h->h_lru_plan) cudaFreeHost(h->h_lru_plan);
-  cudaFree(h->d_lru_chains);
+  h->lru_plan_buf.release();
+  h->lru_chains.release();
   free_index(h->ix);
   free_index(h->ix_spare);
   for (int b = 0; b < 2; ++b) {
@@ -1716,8 +1703,6 @@ void fi_epp_destroy(fi_epp* h) {
     if (h->ev_buf[b]) cudaEventDestroy(h->ev_buf[b]);
   }
   if (h->h_picks) cudaFreeHost(h->h_picks);
-  if (h->h_ranked) cudaFreeHost(h->h_ranked);
-  if (h->h_subsets) cudaFreeHost(h->h_subsets);
   if (h->h_offsets) cudaFreeHost(h->h_offsets);
   if (h->h_h0) cudaFreeHost(h->h_h0);
   if (h->h_nblocks) cudaFreeHost(h->h_nblocks);
@@ -1732,8 +1717,7 @@ void fi_epp_destroy(fi_epp* h) {
   for (int k = 0; k < fi_epp::kTicketRing; ++k)
     if (h->ev_ticket[k]) cudaEventDestroy(h->ev_ticket[k]);
   for (fi_epp::PipeAdd& pa : h->padd) {
-    cudaFree(pa.d_plan);
-    if (pa.h_plan) cudaFreeHost(pa.h_plan);
+    pa.plan.release();
     cudaFree(pa.d_chains);
     if (pa.ev_done) cudaEventDestroy(pa.ev_done);
   }
@@ -2408,13 +2392,6 @@ static int stage_inputs(fi_epp* h, const uint8_t* prompts, const uint64_t* offse
   return FI_OK;
 }
 
-static int copy_chains_out(fi_epp* h, uint64_t* chains_out, uint32_t R, cudaMemcpyKind kind, cudaStream_t s) {
-  const size_t row = (size_t)h->cfg.max_blocks * sizeof(uint64_t);
-  FI_CUDA(cudaMemcpy2DAsync(chains_out, row, h->d_chain, (size_t)h->MP * sizeof(uint64_t), row, R, kind, s));
-  if (kind == cudaMemcpyDeviceToHost) h->stats.d2h_bytes += row * R;
-  return FI_OK;
-}
-
 int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
                       uint64_t* chains_out, uint32_t* nblocks_out) {
   if (!h || !offsets || (!h0 && R) || (!prompts && R && offsets[R])) return FI_ERR_INVALID;
@@ -2426,18 +2403,13 @@ int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets
   if (rc != FI_OK) return rc;
   rc = stage_inputs(h, prompts, offsets, h0, R, total);
   if (rc != FI_OK) return rc;
-  if (h->pipe_seq)  // a pipelined batch's stage A (on s_a) shares d_chain (slot 0) with us
-    FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[(h->pipe_seq - 1) & 1], 0));
-  if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_lru, 0));  // a device-LRU Add may still be reading d_chain
-  if (h->padd_seq) FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_slot_read[0], 0));
+  rc = claim_chain_slot0(h, h->s_main);
+  if (rc != FI_OK) return rc;
   h->last_plain_R = 0;  // d_chain no longer holds a pick batch's chains
-  h->slot_ticket[0] = h->slot_ticket[1] = ~0ull;
   rc = run_hash(h, h->d_prompts, h->d_offsets, h->d_h0, 0, R, h->s_main);
   if (rc != FI_OK) return rc;
-  if (chains_out) {
-    rc = copy_chains_out(h, chains_out, R, cudaMemcpyDeviceToHost, h->s_main);
-    if (rc != FI_OK) return rc;
-  }
+  rc = copy_chains_out(h, h->d_chain, chains_out, R, cudaMemcpyDeviceToHost, h->s_main);
+  if (rc != FI_OK) return rc;
   if (nblocks_out) {
     FI_CUDA(cudaMemcpyAsync(h->h_nblocks, h->d_nblocks, (size_t)R * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_main));
     h->stats.d2h_bytes += (size_t)R * sizeof(uint32_t);
@@ -2447,284 +2419,191 @@ int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets
   return FI_OK;
 }
 
-int fi_epp_pick_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
-                      fi_pick* out, uint64_t* chains_out) {
-  return fi_epp_pick_batch_lora(h, prompts, offsets, h0, nullptr, R, out, chains_out);
+// ---- picks: every entry point below is one PickCall through pick_host, pick_device or pick_submit ----------------
+// the argument checks of every pick call, before the handle is touched (FI_ERR_INVALID); the ranked entry points, which
+// take k >= 1, reject k == 0 themselves
+static bool bad_pick_args(const PickCall& c, bool host) {
+  return !c.offsets || (!c.h0 && c.R) || (!c.out && (c.R || c.k)) || c.k > FI_EPP_MAX_RANKED || (c.k == 0 && c.subsets) ||
+         (host && !c.prompts && c.R && c.offsets[c.R]);
 }
 
-int fi_epp_pick_batch_lora(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
-                           const uint64_t* adapters, uint32_t R, fi_pick* out, uint64_t* chains_out) {
-  if (!h || !offsets || (!h0 && R) || (!out && R) || (!prompts && R && offsets[R])) return FI_ERR_INVALID;
-  std::lock_guard<std::mutex> lk(h->mu);
+// The handle's checks of every pick call, under its lock and before an empty batch returns (a batch over max_batch is
+// never empty).  Subset picks are ranked picks (k >= 1) with per-request candidate bitsets, which are pool-wide: a
+// handle over part of the pool cannot apply them (FI_ERR_STATE, like a sharded pool).
+static int check_pick_handle(fi_epp* h, const PickCall& c) {
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  if (R == 0) return FI_OK;
+  if (c.k && h->world > 1) return fail(h, FI_ERR_STATE, "ranked picks need a single-rank pool");
+  if (c.subsets && (h->cfg.endpoint_begin != 0 || h->cfg.endpoint_count != h->cfg.num_endpoints))
+    return fail(h, FI_ERR_STATE, "subset picks need a single handle over the whole pool");
+  if (c.R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
+  return FI_OK;
+}
+
+// Host buffers: the inputs are staged through pinned memory (run_pick feeds the prompts), and the picks come back
+// through d_picks / h_picks ([R][P]) or the ranked pair ([R][P][k]) before the call returns.
+static int pick_host(fi_epp* h, const PickCall& c) {
+  if (!h || bad_pick_args(c, true)) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  int rc = check_pick_handle(h, c);
+  if (rc != FI_OK || c.R == 0) return rc;
+  const uint32_t R = c.R;
   uint64_t total = 0;
-  int rc = check_batch(h, offsets, R, &total);
+  rc = check_batch(h, c.offsets, R, &total);
   if (rc != FI_OK) return rc;
-  rc = stage_inputs(h, prompts, offsets, h0, R, total, /*copy_prompts=*/false);  // run_pick feeds the prompts
+  PickCall d{h->d_prompts, h->d_offsets, h->d_h0, nullptr, nullptr, R, c.k, h->d_picks, nullptr};  // on device buffers
+  fi_pick* h_out = h->h_picks;
+  if (c.k) {
+    // the k-wide result buffers exist only on handles that rank; sized for max_batch so that R does not regrow them
+    const size_t need = (size_t)h->cfg.max_batch * h->P * c.k;
+    if (need > h->ranked.cap) FI_CUDA(cudaStreamSynchronize(h->s_main));
+    rc = grow_staging(h, h->ranked, need, need, true);
+    if (rc != FI_OK) return rc;
+    d.out = h->ranked.d;
+    h_out = h->ranked.h;
+  }
+  rc = stage_inputs(h, c.prompts, c.offsets, c.h0, R, total, /*copy_prompts=*/false);
   if (rc != FI_OK) return rc;
-  if (adapters) {
-    std::memcpy(h->h_adapters, adapters, (size_t)R * sizeof(uint64_t));
+  if (c.adapters) {
+    std::memcpy(h->h_adapters, c.adapters, (size_t)R * sizeof(uint64_t));
     FI_CUDA(cudaMemcpyAsync(h->d_adapters, h->h_adapters, (size_t)R * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main));
     h->stats.h2d_bytes += (size_t)R * sizeof(uint64_t);
+    d.adapters = h->d_adapters;
   }
-  const HostFeed feed{prompts, offsets};
-  rc = run_pick(h, h->d_prompts, h->d_offsets, h->d_h0, adapters ? h->d_adapters : nullptr, R, h->d_picks, &feed);
-  if (rc != FI_OK) return rc;
-  const size_t pb = (size_t)R * h->P * sizeof(fi_pick);
-  FI_CUDA(cudaMemcpyAsync(h->h_picks, h->d_picks, pb, cudaMemcpyDeviceToHost, h->s_main));
-  h->stats.d2h_bytes += pb;
-  if (chains_out) {
-    rc = copy_chains_out(h, chains_out, R, cudaMemcpyDeviceToHost, h->s_main);
+  if (c.subsets) {
+    // the bitset staging exists only on handles that restrict picks; sized for max_batch
+    const size_t pitch = (h->cfg.num_endpoints + 31) / 32, rows = (size_t)h->cfg.max_batch * pitch;
+    rc = grow_staging(h, h->subsets, rows, rows, true);
     if (rc != FI_OK) return rc;
+    const size_t sb = (size_t)R * pitch * sizeof(uint32_t);
+    std::memcpy(h->subsets.h, c.subsets, sb);
+    FI_CUDA(cudaMemcpyAsync(h->subsets.d, h->subsets.h, sb, cudaMemcpyHostToDevice, h->s_main));
+    h->stats.h2d_bytes += sb;
+    d.subsets = h->subsets.d;
   }
+  rc = run_pick(h, d, &c);
+  if (rc != FI_OK) return rc;
+  const size_t pb = (size_t)R * h->P * std::max(c.k, 1u) * sizeof(fi_pick);
+  FI_CUDA(cudaMemcpyAsync(h_out, d.out, pb, cudaMemcpyDeviceToHost, h->s_main));
+  h->stats.d2h_bytes += pb;
+  rc = copy_chains_out(h, h->d_chain, c.chains_out, R, cudaMemcpyDeviceToHost, h->s_main);
+  if (rc != FI_OK) return rc;
   FI_CUDA(cudaStreamSynchronize(h->s_main));
-  if (h->h_xerr && *h->h_xerr) {  // reported once; the tags are monotonic, so later steps can succeed again
+  if (h->h_xerr && *h->h_xerr) {  // (sharded) reported once; the tags are monotonic, so later steps can succeed again
     *h->h_xerr = 0;
     return fail(h, FI_ERR_COMM, "peer exchange timed out waiting for another rank");
   }
-  std::memcpy(out, h->h_picks, pb);
+  std::memcpy(c.out, h_out, pb);
   return FI_OK;
 }
 
-int fi_epp_pick_batch_device(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
-                             uint64_t total_prompt_bytes, void* d_out, void* d_chains_out, void* stream) {
-  return fi_epp_pick_batch_device_lora(h, d_prompts, d_offsets, d_h0, nullptr, R, total_prompt_bytes, d_out, d_chains_out,
-                                       stream);
-}
-
-int fi_epp_pick_batch_device_lora(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
-                                  const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, void* d_out,
-                                  void* d_chains_out, void* stream) {
-  if (!h || !d_offsets || (!d_h0 && R) || (!d_out && R)) return FI_ERR_INVALID;
+// Device buffers, in the caller's stream order.  The inputs stay where they are: no staging copy and no prompt-bytes
+// limit, so the entry points' total_prompt_bytes is not needed.
+static int pick_device(fi_epp* h, const PickCall& c, void* stream) {
+  if (!h || bad_pick_args(c, false)) return FI_ERR_INVALID;
   std::lock_guard<std::mutex> lk(h->mu);
-  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  if (R == 0) return FI_OK;
-  if (R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
-  (void)total_prompt_bytes;  // inputs stay where they are: no staging copy, no capacity limit
+  int rc = check_pick_handle(h, c);
+  if (rc != FI_OK || c.R == 0) return rc;
   cudaStream_t us = (cudaStream_t)stream;
   FI_CUDA(cudaEventRecord(h->ev_user, us));
   FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_user, 0));
-  int rc = run_pick(h, (const uint8_t*)d_prompts, (const uint64_t*)d_offsets, (const uint64_t*)d_h0,
-                    (const uint64_t*)d_adapters, R, (fi_pick*)d_out);
+  rc = run_pick(h, c, nullptr);
   if (rc != FI_OK) return rc;
-  if (d_chains_out) {
-    rc = copy_chains_out(h, (uint64_t*)d_chains_out, R, cudaMemcpyDeviceToDevice, h->s_main);
-    if (rc != FI_OK) return rc;
-  }
+  rc = copy_chains_out(h, h->d_chain, c.chains_out, c.R, cudaMemcpyDeviceToDevice, h->s_main);
+  if (rc != FI_OK) return rc;
   FI_CUDA(cudaEventRecord(h->ev_done, h->s_main));
   FI_CUDA(cudaStreamWaitEvent(us, h->ev_done, 0));
   return FI_OK;
 }
 
-// ---- ranked picks (docs/SPEC.md S.6a): run_pick with k > 0, which selects the RANKED match-kernel variant --------
-// Subset picks (S.5a) are ranked picks with per-request candidate bitsets, which select its SUBSET twin.  The bitsets
-// are pool-wide, so a handle over part of the pool cannot apply them (FI_ERR_STATE, like a sharded pool).
-static int check_subset_handle(fi_epp* h) {
-  if (h->world > 1 || h->cfg.endpoint_begin != 0 || h->cfg.endpoint_count != h->cfg.num_endpoints)
-    return fail(h, FI_ERR_STATE, "subset picks need a single handle over the whole pool");
-  return FI_OK;
-}
-
-static int pick_ranked_host(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
-                            const uint64_t* adapters, const uint32_t* subsets, uint32_t R, uint32_t k, fi_pick* out,
-                            uint64_t* chains_out) {
-  if (!h || !offsets || (!h0 && R) || !out || (!prompts && R && offsets[R])) return FI_ERR_INVALID;
-  if (k == 0 || k > FI_EPP_MAX_RANKED) return FI_ERR_INVALID;
-  std::lock_guard<std::mutex> lk(h->mu);
-  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  if (h->world > 1) return fail(h, FI_ERR_STATE, "ranked picks need a single-rank pool");
-  if (subsets) {
-    const int rs = check_subset_handle(h);
-    if (rs != FI_OK) return rs;
-  }
-  if (R == 0) return FI_OK;
-  uint64_t total = 0;
-  int rc = check_batch(h, offsets, R, &total);
-  if (rc != FI_OK) return rc;
-  // the k-wide result buffers exist only on handles that rank; sized for max_batch so that R does not regrow them
-  const size_t need = (size_t)h->cfg.max_batch * h->P * k;
-  if (need > h->ranked_cap) {
-    FI_CUDA(cudaStreamSynchronize(h->s_main));
-    cudaFree(h->d_ranked);
-    if (h->h_ranked) cudaFreeHost(h->h_ranked);
-    h->d_ranked = nullptr;
-    h->h_ranked = nullptr;
-    h->ranked_cap = 0;
-    if (cudaMalloc(&h->d_ranked, need * sizeof(fi_pick)) != cudaSuccess ||
-        cudaMallocHost(&h->h_ranked, need * sizeof(fi_pick)) != cudaSuccess) {
-      cudaGetLastError();
-      cudaFree(h->d_ranked);
-      if (h->h_ranked) cudaFreeHost(h->h_ranked);
-      h->d_ranked = nullptr;
-      h->h_ranked = nullptr;
-      return fail(h, FI_ERR_NOMEM, "cannot allocate the ranked pick buffers");
-    }
-    h->ranked_cap = need;
-  }
-  rc = stage_inputs(h, prompts, offsets, h0, R, total, /*copy_prompts=*/false);  // run_pick feeds the prompts
-  if (rc != FI_OK) return rc;
-  if (adapters) {
-    std::memcpy(h->h_adapters, adapters, (size_t)R * sizeof(uint64_t));
-    FI_CUDA(cudaMemcpyAsync(h->d_adapters, h->h_adapters, (size_t)R * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main));
-    h->stats.h2d_bytes += (size_t)R * sizeof(uint64_t);
-  }
-  if (subsets) {
-    // the bitset staging exists only on handles that restrict picks; sized for max_batch
-    const size_t pitch = (h->cfg.num_endpoints + 31) / 32;
-    if (!h->d_subsets) {
-      if (cudaMalloc(&h->d_subsets, (size_t)h->cfg.max_batch * pitch * sizeof(uint32_t)) != cudaSuccess ||
-          cudaMallocHost(&h->h_subsets, (size_t)h->cfg.max_batch * pitch * sizeof(uint32_t)) != cudaSuccess) {
-        cudaGetLastError();
-        cudaFree(h->d_subsets);
-        if (h->h_subsets) cudaFreeHost(h->h_subsets);
-        h->d_subsets = nullptr;
-        h->h_subsets = nullptr;
-        return fail(h, FI_ERR_NOMEM, "cannot allocate the subset staging buffers");
-      }
-    }
-    const size_t sb = (size_t)R * pitch * sizeof(uint32_t);
-    std::memcpy(h->h_subsets, subsets, sb);
-    FI_CUDA(cudaMemcpyAsync(h->d_subsets, h->h_subsets, sb, cudaMemcpyHostToDevice, h->s_main));
-    h->stats.h2d_bytes += sb;
-  }
-  const HostFeed feed{prompts, offsets};
-  rc = run_pick(h, h->d_prompts, h->d_offsets, h->d_h0, adapters ? h->d_adapters : nullptr, R, h->d_ranked, &feed, k,
-                subsets ? h->d_subsets : nullptr);
-  if (rc != FI_OK) return rc;
-  const size_t pb = (size_t)R * h->P * k * sizeof(fi_pick);
-  FI_CUDA(cudaMemcpyAsync(h->h_ranked, h->d_ranked, pb, cudaMemcpyDeviceToHost, h->s_main));
-  h->stats.d2h_bytes += pb;
-  if (chains_out) {
-    rc = copy_chains_out(h, chains_out, R, cudaMemcpyDeviceToHost, h->s_main);
-    if (rc != FI_OK) return rc;
-  }
-  FI_CUDA(cudaStreamSynchronize(h->s_main));
-  std::memcpy(out, h->h_ranked, pb);
-  return FI_OK;
-}
-
-static int pick_ranked_device(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
-                              const void* d_adapters, const void* d_subsets, uint32_t R, uint64_t total_prompt_bytes,
-                              uint32_t k, void* d_out, void* d_chains_out, void* stream) {
-  if (!h || !d_offsets || (!d_h0 && R) || !d_out) return FI_ERR_INVALID;
-  if (k == 0 || k > FI_EPP_MAX_RANKED) return FI_ERR_INVALID;
-  std::lock_guard<std::mutex> lk(h->mu);
-  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  if (h->world > 1) return fail(h, FI_ERR_STATE, "ranked picks need a single-rank pool");
-  if (d_subsets) {
-    const int rs = check_subset_handle(h);
-    if (rs != FI_OK) return rs;
-  }
-  if (R == 0) return FI_OK;
-  if (R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
-  (void)total_prompt_bytes;  // inputs stay where they are: no staging copy, no capacity limit
-  cudaStream_t us = (cudaStream_t)stream;
-  FI_CUDA(cudaEventRecord(h->ev_user, us));
-  FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_user, 0));
-  int rc = run_pick(h, (const uint8_t*)d_prompts, (const uint64_t*)d_offsets, (const uint64_t*)d_h0,
-                    (const uint64_t*)d_adapters, R, (fi_pick*)d_out, nullptr, k, (const uint32_t*)d_subsets);
-  if (rc != FI_OK) return rc;
-  if (d_chains_out) {
-    rc = copy_chains_out(h, (uint64_t*)d_chains_out, R, cudaMemcpyDeviceToDevice, h->s_main);
-    if (rc != FI_OK) return rc;
-  }
-  FI_CUDA(cudaEventRecord(h->ev_done, h->s_main));
-  FI_CUDA(cudaStreamWaitEvent(us, h->ev_done, 0));
-  return FI_OK;
-}
-
-int fi_epp_pick_batch_ranked(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
-                             const uint64_t* adapters, uint32_t R, uint32_t k, fi_pick* out, uint64_t* chains_out) {
-  return pick_ranked_host(h, prompts, offsets, h0, adapters, nullptr, R, k, out, chains_out);
-}
-
-int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
-                                    const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, uint32_t k,
-                                    void* d_out, void* d_chains_out, void* stream) {
-  return pick_ranked_device(h, d_prompts, d_offsets, d_h0, d_adapters, nullptr, R, total_prompt_bytes, k, d_out,
-                            d_chains_out, stream);
-}
-
-int fi_epp_pick_batch_subset(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
-                             const uint64_t* adapters, const uint32_t* subsets, uint32_t R, uint32_t k, fi_pick* out,
-                             uint64_t* chains_out) {
-  return pick_ranked_host(h, prompts, offsets, h0, adapters, subsets, R, k, out, chains_out);
-}
-
-int fi_epp_pick_batch_device_subset(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
-                                    const void* d_adapters, const void* d_subsets, uint32_t R,
-                                    uint64_t total_prompt_bytes, uint32_t k, void* d_out, void* d_chains_out,
-                                    void* stream) {
-  return pick_ranked_device(h, d_prompts, d_offsets, d_h0, d_adapters, d_subsets, R, total_prompt_bytes, k, d_out,
-                            d_chains_out, stream);
-}
-
-int fi_epp_pick_submit(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
-                       uint64_t total_prompt_bytes, void* d_out, void* stream) {
-  if (!h || !d_offsets || (!d_h0 && R) || (!d_out && R)) return FI_ERR_INVALID;
-  bool plain;
-  {
-    std::lock_guard<std::mutex> lk(h->mu);
-    plain = h->world > 1 || !h->fast_hash;  // sharded pools and odd block sizes: the stream-ordered path
-  }
-  uint64_t t = 0;
-  if (plain) {
-    const int rc = fi_epp_pick_batch_device(h, d_prompts, d_offsets, d_h0, R, total_prompt_bytes, d_out, nullptr, stream);
-    if (rc != FI_OK || R == 0) return rc;
-    std::lock_guard<std::mutex> lk(h->mu);
-    return issue_ticket(h, &t);  // the batch's number, as fi_epp_pick_submit_ex would have given it
-  }
-  std::lock_guard<std::mutex> lk(h->mu);
-  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  if (R == 0) return FI_OK;
-  if (R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
-  return submit_pick(h, (const uint8_t*)d_prompts, (const uint64_t*)d_offsets, (const uint64_t*)d_h0, R, (fi_pick*)d_out,
-                     (cudaStream_t)stream, &t);
-}
-
-// Pipelined submit of any pick variant (docs/SPEC.md S.9): the arguments, checks and output of the stream-ordered
-// counterpart (fi_epp_pick_batch_device_lora for k == 0, fi_epp_pick_batch_device_subset otherwise), with the staging
-// of fi_epp_pick_submit.  Handles that fi_epp_pick_submit serves stream-ordered run the counterpart itself.
-int fi_epp_pick_submit_ex(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, const void* d_adapters,
-                          const void* d_subsets, uint32_t R, uint64_t total_prompt_bytes, uint32_t k, void* d_out,
-                          void* d_chains_out, void* stream, uint64_t* ticket) {
-  if (!h || !d_offsets || (!d_h0 && R) || (!d_out && (R || k))) return FI_ERR_INVALID;
-  if (k > FI_EPP_MAX_RANKED || (k == 0 && d_subsets)) return FI_ERR_INVALID;
+// Pipelined submit (docs/SPEC.md S.9): the arguments, checks and output of pick_device, staged through submit_pick.
+// Handles that cannot pipeline (sharded pools, block sizes that are not a multiple of 32) run pick_device itself.  Either
+// way the batch takes the next ticket.  lagged: the index counters may lag (check_counters_lagged); ticket_empty: an
+// empty batch takes a ticket too.
+static int pick_submit(fi_epp* h, const PickCall& c, void* stream, uint64_t* ticket, bool lagged, bool ticket_empty) {
+  if (!h || bad_pick_args(c, false)) return FI_ERR_INVALID;
   bool plain;
   {
     std::lock_guard<std::mutex> lk(h->mu);
     plain = h->world > 1 || !h->fast_hash;
   }
   uint64_t t = 0;
+  int rc;
   if (plain) {
-    const int rc = k ? pick_ranked_device(h, d_prompts, d_offsets, d_h0, d_adapters, d_subsets, R, total_prompt_bytes, k,
-                                          d_out, d_chains_out, stream)
-                     : fi_epp_pick_batch_device_lora(h, d_prompts, d_offsets, d_h0, d_adapters, R, total_prompt_bytes,
-                                                     d_out, d_chains_out, stream);
-    if (rc != FI_OK) return rc;
+    rc = pick_device(h, c, stream);
+    if (rc != FI_OK || (c.R == 0 && !ticket_empty)) return rc;
     std::lock_guard<std::mutex> lk(h->mu);
-    const int rt = issue_ticket(h, &t);
-    if (rt == FI_OK && ticket) *ticket = t;
-    return rt;
-  }
-  std::lock_guard<std::mutex> lk(h->mu);
-  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  if (d_subsets) {
-    const int rs = check_subset_handle(h);
-    if (rs != FI_OK) return rs;
-  }
-  int rc = FI_OK;
-  if (R == 0) {
-    rc = issue_ticket(h, &t);  // an empty batch: complete once everything before it is
+    rc = issue_ticket(h, &t);  // the batch's number, as a pipelined submit would have given it
   } else {
-    if (R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
-    rc = submit_pick(h, (const uint8_t*)d_prompts, (const uint64_t*)d_offsets, (const uint64_t*)d_h0, R, (fi_pick*)d_out,
-                     (cudaStream_t)stream, &t, (const uint64_t*)d_adapters, k, (const uint32_t*)d_subsets,
-                     (uint64_t*)d_chains_out, /*lagged=*/true);
+    std::lock_guard<std::mutex> lk(h->mu);
+    rc = check_pick_handle(h, c);
+    if (rc != FI_OK || (c.R == 0 && !ticket_empty)) return rc;
+    // an empty batch is complete once everything before it is
+    rc = c.R ? submit_pick(h, c, (cudaStream_t)stream, &t, lagged) : issue_ticket(h, &t);
   }
   if (rc == FI_OK && ticket) *ticket = t;
   return rc;
+}
+
+int fi_epp_pick_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
+                      fi_pick* out, uint64_t* chains_out) {
+  return pick_host(h, PickCall{prompts, offsets, h0, nullptr, nullptr, R, 0, out, chains_out});
+}
+
+int fi_epp_pick_batch_lora(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
+                           const uint64_t* adapters, uint32_t R, fi_pick* out, uint64_t* chains_out) {
+  return pick_host(h, PickCall{prompts, offsets, h0, adapters, nullptr, R, 0, out, chains_out});
+}
+
+int fi_epp_pick_batch_device(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
+                             uint64_t total_prompt_bytes, void* d_out, void* d_chains_out, void* stream) {
+  return pick_device(h, device_call(d_prompts, d_offsets, d_h0, nullptr, nullptr, R, 0, d_out, d_chains_out), stream);
+}
+
+int fi_epp_pick_batch_device_lora(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                                  const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, void* d_out,
+                                  void* d_chains_out, void* stream) {
+  return pick_device(h, device_call(d_prompts, d_offsets, d_h0, d_adapters, nullptr, R, 0, d_out, d_chains_out), stream);
+}
+
+int fi_epp_pick_batch_ranked(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
+                             const uint64_t* adapters, uint32_t R, uint32_t k, fi_pick* out, uint64_t* chains_out) {
+  if (k == 0) return FI_ERR_INVALID;
+  return pick_host(h, PickCall{prompts, offsets, h0, adapters, nullptr, R, k, out, chains_out});
+}
+
+int fi_epp_pick_batch_device_ranked(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                                    const void* d_adapters, uint32_t R, uint64_t total_prompt_bytes, uint32_t k,
+                                    void* d_out, void* d_chains_out, void* stream) {
+  if (k == 0) return FI_ERR_INVALID;
+  return pick_device(h, device_call(d_prompts, d_offsets, d_h0, d_adapters, nullptr, R, k, d_out, d_chains_out), stream);
+}
+
+int fi_epp_pick_batch_subset(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
+                             const uint64_t* adapters, const uint32_t* subsets, uint32_t R, uint32_t k, fi_pick* out,
+                             uint64_t* chains_out) {
+  if (k == 0) return FI_ERR_INVALID;
+  return pick_host(h, PickCall{prompts, offsets, h0, adapters, subsets, R, k, out, chains_out});
+}
+
+int fi_epp_pick_batch_device_subset(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0,
+                                    const void* d_adapters, const void* d_subsets, uint32_t R,
+                                    uint64_t total_prompt_bytes, uint32_t k, void* d_out, void* d_chains_out,
+                                    void* stream) {
+  if (k == 0) return FI_ERR_INVALID;
+  return pick_device(h, device_call(d_prompts, d_offsets, d_h0, d_adapters, d_subsets, R, k, d_out, d_chains_out), stream);
+}
+
+int fi_epp_pick_submit(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
+                       uint64_t total_prompt_bytes, void* d_out, void* stream) {
+  return pick_submit(h, device_call(d_prompts, d_offsets, d_h0, nullptr, nullptr, R, 0, d_out, nullptr), stream, nullptr,
+                     /*lagged=*/false, /*ticket_empty=*/false);
+}
+
+int fi_epp_pick_submit_ex(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, const void* d_adapters,
+                          const void* d_subsets, uint32_t R, uint64_t total_prompt_bytes, uint32_t k, void* d_out,
+                          void* d_chains_out, void* stream, uint64_t* ticket) {
+  return pick_submit(h, device_call(d_prompts, d_offsets, d_h0, d_adapters, d_subsets, R, k, d_out, d_chains_out), stream,
+                     ticket, /*lagged=*/true, /*ticket_empty=*/true);
 }
 
 // The pipelined path always runs on the whole GPU: out = {0, 0, 0} (include/fi_epp.h).

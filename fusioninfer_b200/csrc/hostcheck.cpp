@@ -248,6 +248,48 @@ int fihc_lru_plan_check(uint32_t E, uint32_t cap, const uint32_t* endpoints, con
 // lru_touch_bound (lru_plan.h): the per-endpoint touches a sub-batch of fi_epp_index_add_submitted may carry
 uint32_t fihc_lru_touch_bound(uint32_t TS, uint32_t C) { return fi::lru_touch_bound(TS, C); }
 
+// The packed plan (lru_plan.h) read back the way the engine hands it to the LRU kernels: plan each batch with
+// lru_plan_batch, pack it with lru_plan_pack, and read every sub-batch's arrays through lru_plan_offsets.  They must
+// equal the LruPlan vectors, and the sub-batches' sections must cover the lru_plan_words packed words exactly once.
+// 0 if so, else a code; *subs = sub-batches in total.
+int fihc_lru_plan_pack_check(uint32_t E, const uint32_t* endpoints, const uint32_t* nblocks, uint32_t R, uint32_t batches,
+                             uint32_t plan_cap, uint64_t cap_touches, uint32_t cap_requests, uint32_t* subs) {
+  const uint32_t kGuard = 0xA5A5A5A5u;
+  fi::LruPlan pl;
+  uint32_t nsubs = 0;
+  for (uint32_t b = 0; b < batches; ++b) {
+    fi::lru_plan_batch(endpoints + (size_t)b * R, nblocks + (size_t)b * R, R, 0, E, plan_cap, cap_touches, cap_requests, &pl);
+    nsubs += (uint32_t)pl.subs.size();
+    const size_t words = fi::lru_plan_words(pl, E);
+    std::vector<uint32_t> packed(words + 1, kGuard);
+    fi::lru_plan_pack(pl, packed.data());
+    if (packed[words] != kGuard) return 1;  // wrote past the end
+    std::vector<uint32_t> seen(words, 0);
+    auto same = [&](size_t at, const uint32_t* want, size_t n) {
+      for (size_t i = 0; i < n; ++i) {
+        if (at + i >= words || packed[at + i] != want[i]) return false;
+        seen[at + i]++;
+      }
+      return true;
+    };
+    for (size_t sb = 0; sb < pl.subs.size(); ++sb) {
+      const uint32_t k0 = pl.subs[sb].k_begin, nk = pl.subs[sb].k_end - k0;
+      const fi::LruPlanOffsets o = fi::lru_plan_offsets(pl, E, sb);
+      if (!same(o.req_id, pl.req_id.data() + k0, nk)) return 2;
+      if (!same(o.req_ep, pl.req_ep.data() + k0, nk)) return 3;
+      if (!same(o.req_n, pl.req_n.data() + k0, nk)) return 4;
+      if (!same(o.req_off, pl.req_off.data() + k0, nk)) return 5;
+      if (!same(o.ep_list, pl.ep_list.data() + k0, nk)) return 6;
+      if (!same(o.ep_start, pl.ep_start.data() + sb * ((size_t)E + 1), (size_t)E + 1)) return 7;
+      if (!same(o.inc, pl.inc.data() + sb * (size_t)E, E)) return 8;
+    }
+    for (uint32_t s : seen)
+      if (s != 1) return 9;
+  }
+  if (subs) *subs = nsubs;
+  return 0;
+}
+
 // The device LRU's table occupancy under plans cut with lru_touch_bound: per endpoint, `used` (regular slots taken:
 // entries + tombstones) follows lru_maintain_kernel's rule before every sub-batch (kept if (used + min(add, C)) * 10
 // <= 6 TS, else rebuilt to the live entries), then every key the sub-batch touches that is not an entry takes a slot,

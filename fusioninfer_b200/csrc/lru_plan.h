@@ -17,6 +17,7 @@
 #pragma once
 #include <algorithm>
 #include <cstdint>
+#include <cstring>
 #include <vector>
 
 namespace fi {
@@ -107,6 +108,41 @@ inline void lru_plan_batch(const uint32_t* endpoints, const uint32_t* nblocks, u
     cur.k_end++;
   }
   close();
+}
+
+// The plan as the LRU kernels read it: one u32 array (one H2D copy per call), the vectors of LruPlan back to back,
+//   req_id[K] | req_ep[K] | req_n[K] | req_off[K] | ep_list[K] | ep_start[nsub][EL + 1] | inc[nsub][EL]
+inline size_t lru_plan_words(const LruPlan& p, uint32_t EL) {
+  return 5 * p.req_id.size() + p.subs.size() * ((size_t)2 * EL + 1);
+}
+
+// dst: lru_plan_words(p, EL) words (an empty plan writes none).  Packing the vectors back to back gives the layout
+// above because lru_plan_batch sizes ep_start [nsub][EL + 1] and inc [nsub][EL] (fihc_lru_plan_pack_check holds the
+// packer and lru_plan_offsets to each other).
+inline void lru_plan_pack(const LruPlan& p, uint32_t* dst) {
+  for (const std::vector<uint32_t>* v : {&p.req_id, &p.req_ep, &p.req_n, &p.req_off, &p.ep_list, &p.ep_start, &p.inc}) {
+    if (v->empty()) continue;
+    std::memcpy(dst, v->data(), v->size() * sizeof(uint32_t));
+    dst += v->size();
+  }
+}
+
+// where sub-batch sb's arrays start in the packed plan, in words
+struct LruPlanOffsets {
+  size_t req_id, req_ep, req_n, req_off, ep_list, ep_start, inc;
+};
+
+inline LruPlanOffsets lru_plan_offsets(const LruPlan& p, uint32_t EL, size_t sb) {
+  const size_t K = p.req_id.size(), nsub = p.subs.size(), k0 = p.subs[sb].k_begin;
+  LruPlanOffsets o;
+  o.req_id = k0;
+  o.req_ep = K + k0;
+  o.req_n = 2 * K + k0;
+  o.req_off = 3 * K + k0;
+  o.ep_list = 4 * K + k0;
+  o.ep_start = 5 * K + sb * ((size_t)EL + 1);
+  o.inc = 5 * K + nsub * ((size_t)EL + 1) + sb * EL;
+  return o;
 }
 
 }  // namespace fi

@@ -3,7 +3,8 @@
 Its sub-batches are cut with lru_touch_bound (lru_plan.h) so that the device LRU's touch kernel can never find a
 table full, which lets the call go without the overflow readback of fi_epp_index_add_chains.  Checked here through
 libfi_hostcheck.so: the bound against lru_maintain_kernel's thresholds and the insert limit on every table state, a
-model of the tables under random request streams, and the plans' equality with sequential Adds.
+model of the tables under random request streams, and the plans' equality with sequential Adds.  The packed layout
+both Add paths stage a plan in is read back the way the LRU kernels are handed it.
 """
 import ctypes as C
 import os
@@ -27,6 +28,9 @@ def hc():
     lib.fihc_lru_plan_check.restype = C.c_int
     lib.fihc_lru_plan_check.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32,
                                         C.c_uint32, C.c_uint32, C.c_uint64, C.c_uint32, C.c_void_p]
+    lib.fihc_lru_plan_pack_check.restype = C.c_int
+    lib.fihc_lru_plan_pack_check.argtypes = [C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32,
+                                             C.c_uint64, C.c_uint32, C.c_void_p]
     return lib
 
 
@@ -103,6 +107,30 @@ def test_plans_with_the_bound_equal_sequential_adds(hc, ts_mult, cap_touches, ca
                                 cap_touches, cap_requests, C.byref(subs))
     assert rc == 0
     assert subs.value >= 2
+
+
+# each case cuts its sub-batches on a different limit: touches per endpoint, touches, requests
+@pytest.mark.parametrize("plan_cap,cap_touches,cap_requests", [(40, 1 << 30, 1 << 30), (0xFFFFFFFF, 50, 1 << 30),
+                                                               (0xFFFFFFFF, 1 << 30, 9)])
+def test_packed_plan_reads_back_through_the_offsets(hc, plan_cap, cap_touches, cap_requests):
+    """the staging layout of a plan (lru_plan_pack) read back sub-batch by sub-batch through lru_plan_offsets, as the
+    LRU kernels are handed it: every array equals the plan's, and the sections tile the packed words"""
+    rng = np.random.default_rng(7)
+    E, R, pitch, batches = 5, 300, 30, 6
+    eps, _, nb = _stream(rng, E, R, pitch, batches, hot=0.5)
+    eps[eps == 4] = 0xFFFFFFFF  # FI_NO_ENDPOINT: skipped
+    eps[3, :] = 0xFFFFFFFF      # a batch with nothing to add: an empty plan
+
+    def check(plan_cap, cap_touches, cap_requests):
+        subs = C.c_uint32(0)
+        rc = hc.fihc_lru_plan_pack_check(E, eps.ctypes.data, nb.ctypes.data, R, batches, plan_cap, cap_touches,
+                                         cap_requests, C.byref(subs))
+        assert rc == 0
+        return subs.value
+
+    uncut = check(0xFFFFFFFF, 1 << 30, 1 << 30)  # one sub-batch per non-empty batch
+    assert uncut == batches - 1
+    assert check(plan_cap, cap_touches, cap_requests) > 4 * uncut
 
 
 def test_new_entry_points_are_declared_and_bound():
