@@ -14,8 +14,9 @@ HDRS := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/fi_epp.h
 
 RANKED_ORACLE := $(OBJDIR)/libepp_ranked_oracle.so
 SUBSET_ORACLE := $(OBJDIR)/libepp_subset_oracle.so
+CAPACITY_ORACLE := $(OBJDIR)/libepp_capacity_oracle.so
 
-all: $(LIB) $(HOSTCHECK) oracle $(RANKED_ORACLE) $(SUBSET_ORACLE)
+all: $(LIB) $(HOSTCHECK) oracle $(RANKED_ORACLE) $(SUBSET_ORACLE) $(CAPACITY_ORACLE)
 
 $(OBJDIR)/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -46,6 +47,11 @@ $(RANKED_ORACLE): tests/ranked_oracle.cpp oracle/epp_oracle.cpp include/fi_epp.h
 $(SUBSET_ORACLE): tests/subset_oracle.cpp oracle/epp_oracle.cpp include/fi_epp.h
 	@mkdir -p $(OBJDIR)
 	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ tests/subset_oracle.cpp
+
+# the CPU oracle plus per-endpoint LRU capacities (tests/capacity_oracle.cpp), test infrastructure only
+$(CAPACITY_ORACLE): tests/capacity_oracle.cpp oracle/epp_oracle.cpp include/fi_epp.h
+	@mkdir -p $(OBJDIR)
+	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ tests/capacity_oracle.cpp
 
 clean:
 	rm -rf $(OBJDIR) $(LIB) $(HOSTCHECK)

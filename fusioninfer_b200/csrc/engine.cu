@@ -239,6 +239,10 @@ struct fi_epp {
   unsigned long long* d_rm = nullptr;
   LruArena lru_arena;  // backing store of the LRUs (one huge-page mapping)
   std::vector<LruSet> lrus;
+  // [endpoint_count] every local endpoint's LRU capacity (fi_epp_set_lru_capacities; lru_capacity until set): the
+  // host copy of DevLru::cap and of the host LRU's limits, kept whichever LRU serves the handle
+  std::vector<uint32_t> lru_caps;
+  Staging<uint32_t> lru_resize;  // a device resize's rounds: local endpoints | eviction quotas
   std::unique_ptr<WorkerPool> pool;  // host LRU workers (fi_epp_index_add_chains), created on first use
   std::vector<WorkerOps> lru_outs;   // their op lists (capacity kept from batch to batch)
   bool verbose = false;              // FI_EPP_VERBOSE
@@ -250,7 +254,7 @@ struct fi_epp {
   bool dlru_ready = false;  // the device LRU's buffers are all there
   uint32_t lru_table_slots = 0;  // option "lru_table_slots": slots per endpoint table of the device LRU (0: sized by free HBM)
   DevLru dlru{};
-  uint32_t* d_lru_state = nullptr;           // head | tail | count | used | error
+  uint32_t* d_lru_state = nullptr;           // head | tail | count | used | error | cap
   unsigned long long* d_lru_ctr = nullptr;   // [0] SETs emitted, [1] endpoints maintained, [2] CLEARs of the running sub-batch,
                                              // [3] CLEARs total, [4] doomed winners
   struct LruHostStat {
@@ -736,7 +740,7 @@ int alloc_dev_lru(fi_epp* h) {
   const size_t scratch = (size_t)h->lru_touch_cap * (sizeof(uint32_t) + 3 * sizeof(fi_index_op));
   if (slot_bytes + log_bytes + scratch + (256u << 20) > free_b)
     return fail(h, FI_ERR_NOMEM, "device LRU does not fit in free HBM (option device_lru = 0 selects the host LRU)");
-  const size_t state_words = (size_t)7 * EL + 2;
+  const size_t state_words = (size_t)8 * EL + 2;
   FI_CUDA(cudaMalloc(&d.slots, slot_bytes));
   FI_CUDA(cudaMalloc(&d.log, log_bytes));
   FI_CUDA(cudaMalloc(&h->d_lru_state, state_words * sizeof(uint32_t)));
@@ -763,6 +767,10 @@ int alloc_dev_lru(fi_epp* h) {
   d.ovf = d.dcount + EL;
   d.any_ovf = d.ovf + EL;
   d.error = d.any_ovf + 1;
+  d.cap = d.error + 1;
+  // the capacities set so far (possibly before this first Add); pageable source: taken when the call returns
+  if (h->lru_caps.size() != EL) h->lru_caps.assign(EL, C);
+  FI_CUDA(cudaMemcpyAsync(d.cap, h->lru_caps.data(), (size_t)EL * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
   d.n_sets = h->d_lru_ctr;
   d.n_maintained = h->d_lru_ctr + 1;
   d.n_clears = h->d_lru_ctr + 3;
@@ -1056,6 +1064,92 @@ int lru_add_submitted(fi_epp* h, uint32_t slot, const uint32_t* endpoints, const
   h->padd_seq++;
   if (rc != FI_OK) return rc;
   if (e != cudaSuccess) return fail(h, FI_ERR_CUDA, cudaGetErrorString(e));
+  return FI_OK;
+}
+
+// fi_epp_set_lru_capacities on the device LRU: upload the new capacities `caps`, then evict the listed local endpoints
+// down to them and CLEAR the evicted pairs.  lru_shrink_kernel writes its CLEARs to the same buffer as an Add's
+// evictions (2 lru_touch_cap ops) and would drop any beyond it, while a shrink can evict far more (1 024 pods halved
+// from 31 250 entries: 16 M).  So the evictions run in ROUNDS of at most one buffer each, planned on the host from the
+// endpoints' entry counts (a control-plane readback, which waits for the index updates queued so far); an endpoint
+// with more evictions than a round takes is evicted part of the way per round, oldest first, so the rounds together
+// evict exactly what one pass would.  Only a lowered capacity can evict: without one there is no readback and nothing
+// blocks.  Everything that can fail without a CUDA error (the readback, the staging) happens before the capacities
+// reach the device, so a failed call leaves them as they were.  *evicted += entries evicted.
+int lru_device_resize(fi_epp* h, const std::vector<uint32_t>& local, const std::vector<uint32_t>& caps, uint64_t* evicted) {
+  const uint32_t EL = h->cfg.endpoint_count, lo = h->cfg.endpoint_begin;
+  bool lowered = false;
+  for (uint32_t e : local) lowered |= caps[e] < h->lru_caps[e];
+  std::vector<uint32_t> cnt;
+  if (lowered) {  // the entries every endpoint holds once the Adds queued so far have run
+    cnt.resize(EL);
+    FI_CUDA(cudaMemcpyAsync(cnt.data(), h->dlru.count, (size_t)EL * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index));
+    FI_CUDA(cudaStreamSynchronize(h->s_index));
+  }
+  // rounds: (endpoint, quota) pairs, at most clears_cap evictions per round; an endpoint is listed once per round
+  const uint64_t clears_cap = 2 * h->lru_touch_cap;
+  std::vector<uint32_t> r_eps, r_quota;
+  std::vector<size_t> r_begin{0};
+  std::vector<uint64_t> r_total;
+  uint64_t fill = 0;
+  for (uint32_t e : local) {
+    uint64_t over = lowered && cnt[e] > caps[e] ? cnt[e] - caps[e] : 0;
+    while (over) {
+      const uint64_t take = std::min(over, clears_cap - fill);
+      r_eps.push_back(e);
+      r_quota.push_back((uint32_t)take);
+      fill += take;
+      over -= take;
+      *evicted += take;
+      if (fill == clears_cap) {
+        r_begin.push_back(r_eps.size());
+        r_total.push_back(fill);
+        fill = 0;
+      }
+    }
+  }
+  if (fill) {
+    r_begin.push_back(r_eps.size());
+    r_total.push_back(fill);
+  }
+  const size_t pairs = r_eps.size();
+  if (pairs) {
+    // (the previous resize's copy out of the pinned buffer is done: the readback above synchronised s_index)
+    int rc = grow_staging(h, h->lru_resize, 2 * pairs, 2 * pairs, true);
+    if (rc != FI_OK) return rc;
+    std::memcpy(h->lru_resize.h, r_eps.data(), pairs * sizeof(uint32_t));
+    std::memcpy(h->lru_resize.h + pairs, r_quota.data(), pairs * sizeof(uint32_t));
+  }
+  // picks called before this one must not see its evictions
+  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
+  // (pageable source: the copy has taken the data when cudaMemcpyAsync returns)
+  FI_CUDA(cudaMemcpyAsync(h->dlru.cap, caps.data(), (size_t)EL * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+  h->stats.h2d_bytes += (size_t)EL * sizeof(uint32_t);
+  if (pairs) {
+    FI_CUDA(cudaMemcpyAsync(h->lru_resize.d, h->lru_resize.h, 2 * pairs * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+    h->stats.h2d_bytes += 2 * pairs * sizeof(uint32_t);
+  }
+  const GossipLog glog = gossip_log(h);
+  for (size_t k = 0; k < r_total.size(); ++k) {
+    const size_t b = r_begin[k];
+    const uint32_t n = (uint32_t)(r_begin[k + 1] - b);
+    FI_CUDA(cudaMemsetAsync(h->d_lru_ctr + 2, 0, sizeof(unsigned long long), h->s_index));
+    {
+      LaunchScope ls(h, h->s_index, K_INDEX);
+      FI_CUDA(launch_lru_shrink(h->dlru, h->lru_resize.d + b, h->lru_resize.d + pairs + b, n, h->d_lru_clears, h->d_lru_ctr + 2,
+                                clears_cap, lo, h->s_index));
+    }
+    LaunchScope ls(h, h->s_index, K_INDEX);
+    FI_CUDA(launch_index_clear_counted(h->ix, h->d_ctr, h->d_lru_clears, r_total[k], h->d_lru_ctr + 2, lo, EL, h->rank, glog,
+                                       h->s_index));
+  }
+  int rc = lru_refresh_stat(h);
+  if (rc != FI_OK) return rc;
+  // the CLEARs' tombstones reach the rebuild decision of the next index update
+  FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));  // covers the status copy too
+  h->ctr_pending = true;
+  FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
   return FI_OK;
 }
 
@@ -1693,6 +1787,7 @@ void fi_epp_destroy(fi_epp* h) {
   free_dev_lru(h);
   h->lru_plan_buf.release();
   h->lru_chains.release();
+  h->lru_resize.release();
   free_index(h->ix);
   free_index(h->ix_spare);
   for (int b = 0; b < 2; ++b) {
@@ -1843,6 +1938,7 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
     // virtual reservation only: an endpoint's tables become resident when it is first touched
     LruArena* arena = h->lru_arena.reserve((size_t)cfg->endpoint_count * LruSet::bytes_needed(cfg->lru_capacity)) ? &h->lru_arena : nullptr;
     h->lrus = std::vector<LruSet>(cfg->endpoint_count, LruSet(cfg->lru_capacity, arena));
+    h->lru_caps.assign(cfg->endpoint_count, cfg->lru_capacity);
   }
 
   // endpoints + score tables
@@ -2041,6 +2137,70 @@ int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t
     FI_CUDA(cudaMemcpyAsync(&c, h->d_rm, sizeof(c), cudaMemcpyDeviceToHost, h->s_index));
     FI_CUDA(cudaStreamSynchronize(h->s_index));
     *pairs_removed = c;
+  }
+  return FI_OK;
+}
+
+// Per-endpoint LRU capacities (SPEC S.2b; upstream's autoTune).  The listed endpoints' LRUs evict their least recently
+// used keys down to the new capacities, each evicted pair CLEARed as an eviction inside an Add would be; later Adds
+// evict against them.  Ordered like fi_epp_index_apply: behind the ops staged so far and the picks called so far,
+// ahead of every later pick.  The host LRU's limits are set whichever LRU serves the handle (before the first Add it
+// is not chosen yet, and both are empty then); the device LRU reads h->lru_caps when it is allocated.
+int fi_epp_set_lru_capacities(fi_epp* h, const uint32_t* endpoints, const uint32_t* capacities, uint32_t n,
+                              uint64_t* entries_evicted) {
+  if (!h || ((!endpoints || !capacities) && n)) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  if (entries_evicted) *entries_evicted = 0;
+  const uint32_t C = h->cfg.lru_capacity;
+  if (!C) return fail(h, FI_ERR_STATE, "lru_capacity is 0: no LRU to size");
+  for (uint32_t i = 0; i < n; ++i) {
+    if (endpoints[i] >= h->cfg.num_endpoints) return fail(h, FI_ERR_INVALID, "endpoint out of range");
+    if (capacities[i] > C) return fail(h, FI_ERR_INVALID, "LRU capacity above lru_capacity");
+    if (capacities[i] && capacities[i] < h->cfg.max_blocks) return fail(h, FI_ERR_INVALID, "LRU capacity below max_blocks");
+  }
+  if (h->world > 1) return fail(h, FI_ERR_STATE, "sharded pool: fi_epp_set_lru_capacities needs a single-rank handle");
+  const uint32_t lo = h->cfg.endpoint_begin, EL = h->cfg.endpoint_count;
+  std::vector<uint32_t> caps = h->lru_caps;
+  std::vector<uint32_t> local;  // distinct local endpoints listed
+  std::vector<uint8_t> listed(EL, 0);
+  for (uint32_t i = 0; i < n; ++i) {
+    const uint32_t e = endpoints[i] - lo;
+    if (e >= EL) continue;  // another rank's shard
+    caps[e] = capacities[i] ? capacities[i] : C;  // the last entry wins
+    if (!listed[e]) {
+      listed[e] = 1;
+      local.push_back(e);
+    }
+  }
+  if (local.empty()) return FI_OK;
+  int rc = flush_ops(h);  // staged SET / CLEAR groups and host-LRU deltas go first
+  if (rc != FI_OK) return rc;
+  rc = check_counters(h);
+  if (rc != FI_OK) return rc;
+  uint64_t evicted = 0;
+  if (h->lru_mode == 1 && h->dlru_ready) {
+    rc = lru_device_resize(h, local, caps, &evicted);
+    if (rc != FI_OK) return rc;
+  }
+  // host LRU: the evictions are staged like the deltas of an Add (fi_epp_index_apply's ordering); the sets of a
+  // device-LRU handle are empty and only take the limit
+  for (uint32_t e : local) {
+    rc = FI_OK;
+    h->lrus[e].shrink(caps[e], [&](uint64_t key) {
+      if (rc == FI_OK) rc = submit_op(h, key, lo + e, FI_OP_CLEAR);
+      ++evicted;
+    });
+    if (rc != FI_OK) return rc;
+  }
+  h->lru_caps.swap(caps);
+  if (entries_evicted) {
+    rc = flush_ops(h);
+    if (rc != FI_OK) return rc;
+    FI_CUDA(cudaStreamSynchronize(h->s_index));
+    rc = check_counters(h);  // (a broken device-LRU invariant would show here)
+    if (rc != FI_OK) return rc;
+    *entries_evicted = evicted;
   }
   return FI_OK;
 }

@@ -118,6 +118,62 @@ void fihc_lru_touch(void* l, const uint64_t* keys, uint32_t n, uint8_t* inserted
   }
 }
 
+// LruSet::shrink: set the limit, write the evicted keys (oldest first, at most cap); returns how many were evicted
+uint32_t fihc_lru_shrink(void* l, uint32_t limit, uint64_t* evicted, uint32_t cap) {
+  uint32_t n = 0;
+  ((fi::LruSet*)l)->shrink(limit, [&](uint64_t k) {
+    if (n < cap) evicted[n] = k;
+    ++n;
+  });
+  return n;
+}
+uint32_t fihc_lru_limit(void* l) { return ((fi::LruSet*)l)->limit(); }
+// the keys, least recently used first (at most cap written); returns the size
+uint32_t fihc_lru_dump(void* l, uint64_t* out, uint32_t cap) {
+  uint32_t n = 0;
+  ((fi::LruSet*)l)->for_each_oldest_first([&](uint64_t k) {
+    if (n < cap) out[n] = k;
+    ++n;
+  });
+  return n;
+}
+
+// A pool of host LRUs with per-endpoint limits, walked batch by batch with lru_walk_batch (fi_epp_index_add_chains'
+// host phase) and resized with LruSet::shrink (fi_epp_set_lru_capacities): tests/test_lru_capacity_cpu.py drives it
+// against a sequential model.
+struct HcLruPool {
+  std::vector<fi::LruSet> lrus;
+  fi::WorkerPool pool;
+  std::vector<fi::WorkerOps> outs;
+  HcLruPool(uint32_t E, uint32_t cap, uint32_t workers) : lrus(E, fi::LruSet(cap)), pool(workers) {}
+};
+void* fihc_lrupool_new(uint32_t E, uint32_t cap, uint32_t workers) { return new HcLruPool(E, cap, workers); }
+void fihc_lrupool_free(void* p) { delete (HcLruPool*)p; }
+uint32_t fihc_lrupool_shrink(void* p, uint32_t e, uint32_t limit, uint64_t* evicted, uint32_t cap) {
+  return fihc_lru_shrink(&((HcLruPool*)p)->lrus[e], limit, evicted, cap);
+}
+uint32_t fihc_lrupool_dump(void* p, uint32_t e, uint64_t* out, uint32_t cap) {
+  return fihc_lru_dump(&((HcLruPool*)p)->lrus[e], out, cap);
+}
+// one batch of Adds; the ops in the order the engine applies them (segment by segment, a segment's SETs before its
+// CLEARs), at most cap written; returns how many there are
+uint64_t fihc_lrupool_walk(void* p, const uint32_t* endpoints, const uint64_t* chains, uint32_t pitch, const uint32_t* nblocks,
+                           uint32_t R, fi_index_op* ops, uint64_t cap) {
+  HcLruPool& hp = *(HcLruPool*)p;
+  const size_t nseg = fi::lru_walk_batch(hp.lrus, 0, (uint32_t)hp.lrus.size(), endpoints, chains, pitch, nblocks, R, hp.pool, hp.outs);
+  uint64_t n = 0;
+  for (size_t s = 0; s < nseg; ++s)
+    for (int kind = 0; kind < 2; ++kind)
+      for (auto& o : hp.outs) {
+        if (s >= o.nseg) continue;
+        for (const fi_index_op& op : kind == 0 ? o.sets[s] : o.clears[s]) {
+          if (n < cap) ops[n] = op;
+          ++n;
+        }
+      }
+  return n;
+}
+
 // fi_epp_index_add_chains' host phase (lru_batch.h) against the sequential definition: walk the batch on
 // `workers` threads, apply the resulting ops segment by segment (all SETs of a segment, then all its CLEARs — the
 // way the GPU applies a group) to a membership set, and compare that set and the LRU contents with one LRU per

@@ -72,8 +72,8 @@ class LruArena {
 // endpoints are walked by different threads at the same time (false sharing otherwise).
 class alignas(128) LruSet {
  public:
-  explicit LruSet(uint32_t capacity = 0, LruArena* arena = nullptr) : cap_(capacity), arena_(arena) {}
-  LruSet(const LruSet& o) : cap_(o.cap_), arena_(o.arena_) {}  // copies are made only of fresh, empty sets
+  explicit LruSet(uint32_t capacity = 0, LruArena* arena = nullptr) : cap_(capacity), limit_(capacity), arena_(arena) {}
+  LruSet(const LruSet& o) : cap_(o.cap_), limit_(o.limit_), arena_(o.arena_) {}  // copies are made only of fresh, empty sets
   LruSet& operator=(const LruSet&) = delete;
   ~LruSet() {
     if (owned_) std::free(owned_);
@@ -86,6 +86,8 @@ class alignas(128) LruSet {
 
   uint32_t size() const { return size_; }
   uint32_t capacity() const { return cap_; }
+  // the run-time capacity (fi_epp_set_lru_capacities): at most `capacity`, the size the memory is cut for
+  uint32_t limit() const { return limit_; }
 
   // Touch `key`.  Returns true if it was newly inserted; *evicted/ *did_evict
   // report the key pushed out to make room.
@@ -99,7 +101,7 @@ class alignas(128) LruSet {
       return false;
     }
     uint32_t node;
-    if (size_ == cap_) {  // evict the tail, reuse its node
+    if (size_ >= limit_) {  // evict the tail, reuse its node
       node = tail_;
       *evicted = nodes_[node].key;
       *did_evict = true;
@@ -113,8 +115,11 @@ class alignas(128) LruSet {
         const uint32_t t2 = nodes_[tail_].prev;
         if (t2 != kNone) prefetch_slot(nodes_[t2].key);
       }
+    } else if (free_ != kNone) {  // a node a shrink gave back
+      node = free_;
+      free_ = nodes_[node].next;
     } else {
-      node = size_;  // nodes are handed out densely until full
+      node = fresh_++;  // nodes are handed out densely until full
     }
     nodes_[node].key = key;
     link_front(node);
@@ -153,6 +158,31 @@ class alignas(128) LruSet {
     for (uint64_t i = 0; i <= mask_; ++i) map_[i] = Slot{0, kNone, 0};
     size_ = 0;
     head_ = tail_ = kNone;
+    free_ = kNone;
+    fresh_ = 0;
+  }
+
+  // Set the run-time capacity to `limit` (<= capacity()) and evict the least recently used keys until the set holds
+  // at most `limit`: emit(key) for each, oldest first, as touch reports an eviction.  Raising the limit evicts nothing.
+  template <class Emit>
+  void shrink(uint32_t limit, Emit&& emit) {
+    limit_ = limit < cap_ ? limit : cap_;
+    while (size_ > limit_) {
+      const uint32_t node = tail_;
+      const uint64_t key = nodes_[node].key;
+      unlink(node);
+      map_erase(key);
+      nodes_[node].next = free_;
+      free_ = node;
+      --size_;
+      emit(key);
+    }
+  }
+
+  // the keys, least recently used first (diagnostics)
+  template <class Visit>
+  void for_each_oldest_first(Visit&& visit) const {
+    for (uint32_t n = tail_; n != kNone; n = nodes_[n].prev) visit(nodes_[n].key);
   }
 
  private:
@@ -231,8 +261,11 @@ class alignas(128) LruSet {
   }
 
   uint32_t cap_;
+  uint32_t limit_;
   uint32_t size_ = 0;
   uint32_t head_ = kNone, tail_ = kNone;
+  uint32_t free_ = kNone;  // nodes given back by shrink, linked through `next`
+  uint32_t fresh_ = 0;     // nodes [fresh_, cap_) have never been handed out
   uint32_t mask_ = 0;
   Node* nodes_ = nullptr;
   Slot* map_ = nullptr;

@@ -7,7 +7,8 @@
 // resulting membership changes to its own op lists.  The GPU applies a group of ops as "all SETs, then all
 // CLEARs"; that equals the sequential order except when a hash is re-added after its own eviction inside the same
 // batch — then the endpoint's later ops go to the next SEGMENT (segments are applied one after the other), which
-// keeps "last op wins" exact.  Host-only code (no CUDA): tests/test_host_logic.py runs it against a sequential LRU.
+// keeps "last op wins" exact.  Every set evicts against its own limit() (fi_epp_set_lru_capacities).  Host-only
+// code (no CUDA): tests/test_host_logic.py and tests/test_lru_capacity_cpu.py run it against a sequential LRU.
 #pragma once
 #include <algorithm>
 #include <atomic>

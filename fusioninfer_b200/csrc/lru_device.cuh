@@ -25,6 +25,8 @@ struct DevLru {
   uint32_t* ovf;    // [EL] the running sub-batch would overfill this endpoint's table: its requests are deferred
   uint32_t* any_ovf; // some ovf[e] was set by the running touch kernel
   uint32_t* error;  // != 0: an invariant broke (reported by the next host call)
+  uint32_t* cap;    // [EL] the endpoint's LRU capacity (fi_epp_set_lru_capacities), in [max_blocks, capacity]: what
+                    // the LRU holds.  Table and log room are sized and bounded by the uniform `capacity`.
   unsigned long long* n_sets;        // totals (fi_epp_index_stats, fi_epp_lru_counters): SETs emitted,
   unsigned long long* n_clears;      // CLEARs emitted,
   unsigned long long* n_doomed;      // winners that were gone again by the end of their sub-batch,
@@ -59,6 +61,10 @@ cudaError_t launch_lru_append(const DevLru& lru, const LruBatch& b, fi_index_op*
                               uint64_t clears_cap, uint32_t ep_begin, cudaStream_t s);
 cudaError_t launch_lru_evict(const DevLru& lru, fi_index_op* clears, unsigned long long* n_clears, uint64_t clears_cap,
                              uint32_t ep_begin, cudaStream_t s);
+// one round of a resize (fi_epp_set_lru_capacities): evict the quota[i] least recently used entries of local endpoint
+// eps[i] for i < n (device arrays; the host plans the quotas so that a round's CLEARs fit clears_cap)
+cudaError_t launch_lru_shrink(const DevLru& lru, const uint32_t* eps, const uint32_t* quota, uint32_t n, fi_index_op* clears,
+                              unsigned long long* n_clears, uint64_t clears_cap, uint32_t ep_begin, cudaStream_t s);
 // empty the LRUs of the n local endpoints eps[0..n) (device array; n <= 65535)
 cudaError_t launch_lru_reset(const DevLru& lru, const uint32_t* eps, uint32_t n, cudaStream_t s);
 // diagnostics: the live keys of local endpoint e, least recently used first

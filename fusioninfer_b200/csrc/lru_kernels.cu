@@ -22,6 +22,13 @@
 // sub-batches of at most C touches, which always fit (lru_plan.h; endpoints are independent of each other, so
 // deferring one is exact).
 //
+// Per-endpoint capacities (fi_epp_set_lru_capacities, SPEC S.2b).  Endpoint e's LRU holds at most cap[e] <= C keys:
+// scan (`kept`), append (`doomed_below`) and evict (their target) read cap[e], and the exactness argument above holds
+// for each endpoint with its own cap[e].  Everything that bounds room in the table or the log (maintain's `addc`,
+// lru_touch_bound, the conservative pass, the sizes of L and TS) stays on the uniform C: every per-endpoint quantity
+// it bounds is at most the same quantity with C.  A resize evicts with lru_shrink_kernel, in rounds whose CLEARs
+// fit the buffer (engine.cu).
+//
 // Per endpoint e (all in HBM):
 //   table  [TS + 2] LruSlot   open-addressed, linear probing, key → (log position + 1, order of its last touch
 //                             in the running sub-batch).  Slots TS / TS+1 belong to the hashes 0 / ~0 (the
@@ -43,7 +50,7 @@
 //   scan      per endpoint, requests in order: log position of each request's first winner; new head
 //   append    surviving winners write their log record, point the table at it, emit SET if the key was new;
 //             doomed winners leave the table (CLEAR if they were entries before)
-//   evict     endpoints above capacity: walk the log from the tail, evict the oldest live records, emit CLEAR
+//   evict     endpoints above cap[e]: walk the log from the tail, evict the oldest live records, emit CLEAR
 #include "kernels.cuh"
 #include "lru_device.cuh"
 
@@ -232,8 +239,8 @@ __global__ void __launch_bounds__(256) lru_scan_kernel(DevLru lru, LruBatch b) {
     running += __shfl_sync(0xFFFFFFFFu, inc, 31);
   }
   if (lane == 0) {
-    const uint32_t head = lru.head[e];
-    const uint32_t kept = running < lru.capacity ? running : lru.capacity;  // the doomed winners get no record
+    const uint32_t head = lru.head[e], ce = lru.cap[e];
+    const uint32_t kept = running < ce ? running : ce;  // the doomed winners get no record
     lru.hold[e] = head;
     lru.dcount[e] = running;
     if ((uint64_t)head + kept > lru.L) atomicExch(lru.error, 2u);  // cannot happen: maintenance runs first
@@ -250,8 +257,8 @@ __global__ void __launch_bounds__(256) lru_append_kernel(DevLru lru, LruBatch b,
   uint64_t* log = lru.log + (uint64_t)e * lru.L;
   const uint64_t* chain = b.chains + (uint64_t)b.req_id[k] * b.pitch;
   const bool deferred = lru.ovf[e] != 0;
-  const uint32_t D = lru.dcount[e], hold = lru.hold[e];
-  const uint32_t doomed_below = D > lru.capacity ? D - lru.capacity : 0;  // winners of rank < this are gone again
+  const uint32_t D = lru.dcount[e], hold = lru.hold[e], ce = lru.cap[e];
+  const uint32_t doomed_below = D > ce ? D - ce : 0;  // winners of rank < this are gone again
   uint32_t at = b.base[k];  // rank of this request's next winner among the endpoint's winners
   uint32_t fresh = 0, lost = 0, doomed = 0;
   for (uint32_t j0 = 0; j0 < n; j0 += blockDim.x) {  // uniform trip count: block-wide barriers inside
@@ -320,13 +327,11 @@ __global__ void __launch_bounds__(256) lru_append_kernel(DevLru lru, LruBatch b,
   }
 }
 
-// ---- evict: one CTA per endpoint above capacity ------------------------------------------------------
-__global__ void __launch_bounds__(kWideCta) lru_evict_kernel(DevLru lru, fi_index_op* clears, unsigned long long* n_clears,
-                                                        uint64_t clears_cap, uint32_t ep_begin) {
-  const uint32_t e = blockIdx.x;
+// ---- evict: the `want` oldest entries of endpoint e, by the whole CTA -------------------------------------
+__device__ __forceinline__ void lru_evict_oldest(const DevLru& lru, uint32_t e, uint32_t want, fi_index_op* clears,
+                                                 unsigned long long* n_clears, uint64_t clears_cap, uint32_t ep_begin) {
   const uint32_t cnt = lru.count[e];
-  if (cnt <= lru.capacity) return;
-  uint32_t need = cnt - lru.capacity;
+  uint32_t need = want;
   LruSlot* tab = lru.slots + (uint64_t)e * (lru.TS + 2);
   const uint64_t* log = lru.log + (uint64_t)e * lru.L;
   const uint32_t head = lru.head[e];
@@ -365,9 +370,27 @@ __global__ void __launch_bounds__(kWideCta) lru_evict_kernel(DevLru lru, fi_inde
   if (threadIdx.x == 0) {
     if (need) atomicExch(lru.error, 3u);  // fewer live records than entries: cannot happen
     lru.tail[e] = t < head ? t : head;
-    lru.count[e] = lru.capacity + need;
-    atomicAdd(lru.n_clears, (unsigned long long)(cnt - lru.capacity - need));
+    lru.count[e] = cnt - (want - need);
+    atomicAdd(lru.n_clears, (unsigned long long)(want - need));
   }
+}
+
+// one CTA per endpoint: those above their capacity after a sub-batch's appends
+__global__ void __launch_bounds__(kWideCta) lru_evict_kernel(DevLru lru, fi_index_op* clears, unsigned long long* n_clears,
+                                                        uint64_t clears_cap, uint32_t ep_begin) {
+  const uint32_t e = blockIdx.x;
+  const uint32_t cnt = lru.count[e], ce = lru.cap[e];
+  if (cnt <= ce) return;
+  lru_evict_oldest(lru, e, cnt - ce, clears, n_clears, clears_cap, ep_begin);
+}
+
+// one CTA per listed endpoint: one round of a resize, quota[i] evictions of endpoint eps[i]
+__global__ void __launch_bounds__(kWideCta) lru_shrink_kernel(DevLru lru, const uint32_t* __restrict__ eps,
+                                                         const uint32_t* __restrict__ quota, fi_index_op* clears,
+                                                         unsigned long long* n_clears, uint64_t clears_cap, uint32_t ep_begin) {
+  const uint32_t want = quota[blockIdx.x];
+  if (want == 0) return;
+  lru_evict_oldest(lru, eps[blockIdx.x], want, clears, n_clears, clears_cap, ep_begin);
 }
 
 // ---- maintain: compact the log, rebuild the table -------------------------------------------------------
@@ -511,6 +534,12 @@ cudaError_t launch_lru_append(const DevLru& lru, const LruBatch& b, fi_index_op*
 cudaError_t launch_lru_evict(const DevLru& lru, fi_index_op* clears, unsigned long long* n_clears, uint64_t clears_cap,
                              uint32_t ep_begin, cudaStream_t s) {
   lru_evict_kernel<<<lru.EL, kWideCta, 0, s>>>(lru, clears, n_clears, clears_cap, ep_begin);
+  return cudaGetLastError();
+}
+cudaError_t launch_lru_shrink(const DevLru& lru, const uint32_t* eps, const uint32_t* quota, uint32_t n, fi_index_op* clears,
+                              unsigned long long* n_clears, uint64_t clears_cap, uint32_t ep_begin, cudaStream_t s) {
+  if (n == 0) return cudaSuccess;
+  lru_shrink_kernel<<<n, kWideCta, 0, s>>>(lru, eps, quota, clears, n_clears, clears_cap, ep_begin);
   return cudaGetLastError();
 }
 cudaError_t launch_lru_reset(const DevLru& lru, const uint32_t* eps, uint32_t n, cudaStream_t s) {

@@ -33,6 +33,9 @@ namespace fi {
 //   add <= C:  calm <= limit, and C + add <= 2 C <= limit (TS >= 4 C): always;
 //   add > C:   add <= limit - calm + C (table kept) and add <= limit - C (table rebuilt).
 // The bound is the smaller of the two, >= 2 C since TS >= 4 C, so every chain (at most C blocks) fits.
+// C is the uniform lru_capacity even when endpoints have capacities of their own (fi_epp_set_lru_capacities): every
+// c_e <= C, and the argument only uses C as an upper bound on an endpoint's entries (count <= c_e <= C after a
+// rebuild), so it holds unchanged.  Resize evictions only turn entries into tombstones, which `used` already counts.
 inline uint32_t lru_touch_bound(uint32_t TS, uint32_t C) {
   const uint64_t limit = (uint64_t)TS * 85 / 100, calm = (uint64_t)TS * 6 / 10;
   return (uint32_t)std::min<uint64_t>(limit - calm + C, limit - C);

@@ -203,6 +203,21 @@ class EndpointPicker:
                     "fi_epp_index_remove_endpoints")
         return out.value if count else None
 
+    def set_lru_capacities(self, endpoints, capacities, want_evicted: bool = False) -> Optional[int]:
+        """Per-endpoint LRU capacities (upstream autoTune: a pod's LRU sized from its KV-cache block count).
+        capacities[i] is endpoints[i]'s new capacity, 0 meaning lru_capacity; an LRU above its new capacity evicts its
+        least recently used keys (and their index pairs) down to it.  Ordered like index_apply.  want_evicted=True
+        blocks until the evictions are applied and returns how many LRU entries were evicted."""
+        eps = np.ascontiguousarray(np.atleast_1d(np.asarray(endpoints, dtype=np.uint32)))
+        caps = np.ascontiguousarray(np.atleast_1d(np.asarray(capacities, dtype=np.uint32)))
+        if len(caps) != len(eps):
+            raise ValueError("endpoints and capacities differ in length")
+        out = C.c_uint64(0)
+        self._check(self._lib.fi_epp_set_lru_capacities(self._h, _ptr(eps), _ptr(caps), len(eps),
+                                                        C.byref(out) if want_evicted else None),
+                    "fi_epp_set_lru_capacities")
+        return out.value if want_evicted else None
+
     def index_add_chain(self, endpoint: int, hashes: np.ndarray):
         hashes = np.ascontiguousarray(hashes, dtype=np.uint64)
         self._check(

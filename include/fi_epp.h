@@ -27,6 +27,8 @@
  *   prefix indexer.Add / LRU eviction (PreRequest)  → fi_epp_index_add_chains (a batch
  *                                                     of decisions), fi_epp_index_add_chain,
  *                                                     fi_epp_index_apply
+ *   prefix autoTune (LRU sized per pod from its     → fi_epp_set_lru_capacities
+ *   KV-cache block count)
  *   datastore pod metrics refresh (kv, queue, role) → fi_epp_endpoints_update
  *   SchedulerProfile.Run: filter → scorers → picker → fi_epp_pick_batch
  *   pd-profile-handler (decode then prefill)        → fi_epp_pick_batch with
@@ -281,9 +283,27 @@ int fi_epp_index_apply(fi_epp* h, const fi_index_op* ops, uint64_t n);
  * applied); FI_ERR_STATE on a sharded pool. */
 int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t n, uint64_t* pairs_removed);
 
+/* Per-endpoint LRU capacities (docs/SPEC.md S.2b; upstream's autoTune sizes a pod's LRU from the KV-cache blocks the
+ * pod reports).  Every endpoint's LRU capacity starts at lru_capacity; this sets it to capacities[i] for endpoints[i]
+ * (0 = lru_capacity; the last entry of an endpoint listed twice wins).  An LRU that holds more keys than its new
+ * capacity evicts its least recently used ones down to it, and each evicted (endpoint, hash) pair leaves the index,
+ * as an eviction inside an Add does; raising a capacity evicts nothing.  Every later Add (fi_epp_index_add_submitted
+ * of an earlier ticket included) evicts against the new capacity.  fi_epp_index_remove_endpoints empties an LRU but
+ * keeps its capacity.  Ordered like fi_epp_index_apply: ops and removals submitted before the call are applied first,
+ * picks called before it (in-flight fi_epp_pick_submit batches included) do not see its evictions, every later pick
+ * does.  Asynchronous, except that a call which LOWERS a capacity on a handle served by the device LRU blocks: it
+ * reads back the LRUs' entry counts to plan its evictions, and so waits for the index updates queued before it (and
+ * for the picks those wait for).  Endpoints of other shards are ignored; n = 0 is a no-op.  entries_evicted != NULL:
+ * block until applied and write how many LRU entries were evicted.  Errors apply nothing: FI_ERR_INVALID if an
+ * endpoint is >= num_endpoints, a capacity is above lru_capacity, or a non-zero capacity is below max_blocks;
+ * FI_ERR_STATE if lru_capacity is 0 or the pool is sharded.  Capacities set before the first Add apply to whichever
+ * LRU (device or host) serves the handle. */
+int fi_epp_set_lru_capacities(fi_epp* h, const uint32_t* endpoints, const uint32_t* capacities, uint32_t n,
+                              uint64_t* entries_evicted);
+
 /* Upstream indexer.Add(hashes, pod): touch each hash in `endpoint`'s LRU
- * (capacity lru_capacity), emit SET for new entries and CLEAR for evicted
- * ones.  Requires lru_capacity > 0.  Single-rank handles only (FI_ERR_STATE on a sharded pool). */
+ * (capacity lru_capacity, or the endpoint's own from fi_epp_set_lru_capacities), emit SET for new entries and CLEAR
+ * for evicted ones.  Requires lru_capacity > 0.  Single-rank handles only (FI_ERR_STATE on a sharded pool). */
 int fi_epp_index_add_chain(fi_epp* h, uint32_t endpoint, const uint64_t* hashes, uint32_t n);
 
 /* The same for a whole batch of routing decisions — upstream's PreRequest step after a pick batch:
