@@ -28,6 +28,7 @@
 #include <sched.h>
 
 #include "../../include/fi_epp.h"
+#include "cuda_owned.h"
 #include "kernels.cuh"
 #include "lru.h"
 #include "lru_batch.h"
@@ -129,19 +130,77 @@ unsigned usable_cores() {
 // A device staging buffer and its pinned host mirror (h stays null for a device-only buffer), grown by grow_staging
 template <typename T>
 struct Staging {
-  T* d = nullptr;
-  T* h = nullptr;
+  DevPtr<T> d;
+  PinnedPtr<T> h;
   size_t cap = 0;  // elements
-  void release() {
-    cudaFree(d);
-    if (h) cudaFreeHost(h);
-    *this = Staging{};
+};
+
+// The six arrays behind one IndexView, and the view (filled by alloc_index)
+struct IndexTables {
+  IndexView v{};
+  DevPtr<uint64_t> keys, klog;
+  DevPtr<uint32_t> node_of, rows, cnt, rmask;
+};
+
+// The device-resident LRU of a handle (lru_kernels.cu), allocated whole by ensure_dev_lru at the first Add
+struct DevLruStore {
+  DevLru v{};  // points into slots, log, state and ctr
+  DevPtr<LruSlot> slots;
+  DevPtr<uint64_t> log;
+  DevPtr<uint32_t> state;             // head | tail | count | used | hold | dcount | ovf | any_ovf | error | cap
+  DevPtr<unsigned long long> ctr;     // [0] SETs emitted, [1] endpoints maintained, [2] CLEARs of the running sub-batch,
+                                      // [3] CLEARs total, [4] doomed winners
+  struct HostStat {
+    uint32_t error, any_ovf;  // (any_ovf: the touch kernel's overflow flag of the running sub-batch)
+    unsigned long long n_sets, n_maintained, n_clears_cur, n_clears, n_doomed;
+    uint32_t planned_ovf;     // the touch kernel's overflow flag after a fi_epp_index_add_submitted call (must stay 0)
+  };
+  PinnedPtr<HostStat> stat;           // pinned copy, refreshed after every call
+  // per-sub-batch scratch, for touch_cap touches
+  DevPtr<uint32_t> slot_of, wcount, base;
+  DevPtr<fi_index_op> sets, clears;
+  uint64_t touch_cap = 0;
+  Event ev;                           // the previous call's staging has been consumed
+  Event ev_ovf;                       // the touch kernel's overflow flag has reached the host
+};
+
+// Sharded mode (fi_epp_comm_init): the communicator and the buffers of the cross-rank merge and directory gossip
+struct ShardState {
+  ncclComm_t comm = nullptr;
+  DevPtr<fi_pick> d_local;   // [R][P] this rank's picks
+  DevPtr<fi_pick> d_gather;  // [world][R][P]
+  // directory gossip (index_kernels.cu): this rank's transition log of the current round and the buffers the ranks'
+  // logs are gathered into
+  DevPtr<unsigned long long> d_glog_n;  // [2] appear / vanish counts
+  DevPtr<uint64_t> d_glog_a;            // [kOpChunk]
+  DevPtr<uint64_t> d_glog_v;            // [kOpChunk]
+  DevPtr<unsigned long long> d_ghdr;    // [world + 1][2] gathered counts
+  PinnedPtr<unsigned long long> h_ghdr; // pinned copy
+  DevPtr<uint64_t> d_ggather;           // [world][kOpChunk]
+  // peer-memory exchange (kernels.cuh PeerXchg)
+  DevPtr<uint8_t> d_xchg;               // this rank's exchange buffer
+  PinnedPtr<volatile uint32_t> h_xerr;  // poll-timeout flag of the exchange (mapped pinned host word the kernels set)
+  void* peer_ipc[FI_MAX_RANKS] = {};    // mappings opened with cudaIpcOpenMemHandle
+  ~ShardState() {
+    for (void* m : peer_ipc)
+      if (m) cudaIpcCloseMemHandle(m);
+    if (comm) g_nccl.CommDestroy(comm);
   }
 };
 
 }  // namespace
 
 struct fi_epp {
+  // declared first so that they are destroyed last, after every buffer and event the work on them used
+  Stream s_main, s_index;  // compute; index maintenance (side stream)
+  // host-buffer picks feed the prompts in slices: the copy engine runs ahead on s_copy while s_main hashes,
+  // walks and matches the slices that have landed (the step is PCIe-bound: only the last slice's work is exposed)
+  Stream s_copy;
+  // Pipelined device path (fi_epp_pick_submit / fi_epp_pick_wait): stage A (block hashing + chain walk) of
+  // batch k+1 runs on s_a while stage B (match + pick) of batch k runs on s_main; the chain / block-count
+  // buffers are double-buffered (slot = batch parity).
+  Stream s_a;
+
   fi_epp_config cfg;
   std::mutex mu;
   std::string err;
@@ -151,92 +210,69 @@ struct fi_epp {
   uint32_t P = 0;   // profiles
   bool fast_hash = false;
 
-  cudaStream_t s_main = nullptr, s_index = nullptr;  // compute; index maintenance (side stream)
-  // host-buffer picks feed the prompts in slices: the copy engine runs ahead on s_copy while s_main hashes,
-  // walks and matches the slices that have landed (the step is PCIe-bound: only the last slice's work is exposed)
-  cudaStream_t s_copy = nullptr;
   static constexpr int kMaxFeedSlices = 16;
-  cudaEvent_t ev_copy[kMaxFeedSlices] = {};
+  Event ev_copy[kMaxFeedSlices];
   uint32_t feed_slices = 8;  // FI_EPP_FEED_SLICES (1: one copy, then the whole batch)
-  // Pipelined device path (fi_epp_pick_submit / fi_epp_pick_wait): stage A (block hashing + chain walk) of
-  // batch k+1 runs on s_a while stage B (match + pick) of batch k runs on s_main; the chain / block-count
-  // buffers are double-buffered (slot = batch parity).
-  cudaStream_t s_a = nullptr;
-  uint64_t* d_chain2 = nullptr;
-  uint32_t* d_nblocks2 = nullptr;
-  cudaEvent_t ev_in = nullptr, ev_a[2] = {}, ev_b[2] = {};
-  cudaEvent_t ev_pick = nullptr;   // completion of the most recent pick of any kind (recorded on s_main)
-  cudaEvent_t ev_plain = nullptr;  // completion of the most recent stream-ordered (not pipelined) pick
+  // slot 1's chain and block-count buffers, allocated together by the first pipelined submit that needs them
+  DevPtr<uint64_t> d_chain2;
+  DevPtr<uint32_t> d_nblocks2;
+  Event ev_in, ev_a[2], ev_b[2];
+  Event ev_pick;   // completion of the most recent pick of any kind (recorded on s_main)
+  Event ev_plain;  // completion of the most recent stream-ordered (not pipelined) pick
   uint64_t pipe_seq = 0;          // batches submitted
   // Tickets (fi_epp_pick_submit_ex / fi_epp_pick_wait_batch / fi_epp_index_add_submitted): every submit, pipelined or
   // not, takes the next number; ev_ticket[t % kTicketRing] is recorded on s_main when batch t is complete.
   static constexpr int kTicketRing = 8;
-  cudaEvent_t ev_ticket[kTicketRing] = {};
+  Event ev_ticket[kTicketRing];
   uint64_t tickets = 0;
   uint64_t slot_ticket[2] = {~0ull, ~0ull};  // ticket whose chains slot s still holds (~0: none)
   uint32_t slot_R[2] = {0, 0};
-  cudaEvent_t ev_slot_read[2] = {};          // the last copy of slot s's chains for fi_epp_index_add_submitted
-  cudaEvent_t ev_index = nullptr, ev_user = nullptr, ev_done = nullptr, ev_ctr = nullptr;
+  Event ev_slot_read[2];          // the last copy of slot s's chains for fi_epp_index_add_submitted
+  Event ev_index, ev_user, ev_done, ev_ctr;
 
   // request buffers (device)
-  uint8_t* d_prompts = nullptr;
-  uint64_t* d_offsets = nullptr;
-  uint64_t* d_h0 = nullptr;
-  uint64_t* d_chain = nullptr;
-  uint32_t* d_nblocks = nullptr;
-  fi_pick* d_picks = nullptr;   // [R][P] final
+  DevPtr<uint8_t> d_prompts;
+  DevPtr<uint64_t> d_offsets;
+  DevPtr<uint64_t> d_h0;
+  DevPtr<uint64_t> d_chain;
+  DevPtr<uint32_t> d_nblocks;
+  DevPtr<fi_pick> d_picks;      // [R][P] final
   Staging<fi_pick> ranked;      // [R][P][k] of the host ranked pick: allocated by the first such call, grown with k
   Staging<uint32_t> subsets;    // [max_batch][ceil(E/32)] staging of fi_epp_pick_batch_subset: allocated by its first call
-  fi_pick* d_local = nullptr;   // [R][P] this rank's picks (sharded)
-  fi_pick* d_gather = nullptr;  // [world][R][P]
-  // peer-memory exchange (sharded mode; kernels.cuh PeerXchg)
+  std::unique_ptr<ShardState> shard;  // sharded mode only
   PeerXchg px{};                 // px.enabled == 0: NCCL all-gathers are used
-  uint8_t* d_xchg = nullptr;     // this rank's exchange buffer
-  volatile uint32_t* h_xerr = nullptr;  // poll-timeout flag of the exchange (mapped pinned host word the kernels set)
-  void* peer_ipc[FI_MAX_RANKS] = {};  // mappings opened with cudaIpcOpenMemHandle (closed in destroy)
   // sharded mode: every rank hashes every prompt (the default: hashing 16 KiB from local HBM is expected to cost
   // less than receiving 2 KiB of chain over NVLink; not measured on H100s, bench.py --gpus N times both); FI_EPP_SHARD_HASH=
   // split / option "shard_hash" = 1: every rank hashes R/world requests and the chains are all-gathered
   bool split_hash = false;
   uint32_t chain_rows = 0;  // rows allocated in d_chain / d_nblocks (max_batch padded for the gather)
-  // sharded mode: directory gossip (index_kernels.cu): this rank's transition log of the current round and the
-  // buffers the ranks' logs are gathered into
-  unsigned long long* d_glog_n = nullptr;  // [2] appear / vanish counts
-  uint64_t* d_glog_a = nullptr;            // [kOpChunk]
-  uint64_t* d_glog_v = nullptr;            // [kOpChunk]
-  unsigned long long* d_ghdr = nullptr;    // [world][2] gathered counts
-  unsigned long long* h_ghdr = nullptr;    // pinned copy
-  uint64_t* d_ggather = nullptr;           // [world][kOpChunk]
-  unsigned long long* d_probed = nullptr;
-  uint32_t* d_work = nullptr;  // [16] dynamic work-queue counters of in-flight match launches
+  DevPtr<unsigned long long> d_probed;
+  DevPtr<uint32_t> d_work;  // [16] dynamic work-queue counters of in-flight match launches
   // pinned host mirrors
-  fi_pick* h_picks = nullptr;
-  uint64_t* h_offsets = nullptr;
-  uint64_t* h_h0 = nullptr;
-  uint32_t* h_nblocks = nullptr;
+  PinnedPtr<fi_pick> h_picks;
+  PinnedPtr<uint64_t> h_offsets;
+  PinnedPtr<uint64_t> h_h0;
+  PinnedPtr<uint32_t> h_nblocks;
 
   // index
-  IndexView ix{};
-  IndexView ix_spare{};  // rebuild target, allocated at the first rebuild and reused alternately
-  bool spare_ready = false;
-  IndexCounters* d_ctr = nullptr;
-  IndexCounters* h_ctr = nullptr;  // pinned
+  IndexTables ix;
+  std::unique_ptr<IndexTables> ix_spare;  // rebuild target, allocated at the first rebuild and reused alternately
+  DevPtr<IndexCounters> d_ctr;
+  PinnedPtr<IndexCounters> h_ctr;
   bool ctr_pending = false;
   // the last counters read (`used`) and how many new keys the updates queued since then can add at most (one per
   // SET or LRU touch): check_counters_lagged decides from these when the pending counters are not in yet
   uint64_t ctr_used_known = 0, ctr_unchecked = 0;
   uint64_t rebuilds = 0, ops_applied = 0;
-  fi_index_op* h_sets[2] = {nullptr, nullptr};
-  fi_index_op* h_clears[2] = {nullptr, nullptr};
-  fi_index_op* d_sets[2] = {nullptr, nullptr};
-  fi_index_op* d_clears[2] = {nullptr, nullptr};
-  cudaEvent_t ev_buf[2] = {nullptr, nullptr};
+  PinnedPtr<fi_index_op> h_sets[2], h_clears[2];
+  DevPtr<fi_index_op> d_sets[2], d_clears[2];
+  Event ev_buf[2];
   int cur_buf = 0;
   uint64_t n_sets = 0, n_clears = 0;
   std::unordered_set<PairKey, PairHash> cleared;
   // fi_epp_index_remove_endpoints: [0] pairs removed, then (u32) the local endpoints whose device LRU is reset.
   // Allocated at the first call.
-  unsigned long long* d_rm = nullptr;
+  DevPtr<unsigned long long> d_rm;
   LruArena lru_arena;  // backing store of the LRUs (one huge-page mapping)
   std::vector<LruSet> lrus;
   // [endpoint_count] every local endpoint's LRU capacity (fi_epp_set_lru_capacities; lru_capacity until set): the
@@ -251,34 +287,20 @@ struct fi_epp {
   // the two are never mixed on one handle.
   int lru_mode = -1;  // -1: not chosen yet, 0: host LRU, 1: device LRU
   int lru_want = -1;  // option / environment override (-1: automatic)
-  bool dlru_ready = false;  // the device LRU's buffers are all there
   uint32_t lru_table_slots = 0;  // option "lru_table_slots": slots per endpoint table of the device LRU (0: sized by free HBM)
-  DevLru dlru{};
-  uint32_t* d_lru_state = nullptr;           // head | tail | count | used | error | cap
-  unsigned long long* d_lru_ctr = nullptr;   // [0] SETs emitted, [1] endpoints maintained, [2] CLEARs of the running sub-batch,
-                                             // [3] CLEARs total, [4] doomed winners
-  struct LruHostStat {
-    uint32_t error, any_ovf;  // (any_ovf: the touch kernel's overflow flag of the running sub-batch)
-    unsigned long long n_sets, n_maintained, n_clears_cur, n_clears, n_doomed;
-    uint32_t planned_ovf;     // the touch kernel's overflow flag after a fi_epp_index_add_submitted call (must stay 0)
-  };
-  // fi_epp_index_add_submitted: double-buffered plan and chain staging (Add j uses padd[j & 1]; ev_done: consumed)
+  std::unique_ptr<DevLruStore> dlru;  // null until the first device-LRU Add
+  // fi_epp_index_add_submitted: double-buffered plan and chain staging (Add j uses padd[j & 1]; ev_done: consumed).
+  // d_chains and ev_done are allocated together by the buffer's first Add.
   struct PipeAdd {
-    Staging<uint32_t> plan;        // the packed plan (lru_plan.h)
-    uint64_t* d_chains = nullptr;  // [max_batch][MP]
-    cudaEvent_t ev_done = nullptr;
+    Staging<uint32_t> plan;      // the packed plan (lru_plan.h)
+    DevPtr<uint64_t> d_chains;   // [max_batch][MP]
+    Event ev_done;
   };
   PipeAdd padd[2];
   uint64_t padd_seq = 0;
   uint64_t lru_deferred = 0, lru_sub_batches = 0;  // host-side totals
-  LruHostStat* h_lru_stat = nullptr;         // pinned copy, refreshed after every call
   Staging<uint32_t> lru_plan_buf;            // the packed plan of the current call (lru_plan.h)
-  uint32_t *d_lru_slot_of = nullptr, *d_lru_wcount = nullptr, *d_lru_base = nullptr;
-  fi_index_op *d_lru_sets = nullptr, *d_lru_clears = nullptr;
-  uint64_t lru_touch_cap = 0;                // touches per sub-batch the scratch arrays hold
   Staging<uint64_t> lru_chains;              // staging of host chains (device only)
-  cudaEvent_t ev_lru = nullptr;              // the previous call's staging has been consumed
-  cudaEvent_t ev_lru_ovf = nullptr;          // the touch kernel's overflow flag has reached the host
   uint32_t last_plain_R = 0;                 // rows of d_chain the most recent stream-ordered pick wrote
   LruPlan lru_plan;
   unsigned lru_threads = 0;          // 0: FI_EPP_LRU_THREADS, else min(usable cores, 64)
@@ -286,20 +308,19 @@ struct fi_epp {
   // endpoints / score tables
   std::vector<EndpointDev> eps;  // global pool
   bool eps_dirty = true;
-  EndpointDev* d_eps = nullptr;
-  double* d_sc = nullptr;
-  uint32_t* d_elig = nullptr;
-  ZeroBest* d_zero = nullptr;
-  uint32_t* d_ztie = nullptr;
+  DevPtr<EndpointDev> d_eps;
+  DevPtr<double> d_sc;
+  DevPtr<uint32_t> d_elig;
+  DevPtr<ZeroBest> d_zero;
+  DevPtr<uint32_t> d_ztie;
   std::vector<LoraDev> lora;   // local endpoints' adapter residency (lora-affinity-scorer)
   bool lora_dirty = false;
-  LoraDev* d_lora = nullptr;
-  uint64_t* d_adapters = nullptr;  // staging of the host path's per-request adapter ids
-  uint64_t* h_adapters = nullptr;  // pinned
+  DevPtr<LoraDev> d_lora;
+  DevPtr<uint64_t> d_adapters;    // staging of the host path's per-request adapter ids
+  PinnedPtr<uint64_t> h_adapters;
   ScoreTables st{};
 
-  // multi-GPU
-  ncclComm_t comm = nullptr;
+  // multi-GPU (fi_epp_comm_init)
   uint32_t rank = 0, world = 1;
 
   // stats / profiling
@@ -307,13 +328,13 @@ struct fi_epp {
   bool profiling = false;
   bool tracing = false;       // FI_EPP_TRACE=<call index>: print that call's kernel timeline to stderr
   long trace_call = -1;
-  cudaEvent_t ev_trace0 = nullptr;
+  Event ev_trace0;
   struct Ev {
-    cudaEvent_t a, b;
+    Event a, b;
     int kind;
   };
   std::vector<Ev> pending_ev;
-  std::vector<cudaEvent_t> ev_pool;
+  std::vector<Event> ev_pool;
 };
 
 namespace {
@@ -337,25 +358,25 @@ int fail(fi_epp* h, int code, const std::string& m) {
 template <typename T>
 int grow_staging(fi_epp* h, Staging<T>& s, size_t n, size_t alloc, bool pinned) {
   if (n <= s.cap) return FI_OK;
-  s.release();
-  if (cudaMalloc(&s.d, alloc * sizeof(T)) != cudaSuccess ||
-      (pinned && cudaMallocHost(&s.h, alloc * sizeof(T)) != cudaSuccess)) {
+  s = Staging<T>{};
+  Staging<T> t;
+  if (cuda_alloc(t.d, alloc) != cudaSuccess || (pinned && cuda_alloc(t.h, alloc) != cudaSuccess)) {
     cudaGetLastError();
-    s.release();
     return fail(h, FI_ERR_NOMEM, "cannot allocate a staging buffer of " + std::to_string(alloc * sizeof(T)) + " bytes");
   }
-  s.cap = alloc;
+  t.cap = alloc;
+  s = std::move(t);
   return FI_OK;
 }
 
-cudaEvent_t get_event(fi_epp* h) {
+Event get_event(fi_epp* h) {
+  Event e;
   if (!h->ev_pool.empty()) {
-    cudaEvent_t e = h->ev_pool.back();
+    e = std::move(h->ev_pool.back());
     h->ev_pool.pop_back();
-    return e;
+  } else {
+    cuda_create(e, cudaEventDefault);
   }
-  cudaEvent_t e = nullptr;
-  cudaEventCreate(&e);
   return e;
 }
 
@@ -364,19 +385,19 @@ struct LaunchScope {
   fi_epp* h;
   cudaStream_t s;
   int kind;
-  cudaEvent_t a = nullptr, b = nullptr;
+  Event a, b;
   LaunchScope(fi_epp* h_, cudaStream_t s_, int kind_) : h(h_), s(s_), kind(kind_) {
     h->stats.kernel_launches++;
     if (h->profiling || h->tracing) {
       a = get_event(h);
       b = get_event(h);
-      cudaEventRecord(a, s);
+      cudaEventRecord(a.get(), s);
     }
   }
   ~LaunchScope() {
     if (h->profiling || h->tracing) {
-      cudaEventRecord(b, s);
-      h->pending_ev.push_back({a, b, kind});
+      cudaEventRecord(b.get(), s);
+      h->pending_ev.push_back({std::move(a), std::move(b), kind});
     }
   }
 };
@@ -384,7 +405,7 @@ struct LaunchScope {
 void drain_profile(fi_epp* h) {
   for (auto& e : h->pending_ev) {
     float ms = 0.f;
-    if (cudaEventSynchronize(e.b) == cudaSuccess && cudaEventElapsedTime(&ms, e.a, e.b) == cudaSuccess) {
+    if (cudaEventSynchronize(e.b.get()) == cudaSuccess && cudaEventElapsedTime(&ms, e.a.get(), e.b.get()) == cudaSuccess) {
       switch (e.kind) {
         case K_HASH: h->stats.ms_hash_blocks += ms; h->stats.n_hash_blocks++; break;
         case K_MATCH: h->stats.ms_match_pick += ms; h->stats.n_match_pick++; break;
@@ -392,25 +413,10 @@ void drain_profile(fi_epp* h) {
         default: h->stats.ms_other += ms; h->stats.n_other++; break;
       }
     }
-    h->ev_pool.push_back(e.a);
-    h->ev_pool.push_back(e.b);
+    h->ev_pool.push_back(std::move(e.a));
+    h->ev_pool.push_back(std::move(e.b));
   }
   h->pending_ev.clear();
-}
-
-void free_index(IndexView& v) {
-  cudaFree(v.keys);
-  cudaFree(v.node_of);
-  cudaFree(v.klog);
-  cudaFree(v.rows);
-  cudaFree(v.cnt);
-  cudaFree(v.rmask);
-  v.keys = nullptr;
-  v.node_of = nullptr;
-  v.klog = nullptr;
-  v.rows = nullptr;
-  v.cnt = nullptr;
-  v.rmask = nullptr;
 }
 
 size_t index_bytes(uint64_t slots, uint32_t W) {
@@ -421,17 +427,19 @@ size_t index_bytes(uint64_t slots, uint32_t W) {
 // queue the clears that make `v` an empty index (on the index stream)
 int clear_index(fi_epp* h, IndexView& v) {
   const uint64_t total = v.C + 3;
-  FI_CUDA(cudaMemsetAsync(v.keys, 0, total * sizeof(uint64_t), h->s_index));
-  FI_CUDA(cudaMemsetAsync(v.node_of, 0xFF, total * sizeof(uint32_t), h->s_index));  // NODE_INVALID
-  FI_CUDA(cudaMemsetAsync(v.klog, 0, total * sizeof(uint64_t), h->s_index));
-  FI_CUDA(cudaMemsetAsync(v.rows, 0, total * v.W * sizeof(uint32_t), h->s_index));
-  FI_CUDA(cudaMemsetAsync(v.cnt, 0, total * sizeof(uint32_t), h->s_index));
-  FI_CUDA(cudaMemsetAsync(v.rmask, 0, total * sizeof(uint32_t), h->s_index));
+  FI_CUDA(cudaMemsetAsync(v.keys, 0, total * sizeof(uint64_t), h->s_index.get()));
+  FI_CUDA(cudaMemsetAsync(v.node_of, 0xFF, total * sizeof(uint32_t), h->s_index.get()));  // NODE_INVALID
+  FI_CUDA(cudaMemsetAsync(v.klog, 0, total * sizeof(uint64_t), h->s_index.get()));
+  FI_CUDA(cudaMemsetAsync(v.rows, 0, total * v.W * sizeof(uint32_t), h->s_index.get()));
+  FI_CUDA(cudaMemsetAsync(v.cnt, 0, total * sizeof(uint32_t), h->s_index.get()));
+  FI_CUDA(cudaMemsetAsync(v.rmask, 0, total * sizeof(uint32_t), h->s_index.get()));
   return FI_OK;
 }
 
-int alloc_index(fi_epp* h, uint64_t slots, IndexView* out) {
-  IndexView v{};
+// empty index tables of `slots` slots into `out`, which is left as it was on failure
+int alloc_index(fi_epp* h, uint64_t slots, IndexTables& out) {
+  IndexTables t;
+  IndexView& v = t.v;
   v.C = slots;
   v.bmask = slots / BUCKET_KEYS - 1;
   v.W = h->W;
@@ -444,24 +452,26 @@ int alloc_index(fi_epp* h, uint64_t slots, IndexView* out) {
              std::to_string(free_b >> 20) + " MiB of free device memory";
     return FI_ERR_NOMEM;
   }
-  cudaError_t e = cudaMalloc(&v.keys, total * sizeof(uint64_t));
-  if (e == cudaSuccess) e = cudaMalloc(&v.node_of, total * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&v.klog, total * sizeof(uint64_t));
-  if (e == cudaSuccess) e = cudaMalloc(&v.rows, total * v.W * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&v.cnt, total * sizeof(uint32_t));
-  if (e == cudaSuccess) e = cudaMalloc(&v.rmask, total * sizeof(uint32_t));
-  if (e != cudaSuccess) {  // nothing of a partial view survives
+  cudaError_t e = cuda_alloc(t.keys, total);
+  if (e == cudaSuccess) e = cuda_alloc(t.node_of, total);
+  if (e == cudaSuccess) e = cuda_alloc(t.klog, total);
+  if (e == cudaSuccess) e = cuda_alloc(t.rows, total * v.W);
+  if (e == cudaSuccess) e = cuda_alloc(t.cnt, total);
+  if (e == cudaSuccess) e = cuda_alloc(t.rmask, total);
+  if (e != cudaSuccess) {
     cudaGetLastError();
-    free_index(v);
     h->err = std::string("index allocation: ") + cudaGetErrorString(e);
     return e == cudaErrorMemoryAllocation ? FI_ERR_NOMEM : FI_ERR_CUDA;
   }
+  v.keys = t.keys.get();
+  v.node_of = t.node_of.get();
+  v.klog = t.klog.get();
+  v.rows = t.rows.get();
+  v.cnt = t.cnt.get();
+  v.rmask = t.rmask.get();
   int rc = clear_index(h, v);
-  if (rc != FI_OK) {
-    free_index(v);
-    return rc;
-  }
-  *out = v;
+  if (rc != FI_OK) return rc;
+  out = std::move(t);
   return FI_OK;
 }
 
@@ -471,20 +481,21 @@ int alloc_index(fi_epp* h, uint64_t slots, IndexView* out) {
 // before the NEXT rebuild, and that one is ordered behind them (flush_ops makes s_index wait for ev_pick).
 // The spare is allocated once, at the first rebuild (the only point where memory doubles), and then reused.
 int rebuild_index(fi_epp* h) {
-  if (!h->spare_ready) {
-    int rc = alloc_index(h, h->ix.C, &h->ix_spare);  // clears it too
+  if (!h->ix_spare) {
+    auto spare = std::make_unique<IndexTables>();
+    int rc = alloc_index(h, h->ix.v.C, *spare);  // clears it too
     if (rc != FI_OK) return rc;
-    h->spare_ready = true;
+    h->ix_spare = std::move(spare);
   } else {
-    int rc = clear_index(h, h->ix_spare);
+    int rc = clear_index(h, h->ix_spare->v);
     if (rc != FI_OK) return rc;
   }
-  FI_CUDA(cudaMemsetAsync(h->d_ctr, 0, sizeof(IndexCounters), h->s_index));
+  FI_CUDA(cudaMemsetAsync(h->d_ctr.get(), 0, sizeof(IndexCounters), h->s_index.get()));
   {
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_index_rebuild(h->ix, h->ix_spare, h->d_ctr, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_index_rebuild(h->ix.v, h->ix_spare->v, h->d_ctr.get(), h->s_index.get()));
   }
-  std::swap(h->ix, h->ix_spare);
+  std::swap(h->ix, *h->ix_spare);  // owners and views together
   h->rebuilds++;
   return FI_OK;
 }
@@ -493,24 +504,24 @@ int rebuild_index(fi_epp* h) {
 // clogged with tombstones, fail if it is genuinely full
 int check_counters(fi_epp* h) {
   if (!h->ctr_pending) return FI_OK;
-  FI_CUDA(cudaEventSynchronize(h->ev_ctr));
+  FI_CUDA(cudaEventSynchronize(h->ev_ctr.get()));
   h->ctr_pending = false;
   h->ctr_used_known = h->h_ctr->used;
   h->ctr_unchecked = 0;
-  if (h->h_lru_stat && h->h_lru_stat->error)
-    return fail(h, FI_ERR_STATE, "device LRU: invariant " + std::to_string(h->h_lru_stat->error) + " broken");
-  if (h->h_lru_stat && h->h_lru_stat->planned_ovf)
+  if (h->dlru && h->dlru->stat->error)
+    return fail(h, FI_ERR_STATE, "device LRU: invariant " + std::to_string(h->dlru->stat->error) + " broken");
+  if (h->dlru && h->dlru->stat->planned_ovf)
     return fail(h, FI_ERR_STATE, "device LRU: a table overflowed in a sub-batch planned not to (broken invariant)");
   if (h->h_ctr->overflow) return fail(h, FI_ERR_CAPACITY, "index full: raise index_slots");
   const uint64_t used = h->h_ctr->used, tomb = h->h_ctr->tombstones;
-  if (used * 10 > h->ix.C * 7) {
-    if ((used - tomb) * 10 > h->ix.C * 6) return fail(h, FI_ERR_CAPACITY, "index above 60% live keys: raise index_slots");
+  if (used * 10 > h->ix.v.C * 7) {
+    if ((used - tomb) * 10 > h->ix.v.C * 6) return fail(h, FI_ERR_CAPACITY, "index above 60% live keys: raise index_slots");
     // the rebuild reads the old tables on s_index: every pick that still uses them must be ordered before the
     // NEXT rebuild clears them — flush_ops (our only caller that launches work) waits for ev_pick first
-    FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
+    FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
     int rc = rebuild_index(h);
     if (rc != FI_OK) return rc;
-    FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
+    FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   }
   return FI_OK;
 }
@@ -521,8 +532,8 @@ int check_counters(fi_epp* h) {
 // a full index) yet.  Counters that are in are checked as always, and so are the device LRU's error flags.
 int check_counters_lagged(fi_epp* h, uint64_t extra) {
   if (h->ctr_pending && h->world == 1) {
-    const cudaError_t q = cudaEventQuery(h->ev_ctr);
-    if (q == cudaErrorNotReady && (h->ctr_used_known + h->ctr_unchecked + extra) * 10 <= h->ix.C * 7) return FI_OK;
+    const cudaError_t q = cudaEventQuery(h->ev_ctr.get());
+    if (q == cudaErrorNotReady && (h->ctr_used_known + h->ctr_unchecked + extra) * 10 <= h->ix.v.C * 7) return FI_OK;
     if (q != cudaSuccess && q != cudaErrorNotReady) FI_CUDA(q);
   }
   return check_counters(h);
@@ -531,10 +542,10 @@ int check_counters_lagged(fi_epp* h, uint64_t extra) {
 GossipLog gossip_log(fi_epp* h) {
   GossipLog g{};
   if (h->world > 1) {
-    g.n_appear = h->d_glog_n;
-    g.n_vanish = h->d_glog_n + 1;
-    g.appear = h->d_glog_a;
-    g.vanish = h->d_glog_v;
+    g.n_appear = h->shard->d_glog_n.get();
+    g.n_vanish = h->shard->d_glog_n.get() + 1;
+    g.appear = h->shard->d_glog_a.get();
+    g.vanish = h->shard->d_glog_v.get();
     g.cap = kOpChunk;
   }
   return g;
@@ -549,80 +560,82 @@ int flush_ops(fi_epp* h) {
   if (rc != FI_OK) return rc;
   const int b = h->cur_buf;
   // ops submitted after a pick returned must not overtake it on the GPU: the pick sees the index as of its call
-  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
   const GossipLog gl = gossip_log(h);
   if (h->n_sets) {
-    FI_CUDA(cudaMemcpyAsync(h->d_sets[b], h->h_sets[b], h->n_sets * sizeof(fi_index_op), cudaMemcpyHostToDevice, h->s_index));
+    FI_CUDA(cudaMemcpyAsync(h->d_sets[b].get(), h->h_sets[b].get(), h->n_sets * sizeof(fi_index_op), cudaMemcpyHostToDevice, h->s_index.get()));
     h->stats.h2d_bytes += h->n_sets * sizeof(fi_index_op);
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_index_set(h->ix, h->d_ctr, h->d_sets[b], h->n_sets, h->cfg.endpoint_begin, h->cfg.endpoint_count, h->rank,
-                             gl, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_index_set(h->ix.v, h->d_ctr.get(), h->d_sets[b].get(), h->n_sets, h->cfg.endpoint_begin, h->cfg.endpoint_count, h->rank,
+                             gl, h->s_index.get()));
   }
   if (h->n_clears) {
-    FI_CUDA(cudaMemcpyAsync(h->d_clears[b], h->h_clears[b], h->n_clears * sizeof(fi_index_op), cudaMemcpyHostToDevice, h->s_index));
+    FI_CUDA(cudaMemcpyAsync(h->d_clears[b].get(), h->h_clears[b].get(), h->n_clears * sizeof(fi_index_op), cudaMemcpyHostToDevice, h->s_index.get()));
     h->stats.h2d_bytes += h->n_clears * sizeof(fi_index_op);
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_index_clear(h->ix, h->d_ctr, h->d_clears[b], h->n_clears, h->cfg.endpoint_begin, h->cfg.endpoint_count,
-                               h->rank, gl, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_index_clear(h->ix.v, h->d_ctr.get(), h->d_clears[b].get(), h->n_clears, h->cfg.endpoint_begin, h->cfg.endpoint_count,
+                               h->rank, gl, h->s_index.get()));
   }
   h->ops_applied += h->n_sets + h->n_clears;
   h->ctr_unchecked += h->n_sets;
-  FI_CUDA(cudaEventRecord(h->ev_buf[b], h->s_index));
-  FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
-  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_buf[b].get(), h->s_index.get()));
+  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
   h->ctr_pending = true;
-  FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   h->n_sets = h->n_clears = 0;
   h->cleared.clear();
   h->cur_buf ^= 1;
   // the buffer we are about to fill must have been consumed
-  FI_CUDA(cudaEventSynchronize(h->ev_buf[h->cur_buf]));
+  FI_CUDA(cudaEventSynchronize(h->ev_buf[h->cur_buf].get()));
   return FI_OK;
 }
 
-int nccl_allgather_on(fi_epp* h, const void* send, void* recv, size_t bytes, cudaStream_t s);
+int nccl_allgather_on(fi_epp* h, ncclComm_t comm, const void* send, void* recv, size_t bytes, cudaStream_t s);
 
 // Sharded pools, one gossip round (collective: every rank calls it the same number of times): exchange the
 // transition logs written by this round's SET / CLEAR kernels and replay the other ranks' into the local
 // directory — all APPEARs before all VANISHes, like the SETs and CLEARs that produced them.
 int gossip_round(fi_epp* h) {
   if (h->world <= 1) return FI_OK;
+  ShardState& sh = *h->shard;
+  const unsigned long long* hdr = sh.h_ghdr.get();
   const uint32_t Wd = h->world;
-  int rc = nccl_allgather_on(h, h->d_glog_n, h->d_ghdr, 2 * sizeof(unsigned long long), h->s_index);
+  int rc = nccl_allgather_on(h, sh.comm, sh.d_glog_n.get(), sh.d_ghdr.get(), 2 * sizeof(unsigned long long), h->s_index.get());
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaMemcpyAsync(h->h_ghdr, h->d_ghdr, (size_t)Wd * 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->s_index));
-  FI_CUDA(cudaStreamSynchronize(h->s_index));
+  FI_CUDA(cudaMemcpyAsync(sh.h_ghdr.get(), sh.d_ghdr.get(), (size_t)Wd * 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
   uint64_t na = 0, nv = 0;
   for (uint32_t g = 0; g < Wd; ++g) {
-    na = std::max<uint64_t>(na, h->h_ghdr[2 * g]);
-    nv = std::max<uint64_t>(nv, h->h_ghdr[2 * g + 1]);
+    na = std::max<uint64_t>(na, hdr[2 * g]);
+    nv = std::max<uint64_t>(nv, hdr[2 * g + 1]);
   }
   if (na > kOpChunk || nv > kOpChunk) return fail(h, FI_ERR_STATE, "gossip log overflow");
   if (na) {
-    rc = nccl_allgather_on(h, h->d_glog_a, h->d_ggather, na * sizeof(uint64_t), h->s_index);
+    rc = nccl_allgather_on(h, sh.comm, sh.d_glog_a.get(), sh.d_ggather.get(), na * sizeof(uint64_t), h->s_index.get());
     if (rc != FI_OK) return rc;
     for (uint32_t g = 0; g < Wd; ++g) {
-      if (g == h->rank || h->h_ghdr[2 * g] == 0) continue;
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_index_remote_appear(h->ix, h->d_ctr, h->d_ggather + (size_t)g * na, h->h_ghdr[2 * g], g, h->s_index));
+      if (g == h->rank || hdr[2 * g] == 0) continue;
+      LaunchScope ls(h, h->s_index.get(), K_INDEX);
+      FI_CUDA(launch_index_remote_appear(h->ix.v, h->d_ctr.get(), sh.d_ggather.get() + (size_t)g * na, hdr[2 * g], g, h->s_index.get()));
     }
   }
   if (nv) {
-    rc = nccl_allgather_on(h, h->d_glog_v, h->d_ggather, nv * sizeof(uint64_t), h->s_index);
+    rc = nccl_allgather_on(h, sh.comm, sh.d_glog_v.get(), sh.d_ggather.get(), nv * sizeof(uint64_t), h->s_index.get());
     if (rc != FI_OK) return rc;
     for (uint32_t g = 0; g < Wd; ++g) {
-      if (g == h->rank || h->h_ghdr[2 * g + 1] == 0) continue;
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_index_remote_vanish(h->ix, h->d_ctr, h->d_ggather + (size_t)g * nv, h->h_ghdr[2 * g + 1], g, h->s_index));
+      if (g == h->rank || hdr[2 * g + 1] == 0) continue;
+      LaunchScope ls(h, h->s_index.get(), K_INDEX);
+      FI_CUDA(launch_index_remote_vanish(h->ix.v, h->d_ctr.get(), sh.d_ggather.get() + (size_t)g * nv, hdr[2 * g + 1], g, h->s_index.get()));
     }
   }
-  FI_CUDA(cudaMemsetAsync(h->d_glog_n, 0, 2 * sizeof(unsigned long long), h->s_index));
+  FI_CUDA(cudaMemsetAsync(sh.d_glog_n.get(), 0, 2 * sizeof(unsigned long long), h->s_index.get()));
   if (na || nv) {  // the replays allocate nodes too: refresh the counters the rebuild decision reads
-    FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
-    FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
+    FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
+    FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
     h->ctr_pending = true;
   }
-  FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   return FI_OK;
 }
 
@@ -630,14 +643,15 @@ int gossip_round(fi_epp* h) {
 int agree_rounds(fi_epp* h, uint64_t mine, uint64_t* rounds) {
   *rounds = mine;
   if (h->world <= 1) return FI_OK;
+  ShardState& sh = *h->shard;
   unsigned long long v[2] = {mine, 0};
-  FI_CUDA(cudaMemcpyAsync(h->d_ghdr + 2 * (size_t)h->world, v, sizeof(v), cudaMemcpyHostToDevice, h->s_index));
-  int rc = nccl_allgather_on(h, h->d_ghdr + 2 * (size_t)h->world, h->d_ghdr, sizeof(v), h->s_index);
+  FI_CUDA(cudaMemcpyAsync(sh.d_ghdr.get() + 2 * (size_t)h->world, v, sizeof(v), cudaMemcpyHostToDevice, h->s_index.get()));
+  int rc = nccl_allgather_on(h, sh.comm, sh.d_ghdr.get() + 2 * (size_t)h->world, sh.d_ghdr.get(), sizeof(v), h->s_index.get());
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaMemcpyAsync(h->h_ghdr, h->d_ghdr, (size_t)h->world * sizeof(v), cudaMemcpyDeviceToHost, h->s_index));
-  FI_CUDA(cudaStreamSynchronize(h->s_index));
+  FI_CUDA(cudaMemcpyAsync(sh.h_ghdr.get(), sh.d_ghdr.get(), (size_t)h->world * sizeof(v), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
   uint64_t m = 0;
-  for (uint32_t g = 0; g < h->world; ++g) m = std::max<uint64_t>(m, h->h_ghdr[2 * g]);
+  for (uint32_t g = 0; g < h->world; ++g) m = std::max<uint64_t>(m, sh.h_ghdr.get()[2 * g]);
   *rounds = m;
   return FI_OK;
 }
@@ -650,10 +664,10 @@ int submit_op(fi_epp* h, uint64_t hash, uint32_t endpoint, uint32_t op) {
       int rc = flush_ops(h);
       if (rc != FI_OK) return rc;
     }
-    h->h_sets[h->cur_buf][h->n_sets++] = fi_index_op{hash, endpoint, FI_OP_SET};
+    h->h_sets[h->cur_buf].get()[h->n_sets++] = fi_index_op{hash, endpoint, FI_OP_SET};
   } else {
     h->cleared.insert(PairKey{hash, endpoint});
-    h->h_clears[h->cur_buf][h->n_clears++] = fi_index_op{hash, endpoint, FI_OP_CLEAR};
+    h->h_clears[h->cur_buf].get()[h->n_clears++] = fi_index_op{hash, endpoint, FI_OP_CLEAR};
   }
   if (h->n_sets == kOpChunk || h->n_clears == kOpChunk) return flush_ops(h);
   return FI_OK;
@@ -673,48 +687,10 @@ int choose_lru_mode(fi_epp* h) {
   return FI_OK;
 }
 
-void free_dev_lru(fi_epp* h) {
-  cudaFree(h->dlru.slots);
-  cudaFree(h->dlru.log);
-  cudaFree(h->d_lru_state);
-  cudaFree(h->d_lru_ctr);
-  if (h->h_lru_stat) cudaFreeHost(h->h_lru_stat);
-  cudaFree(h->d_lru_slot_of);
-  cudaFree(h->d_lru_wcount);
-  cudaFree(h->d_lru_base);
-  cudaFree(h->d_lru_sets);
-  cudaFree(h->d_lru_clears);
-  if (h->ev_lru) cudaEventDestroy(h->ev_lru);
-  if (h->ev_lru_ovf) cudaEventDestroy(h->ev_lru_ovf);
-  h->dlru = DevLru{};
-  h->d_lru_state = nullptr;
-  h->d_lru_ctr = nullptr;
-  h->h_lru_stat = nullptr;
-  h->d_lru_slot_of = h->d_lru_wcount = h->d_lru_base = nullptr;
-  h->d_lru_sets = h->d_lru_clears = nullptr;
-  h->ev_lru = h->ev_lru_ovf = nullptr;
-  h->dlru_ready = false;
-}
-
-int alloc_dev_lru(fi_epp* h);
-
-int ensure_dev_lru(fi_epp* h) {
-  if (h->dlru_ready) return FI_OK;
-  const int rc = alloc_dev_lru(h);
-  if (rc != FI_OK) {  // nothing of a partial allocation survives (a later call may succeed, e.g. with the host LRU freed)
-    const std::string why = h->err;
-    cudaGetLastError();
-    free_dev_lru(h);
-    h->err = why;
-    return rc;
-  }
-  h->dlru_ready = true;
-  return FI_OK;
-}
-
-int alloc_dev_lru(fi_epp* h) {
+// the device LRU's buffers, all or nothing: `s` is filled only as far as it got when a step fails
+int alloc_dev_lru(fi_epp* h, DevLruStore& s) {
   const uint32_t EL = h->cfg.endpoint_count, C = h->cfg.lru_capacity;
-  DevLru& d = h->dlru;
+  DevLru& d = s.v;
   d.EL = EL;
   d.capacity = C;
   size_t free_b = 0, total_b = 0;
@@ -735,30 +711,32 @@ int alloc_dev_lru(fi_epp* h) {
   d.TS = ts;
   d.L = std::max(d.L, d.TS / 4);
   d.insert_limit = (uint32_t)((uint64_t)d.TS * 85 / 100);
-  const size_t slot_bytes = (size_t)EL * (d.TS + 2) * sizeof(LruSlot), log_bytes = (size_t)EL * d.L * sizeof(uint64_t);
-  h->lru_touch_cap = std::max<uint64_t>((uint64_t)h->cfg.max_batch * h->MP, 1u << 16);
-  const size_t scratch = (size_t)h->lru_touch_cap * (sizeof(uint32_t) + 3 * sizeof(fi_index_op));
-  if (slot_bytes + log_bytes + scratch + (256u << 20) > free_b)
+  const size_t slots = (size_t)EL * (d.TS + 2), log_records = (size_t)EL * d.L;
+  s.touch_cap = std::max<uint64_t>((uint64_t)h->cfg.max_batch * h->MP, 1u << 16);
+  const size_t scratch = (size_t)s.touch_cap * (sizeof(uint32_t) + 3 * sizeof(fi_index_op));
+  if (slots * sizeof(LruSlot) + log_records * sizeof(uint64_t) + scratch + (256u << 20) > free_b)
     return fail(h, FI_ERR_NOMEM, "device LRU does not fit in free HBM (option device_lru = 0 selects the host LRU)");
   const size_t state_words = (size_t)8 * EL + 2;
-  FI_CUDA(cudaMalloc(&d.slots, slot_bytes));
-  FI_CUDA(cudaMalloc(&d.log, log_bytes));
-  FI_CUDA(cudaMalloc(&h->d_lru_state, state_words * sizeof(uint32_t)));
-  FI_CUDA(cudaMalloc(&h->d_lru_ctr, 8 * sizeof(unsigned long long)));
-  FI_CUDA(cudaMallocHost(&h->h_lru_stat, sizeof(fi_epp::LruHostStat)));
-  std::memset(h->h_lru_stat, 0, sizeof(fi_epp::LruHostStat));
-  FI_CUDA(cudaMalloc(&h->d_lru_slot_of, h->lru_touch_cap * sizeof(uint32_t)));
-  FI_CUDA(cudaMalloc(&h->d_lru_sets, h->lru_touch_cap * sizeof(fi_index_op)));
-  FI_CUDA(cudaMalloc(&h->d_lru_clears, 2 * h->lru_touch_cap * sizeof(fi_index_op)));  // doomed keys + evictions
-  FI_CUDA(cudaMalloc(&h->d_lru_wcount, (size_t)h->cfg.max_batch * sizeof(uint32_t)));
-  FI_CUDA(cudaMalloc(&h->d_lru_base, (size_t)h->cfg.max_batch * sizeof(uint32_t)));
-  FI_CUDA(cudaEventCreateWithFlags(&h->ev_lru, cudaEventDisableTiming));
-  FI_CUDA(cudaEventCreateWithFlags(&h->ev_lru_ovf, cudaEventDisableTiming));
-  FI_CUDA(cudaMemsetAsync(d.slots, 0, slot_bytes, h->s_index));
-  FI_CUDA(cudaMemsetAsync(h->d_lru_state, 0, state_words * sizeof(uint32_t), h->s_index));
-  FI_CUDA(cudaMemsetAsync(h->d_lru_ctr, 0, 8 * sizeof(unsigned long long), h->s_index));
-  FI_CUDA(cudaEventRecord(h->ev_lru, h->s_index));
-  d.head = h->d_lru_state;
+  FI_CUDA(cuda_alloc(s.slots, slots));
+  FI_CUDA(cuda_alloc(s.log, log_records));
+  FI_CUDA(cuda_alloc(s.state, state_words));
+  FI_CUDA(cuda_alloc(s.ctr, 8));
+  FI_CUDA(cuda_alloc(s.stat, 1));
+  std::memset(s.stat.get(), 0, sizeof(DevLruStore::HostStat));
+  FI_CUDA(cuda_alloc(s.slot_of, s.touch_cap));
+  FI_CUDA(cuda_alloc(s.sets, s.touch_cap));
+  FI_CUDA(cuda_alloc(s.clears, 2 * s.touch_cap));  // doomed keys + evictions
+  FI_CUDA(cuda_alloc(s.wcount, h->cfg.max_batch));
+  FI_CUDA(cuda_alloc(s.base, h->cfg.max_batch));
+  FI_CUDA(cuda_create(s.ev));
+  FI_CUDA(cuda_create(s.ev_ovf));
+  FI_CUDA(cudaMemsetAsync(s.slots.get(), 0, slots * sizeof(LruSlot), h->s_index.get()));
+  FI_CUDA(cudaMemsetAsync(s.state.get(), 0, state_words * sizeof(uint32_t), h->s_index.get()));
+  FI_CUDA(cudaMemsetAsync(s.ctr.get(), 0, 8 * sizeof(unsigned long long), h->s_index.get()));
+  FI_CUDA(cudaEventRecord(s.ev.get(), h->s_index.get()));
+  d.slots = s.slots.get();
+  d.log = s.log.get();
+  d.head = s.state.get();
   d.tail = d.head + EL;
   d.count = d.tail + EL;
   d.used = d.count + EL;
@@ -770,18 +748,32 @@ int alloc_dev_lru(fi_epp* h) {
   d.cap = d.error + 1;
   // the capacities set so far (possibly before this first Add); pageable source: taken when the call returns
   if (h->lru_caps.size() != EL) h->lru_caps.assign(EL, C);
-  FI_CUDA(cudaMemcpyAsync(d.cap, h->lru_caps.data(), (size_t)EL * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
-  d.n_sets = h->d_lru_ctr;
-  d.n_maintained = h->d_lru_ctr + 1;
-  d.n_clears = h->d_lru_ctr + 3;
-  d.n_doomed = h->d_lru_ctr + 4;
+  FI_CUDA(cudaMemcpyAsync(d.cap, h->lru_caps.data(), (size_t)EL * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
+  d.n_sets = s.ctr.get();
+  d.n_maintained = s.ctr.get() + 1;
+  d.n_clears = s.ctr.get() + 3;
+  d.n_doomed = s.ctr.get() + 4;
+  return FI_OK;
+}
+
+// the device LRU is allocated whole at the first Add; nothing of a failed allocation survives (a later call may
+// succeed, e.g. with the host LRU freed)
+int ensure_dev_lru(fi_epp* h) {
+  if (h->dlru) return FI_OK;
+  auto s = std::make_unique<DevLruStore>();
+  const int rc = alloc_dev_lru(h, *s);
+  if (rc != FI_OK) {
+    cudaGetLastError();
+    return rc;
+  }
+  h->dlru = std::move(s);
   return FI_OK;
 }
 
 // queue the refresh of the pinned LRU status (error flag + totals) behind everything submitted so far
 int lru_refresh_stat(fi_epp* h) {
-  FI_CUDA(cudaMemcpyAsync(&h->h_lru_stat->error, h->dlru.error, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index));
-  FI_CUDA(cudaMemcpyAsync(&h->h_lru_stat->n_sets, h->d_lru_ctr, 5 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->s_index));
+  FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->error, h->dlru->v.error, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->n_sets, h->dlru->ctr.get(), 5 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->s_index.get()));
   return FI_OK;
 }
 
@@ -801,21 +793,21 @@ LruBatch lru_sub_batch(fi_epp* h, const uint32_t* dp, const LruPlan& pl, size_t 
   b.chains = chains;
   b.pitch = pitch;
   b.K = pl.subs[sb].k_end - pl.subs[sb].k_begin;
-  b.slot_of = h->d_lru_slot_of;
-  b.wcount = h->d_lru_wcount;
-  b.base = h->d_lru_base;
-  b.sets = h->d_lru_sets;
+  b.slot_of = h->dlru->slot_of.get();
+  b.wcount = h->dlru->wcount.get();
+  b.base = h->dlru->base.get();
+  b.sets = h->dlru->sets.get();
   return b;
 }
 
 // maintain (log compaction / table rebuild) and touch of one sub-batch
 int lru_enqueue_touch(fi_epp* h, const LruBatch& b, const uint32_t* inc) {
   {
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_lru_maintain(h->dlru, inc, false, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_lru_maintain(h->dlru->v, inc, false, h->s_index.get()));
   }
-  LaunchScope ls(h, h->s_index, K_INDEX);
-  FI_CUDA(launch_lru_touch(h->dlru, b, h->s_index));
+  LaunchScope ls(h, h->s_index.get(), K_INDEX);
+  FI_CUDA(launch_lru_touch(h->dlru->v, b, h->s_index.get()));
   return FI_OK;
 }
 
@@ -823,37 +815,37 @@ int lru_enqueue_touch(fi_epp* h, const LruBatch& b, const uint32_t* inc) {
 // then the overflow flags of the touch are reset); the index counters are copied back for the next rebuild decision
 int lru_enqueue_apply(fi_epp* h, const LruBatch& b, uint64_t touches, const GossipLog& glog, bool clear_ovf) {
   const uint32_t EL = h->cfg.endpoint_count, lo = h->cfg.endpoint_begin;
-  FI_CUDA(cudaMemsetAsync(h->d_lru_ctr + 2, 0, sizeof(unsigned long long), h->s_index));
+  FI_CUDA(cudaMemsetAsync(h->dlru->ctr.get() + 2, 0, sizeof(unsigned long long), h->s_index.get()));
   {
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_lru_count(h->dlru, b, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_lru_count(h->dlru->v, b, h->s_index.get()));
   }
   {
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_lru_scan(h->dlru, b, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_lru_scan(h->dlru->v, b, h->s_index.get()));
   }
   {
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_lru_append(h->dlru, b, h->d_lru_clears, h->d_lru_ctr + 2, 2 * h->lru_touch_cap, lo, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_lru_append(h->dlru->v, b, h->dlru->clears.get(), h->dlru->ctr.get() + 2, 2 * h->dlru->touch_cap, lo, h->s_index.get()));
   }
   {
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_index_set(h->ix, h->d_ctr, h->d_lru_sets, touches, lo, EL, h->rank, glog, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_index_set(h->ix.v, h->d_ctr.get(), h->dlru->sets.get(), touches, lo, EL, h->rank, glog, h->s_index.get()));
   }
   {
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_lru_evict(h->dlru, h->d_lru_clears, h->d_lru_ctr + 2, 2 * h->lru_touch_cap, lo, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_lru_evict(h->dlru->v, h->dlru->clears.get(), h->dlru->ctr.get() + 2, 2 * h->dlru->touch_cap, lo, h->s_index.get()));
   }
   {
     // CLEARs of a sub-batch: at most one per doomed key (<= touches) and one per eviction (<= keys it added)
-    const uint64_t cap = std::min<uint64_t>(2 * h->lru_touch_cap, 2 * touches);
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_index_clear_counted(h->ix, h->d_ctr, h->d_lru_clears, cap, h->d_lru_ctr + 2, lo, EL, h->rank, glog,
-                                       h->s_index));
+    const uint64_t cap = std::min<uint64_t>(2 * h->dlru->touch_cap, 2 * touches);
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_index_clear_counted(h->ix.v, h->d_ctr.get(), h->dlru->clears.get(), cap, h->dlru->ctr.get() + 2, lo, EL, h->rank, glog,
+                                       h->s_index.get()));
   }
-  if (clear_ovf) FI_CUDA(cudaMemsetAsync(h->dlru.ovf, 0, ((size_t)EL + 1) * sizeof(uint32_t), h->s_index));  // ovf[] and any_ovf
-  FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
-  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
+  if (clear_ovf) FI_CUDA(cudaMemsetAsync(h->dlru->v.ovf, 0, ((size_t)EL + 1) * sizeof(uint32_t), h->s_index.get()));  // ovf[] and any_ovf
+  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
   h->ctr_pending = true;
   h->ctr_unchecked += touches;
   return FI_OK;
@@ -881,7 +873,7 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
   // sharded pool: a sub-batch's APPEAR / VANISH transitions must fit the gossip log of one round (at most one SET per
   // touch; CLEARs: evictions <= keys added, plus doomed entries <= touches)
   const bool sharded = h->world > 1;
-  const uint64_t cap_touches = sharded ? std::min<uint64_t>(h->lru_touch_cap, kOpChunk / 2) : h->lru_touch_cap;
+  const uint64_t cap_touches = sharded ? std::min<uint64_t>(h->dlru->touch_cap, kOpChunk / 2) : h->dlru->touch_cap;
   lru_plan_batch(endpoints, nblocks, R, lo, EL, conservative ? h->cfg.lru_capacity : 0xFFFFFFFFu, cap_touches, h->cfg.max_batch, &pl);
   if (pl.subs.empty() && !sharded) return FI_OK;
   const size_t K = pl.req_id.size(), nsub = pl.subs.size();
@@ -893,36 +885,36 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
   }
   const GossipLog glog = gossip_log(h);
   const size_t words = lru_plan_words(pl, EL);
-  FI_CUDA(cudaEventSynchronize(h->ev_lru));  // the previous call's staging (and chain copy) has been consumed
+  FI_CUDA(cudaEventSynchronize(h->dlru->ev.get()));  // the previous call's staging (and chain copy) has been consumed
   rc = grow_staging(h, h->lru_plan_buf, words, words + words / 2 + 1024, true);  // room to spare: plans vary in size
   if (rc != FI_OK) return rc;
-  lru_plan_pack(pl, h->lru_plan_buf.h);
+  lru_plan_pack(pl, h->lru_plan_buf.h.get());
   // the LRU kernels run on the index stream; like every index update they are ordered behind the picks
   // submitted so far (a pick sees the index as of its call)
-  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
   if (words)
-    FI_CUDA(cudaMemcpyAsync(h->lru_plan_buf.d, h->lru_plan_buf.h, words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+    FI_CUDA(cudaMemcpyAsync(h->lru_plan_buf.d.get(), h->lru_plan_buf.h.get(), words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
   h->stats.h2d_bytes += words * sizeof(uint32_t);
   const uint64_t* d_chains = chains;
   if (!on_device && K) {
     const size_t cw = (size_t)R * pitch;
     rc = grow_staging(h, h->lru_chains, cw, cw, false);
     if (rc != FI_OK) return rc;
-    d_chains = h->lru_chains.d;
+    d_chains = h->lru_chains.d.get();
     // only the rows the plan kept are needed; whole-range copy when most are (one DMA), row copies otherwise
     if (K * 2 >= R) {
-      FI_CUDA(cudaMemcpyAsync(h->lru_chains.d, chains, cw * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_index));
+      FI_CUDA(cudaMemcpyAsync(h->lru_chains.d.get(), chains, cw * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_index.get()));
       h->stats.h2d_bytes += cw * sizeof(uint64_t);
     } else {
       for (size_t k = 0; k < K; ++k) {
         const size_t r = pl.req_id[k];
-        FI_CUDA(cudaMemcpyAsync(h->lru_chains.d + r * pitch, chains + r * pitch, (size_t)pl.req_n[k] * sizeof(uint64_t),
-                                cudaMemcpyHostToDevice, h->s_index));
+        FI_CUDA(cudaMemcpyAsync(h->lru_chains.d.get() + r * pitch, chains + r * pitch, (size_t)pl.req_n[k] * sizeof(uint64_t),
+                                cudaMemcpyHostToDevice, h->s_index.get()));
         h->stats.h2d_bytes += (size_t)pl.req_n[k] * sizeof(uint64_t);
       }
     }
   }
-  const uint32_t* dp = h->lru_plan_buf.d;
+  const uint32_t* dp = h->lru_plan_buf.d.get();
   h->lru_sub_batches += nsub;
   std::vector<uint8_t> deferred;  // per request of this call: its endpoint overflowed in the optimistic pass
   std::vector<uint32_t> ovf_host;
@@ -944,19 +936,19 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
     if (rc != FI_OK) return rc;
     // did some endpoint's table refuse keys?  (one host round trip per sub-batch; everything after it is queued
     // without waiting)
-    FI_CUDA(cudaMemcpyAsync(&h->h_lru_stat->any_ovf, h->dlru.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index));
-    FI_CUDA(cudaEventRecord(h->ev_lru_ovf, h->s_index));
-    FI_CUDA(cudaEventSynchronize(h->ev_lru_ovf));
-    const bool any_ovf = h->h_lru_stat->any_ovf != 0;
+    FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->any_ovf, h->dlru->v.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
+    FI_CUDA(cudaEventRecord(h->dlru->ev_ovf.get(), h->s_index.get()));
+    FI_CUDA(cudaEventSynchronize(h->dlru->ev_ovf.get()));
+    const bool any_ovf = h->dlru->stat->any_ovf != 0;
     if (any_ovf) {
       if (conservative) return fail(h, FI_ERR_STATE, "device LRU: overflow in a conservative sub-batch");
       {
-        LaunchScope ls(h, h->s_index, K_INDEX);
-        FI_CUDA(launch_lru_untouch(h->dlru, b, h->s_index));
+        LaunchScope ls(h, h->s_index.get(), K_INDEX);
+        FI_CUDA(launch_lru_untouch(h->dlru->v, b, h->s_index.get()));
       }
       ovf_host.resize(EL);
-      FI_CUDA(cudaMemcpyAsync(ovf_host.data(), h->dlru.ovf, (size_t)EL * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index));
-      FI_CUDA(cudaStreamSynchronize(h->s_index));
+      FI_CUDA(cudaMemcpyAsync(ovf_host.data(), h->dlru->v.ovf, (size_t)EL * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
+      FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
       if (deferred.empty()) deferred.assign(R, 0);
       for (uint32_t k = sbt.k_begin; k < sbt.k_end; ++k)
         if (ovf_host[pl.req_ep[k]]) {
@@ -973,9 +965,9 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
   }
   rc = lru_refresh_stat(h);
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));  // covers the status copy too
-  FI_CUDA(cudaEventRecord(h->ev_lru, h->s_index));
-  FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));  // covers the status copy too
+  FI_CUDA(cudaEventRecord(h->dlru->ev.get(), h->s_index.get()));
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   if (h->verbose) {
     const auto t1 = std::chrono::steady_clock::now();
     std::fprintf(stderr, "[fi_epp] device LRU%s: %u requests (%zu kept), %zu sub-batch(es), %zu deferred, host side %.3f ms\n",
@@ -994,9 +986,9 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
 // the index-stream part of lru_add_submitted: plan upload, sub-batches, status copies
 int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, size_t words, fi_epp::PipeAdd& pa) {
   // like every index update, ordered behind the picks submitted so far (a pick sees the index as of its call)
-  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_slot_read[slot], 0));
-  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
-  FI_CUDA(cudaMemcpyAsync(pa.plan.d, pa.plan.h, words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_slot_read[slot].get(), 0));
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
+  FI_CUDA(cudaMemcpyAsync(pa.plan.d.get(), pa.plan.h.get(), words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
   h->stats.h2d_bytes += words * sizeof(uint32_t);
   const GossipLog glog = gossip_log(h);
   h->lru_sub_batches += pl.subs.size();
@@ -1005,7 +997,7 @@ int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, size_
     int rc = check_counters_lagged(h, touches);  // may rebuild the index (on s_index, before this sub-batch)
     if (rc != FI_OK) return rc;
     const uint32_t* inc = nullptr;
-    const LruBatch b = lru_sub_batch(h, pa.plan.d, pl, sb, pa.d_chains, h->MP, &inc);
+    const LruBatch b = lru_sub_batch(h, pa.plan.d.get(), pl, sb, pa.d_chains.get(), h->MP, &inc);
     rc = lru_enqueue_touch(h, b, inc);
     if (rc != FI_OK) return rc;
     rc = lru_enqueue_apply(h, b, touches, glog, false);
@@ -1013,9 +1005,9 @@ int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, size_
   }
   int rc = lru_refresh_stat(h);
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaMemcpyAsync(&h->h_lru_stat->planned_ovf, h->dlru.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index));
-  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));  // covers the status copies too
-  FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
+  FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->planned_ovf, h->dlru->v.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));  // covers the status copies too
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   return FI_OK;
 }
 
@@ -1039,28 +1031,33 @@ int lru_add_submitted(fi_epp* h, uint32_t slot, const uint32_t* endpoints, const
   rc = flush_ops(h);  // ops staged through fi_epp_index_apply come first
   if (rc != FI_OK) return rc;
   LruPlan& pl = h->lru_plan;
-  lru_plan_batch(endpoints, nblocks, R, lo, EL, lru_touch_bound(h->dlru.TS, h->dlru.capacity), h->lru_touch_cap,
+  lru_plan_batch(endpoints, nblocks, R, lo, EL, lru_touch_bound(h->dlru->v.TS, h->dlru->v.capacity), h->dlru->touch_cap,
                  h->cfg.max_batch, &pl);
   if (pl.subs.empty()) return FI_OK;
   const size_t words = lru_plan_words(pl, EL);
   fi_epp::PipeAdd& pa = h->padd[h->padd_seq & 1];
-  if (pa.ev_done) FI_CUDA(cudaEventSynchronize(pa.ev_done));  // the Add before the previous one is done with it
-  if (!pa.ev_done) {
-    FI_CUDA(cudaEventCreateWithFlags(&pa.ev_done, cudaEventDisableTiming));
-    FI_CUDA(cudaMalloc(&pa.d_chains, (size_t)h->cfg.max_batch * h->MP * sizeof(uint64_t)));
+  if (pa.ev_done) {
+    FI_CUDA(cudaEventSynchronize(pa.ev_done.get()));  // the Add before the previous one is done with it
+  } else {
+    Event ev;
+    DevPtr<uint64_t> chains;
+    FI_CUDA(cuda_create(ev));
+    FI_CUDA(cuda_alloc(chains, (size_t)h->cfg.max_batch * h->MP));
+    pa.ev_done = std::move(ev);
+    pa.d_chains = std::move(chains);
   }
   rc = grow_staging(h, pa.plan, words, words + words / 2 + 1024, true);  // as lru_device_add's
   if (rc != FI_OK) return rc;
-  lru_plan_pack(pl, pa.plan.h);
-  const uint64_t* slot_chain = slot ? h->d_chain2 : h->d_chain;
-  FI_CUDA(cudaStreamWaitEvent(h->s_copy, h->ev_a[slot], 0));  // the batch's chains are written
-  FI_CUDA(cudaMemcpyAsync(pa.d_chains, slot_chain, (size_t)R * h->MP * sizeof(uint64_t), cudaMemcpyDeviceToDevice, h->s_copy));
-  FI_CUDA(cudaEventRecord(h->ev_slot_read[slot], h->s_copy));
+  lru_plan_pack(pl, pa.plan.h.get());
+  const uint64_t* slot_chain = slot ? h->d_chain2.get() : h->d_chain.get();
+  FI_CUDA(cudaStreamWaitEvent(h->s_copy.get(), h->ev_a[slot].get(), 0));  // the batch's chains are written
+  FI_CUDA(cudaMemcpyAsync(pa.d_chains.get(), slot_chain, (size_t)R * h->MP * sizeof(uint64_t), cudaMemcpyDeviceToDevice, h->s_copy.get()));
+  FI_CUDA(cudaEventRecord(h->ev_slot_read[slot].get(), h->s_copy.get()));
   // From here on work that reads pa's buffers is queued: whatever happens, pa.ev_done marks its end (the s_index wait
   // on the chain copy makes it cover that copy too), and the next call takes the other buffers.
   rc = lru_add_submitted_enqueue(h, slot, pl, words, pa);
-  cudaError_t e = cudaStreamWaitEvent(h->s_index, h->ev_slot_read[slot], 0);
-  if (e == cudaSuccess) e = cudaEventRecord(pa.ev_done, h->s_index);
+  cudaError_t e = cudaStreamWaitEvent(h->s_index.get(), h->ev_slot_read[slot].get(), 0);
+  if (e == cudaSuccess) e = cudaEventRecord(pa.ev_done.get(), h->s_index.get());
   h->padd_seq++;
   if (rc != FI_OK) return rc;
   if (e != cudaSuccess) return fail(h, FI_ERR_CUDA, cudaGetErrorString(e));
@@ -1083,11 +1080,11 @@ int lru_device_resize(fi_epp* h, const std::vector<uint32_t>& local, const std::
   std::vector<uint32_t> cnt;
   if (lowered) {  // the entries every endpoint holds once the Adds queued so far have run
     cnt.resize(EL);
-    FI_CUDA(cudaMemcpyAsync(cnt.data(), h->dlru.count, (size_t)EL * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index));
-    FI_CUDA(cudaStreamSynchronize(h->s_index));
+    FI_CUDA(cudaMemcpyAsync(cnt.data(), h->dlru->v.count, (size_t)EL * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
+    FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
   }
   // rounds: (endpoint, quota) pairs, at most clears_cap evictions per round; an endpoint is listed once per round
-  const uint64_t clears_cap = 2 * h->lru_touch_cap;
+  const uint64_t clears_cap = 2 * h->dlru->touch_cap;
   std::vector<uint32_t> r_eps, r_quota;
   std::vector<size_t> r_begin{0};
   std::vector<uint64_t> r_total;
@@ -1117,47 +1114,47 @@ int lru_device_resize(fi_epp* h, const std::vector<uint32_t>& local, const std::
     // (the previous resize's copy out of the pinned buffer is done: the readback above synchronised s_index)
     int rc = grow_staging(h, h->lru_resize, 2 * pairs, 2 * pairs, true);
     if (rc != FI_OK) return rc;
-    std::memcpy(h->lru_resize.h, r_eps.data(), pairs * sizeof(uint32_t));
-    std::memcpy(h->lru_resize.h + pairs, r_quota.data(), pairs * sizeof(uint32_t));
+    std::memcpy(h->lru_resize.h.get(), r_eps.data(), pairs * sizeof(uint32_t));
+    std::memcpy(h->lru_resize.h.get() + pairs, r_quota.data(), pairs * sizeof(uint32_t));
   }
   // picks called before this one must not see its evictions
-  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
   // (pageable source: the copy has taken the data when cudaMemcpyAsync returns)
-  FI_CUDA(cudaMemcpyAsync(h->dlru.cap, caps.data(), (size_t)EL * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+  FI_CUDA(cudaMemcpyAsync(h->dlru->v.cap, caps.data(), (size_t)EL * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
   h->stats.h2d_bytes += (size_t)EL * sizeof(uint32_t);
   if (pairs) {
-    FI_CUDA(cudaMemcpyAsync(h->lru_resize.d, h->lru_resize.h, 2 * pairs * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+    FI_CUDA(cudaMemcpyAsync(h->lru_resize.d.get(), h->lru_resize.h.get(), 2 * pairs * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
     h->stats.h2d_bytes += 2 * pairs * sizeof(uint32_t);
   }
   const GossipLog glog = gossip_log(h);
   for (size_t k = 0; k < r_total.size(); ++k) {
     const size_t b = r_begin[k];
     const uint32_t n = (uint32_t)(r_begin[k + 1] - b);
-    FI_CUDA(cudaMemsetAsync(h->d_lru_ctr + 2, 0, sizeof(unsigned long long), h->s_index));
+    FI_CUDA(cudaMemsetAsync(h->dlru->ctr.get() + 2, 0, sizeof(unsigned long long), h->s_index.get()));
     {
-      LaunchScope ls(h, h->s_index, K_INDEX);
-      FI_CUDA(launch_lru_shrink(h->dlru, h->lru_resize.d + b, h->lru_resize.d + pairs + b, n, h->d_lru_clears, h->d_lru_ctr + 2,
-                                clears_cap, lo, h->s_index));
+      LaunchScope ls(h, h->s_index.get(), K_INDEX);
+      FI_CUDA(launch_lru_shrink(h->dlru->v, h->lru_resize.d.get() + b, h->lru_resize.d.get() + pairs + b, n, h->dlru->clears.get(), h->dlru->ctr.get() + 2,
+                                clears_cap, lo, h->s_index.get()));
     }
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_index_clear_counted(h->ix, h->d_ctr, h->d_lru_clears, r_total[k], h->d_lru_ctr + 2, lo, EL, h->rank, glog,
-                                       h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_index_clear_counted(h->ix.v, h->d_ctr.get(), h->dlru->clears.get(), r_total[k], h->dlru->ctr.get() + 2, lo, EL, h->rank, glog,
+                                       h->s_index.get()));
   }
   int rc = lru_refresh_stat(h);
   if (rc != FI_OK) return rc;
   // the CLEARs' tombstones reach the rebuild decision of the next index update
-  FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
-  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));  // covers the status copy too
+  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));  // covers the status copy too
   h->ctr_pending = true;
-  FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   return FI_OK;
 }
 
 // hash kernels for the request slice [r0, r0+R): prompts → chain (device buffers), on stream s
 int run_hash(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0, uint32_t r0,
              uint32_t R, cudaStream_t s) {
-  uint64_t* chain = h->d_chain + (size_t)r0 * h->MP;
-  uint32_t* nb = h->d_nblocks + r0;
+  uint64_t* chain = h->d_chain.get() + (size_t)r0 * h->MP;
+  uint32_t* nb = h->d_nblocks.get() + r0;
   LaunchScope ls(h, s, K_HASH);
   if (h->fast_hash) {  // block hashing and chain walk in one kernel, no pre-states in HBM
     FI_CUDA(launch_hash_chain(d_prompts, d_offsets + r0, d_h0 + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP,
@@ -1169,16 +1166,18 @@ int run_hash(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, con
   return FI_OK;
 }
 
-int nccl_allgather_on(fi_epp* h, const void* send, void* recv, size_t bytes, cudaStream_t s) {
-  int rc = g_nccl.AllGather(send, recv, bytes, ncclInt8, h->comm, s);
+int nccl_allgather_on(fi_epp* h, ncclComm_t comm, const void* send, void* recv, size_t bytes, cudaStream_t s) {
+  int rc = g_nccl.AllGather(send, recv, bytes, ncclInt8, comm, s);
   if (rc != ncclSuccess)
     return fail(h, FI_ERR_COMM, std::string("ncclAllGather: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "error"));
   return FI_OK;
 }
-int nccl_allgather(fi_epp* h, const void* send, void* recv, size_t bytes) { return nccl_allgather_on(h, send, recv, bytes, h->s_main); }
+int nccl_allgather(fi_epp* h, const void* send, void* recv, size_t bytes) {
+  return nccl_allgather_on(h, h->shard->comm, send, recv, bytes, h->s_main.get());
+}
 
-// Peer-memory exchange set-up (sharded mode): allocate this rank's buffer, exchange its IPC handle over
-// the NCCL communicator, map every peer's buffer.  Falls back to the NCCL all-gather path (px.enabled = 0)
+// Peer-memory exchange set-up (sharded mode, collective): allocate this rank's buffer in `sh`, exchange its IPC handle
+// over sh's communicator, map every peer's buffer, and describe the result in *out.  Falls back to the NCCL all-gather path (px.enabled = 0)
 // when FI_EPP_EXCHANGE=nccl, when there are more than FI_MAX_RANKS ranks, or when any rank cannot map a peer.
 struct XchgBlob {
   cudaIpcMemHandle_t handle;
@@ -1190,53 +1189,51 @@ struct XchgBlob {
 };
 static_assert(sizeof(XchgBlob) == 128, "XchgBlob size");
 
-int setup_peer_exchange(fi_epp* h) {
+int setup_peer_exchange(fi_epp* h, ShardState& sh, uint32_t rank, uint32_t world, PeerXchg* out) {
   const char* mode = std::getenv("FI_EPP_EXCHANGE");
-  const bool want = !(mode && std::strcmp(mode, "nccl") == 0) && h->world <= (uint32_t)FI_MAX_RANKS;
+  const bool want = !(mode && std::strcmp(mode, "nccl") == 0) && world <= (uint32_t)FI_MAX_RANKS;
   const uint64_t R = h->cfg.max_batch;
   auto up = [](uint64_t v) { return (v + 255) & ~255ull; };
   PeerXchg px{};
-  px.world = h->world;
-  px.rank = h->rank;
+  px.world = world;
+  px.rank = rank;
   uint64_t off = 0;
   for (int par = 0; par < 2; ++par) {  // tagged 64-bit words (kernels.cuh PeerXchg)
     px.off_pick[par] = off;
-    off = up(off + (uint64_t)h->world * R * h->P * 4 * sizeof(uint64_t));
+    off = up(off + (uint64_t)world * R * h->P * 4 * sizeof(uint64_t));
   }
   XchgBlob mine{};
   mine.ok = 0;
-  if (want && cudaMalloc(&h->d_xchg, off) == cudaSuccess && cudaMemset(h->d_xchg, 0, off) == cudaSuccess &&
-      cudaHostAlloc((void**)&h->h_xerr, sizeof(uint32_t), cudaHostAllocMapped) == cudaSuccess &&
-      cudaIpcGetMemHandle(&mine.handle, h->d_xchg) == cudaSuccess) {
+  if (want && cuda_alloc(sh.d_xchg, off) == cudaSuccess && cudaMemset(sh.d_xchg.get(), 0, off) == cudaSuccess &&
+      cuda_alloc(sh.h_xerr, 1, cudaHostAllocMapped) == cudaSuccess &&
+      cudaIpcGetMemHandle(&mine.handle, sh.d_xchg.get()) == cudaSuccess) {
     mine.ok = 1;
   }
   cudaGetLastError();
-  mine.ptr = (uint64_t)(uintptr_t)h->d_xchg;
+  mine.ptr = (uint64_t)(uintptr_t)sh.d_xchg.get();
   mine.pid = (int64_t)getpid();
   mine.device = h->cfg.device;
   // round 1: handles; round 2: "I mapped every peer" votes.  Both ride the NCCL communicator.
-  XchgBlob* d_blobs = nullptr;
-  FI_CUDA(cudaMalloc(&d_blobs, (size_t)(h->world + 1) * sizeof(XchgBlob)));
-  std::vector<XchgBlob> all(h->world);
+  DevPtr<XchgBlob> blobs;
+  FI_CUDA(cuda_alloc(blobs, world + 1));
+  XchgBlob* d_blobs = blobs.get();
+  std::vector<XchgBlob> all(world);
   auto gather = [&]() -> int {
-    FI_CUDA(cudaMemcpyAsync(d_blobs + h->world, &mine, sizeof(mine), cudaMemcpyHostToDevice, h->s_main));
-    int rc = nccl_allgather(h, d_blobs + h->world, d_blobs, sizeof(XchgBlob));
+    FI_CUDA(cudaMemcpyAsync(d_blobs + world, &mine, sizeof(mine), cudaMemcpyHostToDevice, h->s_main.get()));
+    int rc = nccl_allgather_on(h, sh.comm, d_blobs + world, d_blobs, sizeof(XchgBlob), h->s_main.get());
     if (rc != FI_OK) return rc;
-    FI_CUDA(cudaMemcpyAsync(all.data(), d_blobs, (size_t)h->world * sizeof(XchgBlob), cudaMemcpyDeviceToHost, h->s_main));
-    FI_CUDA(cudaStreamSynchronize(h->s_main));
+    FI_CUDA(cudaMemcpyAsync(all.data(), d_blobs, (size_t)world * sizeof(XchgBlob), cudaMemcpyDeviceToHost, h->s_main.get()));
+    FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
     return FI_OK;
   };
   int rc = gather();
-  if (rc != FI_OK) {
-    cudaFree(d_blobs);
-    return rc;
-  }
+  if (rc != FI_OK) return rc;
   bool ok = true;
-  for (uint32_t k = 0; k < h->world; ++k) ok = ok && all[k].ok;
+  for (uint32_t k = 0; k < world; ++k) ok = ok && all[k].ok;
   if (ok) {
-    for (uint32_t k = 0; k < h->world && ok; ++k) {
-      if (k == h->rank) {
-        px.base[k] = h->d_xchg;
+    for (uint32_t k = 0; k < world && ok; ++k) {
+      if (k == rank) {
+        px.base[k] = sh.d_xchg.get();
       } else if (all[k].pid == mine.pid) {  // same process: plain peer access
         int can = 0;
         if (all[k].device != h->cfg.device) {
@@ -1254,7 +1251,7 @@ int setup_peer_exchange(fi_epp* h) {
       } else {
         void* m = nullptr;
         if (cudaIpcOpenMemHandle(&m, all[k].handle, cudaIpcMemLazyEnablePeerAccess) == cudaSuccess) {
-          h->peer_ipc[k] = m;
+          sh.peer_ipc[k] = m;
           px.base[k] = (uint8_t*)m;
         } else {
           cudaGetLastError();
@@ -1265,18 +1262,17 @@ int setup_peer_exchange(fi_epp* h) {
   }
   mine.ok = ok ? 1 : 0;
   rc = gather();
-  cudaFree(d_blobs);
   if (rc != FI_OK) return rc;
-  for (uint32_t k = 0; k < h->world; ++k) ok = ok && all[k].ok;
+  for (uint32_t k = 0; k < world; ++k) ok = ok && all[k].ok;
   if (ok) {
     px.enabled = 1;
     px.step = 0;
-    *h->h_xerr = 0;
-    px.err = const_cast<uint32_t*>(h->h_xerr);  // unified addressing: the host pointer is the device pointer
+    *sh.h_xerr = 0;
+    px.err = const_cast<uint32_t*>(sh.h_xerr.get());  // unified addressing: the host pointer is the device pointer
   }
-  h->px = px;
+  *out = px;
   if (std::getenv("FI_EPP_VERBOSE"))
-    std::fprintf(stderr, "[fi_epp] rank %u/%u: sharded exchange over %s\n", h->rank, h->world,
+    std::fprintf(stderr, "[fi_epp] rank %u/%u: sharded exchange over %s\n", rank, world,
                  px.enabled ? "peer memory (in-kernel tagged stores)" : "NCCL all-gather");
   return FI_OK;
 }
@@ -1285,17 +1281,17 @@ int setup_peer_exchange(fi_epp* h) {
 void dump_trace(fi_epp* h, uint32_t R) {
   if (!h->tracing) return;
   static const char* names[] = {"hash_chain", "match_pick", "index", "other"};
-  cudaStreamSynchronize(h->s_main);
+  cudaStreamSynchronize(h->s_main.get());
   std::fprintf(stderr, "[fi_epp trace] rank %u call %ld: R=%u\n", h->rank, h->trace_call, R);
   for (auto& e : h->pending_ev) {
     float t0 = 0.f, t1 = 0.f;
-    cudaEventSynchronize(e.b);
-    cudaEventElapsedTime(&t0, h->ev_trace0, e.a);
-    cudaEventElapsedTime(&t1, h->ev_trace0, e.b);
+    cudaEventSynchronize(e.b.get());
+    cudaEventElapsedTime(&t0, h->ev_trace0.get(), e.a.get());
+    cudaEventElapsedTime(&t1, h->ev_trace0.get(), e.b.get());
     std::fprintf(stderr, "[fi_epp trace]   r%u %-15s start %8.1f us  end %8.1f us  (%6.1f us)\n", h->rank, names[e.kind],
                  t0 * 1e3, t1 * 1e3, (t1 - t0) * 1e3);
-    h->ev_pool.push_back(e.a);
-    h->ev_pool.push_back(e.b);
+    h->ev_pool.push_back(std::move(e.a));
+    h->ev_pool.push_back(std::move(e.b));
   }
   h->pending_ev.clear();
   h->tracing = false;
@@ -1335,17 +1331,17 @@ int copy_chains_out(fi_epp* h, const uint64_t* chain, uint64_t* chains_out, uint
 // submitted so far, the endpoint and adapter tables go up if they changed, and `mp` describes the match of call `c`
 // (device pointers) over the chains at chain / nb.  Sharded: the rank's picks go to d_local, and the merge applies P/D.
 int prepare_match(fi_epp* h, const PickCall& c, const uint64_t* chain, const uint32_t* nb, MatchParams& mp) {
-  FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_index, 0));  // every submitted op is visible
+  FI_CUDA(cudaStreamWaitEvent(h->s_main.get(), h->ev_index.get(), 0));  // every submitted op is visible
   if (h->eps_dirty) {
-    FI_CUDA(cudaMemcpyAsync(h->d_eps, h->eps.data(), h->eps.size() * sizeof(EndpointDev), cudaMemcpyHostToDevice, h->s_main));
+    FI_CUDA(cudaMemcpyAsync(h->d_eps.get(), h->eps.data(), h->eps.size() * sizeof(EndpointDev), cudaMemcpyHostToDevice, h->s_main.get()));
     h->stats.h2d_bytes += h->eps.size() * sizeof(EndpointDev);
-    LaunchScope ls(h, h->s_main, K_OTHER);
-    FI_CUDA(launch_prepare_endpoints(h->d_eps, h->cfg.num_endpoints, h->cfg.endpoint_begin, h->cfg.endpoint_count, h->st,
-                                     h->d_sc, h->d_elig, h->d_zero, h->d_ztie, h->s_main));
+    LaunchScope ls(h, h->s_main.get(), K_OTHER);
+    FI_CUDA(launch_prepare_endpoints(h->d_eps.get(), h->cfg.num_endpoints, h->cfg.endpoint_begin, h->cfg.endpoint_count, h->st,
+                                     h->d_sc.get(), h->d_elig.get(), h->d_zero.get(), h->d_ztie.get(), h->s_main.get()));
     h->eps_dirty = false;  // (eps is pageable host memory: the copy has been staged by the time it returns)
   }
   if (h->lora_dirty) {
-    FI_CUDA(cudaMemcpyAsync(h->d_lora, h->lora.data(), h->lora.size() * sizeof(LoraDev), cudaMemcpyHostToDevice, h->s_main));
+    FI_CUDA(cudaMemcpyAsync(h->d_lora.get(), h->lora.data(), h->lora.size() * sizeof(LoraDev), cudaMemcpyHostToDevice, h->s_main.get()));
     h->stats.h2d_bytes += h->lora.size() * sizeof(LoraDev);
     h->lora_dirty = false;
   }
@@ -1357,7 +1353,7 @@ int prepare_match(fi_epp* h, const PickCall& c, const uint64_t* chain, const uin
   mp.adapters = c.adapters;
   mp.R = c.R;
   mp.MP = h->MP;
-  mp.ix = h->ix;
+  mp.ix = h->ix.v;
   mp.st = h->st;
   mp.ep_begin = h->cfg.endpoint_begin;
   mp.ep_count = h->cfg.endpoint_count;
@@ -1368,14 +1364,14 @@ int prepare_match(fi_epp* h, const PickCall& c, const uint64_t* chain, const uin
   mp.pd_decode = h->cfg.pd_decode_profile;
   mp.pd_prefill = h->cfg.pd_prefill_profile;
   mp.pd_threshold = h->cfg.pd_threshold;
-  mp.out = sharded ? h->d_local : c.out;
-  mp.probed_blocks = h->profiling ? h->d_probed : nullptr;
-  mp.work_counter = h->d_work;
+  mp.out = sharded ? h->shard->d_local.get() : c.out;
+  mp.probed_blocks = h->profiling ? h->d_probed.get() : nullptr;
+  mp.work_counter = h->d_work.get();
   mp.k = c.k;
   if (c.subsets) {
     mp.subsets = c.subsets;
     mp.sub_pitch = (h->cfg.num_endpoints + 31) / 32;
-    mp.eps = h->d_eps;
+    mp.eps = h->d_eps.get();
   }
   return FI_OK;
 }
@@ -1391,13 +1387,13 @@ int prepare_match(fi_epp* h, const PickCall& c, const uint64_t* chain, const uin
 // of a submit waits for the same readers of its own slot, for the match of the batch two back and the last
 // stream-ordered pick (submit_pick).
 int wait_slot_readers(fi_epp* h, uint32_t slot, cudaStream_t s) {
-  if (h->ev_lru) FI_CUDA(cudaStreamWaitEvent(s, h->ev_lru, 0));
-  if (h->padd_seq) FI_CUDA(cudaStreamWaitEvent(s, h->ev_slot_read[slot], 0));
+  if (h->dlru) FI_CUDA(cudaStreamWaitEvent(s, h->dlru->ev.get(), 0));
+  if (h->padd_seq) FI_CUDA(cudaStreamWaitEvent(s, h->ev_slot_read[slot].get(), 0));
   return FI_OK;
 }
 
 int claim_chain_slot0(fi_epp* h, cudaStream_t s) {
-  if (h->pipe_seq) FI_CUDA(cudaStreamWaitEvent(s, h->ev_a[(h->pipe_seq - 1) & 1], 0));
+  if (h->pipe_seq) FI_CUDA(cudaStreamWaitEvent(s, h->ev_a[(h->pipe_seq - 1) & 1].get(), 0));
   const int rc = wait_slot_readers(h, 0, s);
   if (rc == FI_OK) h->slot_ticket[0] = h->slot_ticket[1] = ~0ull;
   return rc;
@@ -1416,14 +1412,14 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
   if (rc != FI_OK) return rc;
   h->tracing = !h->profiling && h->trace_call >= 0 && (long)h->stats.pick_calls == h->trace_call;
   if (h->tracing) {
-    if (!h->ev_trace0) cudaEventCreate(&h->ev_trace0);
-    FI_CUDA(cudaStreamSynchronize(h->s_main));
-    FI_CUDA(cudaEventRecord(h->ev_trace0, h->s_main));
+    if (!h->ev_trace0) cuda_create(h->ev_trace0, cudaEventDefault);
+    FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
+    FI_CUDA(cudaEventRecord(h->ev_trace0.get(), h->s_main.get()));
   }
   MatchParams mp;
-  rc = prepare_match(h, c, h->d_chain, h->d_nblocks, mp);
+  rc = prepare_match(h, c, h->d_chain.get(), h->d_nblocks.get(), mp);
   if (rc != FI_OK) return rc;
-  rc = claim_chain_slot0(h, h->s_main);
+  rc = claim_chain_slot0(h, h->s_main.get());
   if (rc != FI_OK) return rc;
 
   const uint32_t S = h->feed_slices;
@@ -1436,14 +1432,14 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
     for (uint32_t k = 0; k * per < R; ++k, ++used) {
       const uint32_t r0 = k * per, r1 = std::min(R, r0 + per);
       const uint64_t b0 = feed->offsets[r0], b1 = feed->offsets[r1];
-      if (b1 > b0) FI_CUDA(cudaMemcpyAsync(dp + b0, feed->prompts + b0, b1 - b0, cudaMemcpyHostToDevice, h->s_copy));
-      FI_CUDA(cudaEventRecord(h->ev_copy[k], h->s_copy));
+      if (b1 > b0) FI_CUDA(cudaMemcpyAsync(dp + b0, feed->prompts + b0, b1 - b0, cudaMemcpyHostToDevice, h->s_copy.get()));
+      FI_CUDA(cudaEventRecord(h->ev_copy[k].get(), h->s_copy.get()));
     }
     h->stats.h2d_bytes += feed->offsets[R];
     for (uint32_t k = 0; k < used; ++k) {
       const uint32_t r0 = k * per, Rk = std::min(per, R - r0);
-      FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_copy[k], 0));
-      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, Rk, h->s_main);
+      FI_CUDA(cudaStreamWaitEvent(h->s_main.get(), h->ev_copy[k].get(), 0));
+      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, Rk, h->s_main.get());
       if (rc != FI_OK) return rc;
       MatchParams ms = mp;
       ms.chain = mp.chain + (size_t)r0 * h->MP;
@@ -1455,24 +1451,24 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
       ms.r_base = r0;
       ms.R = Rk;
       ms.out = mp.out + (size_t)r0 * h->P * std::max(c.k, 1u);
-      ms.work_counter = h->d_work + k;
-      LaunchScope ls(h, h->s_main, K_MATCH);
-      FI_CUDA(launch_match_pick(ms, h->sm_count, h->s_main));
+      ms.work_counter = h->d_work.get() + k;
+      LaunchScope ls(h, h->s_main.get(), K_MATCH);
+      FI_CUDA(launch_match_pick(ms, h->sm_count, h->s_main.get()));
     }
     return FI_OK;
   }
   if (feed && feed->offsets[R]) {  // one copy, then the whole batch
-    FI_CUDA(cudaMemcpyAsync(const_cast<uint8_t*>(c.prompts), feed->prompts, feed->offsets[R], cudaMemcpyHostToDevice, h->s_main));
+    FI_CUDA(cudaMemcpyAsync(const_cast<uint8_t*>(c.prompts), feed->prompts, feed->offsets[R], cudaMemcpyHostToDevice, h->s_main.get()));
     h->stats.h2d_bytes += feed->offsets[R];
   }
   if (!sharded) {
     // (A sub-batch pipeline over several streams was tried and measured slower on device-resident
     // inputs — DESIGN.md "What did not work": the chain walk costs a flat serial latency at any batch
     // size and small slices pay launch/ramp overheads.)
-    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main);
+    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main.get());
     if (rc != FI_OK) return rc;
-    LaunchScope ls(h, h->s_main, K_MATCH);
-    FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main));
+    LaunchScope ls(h, h->s_main.get(), K_MATCH);
+    FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main.get()));
     return FI_OK;
   }
 
@@ -1484,16 +1480,16 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
     const uint32_t per = (((R + h->world - 1) / h->world) + 31) & ~31u;  // ≤ chain_rows / world
     const uint32_t r0 = std::min(R, h->rank * per), r1 = std::min(R, r0 + per);
     if (r1 > r0) {
-      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, r1 - r0, h->s_main);
+      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, r1 - r0, h->s_main.get());
       if (rc != FI_OK) return rc;
     }
-    rc = nccl_allgather(h, h->d_chain + (size_t)h->rank * per * h->MP, h->d_chain, (size_t)per * h->MP * sizeof(uint64_t));
+    rc = nccl_allgather(h, h->d_chain.get() + (size_t)h->rank * per * h->MP, h->d_chain.get(), (size_t)per * h->MP * sizeof(uint64_t));
     if (rc != FI_OK) return rc;
-    rc = nccl_allgather(h, h->d_nblocks + (size_t)h->rank * per, h->d_nblocks, (size_t)per * sizeof(uint32_t));
+    rc = nccl_allgather(h, h->d_nblocks.get() + (size_t)h->rank * per, h->d_nblocks.get(), (size_t)per * sizeof(uint32_t));
     if (rc != FI_OK) return rc;
     h->stats.n_other += 2;  // two collectives of the step (not kernels of this library)
   } else {
-    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main);
+    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main.get());
     if (rc != FI_OK) return rc;
   }
   const bool p2p = h->px.enabled != 0;
@@ -1501,8 +1497,8 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
     // Peer-memory exchange: match_pick stores this rank's picks as tagged words into every rank's buffer and
     // merge_picks polls per request, so the reduction has no collective call, no barrier between the ranks
     // and no host round trip.  A timeout is reported once (the kernels set the mapped host word).
-    if (*h->h_xerr) {
-      *h->h_xerr = 0;
+    if (*h->shard->h_xerr) {
+      *h->shard->h_xerr = 0;
       return fail(h, FI_ERR_COMM, "peer exchange timed out waiting for another rank");
     }
     h->px.step += 1;
@@ -1510,24 +1506,24 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
     mp.px = h->px;
   }
   {
-    LaunchScope ls(h, h->s_main, K_MATCH);
-    FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main));
+    LaunchScope ls(h, h->s_main.get(), K_MATCH);
+    FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main.get()));
   }
   MergeParams mg{};
   if (p2p) {
-    mg.gathered = reinterpret_cast<const fi_pick*>(h->d_xchg + h->px.off_pick[h->px.step & 1u]);
+    mg.gathered = reinterpret_cast<const fi_pick*>(h->shard->d_xchg.get() + h->px.off_pick[h->px.step & 1u]);
     mg.px = h->px;
   } else {
-    rc = nccl_allgather(h, h->d_local, h->d_gather, (size_t)R * h->P * sizeof(fi_pick));
+    rc = nccl_allgather(h, h->shard->d_local.get(), h->shard->d_gather.get(), (size_t)R * h->P * sizeof(fi_pick));
     if (rc != FI_OK) return rc;
-    mg.gathered = h->d_gather;
+    mg.gathered = h->shard->d_gather.get();
   }
   mg.ranks = h->world;
   mg.R = R;
   mg.P = h->P;
-  mg.nblocks = h->d_nblocks;
+  mg.nblocks = h->d_nblocks.get();
   mg.offsets = c.offsets;
-  mg.chain = h->d_chain;
+  mg.chain = h->d_chain.get();
   mg.h0 = c.h0;
   mg.MP = h->MP;
   mg.E_global = h->cfg.num_endpoints;
@@ -1537,8 +1533,8 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
   mg.pd_threshold = h->cfg.pd_threshold;
   mg.out = c.out;
   {
-    LaunchScope ls(h, h->s_main, K_OTHER);
-    FI_CUDA(launch_merge_picks(mg, h->s_main));
+    LaunchScope ls(h, h->s_main.get(), K_OTHER);
+    FI_CUDA(launch_merge_picks(mg, h->s_main.get()));
   }
   return FI_OK;
 }
@@ -1549,15 +1545,15 @@ int run_pick(fi_epp* h, const PickCall& c, const PickCall* feed) {
   dump_trace(h, c.R);
   h->stats.pick_calls++;
   h->stats.requests += c.R;
-  FI_CUDA(cudaEventRecord(h->ev_pick, h->s_main));  // index updates submitted later wait for this pick
-  FI_CUDA(cudaEventRecord(h->ev_plain, h->s_main));
+  FI_CUDA(cudaEventRecord(h->ev_pick.get(), h->s_main.get()));  // index updates submitted later wait for this pick
+  FI_CUDA(cudaEventRecord(h->ev_plain.get(), h->s_main.get()));
   h->last_plain_R = c.R;
   return FI_OK;
 }
 
 // the next ticket: recorded on s_main behind everything queued there so far (the batch just enqueued)
 int issue_ticket(fi_epp* h, uint64_t* t) {
-  FI_CUDA(cudaEventRecord(h->ev_ticket[h->tickets % fi_epp::kTicketRing], h->s_main));
+  FI_CUDA(cudaEventRecord(h->ev_ticket[h->tickets % fi_epp::kTicketRing].get(), h->s_main.get()));
   *t = h->tickets++;
   return FI_OK;
 }
@@ -1570,60 +1566,64 @@ int submit_pick(fi_epp* h, const PickCall& c, cudaStream_t us, uint64_t* ticket,
   if (rc != FI_OK) return rc;
   rc = lagged ? check_counters_lagged(h, 0) : check_counters(h);
   if (rc != FI_OK) return rc;
-  if (!h->d_chain2) {
-    FI_CUDA(cudaMalloc(&h->d_chain2, (size_t)h->cfg.max_batch * h->MP * sizeof(uint64_t)));
-    FI_CUDA(cudaMalloc(&h->d_nblocks2, (size_t)h->cfg.max_batch * sizeof(uint32_t)));
+  if (!h->d_chain2) {  // slot 1's buffers, both or neither
+    DevPtr<uint64_t> chain;
+    DevPtr<uint32_t> nb;
+    FI_CUDA(cuda_alloc(chain, (size_t)h->cfg.max_batch * h->MP));
+    FI_CUDA(cuda_alloc(nb, h->cfg.max_batch));
+    h->d_chain2 = std::move(chain);
+    h->d_nblocks2 = std::move(nb);
   }
   // FI_EPP_TRACE=<call>: timeline of three consecutive pipelined batches (printed by fi_epp_pick_wait)
   if (!h->profiling && h->trace_call >= 0 && (long)h->stats.pick_calls >= h->trace_call &&
       (long)h->stats.pick_calls < h->trace_call + 3) {
     if ((long)h->stats.pick_calls == h->trace_call) {
-      if (!h->ev_trace0) cudaEventCreate(&h->ev_trace0);
-      FI_CUDA(cudaStreamSynchronize(h->s_main));
-      FI_CUDA(cudaStreamSynchronize(h->s_a));
-      FI_CUDA(cudaEventRecord(h->ev_trace0, h->s_main));
-      FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_trace0, 0));
+      if (!h->ev_trace0) cuda_create(h->ev_trace0, cudaEventDefault);
+      FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
+      FI_CUDA(cudaStreamSynchronize(h->s_a.get()));
+      FI_CUDA(cudaEventRecord(h->ev_trace0.get(), h->s_main.get()));
+      FI_CUDA(cudaStreamWaitEvent(h->s_a.get(), h->ev_trace0.get(), 0));
     }
     h->tracing = true;
   } else if (h->tracing && (long)h->stats.pick_calls >= h->trace_call + 3) {
     h->tracing = false;  // events stay queued until the dump
   }
   const uint32_t slot = (uint32_t)(h->pipe_seq & 1);
-  uint64_t* chain = slot ? h->d_chain2 : h->d_chain;
-  uint32_t* nb = slot ? h->d_nblocks2 : h->d_nblocks;
+  uint64_t* chain = slot ? h->d_chain2.get() : h->d_chain.get();
+  uint32_t* nb = slot ? h->d_nblocks2.get() : h->d_nblocks.get();
   // ---- stage A: inputs are ready in the caller's stream order; the slot's buffers are free once the
   // match of two batches ago is done; slot 0's d_chain / d_nblocks are free once the previous plain pick
   // (if any) is done; and the readers on other streams (claim_chain_slot0)
-  FI_CUDA(cudaEventRecord(h->ev_in, us));
-  FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_in, 0));
-  if (h->pipe_seq >= 2) FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_b[slot], 0));
-  FI_CUDA(cudaStreamWaitEvent(h->s_a, h->ev_plain, 0));
-  rc = wait_slot_readers(h, slot, h->s_a);
+  FI_CUDA(cudaEventRecord(h->ev_in.get(), us));
+  FI_CUDA(cudaStreamWaitEvent(h->s_a.get(), h->ev_in.get(), 0));
+  if (h->pipe_seq >= 2) FI_CUDA(cudaStreamWaitEvent(h->s_a.get(), h->ev_b[slot].get(), 0));
+  FI_CUDA(cudaStreamWaitEvent(h->s_a.get(), h->ev_plain.get(), 0));
+  rc = wait_slot_readers(h, slot, h->s_a.get());
   if (rc != FI_OK) return rc;
   {
     // Block hashing and chain walk in one kernel (hash_kernels.cu hash_chain).  It does not wait for the previous
     // batch's match_pick: a full batch runs half-SM CTAs, and one starts on an SM as soon as two of match's three
     // CTAs there have run out of queue (DESIGN.md §4.0; giving match fewer CTAs per SM so that the two kernels share
     // every SM for the whole step was measured slower: §7).
-    LaunchScope ls(h, h->s_a, K_HASH);
+    LaunchScope ls(h, h->s_a.get(), K_HASH);
     FI_CUDA(launch_hash_chain(c.prompts, c.offsets, c.h0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, chain, nb,
-                              h->sm_count, h->s_a));
+                              h->sm_count, h->s_a.get()));
   }
-  FI_CUDA(cudaEventRecord(h->ev_a[slot], h->s_a));
+  FI_CUDA(cudaEventRecord(h->ev_a[slot].get(), h->s_a.get()));
   // ---- stage B
   MatchParams mp;
   rc = prepare_match(h, c, chain, nb, mp);
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_a[slot], 0));
-  mp.work_counter = h->d_work + 8 + slot;
+  FI_CUDA(cudaStreamWaitEvent(h->s_main.get(), h->ev_a[slot].get(), 0));
+  mp.work_counter = h->d_work.get() + 8 + slot;
   {
-    LaunchScope ls(h, h->s_main, K_MATCH);
-    FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main));
+    LaunchScope ls(h, h->s_main.get(), K_MATCH);
+    FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main.get()));
   }
-  rc = copy_chains_out(h, chain, c.chains_out, R, cudaMemcpyDeviceToDevice, h->s_main);
+  rc = copy_chains_out(h, chain, c.chains_out, R, cudaMemcpyDeviceToDevice, h->s_main.get());
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_b[slot], h->s_main));
-  FI_CUDA(cudaEventRecord(h->ev_pick, h->s_main));
+  FI_CUDA(cudaEventRecord(h->ev_b[slot].get(), h->s_main.get()));
+  FI_CUDA(cudaEventRecord(h->ev_pick.get(), h->s_main.get()));
   rc = issue_ticket(h, ticket);
   if (rc != FI_OK) return rc;
   h->slot_ticket[slot] = *ticket;
@@ -1741,85 +1741,12 @@ void fi_epp_pinned_free(void* p) {
 
 const char* fi_epp_last_error(const fi_epp* h) { return h ? h->err.c_str() : "null handle"; }
 
+// Every resource of the handle has an owner among its members; the streams, declared first, go last.
 void fi_epp_destroy(fi_epp* h) {
   if (!h) return;
   cudaSetDevice(h->cfg.device);
-  if (h->s_main) cudaStreamSynchronize(h->s_main);
-  if (h->s_index) cudaStreamSynchronize(h->s_index);
-  if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
+  for (cudaStream_t s : {h->s_main.get(), h->s_index.get(), h->s_copy.get(), h->s_a.get()}) cudaStreamSynchronize(s);
   drain_profile(h);
-  for (auto e : h->ev_pool) cudaEventDestroy(e);
-  cudaFree(h->d_prompts);
-  cudaFree(h->d_offsets);
-  cudaFree(h->d_h0);
-  cudaFree(h->d_chain);
-  cudaFree(h->d_nblocks);
-  cudaFree(h->d_picks);
-  h->ranked.release();
-  h->subsets.release();
-  cudaFree(h->d_local);
-  cudaFree(h->d_gather);
-  cudaFree(h->d_glog_n);
-  cudaFree(h->d_glog_a);
-  cudaFree(h->d_glog_v);
-  cudaFree(h->d_ghdr);
-  cudaFree(h->d_ggather);
-  if (h->h_ghdr) cudaFreeHost(h->h_ghdr);
-  for (int k = 0; k < FI_MAX_RANKS; ++k)
-    if (h->peer_ipc[k]) cudaIpcCloseMemHandle(h->peer_ipc[k]);
-  cudaFree(h->d_xchg);
-  if (h->h_xerr) cudaFreeHost((void*)h->h_xerr);
-  cudaFree(h->d_probed);
-  cudaFree(h->d_work);
-  cudaFree(h->d_ctr);
-  cudaFree(h->d_rm);
-  cudaFree(h->d_eps);
-  cudaFree(h->d_sc);
-  cudaFree(h->d_elig);
-  cudaFree(h->d_zero);
-  cudaFree(h->d_ztie);
-  cudaFree(h->d_lora);
-  cudaFree(h->d_adapters);
-  if (h->h_adapters) cudaFreeHost(h->h_adapters);
-  h->pool.reset();
-  h->lrus.clear();
-  h->lru_arena.release();
-  free_dev_lru(h);
-  h->lru_plan_buf.release();
-  h->lru_chains.release();
-  h->lru_resize.release();
-  free_index(h->ix);
-  free_index(h->ix_spare);
-  for (int b = 0; b < 2; ++b) {
-    cudaFree(h->d_sets[b]);
-    cudaFree(h->d_clears[b]);
-    if (h->h_sets[b]) cudaFreeHost(h->h_sets[b]);
-    if (h->h_clears[b]) cudaFreeHost(h->h_clears[b]);
-    if (h->ev_buf[b]) cudaEventDestroy(h->ev_buf[b]);
-  }
-  if (h->h_picks) cudaFreeHost(h->h_picks);
-  if (h->h_offsets) cudaFreeHost(h->h_offsets);
-  if (h->h_h0) cudaFreeHost(h->h_h0);
-  if (h->h_nblocks) cudaFreeHost(h->h_nblocks);
-  if (h->h_ctr) cudaFreeHost(h->h_ctr);
-  for (cudaEvent_t e : {h->ev_index, h->ev_user, h->ev_done, h->ev_ctr})
-    if (e) cudaEventDestroy(e);
-  for (int k = 0; k < fi_epp::kMaxFeedSlices; ++k)
-    if (h->ev_copy[k]) cudaEventDestroy(h->ev_copy[k]);
-  for (cudaEvent_t e : {h->ev_in, h->ev_a[0], h->ev_a[1], h->ev_b[0], h->ev_b[1], h->ev_pick, h->ev_plain,
-                        h->ev_slot_read[0], h->ev_slot_read[1]})
-    if (e) cudaEventDestroy(e);
-  for (int k = 0; k < fi_epp::kTicketRing; ++k)
-    if (h->ev_ticket[k]) cudaEventDestroy(h->ev_ticket[k]);
-  for (fi_epp::PipeAdd& pa : h->padd) {
-    pa.plan.release();
-    cudaFree(pa.d_chains);
-    if (pa.ev_done) cudaEventDestroy(pa.ev_done);
-  }
-  cudaFree(h->d_chain2);
-  cudaFree(h->d_nblocks2);
-  for (cudaStream_t s : {h->s_main, h->s_index, h->s_copy, h->s_a})
-    if (s) cudaStreamDestroy(s);
   delete h;
 }
 
@@ -1848,8 +1775,7 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
   }
   auto die = [&](int rc) {
     std::fprintf(stderr, "fi_epp_create: %s\n", h->err.c_str());
-    fi_epp_destroy(up.release());
-    return rc;
+    return rc;  // (`up` releases whatever was created)
   };
 #define FI_TRY(call)                                                    \
   do {                                                                  \
@@ -1879,22 +1805,18 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
     if (h->cfg.index_slots > 0x80000000ull) h->cfg.index_slots = 0x80000000ull;
   }
 
-  FI_TRY(cudaStreamCreateWithFlags(&h->s_main, cudaStreamNonBlocking));
-  FI_TRY(cudaStreamCreateWithFlags(&h->s_index, cudaStreamNonBlocking));
-  FI_TRY(cudaStreamCreateWithFlags(&h->s_copy, cudaStreamNonBlocking));
-  FI_TRY(cudaStreamCreateWithFlags(&h->s_a, cudaStreamNonBlocking));
-  for (cudaEvent_t* e : {&h->ev_in, &h->ev_a[0], &h->ev_a[1], &h->ev_b[0], &h->ev_b[1], &h->ev_pick, &h->ev_plain,
-                         &h->ev_slot_read[0], &h->ev_slot_read[1]})
-    FI_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-  for (int k = 0; k < fi_epp::kTicketRing; ++k) FI_TRY(cudaEventCreateWithFlags(&h->ev_ticket[k], cudaEventDisableTiming));
-  for (int k = 0; k < fi_epp::kMaxFeedSlices; ++k) FI_TRY(cudaEventCreateWithFlags(&h->ev_copy[k], cudaEventDisableTiming));
+  for (Stream* s : {&h->s_main, &h->s_index, &h->s_copy, &h->s_a}) FI_TRY(cuda_create(*s));
+  for (Event* e : {&h->ev_in, &h->ev_a[0], &h->ev_a[1], &h->ev_b[0], &h->ev_b[1], &h->ev_pick, &h->ev_plain,
+                   &h->ev_slot_read[0], &h->ev_slot_read[1]})
+    FI_TRY(cuda_create(*e));
+  for (Event& e : h->ev_ticket) FI_TRY(cuda_create(e));
+  for (Event& e : h->ev_copy) FI_TRY(cuda_create(e));
   if (const char* e = std::getenv("FI_EPP_FEED_SLICES")) {
     const long v = std::strtol(e, nullptr, 10);
     h->feed_slices = (uint32_t)std::min<long>(std::max<long>(v, 1), fi_epp::kMaxFeedSlices);
   }
-  for (cudaEvent_t* e : {&h->ev_index, &h->ev_user, &h->ev_done, &h->ev_ctr})
-    FI_TRY(cudaEventCreateWithFlags(e, cudaEventDisableTiming));
-  FI_TRY(cudaEventRecord(h->ev_index, h->s_index));
+  for (Event* e : {&h->ev_index, &h->ev_user, &h->ev_done, &h->ev_ctr}) FI_TRY(cuda_create(*e));
+  FI_TRY(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   const uint64_t R = cfg->max_batch;
   // rows of the per-request buffers: whole groups of 32 requests (the sliced host feed and the split-hash gather
   // cut the batch on 32-request boundaries), and — for a shard of a bigger pool — room for the in-place all-gather
@@ -1902,37 +1824,37 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
   h->chain_rows = (uint32_t)((R + 31) / 32 * 32);
   if (cfg->endpoint_count < cfg->num_endpoints) h->chain_rows += 32 * (FI_MAX_RANKS + 1);
   if (const char* e = std::getenv("FI_EPP_SHARD_HASH")) h->split_hash = std::strcmp(e, "split") == 0;
-  FI_TRY(cudaMalloc(&h->d_prompts, h->cfg.max_prompt_bytes + 64));
-  FI_TRY(cudaMalloc(&h->d_offsets, (R + 1) * sizeof(uint64_t)));
-  FI_TRY(cudaMalloc(&h->d_h0, R * sizeof(uint64_t)));
-  FI_TRY(cudaMalloc(&h->d_chain, (size_t)h->chain_rows * h->MP * sizeof(uint64_t)));
-  FI_TRY(cudaMalloc(&h->d_nblocks, (size_t)h->chain_rows * sizeof(uint32_t)));
-  FI_TRY(cudaMalloc(&h->d_picks, R * h->P * sizeof(fi_pick)));
-  FI_TRY(cudaMalloc(&h->d_probed, 8 * sizeof(unsigned long long)));
-  FI_TRY(cudaMemset(h->d_probed, 0, 8 * sizeof(unsigned long long)));
-  FI_TRY(cudaMalloc(&h->d_work, 16 * sizeof(uint32_t)));
-  FI_TRY(cudaMemset(h->d_work, 0, 16 * sizeof(uint32_t)));
-  FI_TRY(cudaMallocHost(&h->h_picks, R * h->P * sizeof(fi_pick)));
-  FI_TRY(cudaMallocHost(&h->h_offsets, (R + 1) * sizeof(uint64_t)));
-  FI_TRY(cudaMallocHost(&h->h_h0, R * sizeof(uint64_t)));
-  FI_TRY(cudaMallocHost(&h->h_nblocks, R * sizeof(uint32_t)));
+  FI_TRY(cuda_alloc(h->d_prompts, h->cfg.max_prompt_bytes + 64));
+  FI_TRY(cuda_alloc(h->d_offsets, R + 1));
+  FI_TRY(cuda_alloc(h->d_h0, R));
+  FI_TRY(cuda_alloc(h->d_chain, (size_t)h->chain_rows * h->MP));
+  FI_TRY(cuda_alloc(h->d_nblocks, h->chain_rows));
+  FI_TRY(cuda_alloc(h->d_picks, R * h->P));
+  FI_TRY(cuda_alloc(h->d_probed, 8));
+  FI_TRY(cudaMemset(h->d_probed.get(), 0, 8 * sizeof(unsigned long long)));
+  FI_TRY(cuda_alloc(h->d_work, 16));
+  FI_TRY(cudaMemset(h->d_work.get(), 0, 16 * sizeof(uint32_t)));
+  FI_TRY(cuda_alloc(h->h_picks, R * h->P));
+  FI_TRY(cuda_alloc(h->h_offsets, R + 1));
+  FI_TRY(cuda_alloc(h->h_h0, R));
+  FI_TRY(cuda_alloc(h->h_nblocks, R));
 
   // index
-  FI_TRY(cudaMalloc(&h->d_ctr, sizeof(IndexCounters)));
-  FI_TRY(cudaMemset(h->d_ctr, 0, sizeof(IndexCounters)));
-  FI_TRY(cudaMallocHost(&h->h_ctr, sizeof(IndexCounters)));
-  std::memset(h->h_ctr, 0, sizeof(IndexCounters));
+  FI_TRY(cuda_alloc(h->d_ctr, 1));
+  FI_TRY(cudaMemset(h->d_ctr.get(), 0, sizeof(IndexCounters)));
+  FI_TRY(cuda_alloc(h->h_ctr, 1));
+  std::memset(h->h_ctr.get(), 0, sizeof(IndexCounters));
   {
-    int rc = alloc_index(h, h->cfg.index_slots, &h->ix);
+    int rc = alloc_index(h, h->cfg.index_slots, h->ix);
     if (rc != FI_OK) return die(rc);
   }
   for (int b = 0; b < 2; ++b) {
-    FI_TRY(cudaMallocHost(&h->h_sets[b], kOpChunk * sizeof(fi_index_op)));
-    FI_TRY(cudaMallocHost(&h->h_clears[b], kOpChunk * sizeof(fi_index_op)));
-    FI_TRY(cudaMalloc(&h->d_sets[b], kOpChunk * sizeof(fi_index_op)));
-    FI_TRY(cudaMalloc(&h->d_clears[b], kOpChunk * sizeof(fi_index_op)));
-    FI_TRY(cudaEventCreateWithFlags(&h->ev_buf[b], cudaEventDisableTiming));
-    FI_TRY(cudaEventRecord(h->ev_buf[b], h->s_index));
+    FI_TRY(cuda_alloc(h->h_sets[b], kOpChunk));
+    FI_TRY(cuda_alloc(h->h_clears[b], kOpChunk));
+    FI_TRY(cuda_alloc(h->d_sets[b], kOpChunk));
+    FI_TRY(cuda_alloc(h->d_clears[b], kOpChunk));
+    FI_TRY(cuda_create(h->ev_buf[b]));
+    FI_TRY(cudaEventRecord(h->ev_buf[b].get(), h->s_index.get()));
   }
   if (cfg->lru_capacity) {
     // virtual reservation only: an endpoint's tables become resident when it is first touched
@@ -1944,26 +1866,26 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
   // endpoints + score tables
   h->eps.assign(cfg->num_endpoints, EndpointDev{0.0, 0, 0, 0, 0});
   const uint32_t Epad = h->W * 32;
-  FI_TRY(cudaMalloc(&h->d_eps, (size_t)cfg->num_endpoints * sizeof(EndpointDev)));
-  FI_TRY(cudaMalloc(&h->d_sc, (size_t)FI_EPP_MAX_PROFILES * FI_EPP_MAX_SCORERS * Epad * sizeof(double)));
-  FI_TRY(cudaMalloc(&h->d_elig, (size_t)FI_EPP_MAX_PROFILES * h->W * sizeof(uint32_t)));
-  FI_TRY(cudaMalloc(&h->d_zero, FI_EPP_MAX_PROFILES * sizeof(ZeroBest)));
-  FI_TRY(cudaMalloc(&h->d_ztie, (size_t)FI_EPP_MAX_PROFILES * h->W * sizeof(uint32_t)));
-  FI_TRY(cudaMemset(h->d_ztie, 0, (size_t)FI_EPP_MAX_PROFILES * h->W * sizeof(uint32_t)));
-  FI_TRY(cudaMemset(h->d_sc, 0, (size_t)FI_EPP_MAX_PROFILES * FI_EPP_MAX_SCORERS * Epad * sizeof(double)));
-  FI_TRY(cudaMemset(h->d_elig, 0, (size_t)FI_EPP_MAX_PROFILES * h->W * sizeof(uint32_t)));
+  FI_TRY(cuda_alloc(h->d_eps, cfg->num_endpoints));
+  FI_TRY(cuda_alloc(h->d_sc, (size_t)FI_EPP_MAX_PROFILES * FI_EPP_MAX_SCORERS * Epad));
+  FI_TRY(cuda_alloc(h->d_elig, (size_t)FI_EPP_MAX_PROFILES * h->W));
+  FI_TRY(cuda_alloc(h->d_zero, FI_EPP_MAX_PROFILES));
+  FI_TRY(cuda_alloc(h->d_ztie, (size_t)FI_EPP_MAX_PROFILES * h->W));
+  FI_TRY(cudaMemset(h->d_ztie.get(), 0, (size_t)FI_EPP_MAX_PROFILES * h->W * sizeof(uint32_t)));
+  FI_TRY(cudaMemset(h->d_sc.get(), 0, (size_t)FI_EPP_MAX_PROFILES * FI_EPP_MAX_SCORERS * Epad * sizeof(double)));
+  FI_TRY(cudaMemset(h->d_elig.get(), 0, (size_t)FI_EPP_MAX_PROFILES * h->W * sizeof(uint32_t)));
   h->st.n_profiles = h->P;
   h->st.Epad = Epad;
-  h->st.sc = h->d_sc;
-  h->st.elig = h->d_elig;
-  h->st.zero = h->d_zero;
-  h->st.ztie = h->d_ztie;
+  h->st.sc = h->d_sc.get();
+  h->st.elig = h->d_elig.get();
+  h->st.zero = h->d_zero.get();
+  h->st.ztie = h->d_ztie.get();
   h->lora.assign(Epad, LoraDev{});
-  FI_TRY(cudaMalloc(&h->d_lora, (size_t)Epad * sizeof(LoraDev)));
-  FI_TRY(cudaMemset(h->d_lora, 0, (size_t)Epad * sizeof(LoraDev)));
-  FI_TRY(cudaMalloc(&h->d_adapters, R * sizeof(uint64_t)));
-  FI_TRY(cudaMallocHost(&h->h_adapters, R * sizeof(uint64_t)));
-  h->st.lora = h->d_lora;
+  FI_TRY(cuda_alloc(h->d_lora, Epad));
+  FI_TRY(cudaMemset(h->d_lora.get(), 0, (size_t)Epad * sizeof(LoraDev)));
+  FI_TRY(cuda_alloc(h->d_adapters, R));
+  FI_TRY(cuda_alloc(h->h_adapters, R));
+  h->st.lora = h->d_lora.get();
   h->st.has_lora = 0;
   for (uint32_t p = 0; p < h->P; ++p)
     for (uint32_t s = 0; s < cfg->profiles[p].n_scorers; ++s)
@@ -1979,7 +1901,7 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
       d.weight[s] = (double)cfg->profiles[p].scorers[s].weight;
     }
   }
-  FI_TRY(cudaStreamSynchronize(h->s_index));
+  FI_TRY(cudaStreamSynchronize(h->s_index.get()));
   FI_TRY(cudaDeviceSynchronize());
 #undef FI_TRY
   *out = up.release();
@@ -2109,33 +2031,33 @@ int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t
   if (rc != FI_OK) return rc;
   rc = check_counters(h);
   if (rc != FI_OK) return rc;
-  if (!h->d_rm) FI_CUDA(cudaMalloc(&h->d_rm, sizeof(unsigned long long) + (size_t)EL * sizeof(uint32_t)));
-  uint32_t* d_eps = reinterpret_cast<uint32_t*>(h->d_rm + 1);
+  if (!h->d_rm) FI_CUDA(cuda_alloc(h->d_rm, 1 + ((size_t)EL + 1) / 2));
+  uint32_t* d_eps = reinterpret_cast<uint32_t*>(h->d_rm.get() + 1);
   // picks called before this one must not see the removal
-  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_pick, 0));
-  FI_CUDA(cudaMemsetAsync(h->d_rm, 0, sizeof(unsigned long long), h->s_index));
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
+  FI_CUDA(cudaMemsetAsync(h->d_rm.get(), 0, sizeof(unsigned long long), h->s_index.get()));
   {
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_index_remove_sweep(h->ix, h->d_ctr, rs, remove_whole_rows(rs, h->W), h->rank, h->d_rm, h->sm_count, h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_index_remove_sweep(h->ix.v, h->d_ctr.get(), rs, remove_whole_rows(rs, h->W), h->rank, h->d_rm.get(), h->sm_count, h->s_index.get()));
   }
-  if (h->lru_mode == 1 && h->dlru_ready) {
+  if (h->lru_mode == 1 && h->dlru) {
     // (pageable source: the copy has taken the data when cudaMemcpyAsync returns)
-    FI_CUDA(cudaMemcpyAsync(d_eps, local.data(), local.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index));
+    FI_CUDA(cudaMemcpyAsync(d_eps, local.data(), local.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
     h->stats.h2d_bytes += local.size() * sizeof(uint32_t);
-    LaunchScope ls(h, h->s_index, K_INDEX);
-    FI_CUDA(launch_lru_reset(h->dlru, d_eps, (uint32_t)local.size(), h->s_index));
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_lru_reset(h->dlru->v, d_eps, (uint32_t)local.size(), h->s_index.get()));
   }
   for (uint32_t e : local)
     if (e < h->lrus.size()) h->lrus[e].clear();
   // the sweep's tombstones reach the rebuild decision of the next index update
-  FI_CUDA(cudaMemcpyAsync(h->h_ctr, h->d_ctr, sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index));
-  FI_CUDA(cudaEventRecord(h->ev_ctr, h->s_index));
+  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
   h->ctr_pending = true;
-  FI_CUDA(cudaEventRecord(h->ev_index, h->s_index));
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   if (pairs_removed) {
     unsigned long long c = 0;
-    FI_CUDA(cudaMemcpyAsync(&c, h->d_rm, sizeof(c), cudaMemcpyDeviceToHost, h->s_index));
-    FI_CUDA(cudaStreamSynchronize(h->s_index));
+    FI_CUDA(cudaMemcpyAsync(&c, h->d_rm.get(), sizeof(c), cudaMemcpyDeviceToHost, h->s_index.get()));
+    FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
     *pairs_removed = c;
   }
   return FI_OK;
@@ -2179,7 +2101,7 @@ int fi_epp_set_lru_capacities(fi_epp* h, const uint32_t* endpoints, const uint32
   rc = check_counters(h);
   if (rc != FI_OK) return rc;
   uint64_t evicted = 0;
-  if (h->lru_mode == 1 && h->dlru_ready) {
+  if (h->lru_mode == 1 && h->dlru) {
     rc = lru_device_resize(h, local, caps, &evicted);
     if (rc != FI_OK) return rc;
   }
@@ -2197,7 +2119,7 @@ int fi_epp_set_lru_capacities(fi_epp* h, const uint32_t* endpoints, const uint32
   if (entries_evicted) {
     rc = flush_ops(h);
     if (rc != FI_OK) return rc;
-    FI_CUDA(cudaStreamSynchronize(h->s_index));
+    FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
     rc = check_counters(h);  // (a broken device-LRU invariant would show here)
     if (rc != FI_OK) return rc;
     *entries_evicted = evicted;
@@ -2322,7 +2244,7 @@ int fi_epp_index_add_chains(fi_epp* h, const uint32_t* endpoints, const uint64_t
             const size_t room = (size_t)(kOpChunk - fillc);
             const size_t take = std::min(room, v.size() - done);
             if (!dry && take) {
-              fi_index_op* base = kind == 0 ? h->h_sets[h->cur_buf] : h->h_clears[h->cur_buf];
+              fi_index_op* base = kind == 0 ? h->h_sets[h->cur_buf].get() : h->h_clears[h->cur_buf].get();
               jobs.push_back(CopyJob{base + fillc, v.data() + done, take});
             }
             fillc += take;
@@ -2401,7 +2323,7 @@ int fi_epp_index_add_chains_device(fi_epp* h, const uint32_t* endpoints, const v
   if (!h->cfg.lru_capacity) return fail(h, FI_ERR_STATE, "lru_capacity is 0: no LRU");
   if (!d_chains) {  // the chains of the handle's most recent stream-ordered pick, still in its own buffer
     if (R > h->last_plain_R) return fail(h, FI_ERR_STATE, "no pick batch of that size to take the chains from");
-    d_chains = h->d_chain;
+    d_chains = h->d_chain.get();
     pitch_blocks = h->MP;
   }
   for (uint32_t r = 0; r < R; ++r) {
@@ -2412,8 +2334,8 @@ int fi_epp_index_add_chains_device(fi_epp* h, const uint32_t* endpoints, const v
   if (rc != FI_OK) return rc;
   if (h->lru_mode != 1) return fail(h, FI_ERR_STATE, "fi_epp_index_add_chains_device needs the device LRU");
   // the chains were produced on the caller's stream
-  FI_CUDA(cudaEventRecord(h->ev_user, (cudaStream_t)stream));
-  FI_CUDA(cudaStreamWaitEvent(h->s_index, h->ev_user, 0));
+  FI_CUDA(cudaEventRecord(h->ev_user.get(), (cudaStream_t)stream));
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_user.get(), 0));
   return lru_device_add(h, endpoints, static_cast<const uint64_t*>(d_chains), true, pitch_blocks, nblocks, R);
 }
 
@@ -2425,22 +2347,16 @@ int fi_epp_lru_dump(fi_epp* h, uint32_t endpoint, uint64_t* out, uint32_t cap, u
   *n_out = 0;
   const uint32_t e = endpoint - h->cfg.endpoint_begin;
   if (e >= h->cfg.endpoint_count) return fail(h, FI_ERR_INVALID, "endpoint outside this handle's shard");
-  if (h->lru_mode != 1 || !h->dlru_ready) return h->lru_mode == 0 ? fail(h, FI_ERR_STATE, "the handle runs the host LRU") : FI_OK;
-  uint64_t* d_out = nullptr;
-  uint32_t* d_n = nullptr;
-  FI_CUDA(cudaMalloc(&d_out, ((size_t)h->dlru.capacity + 1) * sizeof(uint64_t)));
-  if (cudaMalloc(&d_n, sizeof(uint32_t)) != cudaSuccess) {
-    cudaFree(d_out);
-    return fail(h, FI_ERR_NOMEM, "cudaMalloc failed");
-  }
+  if (h->lru_mode != 1 || !h->dlru) return h->lru_mode == 0 ? fail(h, FI_ERR_STATE, "the handle runs the host LRU") : FI_OK;
+  DevPtr<uint64_t> d_out;
+  DevPtr<uint32_t> d_n;
+  FI_CUDA(cuda_alloc(d_out, (size_t)h->dlru->v.capacity + 1));
+  if (cuda_alloc(d_n, 1) != cudaSuccess) return fail(h, FI_ERR_NOMEM, "cudaMalloc failed");
   uint32_t n = 0;
-  cudaError_t er = launch_lru_dump(h->dlru, e, d_out, d_n, h->s_index);
-  if (er == cudaSuccess) er = cudaMemcpyAsync(&n, d_n, sizeof(n), cudaMemcpyDeviceToHost, h->s_index);
-  if (er == cudaSuccess) er = cudaStreamSynchronize(h->s_index);
-  if (er == cudaSuccess && n) er = cudaMemcpy(out, d_out, (size_t)std::min(n, cap) * sizeof(uint64_t), cudaMemcpyDeviceToHost);
-  cudaFree(d_out);
-  cudaFree(d_n);
-  if (er != cudaSuccess) return fail(h, FI_ERR_CUDA, cudaGetErrorString(er));
+  FI_CUDA(launch_lru_dump(h->dlru->v, e, d_out.get(), d_n.get(), h->s_index.get()));
+  FI_CUDA(cudaMemcpyAsync(&n, d_n.get(), sizeof(n), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
+  if (n) FI_CUDA(cudaMemcpy(out, d_out.get(), (size_t)std::min(n, cap) * sizeof(uint64_t), cudaMemcpyDeviceToHost));
   *n_out = n;
   return FI_OK;
 }
@@ -2452,12 +2368,12 @@ int fi_epp_lru_counters(fi_epp* h, uint64_t out[6]) {
   std::lock_guard<std::mutex> lk(h->mu);
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   for (int i = 0; i < 6; ++i) out[i] = 0;
-  if (h->lru_mode != 1 || !h->dlru_ready) return FI_OK;
-  FI_CUDA(cudaStreamSynchronize(h->s_index));
-  out[0] = h->h_lru_stat->n_sets;
-  out[1] = h->h_lru_stat->n_clears;
-  out[2] = h->h_lru_stat->n_doomed;
-  out[3] = h->h_lru_stat->n_maintained;
+  if (h->lru_mode != 1 || !h->dlru) return FI_OK;
+  FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
+  out[0] = h->dlru->stat->n_sets;
+  out[1] = h->dlru->stat->n_clears;
+  out[2] = h->dlru->stat->n_doomed;
+  out[3] = h->dlru->stat->n_maintained;
   out[4] = h->lru_deferred;
   out[5] = h->lru_sub_batches;
   return FI_OK;
@@ -2469,7 +2385,7 @@ int fi_epp_index_sync(fi_epp* h) {
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   int rc = flush_ops(h);
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaStreamSynchronize(h->s_index));
+  FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
   return check_counters(h);
 }
 
@@ -2479,20 +2395,20 @@ int fi_epp_index_stats(fi_epp* h, fi_index_stats* out) {
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   int rc = flush_ops(h);
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaStreamSynchronize(h->s_index));
+  FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
   IndexCounters c;
-  FI_CUDA(cudaMemcpy(&c, h->d_ctr, sizeof(c), cudaMemcpyDeviceToHost));
-  out->slots = h->ix.C;
+  FI_CUDA(cudaMemcpy(&c, h->d_ctr.get(), sizeof(c), cudaMemcpyDeviceToHost));
+  out->slots = h->ix.v.C;
   out->used = c.used;
   out->tombstones = c.tombstones;
   out->rebuilds = h->rebuilds;
   out->ops_applied = h->ops_applied;
   uint64_t l = 0;
-  if (h->lru_mode == 1 && h->dlru_ready) {
-    std::vector<uint32_t> cnt(h->dlru.EL);
-    FI_CUDA(cudaMemcpy(cnt.data(), h->dlru.count, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
+  if (h->lru_mode == 1 && h->dlru) {
+    std::vector<uint32_t> cnt(h->dlru->v.EL);
+    FI_CUDA(cudaMemcpy(cnt.data(), h->dlru->v.count, cnt.size() * sizeof(uint32_t), cudaMemcpyDeviceToHost));
     for (uint32_t c2 : cnt) l += c2;
-    out->ops_applied += h->h_lru_stat->n_sets + h->h_lru_stat->n_clears;
+    out->ops_applied += h->dlru->stat->n_sets + h->dlru->stat->n_clears;
   } else {
     for (auto& s : h->lrus) l += s.size();
   }
@@ -2508,23 +2424,17 @@ int fi_epp_index_contains(fi_epp* h, const fi_index_op* q, uint64_t n, uint8_t* 
   int rc = flush_ops(h);
   if (rc != FI_OK) return rc;
   if (n == 0) return FI_OK;
-  fi_index_op* dq = nullptr;
-  uint8_t* dout = nullptr;
-  FI_CUDA(cudaMalloc(&dq, n * sizeof(fi_index_op)));
-  if (cudaMalloc(&dout, n) != cudaSuccess) {
-    cudaFree(dq);
-    return fail(h, FI_ERR_NOMEM, "cudaMalloc failed");
+  DevPtr<fi_index_op> dq;
+  DevPtr<uint8_t> dout;
+  FI_CUDA(cuda_alloc(dq, n));
+  if (cuda_alloc(dout, n) != cudaSuccess) return fail(h, FI_ERR_NOMEM, "cudaMalloc failed");
+  FI_CUDA(cudaMemcpyAsync(dq.get(), q, n * sizeof(fi_index_op), cudaMemcpyHostToDevice, h->s_index.get()));
+  {
+    LaunchScope ls(h, h->s_index.get(), K_OTHER);
+    FI_CUDA(launch_index_contains(h->ix.v, dq.get(), n, h->cfg.endpoint_begin, h->cfg.endpoint_count, dout.get(), h->s_index.get()));
   }
-  cudaError_t e = cudaMemcpyAsync(dq, q, n * sizeof(fi_index_op), cudaMemcpyHostToDevice, h->s_index);
-  if (e == cudaSuccess) {
-    LaunchScope ls(h, h->s_index, K_OTHER);
-    e = launch_index_contains(h->ix, dq, n, h->cfg.endpoint_begin, h->cfg.endpoint_count, dout, h->s_index);
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out, dout, n, cudaMemcpyDeviceToHost, h->s_index);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->s_index);
-  cudaFree(dq);
-  cudaFree(dout);
-  if (e != cudaSuccess) return fail(h, FI_ERR_CUDA, cudaGetErrorString(e));
+  FI_CUDA(cudaMemcpyAsync(out, dout.get(), n, cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
   return FI_OK;
 }
 
@@ -2540,12 +2450,12 @@ static int check_batch(fi_epp* h, const uint64_t* offsets, uint32_t R, uint64_t*
 
 static int stage_inputs(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
                         uint64_t total, bool copy_prompts = true) {
-  std::memcpy(h->h_offsets, offsets, (size_t)(R + 1) * sizeof(uint64_t));
-  std::memcpy(h->h_h0, h0, (size_t)R * sizeof(uint64_t));
-  FI_CUDA(cudaMemcpyAsync(h->d_offsets, h->h_offsets, (size_t)(R + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main));
-  FI_CUDA(cudaMemcpyAsync(h->d_h0, h->h_h0, (size_t)R * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main));
+  std::memcpy(h->h_offsets.get(), offsets, (size_t)(R + 1) * sizeof(uint64_t));
+  std::memcpy(h->h_h0.get(), h0, (size_t)R * sizeof(uint64_t));
+  FI_CUDA(cudaMemcpyAsync(h->d_offsets.get(), h->h_offsets.get(), (size_t)(R + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main.get()));
+  FI_CUDA(cudaMemcpyAsync(h->d_h0.get(), h->h_h0.get(), (size_t)R * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main.get()));
   if (total && copy_prompts) {
-    FI_CUDA(cudaMemcpyAsync(h->d_prompts, prompts, total, cudaMemcpyHostToDevice, h->s_main));
+    FI_CUDA(cudaMemcpyAsync(h->d_prompts.get(), prompts, total, cudaMemcpyHostToDevice, h->s_main.get()));
     h->stats.h2d_bytes += total;
   }
   h->stats.h2d_bytes += (size_t)(2 * R + 1) * sizeof(uint64_t);
@@ -2563,19 +2473,19 @@ int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets
   if (rc != FI_OK) return rc;
   rc = stage_inputs(h, prompts, offsets, h0, R, total);
   if (rc != FI_OK) return rc;
-  rc = claim_chain_slot0(h, h->s_main);
+  rc = claim_chain_slot0(h, h->s_main.get());
   if (rc != FI_OK) return rc;
   h->last_plain_R = 0;  // d_chain no longer holds a pick batch's chains
-  rc = run_hash(h, h->d_prompts, h->d_offsets, h->d_h0, 0, R, h->s_main);
+  rc = run_hash(h, h->d_prompts.get(), h->d_offsets.get(), h->d_h0.get(), 0, R, h->s_main.get());
   if (rc != FI_OK) return rc;
-  rc = copy_chains_out(h, h->d_chain, chains_out, R, cudaMemcpyDeviceToHost, h->s_main);
+  rc = copy_chains_out(h, h->d_chain.get(), chains_out, R, cudaMemcpyDeviceToHost, h->s_main.get());
   if (rc != FI_OK) return rc;
   if (nblocks_out) {
-    FI_CUDA(cudaMemcpyAsync(h->h_nblocks, h->d_nblocks, (size_t)R * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_main));
+    FI_CUDA(cudaMemcpyAsync(h->h_nblocks.get(), h->d_nblocks.get(), (size_t)R * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_main.get()));
     h->stats.d2h_bytes += (size_t)R * sizeof(uint32_t);
   }
-  FI_CUDA(cudaStreamSynchronize(h->s_main));
-  if (nblocks_out) std::memcpy(nblocks_out, h->h_nblocks, (size_t)R * sizeof(uint32_t));
+  FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
+  if (nblocks_out) std::memcpy(nblocks_out, h->h_nblocks.get(), (size_t)R * sizeof(uint32_t));
   return FI_OK;
 }
 
@@ -2610,24 +2520,24 @@ static int pick_host(fi_epp* h, const PickCall& c) {
   uint64_t total = 0;
   rc = check_batch(h, c.offsets, R, &total);
   if (rc != FI_OK) return rc;
-  PickCall d{h->d_prompts, h->d_offsets, h->d_h0, nullptr, nullptr, R, c.k, h->d_picks, nullptr};  // on device buffers
-  fi_pick* h_out = h->h_picks;
+  PickCall d{h->d_prompts.get(), h->d_offsets.get(), h->d_h0.get(), nullptr, nullptr, R, c.k, h->d_picks.get(), nullptr};  // on device buffers
+  fi_pick* h_out = h->h_picks.get();
   if (c.k) {
     // the k-wide result buffers exist only on handles that rank; sized for max_batch so that R does not regrow them
     const size_t need = (size_t)h->cfg.max_batch * h->P * c.k;
-    if (need > h->ranked.cap) FI_CUDA(cudaStreamSynchronize(h->s_main));
+    if (need > h->ranked.cap) FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
     rc = grow_staging(h, h->ranked, need, need, true);
     if (rc != FI_OK) return rc;
-    d.out = h->ranked.d;
-    h_out = h->ranked.h;
+    d.out = h->ranked.d.get();
+    h_out = h->ranked.h.get();
   }
   rc = stage_inputs(h, c.prompts, c.offsets, c.h0, R, total, /*copy_prompts=*/false);
   if (rc != FI_OK) return rc;
   if (c.adapters) {
-    std::memcpy(h->h_adapters, c.adapters, (size_t)R * sizeof(uint64_t));
-    FI_CUDA(cudaMemcpyAsync(h->d_adapters, h->h_adapters, (size_t)R * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main));
+    std::memcpy(h->h_adapters.get(), c.adapters, (size_t)R * sizeof(uint64_t));
+    FI_CUDA(cudaMemcpyAsync(h->d_adapters.get(), h->h_adapters.get(), (size_t)R * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_main.get()));
     h->stats.h2d_bytes += (size_t)R * sizeof(uint64_t);
-    d.adapters = h->d_adapters;
+    d.adapters = h->d_adapters.get();
   }
   if (c.subsets) {
     // the bitset staging exists only on handles that restrict picks; sized for max_batch
@@ -2635,21 +2545,22 @@ static int pick_host(fi_epp* h, const PickCall& c) {
     rc = grow_staging(h, h->subsets, rows, rows, true);
     if (rc != FI_OK) return rc;
     const size_t sb = (size_t)R * pitch * sizeof(uint32_t);
-    std::memcpy(h->subsets.h, c.subsets, sb);
-    FI_CUDA(cudaMemcpyAsync(h->subsets.d, h->subsets.h, sb, cudaMemcpyHostToDevice, h->s_main));
+    std::memcpy(h->subsets.h.get(), c.subsets, sb);
+    FI_CUDA(cudaMemcpyAsync(h->subsets.d.get(), h->subsets.h.get(), sb, cudaMemcpyHostToDevice, h->s_main.get()));
     h->stats.h2d_bytes += sb;
-    d.subsets = h->subsets.d;
+    d.subsets = h->subsets.d.get();
   }
   rc = run_pick(h, d, &c);
   if (rc != FI_OK) return rc;
   const size_t pb = (size_t)R * h->P * std::max(c.k, 1u) * sizeof(fi_pick);
-  FI_CUDA(cudaMemcpyAsync(h_out, d.out, pb, cudaMemcpyDeviceToHost, h->s_main));
+  FI_CUDA(cudaMemcpyAsync(h_out, d.out, pb, cudaMemcpyDeviceToHost, h->s_main.get()));
   h->stats.d2h_bytes += pb;
-  rc = copy_chains_out(h, h->d_chain, c.chains_out, R, cudaMemcpyDeviceToHost, h->s_main);
+  rc = copy_chains_out(h, h->d_chain.get(), c.chains_out, R, cudaMemcpyDeviceToHost, h->s_main.get());
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaStreamSynchronize(h->s_main));
-  if (h->h_xerr && *h->h_xerr) {  // (sharded) reported once; the tags are monotonic, so later steps can succeed again
-    *h->h_xerr = 0;
+  FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
+  volatile uint32_t* xerr = h->shard ? h->shard->h_xerr.get() : nullptr;
+  if (xerr && *xerr) {  // (sharded) reported once; the tags are monotonic, so later steps can succeed again
+    *xerr = 0;
     return fail(h, FI_ERR_COMM, "peer exchange timed out waiting for another rank");
   }
   std::memcpy(c.out, h_out, pb);
@@ -2664,14 +2575,14 @@ static int pick_device(fi_epp* h, const PickCall& c, void* stream) {
   int rc = check_pick_handle(h, c);
   if (rc != FI_OK || c.R == 0) return rc;
   cudaStream_t us = (cudaStream_t)stream;
-  FI_CUDA(cudaEventRecord(h->ev_user, us));
-  FI_CUDA(cudaStreamWaitEvent(h->s_main, h->ev_user, 0));
+  FI_CUDA(cudaEventRecord(h->ev_user.get(), us));
+  FI_CUDA(cudaStreamWaitEvent(h->s_main.get(), h->ev_user.get(), 0));
   rc = run_pick(h, c, nullptr);
   if (rc != FI_OK) return rc;
-  rc = copy_chains_out(h, h->d_chain, c.chains_out, c.R, cudaMemcpyDeviceToDevice, h->s_main);
+  rc = copy_chains_out(h, h->d_chain.get(), c.chains_out, c.R, cudaMemcpyDeviceToDevice, h->s_main.get());
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_done, h->s_main));
-  FI_CUDA(cudaStreamWaitEvent(us, h->ev_done, 0));
+  FI_CUDA(cudaEventRecord(h->ev_done.get(), h->s_main.get()));
+  FI_CUDA(cudaStreamWaitEvent(us, h->ev_done.get(), 0));
   return FI_OK;
 }
 
@@ -2777,7 +2688,7 @@ int fi_epp_pick_wait(fi_epp* h, void* stream) {
   if (!h) return FI_ERR_INVALID;
   std::lock_guard<std::mutex> lk(h->mu);
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  FI_CUDA(cudaStreamWaitEvent((cudaStream_t)stream, h->ev_pick, 0));  // s_main runs the batches in order
+  FI_CUDA(cudaStreamWaitEvent((cudaStream_t)stream, h->ev_pick.get(), 0));  // s_main runs the batches in order
   if (!h->profiling && !h->pending_ev.empty() && h->ev_trace0) {
     h->tracing = true;
     dump_trace(h, 0);
@@ -2793,7 +2704,7 @@ int fi_epp_pick_wait_batch(fi_epp* h, uint64_t ticket, void* stream) {
   // s_main completes the batches in order: a ticket older than the ring is done by the oldest one it still tracks
   const uint64_t oldest = h->tickets - std::min<uint64_t>(h->tickets, fi_epp::kTicketRing);
   const uint64_t t = std::max(ticket, oldest);
-  FI_CUDA(cudaStreamWaitEvent((cudaStream_t)stream, h->ev_ticket[t % fi_epp::kTicketRing], 0));
+  FI_CUDA(cudaStreamWaitEvent((cudaStream_t)stream, h->ev_ticket[t % fi_epp::kTicketRing].get(), 0));
   if (!h->profiling && !h->pending_ev.empty() && h->ev_trace0) {
     h->tracing = true;
     dump_trace(h, 0);
@@ -2847,7 +2758,7 @@ int fi_epp_comm_init(fi_epp* h, const uint8_t id_bytes[FI_EPP_UNIQUE_ID_BYTES], 
   if (!h || !id_bytes || world == 0 || rank >= world) return FI_ERR_INVALID;
   std::lock_guard<std::mutex> lk(h->mu);
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  if (h->comm) return fail(h, FI_ERR_STATE, "communicator already initialised");
+  if (h->shard) return fail(h, FI_ERR_STATE, "communicator already initialised");
   if (world > 32) return fail(h, FI_ERR_INVALID, "more than 32 ranks: the directory keeps one presence bit per rank");
   if (h->ops_applied || h->n_sets || h->n_clears)
     return fail(h, FI_ERR_STATE, "fi_epp_comm_init must precede the first index update (the directory is built by gossip)");
@@ -2861,27 +2772,33 @@ int fi_epp_comm_init(fi_epp* h, const uint8_t id_bytes[FI_EPP_UNIQUE_ID_BYTES], 
     std::string e;
     if (!g_nccl.load(&e)) return fail(h, FI_ERR_COMM, e);
   }
+  // the shard state is built whole before the handle takes it: a failed call leaves a single-rank handle
+  auto sh = std::make_unique<ShardState>();
   ncclUniqueId id;
   std::memcpy(&id, id_bytes, sizeof(id));
-  int rc = g_nccl.CommInitRank(&h->comm, (int)world, id, (int)rank);
+  int rc = g_nccl.CommInitRank(&sh->comm, (int)world, id, (int)rank);
   if (rc != ncclSuccess) {
-    h->comm = nullptr;
+    sh->comm = nullptr;
     return fail(h, FI_ERR_COMM, std::string("ncclCommInitRank: ") + (g_nccl.GetErrorString ? g_nccl.GetErrorString(rc) : "error"));
   }
   const uint64_t R = h->cfg.max_batch;
-  FI_CUDA(cudaMalloc(&h->d_local, R * h->P * sizeof(fi_pick)));
-  FI_CUDA(cudaMalloc(&h->d_gather, (size_t)world * R * h->P * sizeof(fi_pick)));
-  // directory gossip (index_kernels.cu): this rank's transition log + gather buffers
-  FI_CUDA(cudaMalloc(&h->d_glog_n, 2 * sizeof(unsigned long long)));
-  FI_CUDA(cudaMemset(h->d_glog_n, 0, 2 * sizeof(unsigned long long)));
-  FI_CUDA(cudaMalloc(&h->d_glog_a, kOpChunk * sizeof(uint64_t)));
-  FI_CUDA(cudaMalloc(&h->d_glog_v, kOpChunk * sizeof(uint64_t)));
-  FI_CUDA(cudaMalloc(&h->d_ghdr, (size_t)(world + 1) * 2 * sizeof(unsigned long long)));
-  FI_CUDA(cudaMallocHost(&h->h_ghdr, (size_t)(world + 1) * 2 * sizeof(unsigned long long)));
-  FI_CUDA(cudaMalloc(&h->d_ggather, (size_t)world * kOpChunk * sizeof(uint64_t)));
+  FI_CUDA(cuda_alloc(sh->d_local, R * h->P));
+  FI_CUDA(cuda_alloc(sh->d_gather, (size_t)world * R * h->P));
+  FI_CUDA(cuda_alloc(sh->d_glog_n, 2));
+  FI_CUDA(cudaMemset(sh->d_glog_n.get(), 0, 2 * sizeof(unsigned long long)));
+  FI_CUDA(cuda_alloc(sh->d_glog_a, kOpChunk));
+  FI_CUDA(cuda_alloc(sh->d_glog_v, kOpChunk));
+  FI_CUDA(cuda_alloc(sh->d_ghdr, (size_t)(world + 1) * 2));
+  FI_CUDA(cuda_alloc(sh->h_ghdr, (size_t)(world + 1) * 2));
+  FI_CUDA(cuda_alloc(sh->d_ggather, (size_t)world * kOpChunk));
+  PeerXchg px{};
+  rc = setup_peer_exchange(h, *sh, rank, world, &px);
+  if (rc != FI_OK) return rc;
+  h->shard = std::move(sh);
+  h->px = px;
   h->rank = rank;
   h->world = world;
-  return setup_peer_exchange(h);
+  return FI_OK;
 }
 
 int fi_epp_comm_exchange(fi_epp* h) {
@@ -2924,7 +2841,7 @@ int fi_epp_set_option(fi_epp* h, const char* name, int64_t value) {
   }
   if (n == "lru_table_slots") {
     if (value < 0 || value > (1ll << 30)) return fail(h, FI_ERR_INVALID, "lru_table_slots: 0 .. 2^30");
-    if (h->dlru_ready) return fail(h, FI_ERR_STATE, "lru_table_slots: the device LRU is already allocated");
+    if (h->dlru) return fail(h, FI_ERR_STATE, "lru_table_slots: the device LRU is already allocated");
     h->lru_table_slots = (uint32_t)value;
     return FI_OK;
   }
@@ -2952,9 +2869,9 @@ int fi_epp_get_stats(fi_epp* h, fi_epp_stats* out) {
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   drain_profile(h);
   if (h->profiling) {
-    FI_CUDA(cudaStreamSynchronize(h->s_main));
+    FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
     unsigned long long pb[8] = {0};
-    FI_CUDA(cudaMemcpy(pb, h->d_probed, sizeof(pb), cudaMemcpyDeviceToHost));
+    FI_CUDA(cudaMemcpy(pb, h->d_probed.get(), sizeof(pb), cudaMemcpyDeviceToHost));
     h->stats.probed_blocks = pb[0];
     if (pb[5] && h->verbose)  // FI_MATCH_TIMING build: where a request's time goes inside match_pick
       std::fprintf(stderr, "[fi_epp] match_pick phases, cycles per request over %llu requests: stage %.0f, first lookup %.0f, "
@@ -2970,8 +2887,8 @@ int fi_epp_reset_stats(fi_epp* h) {
   std::lock_guard<std::mutex> lk(h->mu);
   cudaSetDevice(h->cfg.device);
   drain_profile(h);
-  cudaStreamSynchronize(h->s_main);
-  cudaMemset(h->d_probed, 0, 8 * sizeof(unsigned long long));
+  cudaStreamSynchronize(h->s_main.get());
+  cudaMemset(h->d_probed.get(), 0, 8 * sizeof(unsigned long long));
   h->stats = fi_epp_stats{};
   return FI_OK;
 }
