@@ -267,9 +267,11 @@ struct fi_epp {
   PinnedPtr<fi_index_op> h_sets[2], h_clears[2];
   DevPtr<fi_index_op> d_sets[2], d_clears[2];
   Event ev_buf[2];
+  // the open op group (submit_op states the rule that keeps it exact)
   int cur_buf = 0;
   uint64_t n_sets = 0, n_clears = 0;
   std::unordered_set<PairKey, PairHash> cleared;
+  bool clears_untracked = false;
   // fi_epp_index_remove_endpoints: [0] pairs removed, then (u32) the local endpoints whose device LRU is reset.
   // Allocated at the first call.
   DevPtr<unsigned long long> d_rm;
@@ -551,6 +553,14 @@ GossipLog gossip_log(fi_epp* h) {
   return g;
 }
 
+// queue the copy of the index counters that the next check_counters reads
+int read_counters(fi_epp* h) {
+  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
+  h->ctr_pending = true;
+  return FI_OK;
+}
+
 // launch the staged SET then CLEAR ops of the current group on the index stream.
 // Asynchronous: the only waits are for the *previous* group's counters (rebuild /
 // overflow decisions lag one group) and for the staging buffer being reused.
@@ -579,12 +589,12 @@ int flush_ops(fi_epp* h) {
   h->ops_applied += h->n_sets + h->n_clears;
   h->ctr_unchecked += h->n_sets;
   FI_CUDA(cudaEventRecord(h->ev_buf[b].get(), h->s_index.get()));
-  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
-  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
-  h->ctr_pending = true;
+  rc = read_counters(h);
+  if (rc != FI_OK) return rc;
   FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   h->n_sets = h->n_clears = 0;
   h->cleared.clear();
+  h->clears_untracked = false;
   h->cur_buf ^= 1;
   // the buffer we are about to fill must have been consumed
   FI_CUDA(cudaEventSynchronize(h->ev_buf[h->cur_buf].get()));
@@ -631,36 +641,48 @@ int gossip_round(fi_epp* h) {
   }
   FI_CUDA(cudaMemsetAsync(sh.d_glog_n.get(), 0, 2 * sizeof(unsigned long long), h->s_index.get()));
   if (na || nv) {  // the replays allocate nodes too: refresh the counters the rebuild decision reads
-    FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
-    FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
-    h->ctr_pending = true;
+    rc = read_counters(h);
+    if (rc != FI_OK) return rc;
   }
   FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   return FI_OK;
 }
 
-// Sharded pools: agree on how many gossip rounds a collective index call needs (the ranks' op counts differ)
-int agree_rounds(fi_epp* h, uint64_t mine, uint64_t* rounds) {
-  *rounds = mine;
-  if (h->world <= 1) return FI_OK;
-  ShardState& sh = *h->shard;
-  unsigned long long v[2] = {mine, 0};
-  FI_CUDA(cudaMemcpyAsync(sh.d_ghdr.get() + 2 * (size_t)h->world, v, sizeof(v), cudaMemcpyHostToDevice, h->s_index.get()));
-  int rc = nccl_allgather_on(h, sh.comm, sh.d_ghdr.get() + 2 * (size_t)h->world, sh.d_ghdr.get(), sizeof(v), h->s_index.get());
-  if (rc != FI_OK) return rc;
-  FI_CUDA(cudaMemcpyAsync(sh.h_ghdr.get(), sh.d_ghdr.get(), (size_t)h->world * sizeof(v), cudaMemcpyDeviceToHost, h->s_index.get()));
-  FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
-  uint64_t m = 0;
-  for (uint32_t g = 0; g < h->world; ++g) m = std::max<uint64_t>(m, sh.h_ghdr.get()[2 * g]);
-  *rounds = m;
-  return FI_OK;
+// One collective index update of a sharded pool = `rounds` gossip rounds on every rank: the ranks agree on the
+// largest of their round counts `mine`, and `step(i)` stages and flushes this rank's share of round i (nothing if it
+// has fewer).  A rank whose arguments were rejected (my_err) still takes part, with zero rounds, so that the others do
+// not hang.  Single rank: just the steps.
+int run_rounds(fi_epp* h, uint64_t mine, int my_err, const std::function<int(uint64_t)>& step) {
+  if (my_err != FI_OK) {
+    if (h->world <= 1) return my_err;
+    mine = 0;
+  }
+  uint64_t rounds = mine;
+  if (h->world > 1) {
+    ShardState& sh = *h->shard;
+    unsigned long long v[2] = {mine, 0};
+    FI_CUDA(cudaMemcpyAsync(sh.d_ghdr.get() + 2 * (size_t)h->world, v, sizeof(v), cudaMemcpyHostToDevice, h->s_index.get()));
+    int rc = nccl_allgather_on(h, sh.comm, sh.d_ghdr.get() + 2 * (size_t)h->world, sh.d_ghdr.get(), sizeof(v), h->s_index.get());
+    if (rc != FI_OK) return rc;
+    FI_CUDA(cudaMemcpyAsync(sh.h_ghdr.get(), sh.d_ghdr.get(), (size_t)h->world * sizeof(v), cudaMemcpyDeviceToHost, h->s_index.get()));
+    FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
+    for (uint32_t g = 0; g < h->world; ++g) rounds = std::max<uint64_t>(rounds, sh.h_ghdr.get()[2 * g]);
+  }
+  for (uint64_t i = 0; i < rounds; ++i) {
+    int rc = i < mine ? step(i) : FI_OK;
+    if (rc == FI_OK) rc = gossip_round(h);
+    if (rc != FI_OK) return rc;
+  }
+  return my_err;
 }
 
-// stage one op (already filtered to this shard).  Within a launch group SETs run
-// before CLEARs, so a SET that follows a CLEAR of the same pair starts a new group.
+// Stage one op (already filtered to this shard) in the open group.  The GPU applies a group as all its SETs, then all
+// its CLEARs, so a SET that follows a CLEAR of the same pair starts a new group.  `cleared` holds the pairs CLEARed in
+// the group, unless clears_untracked: fi_epp_index_add_chains stages its CLEARs in bulk without recording them, and
+// until the next flush every SET then counts as following a CLEAR of its pair if the group holds any CLEAR.
 int submit_op(fi_epp* h, uint64_t hash, uint32_t endpoint, uint32_t op) {
   if (op == FI_OP_SET) {
-    if (!h->cleared.empty() && h->cleared.count(PairKey{hash, endpoint})) {
+    if (h->n_clears && (h->clears_untracked || h->cleared.count(PairKey{hash, endpoint}))) {
       int rc = flush_ops(h);
       if (rc != FI_OK) return rc;
     }
@@ -684,6 +706,17 @@ int choose_lru_mode(fi_epp* h) {
   const bool possible = h->cfg.lru_capacity >= h->cfg.max_blocks && h->cfg.lru_capacity <= (1u << 28);
   if (want == 1 && !possible) return fail(h, FI_ERR_STATE, "device_lru needs lru_capacity >= max_blocks");
   h->lru_mode = (want < 0 ? possible : want == 1) ? 1 : 0;
+  return FI_OK;
+}
+
+// the per-request arguments of a batched Add: every endpoint in range or FI_NO_ENDPOINT, every chain at most
+// max_nblocks long (`bound` names that limit)
+int check_add_requests(fi_epp* h, const uint32_t* endpoints, const uint32_t* nblocks, uint32_t R, uint32_t max_nblocks,
+                       const char* bound) {
+  for (uint32_t r = 0; r < R; ++r) {
+    if (endpoints[r] != FI_NO_ENDPOINT && endpoints[r] >= h->cfg.num_endpoints) return fail(h, FI_ERR_INVALID, "endpoint out of range");
+    if (nblocks[r] > max_nblocks) return fail(h, FI_ERR_INVALID, std::string("nblocks[r] larger than ") + bound);
+  }
   return FI_OK;
 }
 
@@ -844,10 +877,65 @@ int lru_enqueue_apply(fi_epp* h, const LruBatch& b, uint64_t touches, const Goss
                                        h->s_index.get()));
   }
   if (clear_ovf) FI_CUDA(cudaMemsetAsync(h->dlru->v.ovf, 0, ((size_t)EL + 1) * sizeof(uint32_t), h->s_index.get()));  // ovf[] and any_ovf
-  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
-  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
-  h->ctr_pending = true;
   h->ctr_unchecked += touches;
+  return read_counters(h);
+}
+
+// The prologue of both device-LRU Adds: the LRU exists, every local chain fits lru_capacity, and the ops staged
+// through fi_epp_index_apply go first.
+int lru_add_begin(fi_epp* h, const uint32_t* endpoints, const uint32_t* nblocks, uint32_t R) {
+  int rc = ensure_dev_lru(h);
+  if (rc != FI_OK) return rc;
+  for (uint32_t r = 0; r < R; ++r)
+    if (nblocks[r] > h->cfg.lru_capacity && endpoints[r] - h->cfg.endpoint_begin < h->cfg.endpoint_count)
+      return fail(h, FI_ERR_INVALID, "device LRU: a chain longer than lru_capacity");
+  return flush_ops(h);
+}
+
+// Pack plan `pl` into `buf` once `done` says the device has consumed the plan staged there before, and upload it on
+// the index stream.  Like every index update, ordered behind the picks submitted so far (a pick sees the index as of
+// its call).
+int lru_stage_plan(fi_epp* h, Staging<uint32_t>& buf, const LruPlan& pl, cudaEvent_t done) {
+  const size_t words = lru_plan_words(pl, h->cfg.endpoint_count);
+  FI_CUDA(cudaEventSynchronize(done));
+  int rc = grow_staging(h, buf, words, words + words / 2 + 1024, true);  // room to spare: plans vary in size
+  if (rc != FI_OK) return rc;
+  lru_plan_pack(pl, buf.h.get());
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
+  if (words) FI_CUDA(cudaMemcpyAsync(buf.d.get(), buf.h.get(), words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
+  h->stats.h2d_bytes += words * sizeof(uint32_t);
+  return FI_OK;
+}
+
+// The epilogue of both device-LRU Adds, behind their sub-batches: the LRU status refresh, then ev_ctr (which covers
+// the status copies), `done` (if given) and ev_index.
+int lru_add_end(fi_epp* h, cudaEvent_t done) {
+  int rc = lru_refresh_stat(h);
+  if (rc != FI_OK) return rc;
+  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
+  if (done) FI_CUDA(cudaEventRecord(done, h->s_index.get()));
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
+  return FI_OK;
+}
+
+// copy the rows of host `chains` that plan `pl` keeps to the device staging; *d_chains = where they are
+int lru_stage_chains(fi_epp* h, const uint64_t* chains, uint32_t pitch, uint32_t R, const LruPlan& pl, const uint64_t** d_chains) {
+  const size_t K = pl.req_id.size(), cw = (size_t)R * pitch;
+  int rc = grow_staging(h, h->lru_chains, cw, cw, false);
+  if (rc != FI_OK) return rc;
+  *d_chains = h->lru_chains.d.get();
+  // whole-range copy when most rows are kept (one DMA), row copies otherwise
+  if (K * 2 >= R) {
+    FI_CUDA(cudaMemcpyAsync(h->lru_chains.d.get(), chains, cw * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_index.get()));
+    h->stats.h2d_bytes += cw * sizeof(uint64_t);
+    return FI_OK;
+  }
+  for (size_t k = 0; k < K; ++k) {
+    const size_t r = pl.req_id[k];
+    FI_CUDA(cudaMemcpyAsync(h->lru_chains.d.get() + r * pitch, chains + r * pitch, (size_t)pl.req_n[k] * sizeof(uint64_t),
+                            cudaMemcpyHostToDevice, h->s_index.get()));
+    h->stats.h2d_bytes += (size_t)pl.req_n[k] * sizeof(uint64_t);
+  }
   return FI_OK;
 }
 
@@ -855,141 +943,100 @@ int lru_enqueue_apply(fi_epp* h, const LruBatch& b, uint64_t touches, const Goss
 // (copied to the device first) or, with on_device, memory the index stream can read.  The first pass is
 // OPTIMISTIC: sub-batches are cut only by the scratch arrays' size, and an endpoint whose table cannot take the
 // batch's distinct keys is rolled back and deferred; the deferred requests then run in a second, conservative pass
-// (at most lru_capacity touches per endpoint and sub-batch: always fits).
+// (at most lru_capacity touches per endpoint and sub-batch: always fits).  On a sharded pool both passes are
+// collective (one gossip round per sub-batch) and every rank takes part in both, one whose arguments were rejected
+// (my_err) with no sub-batches.
 int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains, bool on_device, uint32_t pitch,
-                   const uint32_t* nblocks, uint32_t R, bool conservative = false) {
-  int rc = ensure_dev_lru(h);
-  if (rc != FI_OK) return rc;
+                   const uint32_t* nblocks, uint32_t R, int my_err) {
+  if (my_err == FI_OK) my_err = lru_add_begin(h, endpoints, nblocks, R);
   const uint32_t EL = h->cfg.endpoint_count, lo = h->cfg.endpoint_begin;
-  for (uint32_t r = 0; r < R; ++r)
-    if (nblocks[r] > h->cfg.lru_capacity && endpoints[r] - lo < EL)
-      return fail(h, FI_ERR_INVALID, "device LRU: a chain longer than lru_capacity");
-  rc = flush_ops(h);  // ops staged through fi_epp_index_apply come first
-  if (rc != FI_OK) return rc;
-  rc = check_counters(h);
-  if (rc != FI_OK) return rc;
-  const auto t0 = std::chrono::steady_clock::now();
-  LruPlan& pl = h->lru_plan;
-  // sharded pool: a sub-batch's APPEAR / VANISH transitions must fit the gossip log of one round (at most one SET per
-  // touch; CLEARs: evictions <= keys added, plus doomed entries <= touches)
   const bool sharded = h->world > 1;
-  const uint64_t cap_touches = sharded ? std::min<uint64_t>(h->dlru->touch_cap, kOpChunk / 2) : h->dlru->touch_cap;
-  lru_plan_batch(endpoints, nblocks, R, lo, EL, conservative ? h->cfg.lru_capacity : 0xFFFFFFFFu, cap_touches, h->cfg.max_batch, &pl);
-  if (pl.subs.empty() && !sharded) return FI_OK;
-  const size_t K = pl.req_id.size(), nsub = pl.subs.size();
-  // collective on a sharded pool: the ranks' sub-batch counts differ, every one is a gossip round for all
-  uint64_t rounds = nsub;
-  if (sharded) {
-    rc = agree_rounds(h, nsub, &rounds);
-    if (rc != FI_OK) return rc;
-  }
-  const GossipLog glog = gossip_log(h);
-  const size_t words = lru_plan_words(pl, EL);
-  FI_CUDA(cudaEventSynchronize(h->dlru->ev.get()));  // the previous call's staging (and chain copy) has been consumed
-  rc = grow_staging(h, h->lru_plan_buf, words, words + words / 2 + 1024, true);  // room to spare: plans vary in size
-  if (rc != FI_OK) return rc;
-  lru_plan_pack(pl, h->lru_plan_buf.h.get());
-  // the LRU kernels run on the index stream; like every index update they are ordered behind the picks
-  // submitted so far (a pick sees the index as of its call)
-  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
-  if (words)
-    FI_CUDA(cudaMemcpyAsync(h->lru_plan_buf.d.get(), h->lru_plan_buf.h.get(), words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
-  h->stats.h2d_bytes += words * sizeof(uint32_t);
-  const uint64_t* d_chains = chains;
-  if (!on_device && K) {
-    const size_t cw = (size_t)R * pitch;
-    rc = grow_staging(h, h->lru_chains, cw, cw, false);
-    if (rc != FI_OK) return rc;
-    d_chains = h->lru_chains.d.get();
-    // only the rows the plan kept are needed; whole-range copy when most are (one DMA), row copies otherwise
-    if (K * 2 >= R) {
-      FI_CUDA(cudaMemcpyAsync(h->lru_chains.d.get(), chains, cw * sizeof(uint64_t), cudaMemcpyHostToDevice, h->s_index.get()));
-      h->stats.h2d_bytes += cw * sizeof(uint64_t);
-    } else {
-      for (size_t k = 0; k < K; ++k) {
-        const size_t r = pl.req_id[k];
-        FI_CUDA(cudaMemcpyAsync(h->lru_chains.d.get() + r * pitch, chains + r * pitch, (size_t)pl.req_n[k] * sizeof(uint64_t),
-                                cudaMemcpyHostToDevice, h->s_index.get()));
-        h->stats.h2d_bytes += (size_t)pl.req_n[k] * sizeof(uint64_t);
+  LruPlan& pl = h->lru_plan;
+  std::vector<uint32_t> ep2;  // the conservative pass's endpoints: the deferred requests' (FI_NO_ENDPOINT elsewhere)
+  for (const bool conservative : {false, true}) {
+    if (my_err == FI_OK) my_err = check_counters(h);
+    const auto t0 = std::chrono::steady_clock::now();
+    size_t K = 0, nsub = 0;
+    if (my_err == FI_OK) {
+      // sharded pool: a sub-batch's APPEAR / VANISH transitions must fit the gossip log of one round (at most one SET
+      // per touch; CLEARs: evictions <= keys added, plus doomed entries <= touches)
+      const uint64_t cap_touches = sharded ? std::min<uint64_t>(h->dlru->touch_cap, kOpChunk / 2) : h->dlru->touch_cap;
+      lru_plan_batch(endpoints, nblocks, R, lo, EL, conservative ? h->cfg.lru_capacity : 0xFFFFFFFFu, cap_touches, h->cfg.max_batch, &pl);
+      if (pl.subs.empty() && !sharded) return FI_OK;
+      K = pl.req_id.size();
+      nsub = pl.subs.size();
+      my_err = lru_stage_plan(h, h->lru_plan_buf, pl, h->dlru->ev.get());  // (dlru->ev covers the chain staging too)
+    }
+    if (my_err == FI_OK && !on_device && K) my_err = lru_stage_chains(h, chains, pitch, R, pl, &chains);
+    if (my_err == FI_OK) h->lru_sub_batches += nsub;
+    const GossipLog glog = gossip_log(h);
+    std::vector<uint8_t> deferred;  // per request of this call: its endpoint overflowed in the optimistic pass
+    std::vector<uint32_t> ovf_host;
+    size_t n_deferred = 0;
+    int rc = run_rounds(h, nsub, my_err, [&](uint64_t sb) -> int {
+      if (sb) {  // the index counters of the previous sub-batch decide about a rebuild before more keys arrive
+        const int rc2 = check_counters(h);
+        if (rc2 != FI_OK) return rc2;
       }
-    }
-  }
-  const uint32_t* dp = h->lru_plan_buf.d.get();
-  h->lru_sub_batches += nsub;
-  std::vector<uint8_t> deferred;  // per request of this call: its endpoint overflowed in the optimistic pass
-  std::vector<uint32_t> ovf_host;
-  size_t n_deferred = 0;
-  for (size_t sb = 0; sb < rounds; ++sb) {
-    if (sb >= nsub) {  // (sharded) this rank is done: it only takes part in the others' gossip rounds
-      rc = gossip_round(h);
-      if (rc != FI_OK) return rc;
-      continue;
-    }
-    if (sb) {  // the index counters of the previous sub-batch decide about a rebuild before more keys arrive
-      rc = check_counters(h);
-      if (rc != FI_OK) return rc;
-    }
-    const LruSubBatch& sbt = pl.subs[sb];
-    const uint32_t* inc = nullptr;
-    const LruBatch b = lru_sub_batch(h, dp, pl, sb, d_chains, pitch, &inc);
-    rc = lru_enqueue_touch(h, b, inc);
-    if (rc != FI_OK) return rc;
-    // did some endpoint's table refuse keys?  (one host round trip per sub-batch; everything after it is queued
-    // without waiting)
-    FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->any_ovf, h->dlru->v.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
-    FI_CUDA(cudaEventRecord(h->dlru->ev_ovf.get(), h->s_index.get()));
-    FI_CUDA(cudaEventSynchronize(h->dlru->ev_ovf.get()));
-    const bool any_ovf = h->dlru->stat->any_ovf != 0;
-    if (any_ovf) {
-      if (conservative) return fail(h, FI_ERR_STATE, "device LRU: overflow in a conservative sub-batch");
-      {
-        LaunchScope ls(h, h->s_index.get(), K_INDEX);
-        FI_CUDA(launch_lru_untouch(h->dlru->v, b, h->s_index.get()));
-      }
-      ovf_host.resize(EL);
-      FI_CUDA(cudaMemcpyAsync(ovf_host.data(), h->dlru->v.ovf, (size_t)EL * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
-      FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
-      if (deferred.empty()) deferred.assign(R, 0);
-      for (uint32_t k = sbt.k_begin; k < sbt.k_end; ++k)
-        if (ovf_host[pl.req_ep[k]]) {
-          deferred[pl.req_id[k]] = 1;
-          ++n_deferred;
+      const LruSubBatch& sbt = pl.subs[sb];
+      const uint32_t* inc = nullptr;
+      const LruBatch b = lru_sub_batch(h, h->lru_plan_buf.d.get(), pl, sb, chains, pitch, &inc);
+      const int rc2 = lru_enqueue_touch(h, b, inc);
+      if (rc2 != FI_OK) return rc2;
+      // did some endpoint's table refuse keys?  (one host round trip per sub-batch; everything after it is queued
+      // without waiting)
+      FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->any_ovf, h->dlru->v.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
+      FI_CUDA(cudaEventRecord(h->dlru->ev_ovf.get(), h->s_index.get()));
+      FI_CUDA(cudaEventSynchronize(h->dlru->ev_ovf.get()));
+      const bool any_ovf = h->dlru->stat->any_ovf != 0;
+      if (any_ovf) {
+        if (conservative) return fail(h, FI_ERR_STATE, "device LRU: overflow in a conservative sub-batch");
+        {
+          LaunchScope ls(h, h->s_index.get(), K_INDEX);
+          FI_CUDA(launch_lru_untouch(h->dlru->v, b, h->s_index.get()));
         }
-    }
-    rc = lru_enqueue_apply(h, b, sbt.touches, glog, any_ovf);
+        ovf_host.resize(EL);
+        FI_CUDA(cudaMemcpyAsync(ovf_host.data(), h->dlru->v.ovf, (size_t)EL * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
+        FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
+        if (deferred.empty()) deferred.assign(R, 0);
+        for (uint32_t k = sbt.k_begin; k < sbt.k_end; ++k)
+          if (ovf_host[pl.req_ep[k]]) {
+            deferred[pl.req_id[k]] = 1;
+            ++n_deferred;
+          }
+      }
+      return lru_enqueue_apply(h, b, sbt.touches, glog, any_ovf);
+    });
+    if (rc != (sharded ? my_err : FI_OK)) return rc;  // (a sharded rank with my_err goes on to the second pass)
+    if (my_err != FI_OK) continue;
+    rc = lru_add_end(h, h->dlru->ev.get());
     if (rc != FI_OK) return rc;
-    if (sharded) {  // the other ranks replay this sub-batch's transitions into their directories (and we theirs)
-      rc = gossip_round(h);
-      if (rc != FI_OK) return rc;
+    if (h->verbose) {
+      const auto t1 = std::chrono::steady_clock::now();
+      std::fprintf(stderr, "[fi_epp] device LRU%s: %u requests (%zu kept), %zu sub-batch(es), %zu deferred, host side %.3f ms\n",
+                   conservative ? " (conservative pass)" : "", R, K, nsub, n_deferred,
+                   std::chrono::duration<double, std::milli>(t1 - t0).count());
     }
+    h->lru_deferred += n_deferred;
+    // (sharded: every rank enters the second pass, most with nothing to do)
+    if (conservative || (!n_deferred && !sharded)) return FI_OK;
+    ep2.assign(R, FI_NO_ENDPOINT);
+    for (uint32_t r = 0; r < R; ++r)
+      if (n_deferred && deferred[r]) ep2[r] = endpoints[r];
+    endpoints = ep2.data();
+    on_device = true;  // `chains` is in device memory now
   }
-  rc = lru_refresh_stat(h);
-  if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));  // covers the status copy too
-  FI_CUDA(cudaEventRecord(h->dlru->ev.get(), h->s_index.get()));
-  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
-  if (h->verbose) {
-    const auto t1 = std::chrono::steady_clock::now();
-    std::fprintf(stderr, "[fi_epp] device LRU%s: %u requests (%zu kept), %zu sub-batch(es), %zu deferred, host side %.3f ms\n",
-                 conservative ? " (conservative pass)" : "", R, K, nsub, n_deferred,
-                 std::chrono::duration<double, std::milli>(t1 - t0).count());
-  }
-  h->lru_deferred += n_deferred;
-  if (n_deferred || (sharded && !conservative)) {  // (sharded: every rank enters the second pass, most with nothing to do)
-    std::vector<uint32_t> ep2(R);
-    for (uint32_t r = 0; r < R; ++r) ep2[r] = (n_deferred && deferred[r]) ? endpoints[r] : FI_NO_ENDPOINT;
-    return lru_device_add(h, ep2.data(), d_chains, true, pitch, nblocks, R, true);
-  }
-  return FI_OK;
+  return my_err;
 }
 
-// the index-stream part of lru_add_submitted: plan upload, sub-batches, status copies
-int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, size_t words, fi_epp::PipeAdd& pa) {
-  // like every index update, ordered behind the picks submitted so far (a pick sees the index as of its call)
+// the index-stream part of lru_add_submitted behind the plan upload: the chain copy out of the slot, the sub-batches,
+// the status copies
+int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, fi_epp::PipeAdd& pa, uint32_t R) {
+  const uint64_t* slot_chain = slot ? h->d_chain2.get() : h->d_chain.get();
+  FI_CUDA(cudaStreamWaitEvent(h->s_copy.get(), h->ev_a[slot].get(), 0));  // the batch's chains are written
+  FI_CUDA(cudaMemcpyAsync(pa.d_chains.get(), slot_chain, (size_t)R * h->MP * sizeof(uint64_t), cudaMemcpyDeviceToDevice, h->s_copy.get()));
+  FI_CUDA(cudaEventRecord(h->ev_slot_read[slot].get(), h->s_copy.get()));
   FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_slot_read[slot].get(), 0));
-  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
-  FI_CUDA(cudaMemcpyAsync(pa.plan.d.get(), pa.plan.h.get(), words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
-  h->stats.h2d_bytes += words * sizeof(uint32_t);
   const GossipLog glog = gossip_log(h);
   h->lru_sub_batches += pl.subs.size();
   for (size_t sb = 0; sb < pl.subs.size(); ++sb) {
@@ -1003,12 +1050,8 @@ int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, size_
     rc = lru_enqueue_apply(h, b, touches, glog, false);
     if (rc != FI_OK) return rc;
   }
-  int rc = lru_refresh_stat(h);
-  if (rc != FI_OK) return rc;
   FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->planned_ovf, h->dlru->v.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
-  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));  // covers the status copies too
-  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
-  return FI_OK;
+  return lru_add_end(h, nullptr);
 }
 
 // fi_epp_index_add_submitted: indexer.Add(chain_r, endpoints[r]) for the batch whose chains pipeline slot `slot`
@@ -1022,23 +1065,14 @@ int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, size_
 //  - the chains are first copied out of the slot on s_copy, as soon as the batch's hashing is done, so that the submit
 //    that reuses the slot waits for that copy only and not for this Add, which runs behind the picks in flight.
 int lru_add_submitted(fi_epp* h, uint32_t slot, const uint32_t* endpoints, const uint32_t* nblocks, uint32_t R) {
-  int rc = ensure_dev_lru(h);
-  if (rc != FI_OK) return rc;
-  const uint32_t EL = h->cfg.endpoint_count, lo = h->cfg.endpoint_begin;
-  for (uint32_t r = 0; r < R; ++r)
-    if (nblocks[r] > h->cfg.lru_capacity && endpoints[r] - lo < EL)
-      return fail(h, FI_ERR_INVALID, "device LRU: a chain longer than lru_capacity");
-  rc = flush_ops(h);  // ops staged through fi_epp_index_apply come first
+  int rc = lru_add_begin(h, endpoints, nblocks, R);
   if (rc != FI_OK) return rc;
   LruPlan& pl = h->lru_plan;
-  lru_plan_batch(endpoints, nblocks, R, lo, EL, lru_touch_bound(h->dlru->v.TS, h->dlru->v.capacity), h->dlru->touch_cap,
-                 h->cfg.max_batch, &pl);
+  lru_plan_batch(endpoints, nblocks, R, h->cfg.endpoint_begin, h->cfg.endpoint_count, lru_touch_bound(h->dlru->v.TS, h->dlru->v.capacity),
+                 h->dlru->touch_cap, h->cfg.max_batch, &pl);
   if (pl.subs.empty()) return FI_OK;
-  const size_t words = lru_plan_words(pl, EL);
   fi_epp::PipeAdd& pa = h->padd[h->padd_seq & 1];
-  if (pa.ev_done) {
-    FI_CUDA(cudaEventSynchronize(pa.ev_done.get()));  // the Add before the previous one is done with it
-  } else {
+  if (!pa.ev_done) {
     Event ev;
     DevPtr<uint64_t> chains;
     FI_CUDA(cuda_create(ev));
@@ -1046,16 +1080,11 @@ int lru_add_submitted(fi_epp* h, uint32_t slot, const uint32_t* endpoints, const
     pa.ev_done = std::move(ev);
     pa.d_chains = std::move(chains);
   }
-  rc = grow_staging(h, pa.plan, words, words + words / 2 + 1024, true);  // as lru_device_add's
+  rc = lru_stage_plan(h, pa.plan, pl, pa.ev_done.get());  // waits for the Add before the previous one
   if (rc != FI_OK) return rc;
-  lru_plan_pack(pl, pa.plan.h.get());
-  const uint64_t* slot_chain = slot ? h->d_chain2.get() : h->d_chain.get();
-  FI_CUDA(cudaStreamWaitEvent(h->s_copy.get(), h->ev_a[slot].get(), 0));  // the batch's chains are written
-  FI_CUDA(cudaMemcpyAsync(pa.d_chains.get(), slot_chain, (size_t)R * h->MP * sizeof(uint64_t), cudaMemcpyDeviceToDevice, h->s_copy.get()));
-  FI_CUDA(cudaEventRecord(h->ev_slot_read[slot].get(), h->s_copy.get()));
   // From here on work that reads pa's buffers is queued: whatever happens, pa.ev_done marks its end (the s_index wait
   // on the chain copy makes it cover that copy too), and the next call takes the other buffers.
-  rc = lru_add_submitted_enqueue(h, slot, pl, words, pa);
+  rc = lru_add_submitted_enqueue(h, slot, pl, pa, R);
   cudaError_t e = cudaStreamWaitEvent(h->s_index.get(), h->ev_slot_read[slot].get(), 0);
   if (e == cudaSuccess) e = cudaEventRecord(pa.ev_done.get(), h->s_index.get());
   h->padd_seq++;
@@ -1142,10 +1171,9 @@ int lru_device_resize(fi_epp* h, const std::vector<uint32_t>& local, const std::
   }
   int rc = lru_refresh_stat(h);
   if (rc != FI_OK) return rc;
-  // the CLEARs' tombstones reach the rebuild decision of the next index update
-  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
-  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));  // covers the status copy too
-  h->ctr_pending = true;
+  // the CLEARs' tombstones reach the rebuild decision of the next index update (ev_ctr covers the status copy too)
+  rc = read_counters(h);
+  if (rc != FI_OK) return rc;
   FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   return FI_OK;
 }
@@ -1949,32 +1977,6 @@ int fi_epp_endpoints_lora_update(fi_epp* h, const fi_endpoint_lora* s, uint32_t 
   return FI_OK;
 }
 
-// One collective index update of a sharded pool = `rounds` gossip rounds on every rank; `step(i)` stages and
-// flushes this rank's share of round i (nothing if it has fewer).  Single rank: just the steps.
-static int run_rounds(fi_epp* h, uint64_t mine, int my_err, const std::function<int(uint64_t)>& step) {
-  if (h->world <= 1) {
-    if (my_err != FI_OK) return my_err;
-    for (uint64_t i = 0; i < mine; ++i) {
-      int rc = step(i);
-      if (rc != FI_OK) return rc;
-    }
-    return FI_OK;
-  }
-  // a rank whose arguments were rejected still takes part (with zero rounds) so that the others do not hang
-  uint64_t rounds = 0;
-  int rc = agree_rounds(h, my_err == FI_OK ? mine : 0, &rounds);
-  if (rc != FI_OK) return rc;
-  for (uint64_t i = 0; i < rounds; ++i) {
-    if (my_err == FI_OK && i < mine) {
-      rc = step(i);
-      if (rc != FI_OK) return rc;
-    }
-    rc = gossip_round(h);
-    if (rc != FI_OK) return rc;
-  }
-  return my_err;
-}
-
 int fi_epp_index_apply(fi_epp* h, const fi_index_op* ops, uint64_t n) {
   if (!h || (!ops && n)) return FI_ERR_INVALID;
   std::lock_guard<std::mutex> lk(h->mu);
@@ -2050,9 +2052,8 @@ int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t
   for (uint32_t e : local)
     if (e < h->lrus.size()) h->lrus[e].clear();
   // the sweep's tombstones reach the rebuild decision of the next index update
-  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
-  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
-  h->ctr_pending = true;
+  rc = read_counters(h);
+  if (rc != FI_OK) return rc;
   FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   if (pairs_removed) {
     unsigned long long c = 0;
@@ -2138,7 +2139,7 @@ int fi_epp_index_add_chain(fi_epp* h, uint32_t endpoint, const uint64_t* hashes,
   if (e >= h->cfg.endpoint_count) return FI_OK;  // another rank's shard
   int rc = choose_lru_mode(h);
   if (rc != FI_OK) return rc;
-  if (h->lru_mode == 1) return lru_device_add(h, &endpoint, hashes, false, n, &n, 1);
+  if (h->lru_mode == 1) return lru_device_add(h, &endpoint, hashes, false, n, &n, 1, FI_OK);
   rc = check_counters(h);
   if (rc != FI_OK) return rc;
   LruSet& l = h->lrus[e];
@@ -2160,16 +2161,6 @@ int fi_epp_index_add_chain(fi_epp* h, uint32_t endpoint, const uint64_t* hashes,
   return FI_OK;
 }
 
-namespace {
-
-struct CopyJob {
-  fi_index_op* dst;
-  const fi_index_op* src;
-  size_t n;
-};
-
-}  // namespace
-
 // Upstream PreRequest for a whole batch of decisions: indexer.Add(chain_r, endpoints[r]) for r = 0..R-1, in
 // request order per endpoint (the endpoints' LRUs are independent of each other, so they are walked in
 // parallel on the host worker pool; the result equals R sequential fi_epp_index_add_chain calls).
@@ -2178,20 +2169,19 @@ int fi_epp_index_add_chains(fi_epp* h, const uint32_t* endpoints, const uint64_t
   if (!h || ((!endpoints || !chains || !nblocks) && R)) return FI_ERR_INVALID;
   std::lock_guard<std::mutex> lk(h->mu);
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  int err = FI_OK;
-  if (!h->cfg.lru_capacity) err = fail(h, FI_ERR_STATE, "lru_capacity is 0: the host LRU is disabled");
-  for (uint32_t r = 0; r < R && err == FI_OK; ++r) {
-    if (endpoints[r] != FI_NO_ENDPOINT && endpoints[r] >= h->cfg.num_endpoints) err = fail(h, FI_ERR_INVALID, "endpoint out of range");
-    else if (nblocks[r] > pitch_blocks) err = fail(h, FI_ERR_INVALID, "nblocks[r] larger than the chain pitch");
-  }
-  if (err == FI_OK) err = choose_lru_mode(h);
-  if (err == FI_OK && h->lru_mode == 1) return lru_device_add(h, endpoints, chains, false, pitch_blocks, nblocks, R);
+  // The LRU depends on configuration and options only, so every rank of a sharded pool runs the same one and takes
+  // part in its collective, a rank whose arguments were rejected (err) too.
+  const int mode_err = choose_lru_mode(h);
+  int err = h->cfg.lru_capacity ? check_add_requests(h, endpoints, nblocks, R, pitch_blocks, "the chain pitch")
+                                : fail(h, FI_ERR_STATE, "lru_capacity is 0: the host LRU is disabled");
+  if (err == FI_OK) err = mode_err;
+  if (h->lru_mode == 1) return lru_device_add(h, endpoints, chains, false, pitch_blocks, nblocks, R, err);
   if (err == FI_OK) err = check_counters(h);
 
-  // ---- 1./2. bucket the requests by endpoint and walk the LRUs on the worker pool (lru_batch.h)
-  const uint32_t lo = h->cfg.endpoint_begin, EL = h->cfg.endpoint_count;
+  // bucket the requests by endpoint, walk the LRUs on the worker pool and plan the staging (lru_batch.h)
   std::vector<WorkerOps>& outs = h->lru_outs;  // persistent: capacity survives from batch to batch
   size_t nseg = 0;
+  std::vector<StageGroup> groups;
   const auto t_start = std::chrono::steady_clock::now();
   if (!h->pool) {
     unsigned t = std::min(usable_cores(), 128u);
@@ -2199,118 +2189,45 @@ int fi_epp_index_add_chains(fi_epp* h, const uint32_t* endpoints, const uint64_t
     if (h->lru_threads) t = h->lru_threads;
     h->pool.reset(new WorkerPool(t));
   }
-  if (err == FI_OK) nseg = lru_walk_batch(h->lrus, lo, EL, endpoints, chains, pitch_blocks, nblocks, R, *h->pool, outs);
-  else for (auto& o : outs) o.begin_batch();
+  if (err == FI_OK) nseg = lru_walk_batch(h->lrus, h->cfg.endpoint_begin, h->cfg.endpoint_count, endpoints, chains, pitch_blocks, nblocks, R, *h->pool, outs);
   const auto t_walked = std::chrono::steady_clock::now();
+  if (err == FI_OK) groups = plan_staging(outs, nseg, h->n_sets, h->n_clears, kOpChunk);
 
-  // ---- 3. stage segment by segment (SETs, then CLEARs), flushing whenever a staging buffer is full.
-  // `flushes` is first counted (dry run) so that the ranks of a sharded pool can agree on the rounds.
-  std::vector<CopyJob> jobs;
-  auto run_jobs = [&]() {
-    if (jobs.empty()) return;
-    // big copies into the pinned staging buffers go through the worker pool
-    std::vector<CopyJob> pieces;
+  // Step i copies group i into the staging buffers and flushes it.  A single rank leaves the tail staged: it is
+  // launched with the next flush, at the latest by the next pick / sync.  On a sharded pool every group is one gossip
+  // round, the tail included.
+  struct CopyJob {
+    fi_index_op* dst;
+    const fi_index_op* src;
+    size_t n;
+  };
+  const int rc = run_rounds(h, groups.size(), err, [&](uint64_t i) -> int {
+    const StageGroup& g = groups[i];
+    std::vector<CopyJob> jobs;  // big copies into the pinned staging buffers go through the worker pool
     const size_t kPiece = 1u << 16;
-    for (const CopyJob& j : jobs)
-      for (size_t o = 0; o < j.n; o += kPiece) pieces.push_back(CopyJob{j.dst + o, j.src + o, std::min(kPiece, j.n - o)});
-    h->pool->run((uint32_t)pieces.size(), [&](uint32_t t, unsigned) {
-      std::memcpy(pieces[t].dst, pieces[t].src, pieces[t].n * sizeof(fi_index_op));
+    for (const StagePiece& p : g.pieces) {
+      const fi_index_op* src = (p.clear ? outs[p.worker].clears : outs[p.worker].sets)[p.seg].data() + p.src;
+      fi_index_op* dst = (p.clear ? h->h_clears : h->h_sets)[h->cur_buf].get() + p.dst;
+      for (size_t o = 0; o < p.n; o += kPiece) jobs.push_back(CopyJob{dst + o, src + o, std::min(kPiece, p.n - o)});
+    }
+    h->pool->run((uint32_t)jobs.size(), [&](uint32_t t, unsigned) {
+      std::memcpy(jobs[t].dst, jobs[t].src, jobs[t].n * sizeof(fi_index_op));
     });
-    jobs.clear();
-  };
-  // walk(dry): returns the number of flushes; !dry performs them through do_flush
-  auto walk = [&](bool dry, const std::function<int()>& do_flush, uint64_t* n_flush) -> int {
-    uint64_t ns = dry ? 0 : h->n_sets, nc = dry ? 0 : h->n_clears, flushes = 0;
-    auto flush = [&]() -> int {
-      ++flushes;
-      if (!dry) {
-        run_jobs();
-        h->n_sets = ns;
-        h->n_clears = nc;
-        int rc = do_flush();
-        if (rc != FI_OK) return rc;
-      }
-      ns = nc = 0;
-      return FI_OK;
-    };
-    for (size_t seg = 0; seg < nseg; ++seg) {
-      for (int kind = 0; kind < 2; ++kind) {
-        for (auto& o : outs) {
-          if (o.nseg <= seg) continue;
-          const std::vector<fi_index_op>& v = kind == 0 ? o.sets[seg] : o.clears[seg];
-          size_t done = 0;
-          while (done < v.size()) {
-            uint64_t& fillc = kind == 0 ? ns : nc;
-            const size_t room = (size_t)(kOpChunk - fillc);
-            const size_t take = std::min(room, v.size() - done);
-            if (!dry && take) {
-              fi_index_op* base = kind == 0 ? h->h_sets[h->cur_buf].get() : h->h_clears[h->cur_buf].get();
-              jobs.push_back(CopyJob{base + fillc, v.data() + done, take});
-            }
-            fillc += take;
-            done += take;
-            if (fillc == kOpChunk) {
-              int rc = flush();
-              if (rc != FI_OK) return rc;
-            }
-          }
-        }
-      }
-      if (seg + 1 < nseg && (ns || nc)) {  // segment boundary: the next segment's SETs must run after these CLEARs
-        int rc = flush();
-        if (rc != FI_OK) return rc;
-      }
-    }
-    if (!dry) {
-      run_jobs();
-      h->n_sets = ns;
-      h->n_clears = nc;
-    }
-    if (n_flush) *n_flush = flushes;
-    return FI_OK;
-  };
-
-  if (h->world <= 1) {
-    if (err != FI_OK) return err;
-    // the tail stays staged: it is launched with the next flush — at the latest by the next pick / sync
-    int rc1 = walk(false, [&]() { return flush_ops(h); }, nullptr);
-    if (h->verbose) {
-      const auto t_end = std::chrono::steady_clock::now();
-      size_t nops = 0;
-      for (auto& o : outs)
-        for (size_t sg = 0; sg < o.nseg; ++sg) nops += o.sets[sg].size() + o.clears[sg].size();
-      std::fprintf(stderr, "[fi_epp] add_chains: %u requests, %zu ops, %zu segment(s), %u workers: LRU walk %.2f ms, staging %.2f ms\n",
-                   R, nops, nseg, h->pool->size(), std::chrono::duration<double, std::milli>(t_walked - t_start).count(),
-                   std::chrono::duration<double, std::milli>(t_end - t_walked).count());
-    }
-    return rc1;
+    h->n_sets = g.n_sets;
+    h->n_clears = g.n_clears;
+    h->clears_untracked |= g.n_clears > 0;
+    return i + 1 < groups.size() || h->world > 1 ? flush_ops(h) : FI_OK;
+  });
+  if (h->verbose && err == FI_OK) {
+    const auto t_end = std::chrono::steady_clock::now();
+    size_t nops = 0;
+    for (auto& o : outs)
+      for (size_t sg = 0; sg < o.nseg; ++sg) nops += o.sets[sg].size() + o.clears[sg].size();
+    std::fprintf(stderr, "[fi_epp] add_chains: %u requests, %zu ops, %zu segment(s), %u workers: LRU walk %.2f ms, staging %.2f ms\n",
+                 R, nops, nseg, h->pool->size(), std::chrono::duration<double, std::milli>(t_walked - t_start).count(),
+                 std::chrono::duration<double, std::milli>(t_end - t_walked).count());
   }
-  // sharded: every flush is one gossip round, the tail included
-  uint64_t mine = 0;
-  if (err == FI_OK) {
-    walk(true, nullptr, &mine);
-    mine += 1;  // the tail
-  }
-  uint64_t rounds = 0;
-  int rc = agree_rounds(h, err == FI_OK ? mine : 0, &rounds);
-  if (rc != FI_OK) return rc;
-  uint64_t did = 0;
-  if (err == FI_OK) {
-    rc = walk(false, [&]() -> int {
-      int r2 = flush_ops(h);
-      if (r2 != FI_OK) return r2;
-      ++did;
-      return gossip_round(h);
-    }, nullptr);
-    if (rc != FI_OK) return rc;
-    rc = flush_ops(h);  // the tail
-    if (rc != FI_OK) return rc;
-  }
-  for (; did < rounds; ++did) {
-    rc = gossip_round(h);
-    if (rc != FI_OK) return rc;
-  }
-  return err;
+  return rc;
 }
 
 // The same with the chains already in device memory (e.g. the chains_out of fi_epp_pick_batch_device): nothing
@@ -2320,23 +2237,26 @@ int fi_epp_index_add_chains_device(fi_epp* h, const uint32_t* endpoints, const v
   if (!h || ((!endpoints || !nblocks) && R)) return FI_ERR_INVALID;
   std::lock_guard<std::mutex> lk(h->mu);
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
-  if (!h->cfg.lru_capacity) return fail(h, FI_ERR_STATE, "lru_capacity is 0: no LRU");
-  if (!d_chains) {  // the chains of the handle's most recent stream-ordered pick, still in its own buffer
-    if (R > h->last_plain_R) return fail(h, FI_ERR_STATE, "no pick batch of that size to take the chains from");
-    d_chains = h->d_chain.get();
-    pitch_blocks = h->MP;
+  const int mode_err = choose_lru_mode(h);  // (as in fi_epp_index_add_chains)
+  int err = FI_OK;
+  if (!h->cfg.lru_capacity) {
+    err = fail(h, FI_ERR_STATE, "lru_capacity is 0: no LRU");
+  } else if (!d_chains && R > h->last_plain_R) {
+    err = fail(h, FI_ERR_STATE, "no pick batch of that size to take the chains from");
+  } else {
+    if (!d_chains) {  // the chains of the handle's most recent stream-ordered pick, still in its own buffer
+      d_chains = h->d_chain.get();
+      pitch_blocks = h->MP;
+    }
+    err = check_add_requests(h, endpoints, nblocks, R, pitch_blocks, "the chain pitch");
   }
-  for (uint32_t r = 0; r < R; ++r) {
-    if (endpoints[r] != FI_NO_ENDPOINT && endpoints[r] >= h->cfg.num_endpoints) return fail(h, FI_ERR_INVALID, "endpoint out of range");
-    if (nblocks[r] > pitch_blocks) return fail(h, FI_ERR_INVALID, "nblocks[r] larger than the chain pitch");
+  if (err == FI_OK) err = mode_err;
+  if (h->lru_mode != 1) return err != FI_OK ? err : fail(h, FI_ERR_STATE, "fi_epp_index_add_chains_device needs the device LRU");
+  if (err == FI_OK) {  // the chains were produced on the caller's stream
+    FI_CUDA(cudaEventRecord(h->ev_user.get(), (cudaStream_t)stream));
+    FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_user.get(), 0));
   }
-  int rc = choose_lru_mode(h);
-  if (rc != FI_OK) return rc;
-  if (h->lru_mode != 1) return fail(h, FI_ERR_STATE, "fi_epp_index_add_chains_device needs the device LRU");
-  // the chains were produced on the caller's stream
-  FI_CUDA(cudaEventRecord(h->ev_user.get(), (cudaStream_t)stream));
-  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_user.get(), 0));
-  return lru_device_add(h, endpoints, static_cast<const uint64_t*>(d_chains), true, pitch_blocks, nblocks, R);
+  return lru_device_add(h, endpoints, static_cast<const uint64_t*>(d_chains), true, pitch_blocks, nblocks, R, err);
 }
 
 // Diagnostics: the device LRU's content for one endpoint, least recently used first.
@@ -2729,11 +2649,9 @@ int fi_epp_index_add_submitted(fi_epp* h, uint64_t ticket, const uint32_t* endpo
     return fail(h, FI_ERR_STATE, "the chains of that batch are gone (two later submits, a stream-ordered pick or hash "
                                  "since, or a batch that was not pipelined)");
   if (R > h->slot_R[slot]) return fail(h, FI_ERR_STATE, "R larger than the submitted batch");
-  for (uint32_t r = 0; r < R; ++r) {
-    if (endpoints[r] != FI_NO_ENDPOINT && endpoints[r] >= h->cfg.num_endpoints) return fail(h, FI_ERR_INVALID, "endpoint out of range");
-    if (nblocks[r] > h->cfg.max_blocks) return fail(h, FI_ERR_INVALID, "nblocks[r] larger than max_blocks");
-  }
-  int rc = choose_lru_mode(h);
+  int rc = check_add_requests(h, endpoints, nblocks, R, h->cfg.max_blocks, "max_blocks");
+  if (rc != FI_OK) return rc;
+  rc = choose_lru_mode(h);
   if (rc != FI_OK) return rc;
   if (h->lru_mode != 1) return fail(h, FI_ERR_STATE, "fi_epp_index_add_submitted needs the device LRU");
   return lru_add_submitted(h, (uint32_t)slot, endpoints, nblocks, R);

@@ -174,6 +174,62 @@ uint64_t fihc_lrupool_walk(void* p, const uint32_t* endpoints, const uint64_t* c
   return n;
 }
 
+// plan_staging (lru_batch.h) of W workers' ops given by counts: worker w used wseg[w] <= nseg segments, and
+// counts[(w * nseg + s) * 2 + kind] is how many SETs (kind 0) / CLEARs (kind 1) it has in segment s.  Writes each
+// piece as 7 words (group, worker, seg, clear, src, n, dst), at most piece_cap of them, and each group's fill
+// (n_sets, n_clears), at most group_cap groups; *n_pieces = pieces.  Returns the number of groups.
+uint64_t fihc_plan_staging(uint32_t W, uint32_t nseg, const uint32_t* wseg, const uint64_t* counts, uint64_t ns0, uint64_t nc0,
+                           uint64_t chunk, uint64_t* pieces, uint64_t piece_cap, uint64_t* fills, uint64_t group_cap,
+                           uint64_t* n_pieces) {
+  std::vector<fi::WorkerOps> outs(W);
+  for (uint32_t w = 0; w < W; ++w)
+    for (uint32_t s = 0; s < wseg[w]; ++s) {
+      outs[w].sets_of(s).resize(counts[((size_t)w * nseg + s) * 2]);
+      outs[w].clears_of(s).resize(counts[((size_t)w * nseg + s) * 2 + 1]);
+    }
+  const std::vector<fi::StageGroup> groups = fi::plan_staging(outs, nseg, ns0, nc0, chunk);
+  uint64_t n = 0;
+  for (size_t g = 0; g < groups.size(); ++g) {
+    if (g < group_cap) {
+      fills[2 * g] = groups[g].n_sets;
+      fills[2 * g + 1] = groups[g].n_clears;
+    }
+    for (const fi::StagePiece& p : groups[g].pieces) {
+      if (n < piece_cap) {
+        const uint64_t row[7] = {g, p.worker, p.seg, p.clear, p.src, p.n, p.dst};
+        std::memcpy(pieces + 7 * n, row, sizeof(row));
+      }
+      ++n;
+    }
+  }
+  *n_pieces = n;
+  return groups.size();
+}
+
+// One fi_epp_index_add_chains on a pool: walk the batch, plan its staging behind an open group of ns0 SETs and nc0
+// CLEARs, and write the ops in the order they are staged, each with its group (ops[i], group[i]; at most cap).
+// Returns how many ops there are; *n_groups = groups (the last one, the tail, stays open).
+uint64_t fihc_lrupool_stage(void* p, const uint32_t* endpoints, const uint64_t* chains, uint32_t pitch, const uint32_t* nblocks,
+                            uint32_t R, uint64_t ns0, uint64_t nc0, uint64_t chunk, fi_index_op* ops, uint32_t* group, uint64_t cap,
+                            uint64_t* n_groups) {
+  HcLruPool& hp = *(HcLruPool*)p;
+  const size_t nseg = fi::lru_walk_batch(hp.lrus, 0, (uint32_t)hp.lrus.size(), endpoints, chains, pitch, nblocks, R, hp.pool, hp.outs);
+  const std::vector<fi::StageGroup> groups = fi::plan_staging(hp.outs, nseg, ns0, nc0, chunk);
+  uint64_t n = 0;
+  for (uint32_t g = 0; g < groups.size(); ++g)
+    for (const fi::StagePiece& sp : groups[g].pieces) {
+      const fi::WorkerOps& o = hp.outs[sp.worker];
+      const fi_index_op* src = (sp.clear ? o.clears : o.sets)[sp.seg].data() + sp.src;
+      for (size_t i = 0; i < sp.n; ++i, ++n)
+        if (n < cap) {
+          ops[n] = src[i];
+          group[n] = g;
+        }
+    }
+  *n_groups = groups.size();
+  return n;
+}
+
 // fi_epp_index_add_chains' host phase (lru_batch.h) against the sequential definition: walk the batch on
 // `workers` threads, apply the resulting ops segment by segment (all SETs of a segment, then all its CLEARs — the
 // way the GPU applies a group) to a membership set, and compare that set and the LRU contents with one LRU per

@@ -8,7 +8,8 @@
 // CLEARs"; that equals the sequential order except when a hash is re-added after its own eviction inside the same
 // batch — then the endpoint's later ops go to the next SEGMENT (segments are applied one after the other), which
 // keeps "last op wins" exact.  Every set evicts against its own limit() (fi_epp_set_lru_capacities).  Host-only
-// code (no CUDA): tests/test_host_logic.py and tests/test_lru_capacity_cpu.py run it against a sequential LRU.
+// code (no CUDA): tests/test_host_logic.py and tests/test_lru_capacity_cpu.py run it against a sequential LRU, and
+// tests/test_add_staging_cpu.py checks the staging plan (plan_staging).
 #pragma once
 #include <algorithm>
 #include <atomic>
@@ -240,6 +241,52 @@ inline size_t lru_walk_batch(std::vector<LruSet>& lrus, uint32_t lo, uint32_t EL
   size_t nseg = 0;
   for (auto& o : outs) nseg = std::max(nseg, o.nseg);
   return nseg;
+}
+
+// One copy of a staging plan: ops [src, src + n) of outs[worker].sets[seg] (or .clears[seg]) go to offset dst of the
+// group's SET (or CLEAR) buffer.
+struct StagePiece {
+  uint32_t worker, seg;
+  bool clear;
+  size_t src, n;
+  uint64_t dst;
+};
+struct StageGroup {
+  std::vector<StagePiece> pieces;
+  uint64_t n_sets = 0, n_clears = 0;  // the group's fill once its pieces are copied
+};
+
+// Where the ops of one walk are staged (fi_epp_index_add_chains).  The open group already holds ns0 SETs and nc0
+// CLEARs; the walk's ops follow segment by segment, a segment's SETs before its CLEARs, worker by worker.  A group is
+// closed (flushed) when a buffer of `chunk` ops is full, and at a segment boundary when anything is staged.  The ops
+// staged before the call count as a segment of their own: when they include CLEARs the plan begins with a flush, so
+// that no SET of this call shares a group with them.  Every group but the last (the tail) ends with a flush.  Counts
+// and offsets only: the ops themselves are not read.
+inline std::vector<StageGroup> plan_staging(const std::vector<WorkerOps>& outs, size_t nseg, uint64_t ns0, uint64_t nc0,
+                                            uint64_t chunk) {
+  std::vector<StageGroup> groups(1);
+  groups[0].n_sets = ns0;
+  groups[0].n_clears = nc0;
+  if (nc0) groups.emplace_back();
+  for (size_t seg = 0; seg < nseg; ++seg) {
+    for (int kind = 0; kind < 2; ++kind)
+      for (uint32_t w = 0; w < outs.size(); ++w) {
+        if (outs[w].nseg <= seg) continue;
+        const size_t n = (kind ? outs[w].clears[seg] : outs[w].sets[seg]).size();
+        for (size_t done = 0; done < n;) {
+          StageGroup& g = groups.back();
+          uint64_t& fill = kind ? g.n_clears : g.n_sets;
+          const size_t take = std::min<uint64_t>(chunk - fill, n - done);
+          g.pieces.push_back(StagePiece{w, (uint32_t)seg, kind == 1, done, take, fill});
+          fill += take;
+          done += take;
+          if (fill == chunk) groups.emplace_back();
+        }
+      }
+    // the next segment's SETs must run after these CLEARs
+    if (seg + 1 < nseg && (groups.back().n_sets || groups.back().n_clears)) groups.emplace_back();
+  }
+  return groups;
 }
 
 }  // namespace fi
