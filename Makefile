@@ -12,11 +12,9 @@ CU_SRCS := $(CSRC)/hash_kernels.cu $(CSRC)/index_kernels.cu $(CSRC)/lru_kernels.
 CU_OBJS := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(CU_SRCS))
 HDRS := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/fi_epp.h
 
-RANKED_ORACLE := $(OBJDIR)/libepp_ranked_oracle.so
-SUBSET_ORACLE := $(OBJDIR)/libepp_subset_oracle.so
-CAPACITY_ORACLE := $(OBJDIR)/libepp_capacity_oracle.so
+EXT_ORACLE := $(OBJDIR)/libepp_ext_oracle.so
 
-all: $(LIB) $(HOSTCHECK) oracle $(RANKED_ORACLE) $(SUBSET_ORACLE) $(CAPACITY_ORACLE)
+all: $(LIB) $(HOSTCHECK) oracle $(EXT_ORACLE)
 
 $(OBJDIR)/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -38,20 +36,11 @@ $(HOSTCHECK): $(CSRC)/hostcheck.cpp $(CSRC)/xxh64.cuh $(CSRC)/bitslice.cuh $(CSR
 oracle:
 	$(MAKE) -C oracle
 
-# the CPU oracle plus its ranked pick (tests/ranked_oracle.cpp), test infrastructure only
-$(RANKED_ORACLE): tests/ranked_oracle.cpp oracle/epp_oracle.cpp include/fi_epp.h
+# a test-side extension of the CPU oracle, tests/<name>.cpp -> build/libepp_<name>.so (test infrastructure only):
+# tests/ext_oracle.cpp adds the ranked / subset pick and per-endpoint LRU capacities
+$(OBJDIR)/libepp_%.so: tests/%.cpp oracle/epp_oracle.cpp include/fi_epp.h
 	@mkdir -p $(OBJDIR)
-	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ tests/ranked_oracle.cpp
-
-# the CPU oracle plus its subset pick (tests/subset_oracle.cpp), test infrastructure only
-$(SUBSET_ORACLE): tests/subset_oracle.cpp oracle/epp_oracle.cpp include/fi_epp.h
-	@mkdir -p $(OBJDIR)
-	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ tests/subset_oracle.cpp
-
-# the CPU oracle plus per-endpoint LRU capacities (tests/capacity_oracle.cpp), test infrastructure only
-$(CAPACITY_ORACLE): tests/capacity_oracle.cpp oracle/epp_oracle.cpp include/fi_epp.h
-	@mkdir -p $(OBJDIR)
-	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ tests/capacity_oracle.cpp
+	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ $<
 
 clean:
 	rm -rf $(OBJDIR) $(LIB) $(HOSTCHECK)

@@ -1,4 +1,4 @@
-"""GPU (-m gpu): indexer.Add calls in a row, with no pick or sync between them, against the capacity oracle.
+"""GPU (-m gpu): indexer.Add calls in a row, with no pick or sync between them, against the CPU oracle.
 
 On the host LRU (device_lru = 0) the Adds stage their index ops in an open group that the GPU applies as all SETs, then
 all CLEARs.  A CLEAR staged by one call and a SET of the same pair staged by the next must not share a group, whichever
@@ -12,13 +12,13 @@ import pytest
 from fusioninfer_b200 import EndpointPicker
 from fusioninfer_b200 import _abi as abi
 from tests import helpers as H
-from tests.capacity_oracle import CapacityOracle
+from tests.ext_oracle import ExtOracle
 
 pytestmark = pytest.mark.gpu
 
 
 class _Pair:
-    """a handle and the capacity oracle fed the same Adds; `ever` = every key added so far"""
+    """a handle and the CPU oracle (tests/ext_oracle.cpp) fed the same Adds; `ever` = every key added so far"""
 
     def __init__(self, device_lru, E=4, cap=8, max_blocks=4, table_slots=0):
         wl = H.small_workload(E=E, R=8, T=max_blocks * 16, max_blocks=max_blocks, lru_capacity=0)
@@ -27,7 +27,7 @@ class _Pair:
         self.gpu.set_option("device_lru", device_lru)
         if table_slots:
             self.gpu.set_option("lru_table_slots", table_slots)
-        self.ref = CapacityOracle(self.cfg)
+        self.ref = ExtOracle(self.cfg)
         self.E, self.mb, self.ever = E, max_blocks, set()
 
     def add_chains(self, eps, chains):

@@ -4,8 +4,8 @@ tests/collide.py places keys exactly where a test wants them: full home buckets,
 (slot) to the first, runs that merge, tombstones at the start, middle and end of runs, one new key claimed by several
 CTAs at once.  Its models replay every call and the tests assert that each crafted layout really happened (a probe
 that wraps, a key behind tombstones, a miss decided past its home), so a drift between a constructor and the kernels
-cannot leave a test checking nothing.  Membership is compared with oracle/epp_oracle.cpp, picks with the ranked
-oracle, removals with tests/remove_ref.py, and the device LRU's recency order with tests/capacity_oracle.py.
+cannot leave a test checking nothing.  Membership is compared with oracle/epp_oracle.cpp, picks (ranked ones too) and
+the device LRU's recency order with its extension tests/ext_oracle.cpp, and removals with tests/remove_ref.py.
 """
 import numpy as np
 import pytest
@@ -15,8 +15,7 @@ from fusioninfer_b200 import _abi as abi
 from oracle import epp_oracle as eo
 from tests import collide as X
 from tests import helpers as H
-from tests.capacity_oracle import CapacityOracle
-from tests.ranked_oracle import RankedOracle
+from tests.ext_oracle import ExtOracle
 from tests.remove_ref import RemovalOracle
 
 pytestmark = pytest.mark.gpu
@@ -216,7 +215,7 @@ class _PickScene:
 
     SLOTS, R, MB, BB, BATCH = 4096, 48, 32, 64, 4800
 
-    def __init__(self, E, mode, shuffled, seed=11, ref_cls=RankedOracle):
+    def __init__(self, E, mode, shuffled, seed=11, ref_cls=ExtOracle):
         self.E, self.mode = E, mode
         self.cfg = make_config(num_endpoints=E, block_bytes=self.BB, max_blocks=self.MB, lru_capacity=0, max_batch=self.BATCH,
                                profiles=WEIGHTED, match_mode=mode, index_slots=self.SLOTS)
@@ -387,7 +386,8 @@ def test_removal_through_runs(mode):
 
 # ---- d. the device LRU -------------------------------------------------------------------------------------------------
 class _Lru:
-    """a device-LRU handle (lru_table_slots pinned), the capacity oracle and one LruModel per endpoint"""
+    """a device-LRU handle (lru_table_slots pinned), the oracle with per-endpoint capacities and one LruModel per
+    endpoint"""
 
     C, MB, E = 64, 32, 4
 
@@ -397,7 +397,7 @@ class _Lru:
         self.gpu = EndpointPicker(self.cfg)
         self.gpu.set_option("device_lru", 1)
         self.gpu.set_option("lru_table_slots", ts_option)
-        self.ref = CapacityOracle(self.cfg)
+        self.ref = ExtOracle(self.cfg)
         self.TS = X.dlru_table_slots(self.C, ts_option)
         self.models = [X.LruModel(self.TS, self.C) for _ in range(self.E)]
         self.caps = [self.C] * self.E

@@ -1,6 +1,6 @@
 """GPU (-m gpu): per-endpoint LRU capacities (fi_epp_set_lru_capacities, SPEC S.2b) against the CPU reference.
 
-The reference is tests/capacity_oracle.cpp: the CPU oracle with an LRU capacity per endpoint.  Every check is
+The reference is tests/ext_oracle.cpp: the CPU oracle with an LRU capacity per endpoint.  Every check is
 bit-exact: the device LRU's recency order (fi_epp_lru_dump) against the reference's, index
 membership (fi_epp_index_contains) and picks against the oracle's.  Where a test takes `device_lru`, it runs on the
 device LRU and on the host LRU (device_lru = 0), whose recency order is not observable (membership and picks are).
@@ -15,7 +15,7 @@ from fusioninfer_b200 import _abi as abi
 from fusioninfer_b200.dist import shard_range
 from fusioninfer_b200.picker import FiEppError
 from tests import helpers as H
-from tests.capacity_oracle import CapacityOracle
+from tests.ext_oracle import ExtOracle
 
 pytestmark = pytest.mark.gpu
 P, K, Q = H.P, H.K, H.Q
@@ -31,7 +31,7 @@ class _Run:
         self.gpu = EndpointPicker(self.cfg)
         self.gpu.set_option("device_lru", device_lru)
         self.device_lru = device_lru
-        self.ref = CapacityOracle(self.cfg, track_removal=track_removal)
+        self.ref = ExtOracle(self.cfg, track_removal=track_removal)
         st = self.wl.endpoint_states()
         self.gpu.update_endpoints(st)
         self.ref.update_endpoints(st)
@@ -160,7 +160,7 @@ def test_rounds_exceed_the_clear_buffer(case):
     E, cap, filled = (64, 4096, list(range(64))) if case == "many_endpoints" else (2, 196 * pitch, [0])
     wl = H.small_workload(E=E, R=8, max_blocks=mb, lru_capacity=0)
     cfg = H.config_for(wl, profiles=WEIGHTED, lru_capacity=cap, max_batch=8, index_slots=1 << 20)
-    gpu, ref = EndpointPicker(cfg), CapacityOracle(cfg)
+    gpu, ref = EndpointPicker(cfg), ExtOracle(cfg)
     rng = np.random.default_rng(3)
     keys = rng.integers(1, 2**63, size=len(filled) * cap, dtype=np.uint64)
     rows = keys.reshape(-1, pitch)

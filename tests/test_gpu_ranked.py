@@ -1,7 +1,7 @@
 """GPU (-m gpu): the ranked pick (fi_epp_pick_batch_ranked / _device_ranked, docs/SPEC.md S.6a).
 
 Every comparison is bit-exact (scores as raw 64-bit patterns): k = 1 against the single pick of the same handle,
-k > 1 against the ranked CPU oracle (tests/ranked_oracle.cpp), on every row shape of the match kernel.
+k > 1 against the CPU oracle's ranked pick (tests/ext_oracle.cpp), on every row shape of the match kernel.
 """
 import ctypes as C
 import threading
@@ -14,7 +14,7 @@ from fusioninfer_b200 import _abi as abi
 from fusioninfer_b200.dist import shard_range
 from fusioninfer_b200.picker import FiEppError
 from tests import helpers as H
-from tests.ranked_oracle import RankedOracle
+from tests.ext_oracle import ExtOracle
 
 pytestmark = pytest.mark.gpu
 P, K, Q, L = H.P, H.K, H.Q, abi.FI_SCORER_LORA
@@ -61,7 +61,7 @@ def _setup(wl, case, mode, rng, **kw):
     if case == "pd":  # a threshold that splits the batch between prefill and skip
         spec["pd"] = dict(spec["pd"], threshold=0.6 * wl.T * 4)
     cfg = H.config_for(wl, match_mode=mode, max_prompt_bytes=wl.R * wl.T * 4, **spec, **kw)
-    gpu, cpu = EndpointPicker(cfg), RankedOracle(cfg)
+    gpu, cpu = EndpointPicker(cfg), ExtOracle(cfg)
     st = _states(wl, rng)
     gpu.update_endpoints(st)
     cpu.update_endpoints(st)
@@ -119,7 +119,7 @@ def test_ranked_equals_the_oracle_on_every_row_shape(E, mode):
                 {"name": "prefix", "role_mask": 3, "scorers": [(P, 100)]},
                 {"name": "none", "role_mask": NOBODY, "scorers": [(P, 1)]}]
     cfg = H.config_for(wl, match_mode=mode, profiles=profiles)
-    gpu, cpu = EndpointPicker(cfg), RankedOracle(cfg)
+    gpu, cpu = EndpointPicker(cfg), ExtOracle(cfg)
     st = _states(wl, rng, roles=False)
     st["role_mask"] = rng.integers(1, 8, E).astype(np.uint32)
     gpu.update_endpoints(st)
@@ -246,7 +246,7 @@ def test_sub_range_handle_reports_global_endpoints():
     begin, count = 100, 150
     profiles = [{"name": "default", "scorers": [(P, 100), (K, 13)]}]
     gpu = EndpointPicker(H.config_for(wl, profiles=profiles, endpoint_begin=begin, endpoint_count=count))
-    cpu = RankedOracle(H.config_for(wl, profiles=profiles))
+    cpu = ExtOracle(H.config_for(wl, profiles=profiles))
     st = _states(wl, rng, roles=False)
     gpu.update_endpoints(st)
     st = st.copy()

@@ -15,8 +15,7 @@ from fusioninfer_b200.picker import FiEppError
 from oracle import epp_oracle as eo
 from tests import score_edges as S
 from tests.helpers import describe_diff
-from tests.ranked_oracle import RankedOracle
-from tests.subset_oracle import SubsetOracle
+from tests.ext_oracle import ExtOracle
 
 pytestmark = pytest.mark.gpu
 
@@ -44,21 +43,21 @@ def test_every_entry_point_on_the_edges(kind, E):
     c = S.gpu_case(kind, E)
     cfg = c.config()
     Pn = len(c.profiles)
-    g, ro, so = EndpointPicker(cfg), RankedOracle(cfg), SubsetOracle(cfg)
-    for x in (g, ro, so):
+    g, o = EndpointPicker(cfg), ExtOracle(cfg)
+    for x in (g, o):
         c.load(x)
     spec = S.Spec(c)
     ad = c.adapters
 
     # the single pick: zero-match shortcut (no LoRA scorer) or every endpoint scored (LoRA)
     single = g.pick_batch(c.tok, c.offs, c.h0, adapters=ad)
-    _eq(single, ro.pick_batch(c.tok, c.offs, c.h0, adapters=ad), "pick_batch vs the oracle")
+    _eq(single, o.pick_batch(c.tok, c.offs, c.h0, adapters=ad), "pick_batch vs the oracle")
     _eq(single, spec.picks(), "pick_batch vs spec_total")
 
     # ranked: k = 16 is above the eligible count of the small pools and of the edge cases' "few" profile
     for k in (1, 5, 16):
         got = g.pick_batch_ranked(c.tok, c.offs, c.h0, k, adapters=ad)
-        _eq(got, ro.pick_batch_ranked(c.tok, c.offs, c.h0, k, adapters=ad), f"pick_batch_ranked k={k} vs the oracle")
+        _eq(got, o.pick_batch_ranked(c.tok, c.offs, c.h0, k, adapters=ad), f"pick_batch_ranked k={k} vs the oracle")
         _eq(np.ascontiguousarray(got[:, :, 0]), single, f"pick_batch_ranked k={k} entry 0 vs pick_batch")
     if kind == "edges" or E == 3:
         elig = int(spec.elig[1 if kind == "edges" else 0].sum())
@@ -68,7 +67,7 @@ def test_every_entry_point_on_the_edges(kind, E):
     sub = S.subset_rows(c, seed=E)
     for k in (1, 5):
         got = g.pick_batch_subset(c.tok, c.offs, c.h0, sub, k, adapters=ad)
-        _eq(got, so.pick_batch_subset(c.tok, c.offs, c.h0, sub, k, adapters=ad), f"pick_batch_subset k={k} vs the oracle")
+        _eq(got, o.pick_batch_subset(c.tok, c.offs, c.h0, sub, k, adapters=ad), f"pick_batch_subset k={k} vs the oracle")
     if E <= 100:
         _eq(got, spec.ranked(5, sub), "pick_batch_subset k=5 vs the subset-aware spec")
 
@@ -87,10 +86,9 @@ def test_every_entry_point_on_the_edges(kind, E):
     assert t5 == t0 + 1
     _eq(d0[3].cpu().numpy().view(S.PICK_DTYPE).reshape(c.R, Pn), single, "pick_submit_ex k=0 vs pick_batch")
     _eq(d5[3].cpu().numpy().view(S.PICK_DTYPE).reshape(c.R, Pn, 5),
-        so.pick_batch_subset(c.tok, c.offs, c.h0, sub, 5, adapters=ad), "pick_submit_ex k=5 with subsets vs the oracle")
+        o.pick_batch_subset(c.tok, c.offs, c.h0, sub, 5, adapters=ad), "pick_submit_ex k=5 with subsets vs the oracle")
     g.close()
-    ro.close()
-    so.close()
+    o.close()
 
 
 @pytest.mark.parametrize("E", [40, 1024])

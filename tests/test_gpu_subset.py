@@ -1,8 +1,8 @@
 """GPU (-m gpu): subset picks (fi_epp_pick_batch_subset / _device_subset, docs/SPEC.md S.5a).
 
 Every comparison is bit-exact (scores as raw 64-bit patterns): no subset and all-ones subsets against the ranked and
-single picks of the same handle, random subsets against the subset CPU oracle (tests/subset_oracle.cpp), on every
-row shape of the match kernel.
+single picks of the same handle, random subsets against the CPU oracle's subset pick (tests/ext_oracle.cpp), on
+every row shape of the match kernel.
 """
 import ctypes as C
 
@@ -13,7 +13,7 @@ from fusioninfer_b200 import EndpointPicker, subset_bitsets
 from fusioninfer_b200 import _abi as abi
 from fusioninfer_b200.picker import FiEppError
 from tests import helpers as H
-from tests.subset_oracle import SubsetOracle
+from tests.ext_oracle import ExtOracle
 from tests.test_gpu_ranked import CASES, _cold, _device_batch, _eq, _lora, _states
 
 pytestmark = pytest.mark.gpu
@@ -25,7 +25,7 @@ def _setup(wl, case, mode, rng, **kw):
     if case == "pd":  # a threshold that splits the batch between prefill and skip
         spec["pd"] = dict(spec["pd"], threshold=0.6 * wl.T * 4)
     cfg = H.config_for(wl, match_mode=mode, max_prompt_bytes=wl.R * wl.T * 4, **spec, **kw)
-    gpu, cpu = EndpointPicker(cfg), SubsetOracle(cfg)
+    gpu, cpu = EndpointPicker(cfg), ExtOracle(cfg)
     st = _states(wl, rng)
     gpu.update_endpoints(st)
     cpu.update_endpoints(st)

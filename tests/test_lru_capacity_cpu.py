@@ -1,6 +1,6 @@
-"""CPU: per-endpoint LRU capacities (fi_epp_set_lru_capacities, SPEC S.2b) in the capacity oracle and in the host LRU.
+"""CPU: per-endpoint LRU capacities (fi_epp_set_lru_capacities, SPEC S.2b) in the CPU oracle and in the host LRU.
 
-The capacity oracle (tests/capacity_oracle.cpp, the CPU oracle with a capacity per endpoint) is what the GPU tests
+The oracle's extension (tests/ext_oracle.cpp, the CPU oracle with a capacity per endpoint) is what the GPU tests
 compare against; here it is checked against the oracle's own Adds (uniform capacities) and against an ordered-dict
 model of the same calls (random capacities).  The host LRU's LruSet::shrink and the
 batched host walk (lru_batch.h) with mixed limits are driven through libfi_hostcheck.so against the same model.
@@ -16,7 +16,7 @@ import pytest
 from fusioninfer_b200 import _abi as abi
 from oracle import epp_oracle as eo
 from tests import helpers as H
-from tests.capacity_oracle import CapacityOracle
+from tests.ext_oracle import ExtOracle
 
 
 class _Model:
@@ -65,7 +65,7 @@ def test_reference_with_uniform_capacities_is_the_oracle():
     rng = random.Random(3)
     universe = _universe(rng, 40)
     for variant in ("never", "lru_capacity", "zero"):
-        ref, cpu = CapacityOracle(cfg), eo.Oracle(cfg)
+        ref, cpu = ExtOracle(cfg), eo.Oracle(cfg)
         if variant != "never":
             assert ref.set_lru_capacities(list(range(E)), [cap if variant == "lru_capacity" else 0] * E) == []
         for _ in range(40):
@@ -91,7 +91,7 @@ def test_reference_with_random_capacities_matches_model():
     (shrinks, grows, duplicates in one call) between random Adds and direct ops."""
     E, cap, mb = 8, 24, 4
     cfg = H.make_config(num_endpoints=E, max_batch=8, max_blocks=mb, lru_capacity=cap)
-    ref, model = CapacityOracle(cfg), _Model(E, cap)
+    ref, model = ExtOracle(cfg), _Model(E, cap)
     rng = random.Random(11)
     universe = _universe(rng, 120)
     for step in range(60):

@@ -1,8 +1,8 @@
 """CPU: the ranked pick's configuration entry point and its oracle (docs/SPEC.md S.6a).
 
 fi_epp_config_picker_endpoints reads each profile's max-score-picker maxNumOfEndpoints through the same loader as
-fi_epp_config_from_yaml.  The ranked oracle (tests/ranked_oracle.cpp) is checked against a ranking built here with
-numpy from tests/restate.py's independent match, eligibility and score pieces.
+fi_epp_config_from_yaml.  The oracle's ranked pick (tests/ext_oracle.cpp; the subset pick with no subsets) is checked
+against a ranking built here with numpy from tests/restate.py's independent match, eligibility and score pieces.
 """
 import ctypes as C
 
@@ -14,7 +14,7 @@ from fusioninfer_b200 import config_from_yaml, make_config, synth
 from fusioninfer_b200.picker import FiEppError, config_picker_endpoints
 from tests import helpers as H
 from tests import restate
-from tests.ranked_oracle import RankedOracle
+from tests.ext_oracle import ExtOracle
 from tests.test_host_logic import PD_YAML, PREFIX_YAML, _single
 
 P, K, Q, L = H.P, H.K, H.Q, abi.FI_SCORER_LORA
@@ -92,7 +92,7 @@ def test_picker_endpoints_null_arguments():
     assert lib.fi_epp_config_picker_endpoints(raw, len(raw), None, None, 0) == abi.FI_ERR_INVALID
 
 
-# ---- the ranked oracle against a numpy ranking from tests/restate.py -----------------------------------------------
+# ---- the oracle's ranked pick against a numpy ranking from tests/restate.py -----------------------------------------
 def _numpy_ranking(rs, prompts, offsets, h0, k, adapters=None):
     """[R, P, k] (endpoint, match, n, total) rows: every eligible endpoint's total from restate's pieces, ordered by
     np.lexsort on (rotation distance, -total)"""
@@ -183,7 +183,7 @@ def test_ranked_oracle_matches_numpy_ranking(case, mode, E):
     wl = synth.Workload(R=24, E=E, T=160, seed=synth.SEEDS[1], max_blocks=8, lru_capacity=64, holes=True)
     cfg = make_config(num_endpoints=E, block_bytes=wl.block_bytes, max_blocks=wl.max_blocks, max_batch=wl.R,
                       match_mode=mode, **CASES[case])
-    orc, rs = RankedOracle(cfg), restate.from_config(cfg)
+    orc, rs = ExtOracle(cfg), restate.from_config(cfg)
     st = _random_states(E, rng)
     orc.update_endpoints(st)
     rs.update_endpoints(st)

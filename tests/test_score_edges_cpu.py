@@ -1,7 +1,8 @@
 """CPU: the scoring edge cases of tests/score_edges.py through the three CPU restatements of docs/SPEC.md — the
 oracle, tests/restate.py and the exact Fraction reference spec_total — which must agree bit for bit; the ranked and
-subset oracles against the single pick and the subset-aware reference; and proof that every modelled kernel mistake
-changes an expected output of the cases, so the bit-exact GPU comparisons of test_gpu_score_edges.py can see it."""
+subset picks of tests/ext_oracle.cpp against the single pick and the subset-aware reference; and proof that every
+modelled kernel mistake changes an expected output of the cases, so the bit-exact GPU comparisons of
+test_gpu_score_edges.py can see it."""
 import functools
 
 import numpy as np
@@ -12,8 +13,7 @@ from oracle import epp_oracle as eo
 from tests import restate
 from tests import score_edges as S
 from tests.helpers import describe_diff
-from tests.ranked_oracle import RankedOracle
-from tests.subset_oracle import SubsetOracle
+from tests.ext_oracle import ExtOracle
 
 MODES = [abi.FI_MATCH_UPSTREAM, abi.FI_MATCH_LPM]
 POOLS = [3, 40, 100]
@@ -53,23 +53,21 @@ def test_oracle_restatement_and_exact_reference_agree(kind, E, mode):
 def test_ranked_and_subset_oracles_on_the_edges(kind, E, mode):
     c = _case(kind, E, mode)
     cfg = c.config()
-    ro, so = RankedOracle(cfg), SubsetOracle(cfg)
-    c.load(ro)
-    c.load(so)
+    o = ExtOracle(cfg)
+    c.load(o)
     spec = S.Spec(c)
     single = spec.picks()
     for k in (1, 5, 16):
-        ranked = ro.pick_batch_ranked(c.tok, c.offs, c.h0, k, adapters=c.adapters)
+        ranked = o.pick_batch_ranked(c.tok, c.offs, c.h0, k, adapters=c.adapters)
         _eq(np.ascontiguousarray(ranked[:, :, 0]), single, f"ranked k={k} entry 0 vs the single pick")
         _eq(ranked, spec.ranked(k), f"ranked k={k} vs spec")
         full = np.full((c.R, (E + 31) // 32), 0xFFFFFFFF, dtype=np.uint32)
-        _eq(so.pick_batch_subset(c.tok, c.offs, c.h0, full, k, adapters=c.adapters), ranked, f"full subset k={k} vs ranked")
+        _eq(o.pick_batch_subset(c.tok, c.offs, c.h0, full, k, adapters=c.adapters), ranked, f"full subset k={k} vs ranked")
     sub = S.subset_rows(c, seed=E + mode)
     for k in (1, 5):
-        _eq(so.pick_batch_subset(c.tok, c.offs, c.h0, sub, k, adapters=c.adapters), spec.ranked(k, sub),
+        _eq(o.pick_batch_subset(c.tok, c.offs, c.h0, sub, k, adapters=c.adapters), spec.ranked(k, sub),
             f"proper subsets k={k} vs the subset-aware spec")
-    ro.close()
-    so.close()
+    o.close()
 
 
 def test_queue_extremes_inside_and_outside_the_subsets():

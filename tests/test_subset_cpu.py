@@ -1,4 +1,5 @@
-"""CPU: the subset pick's oracle on hand-worked cases (docs/SPEC.md S.5a), its bitset helper and its C binding.
+"""CPU: the subset pick of the oracle extension (tests/ext_oracle.cpp) on hand-worked cases (docs/SPEC.md S.5a), its
+bitset helper and its C binding.
 
 Each case is small enough to work out by hand: four endpoints, one four-block prompt, and the index rows set
 explicitly from the prompt's own chain.
@@ -12,8 +13,7 @@ import pytest
 from fusioninfer_b200 import _abi as abi
 from fusioninfer_b200 import make_config, subset_bitsets, synth
 from tests import helpers as H
-from tests.ranked_oracle import RankedOracle
-from tests.subset_oracle import SubsetOracle
+from tests.ext_oracle import ExtOracle
 
 P, K, Q = H.P, H.K, H.Q
 NO = abi.FI_NO_ENDPOINT
@@ -24,7 +24,7 @@ H0 = 0x1234
 def _oracle(profiles, E=4, pd=None, mode=abi.FI_MATCH_UPSTREAM, queue=None, roles=None, alive=None):
     cfg = make_config(num_endpoints=E, block_bytes=B, max_blocks=8, max_batch=16, match_mode=mode, profiles=profiles,
                       pd=pd)
-    o = SubsetOracle(cfg)
+    o = ExtOracle(cfg)
     o.update_endpoints(H.states_array(E, queue=queue, roles=roles, alive=alive))
     return o
 
@@ -128,6 +128,10 @@ def test_k_beyond_the_subset_is_padded():
 
 @pytest.mark.parametrize("mode", [abi.FI_MATCH_UPSTREAM, abi.FI_MATCH_LPM])
 def test_no_subset_and_all_ones_equal_the_ranked_oracle(mode):
+    """No subset is the ranked pick itself (one function, which test_ranked_cpu.py's
+    test_ranked_oracle_matches_numpy_ranking checks against tests/restate.py).  All-ones rows must equal it: the queue
+    range over a full row is the pool's.  Entry 0 of both is the oracle's single pick (epo_pick_batch, code the ranked
+    pick does not share).  A subset never adds an endpoint."""
     rng = np.random.default_rng(9 + mode)
     E = 40
     wl = synth.Workload(R=24, E=E, T=160, seed=synth.SEEDS[1], max_blocks=8, lru_capacity=64, holes=True)
@@ -135,26 +139,25 @@ def test_no_subset_and_all_ones_equal_the_ranked_oracle(mode):
                 {"name": "a", "role_mask": 3, "scorers": [(P, 10), (Q, 3)]}]
     cfg = make_config(num_endpoints=E, block_bytes=wl.block_bytes, max_blocks=wl.max_blocks, max_batch=wl.R,
                       match_mode=mode, profiles=profiles)
-    sub, ranked = SubsetOracle(cfg), RankedOracle(cfg)
-    st = H.states_array(E, kv=rng.integers(0, 8, E) / 8.0, queue=rng.integers(0, 6, E),
-                        roles=rng.integers(1, 8, E).astype(np.uint32), alive=np.where(rng.random(E) < 0.2, 0, 1))
-    for o in (sub, ranked):
-        o.update_endpoints(st)
-        for ops in wl.index_ops():
-            o.index_apply(ops)
+    o = ExtOracle(cfg)
+    o.update_endpoints(H.states_array(E, kv=rng.integers(0, 8, E) / 8.0, queue=rng.integers(0, 6, E),
+                                      roles=rng.integers(1, 8, E).astype(np.uint32),
+                                      alive=np.where(rng.random(E) < 0.2, 0, 1)))
+    for ops in wl.index_ops():
+        o.index_apply(ops)
     tok, offs = wl.prompts()
+    single = o.pick_batch(tok, offs, wl.h0)
     for k in (1, 5):
-        want = ranked.pick_batch_ranked(tok, offs, wl.h0, k)
-        assert H.picks_equal(sub.pick_batch_subset(tok, offs, wl.h0, None, k), want)
-        assert H.picks_equal(sub.pick_batch_subset(tok, offs, wl.h0, subset_bitsets([None] * wl.R, E), k), want)
+        want = o.pick_batch_ranked(tok, offs, wl.h0, k)
+        assert H.picks_equal(np.ascontiguousarray(want[:, :, 0]), single)
+        assert H.picks_equal(o.pick_batch_subset(tok, offs, wl.h0, subset_bitsets([None] * wl.R, E), k), want)
     # a subset never adds an endpoint: every listed pick is a candidate of its request
     lists = [sorted(rng.choice(E, 6, replace=False).tolist()) for _ in range(wl.R)]
-    got = sub.pick_batch_subset(tok, offs, wl.h0, subset_bitsets(lists, E), 3)
+    got = o.pick_batch_subset(tok, offs, wl.h0, subset_bitsets(lists, E), 3)
     for r in range(wl.R):
         real = got["endpoint"][r][got["endpoint"][r] != NO]
         assert set(real.tolist()) <= set(lists[r])
-    sub.close()
-    ranked.close()
+    o.close()
 
 
 def test_subset_bitsets():

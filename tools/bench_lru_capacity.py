@@ -8,7 +8,7 @@
      hetero    a third of the pods at 31 250, a third at 15 625, a third at 7 813.
    Reported: decisions/s over the timed steps.  Exactness: `never` is checked bit for bit against the oracle on the
    first --oracle-steps steps; `uniform` must give byte-identical picks to `never` at every step; `hetero` is checked
-   bit for bit against the capacity oracle (the CPU oracle with per-endpoint capacities, tests/capacity_oracle.cpp,
+   bit for bit against the capacity oracle (the CPU oracle with per-endpoint capacities, tests/ext_oracle.cpp,
    built by `make`) fed the same calls, on the first --oracle-steps steps.
 2. Resize: the time of fi_epp_set_lru_capacities(want_evicted) halving the capacity of 1, 64 and 1 024 pods of a
    full index (a fresh handle each), and the entries evicted.
@@ -68,7 +68,7 @@ def main():
 
     from fusioninfer_b200 import EndpointPicker, PinnedBuffer, make_config, synth
     from oracle import epp_oracle as eo
-    from tests.capacity_oracle import CapacityOracle
+    from tests.ext_oracle import ExtOracle
 
     wl = synth.baseline_workload(args.cfg)
     profiles, pd = synth.baseline_profiles(args.cfg)
@@ -114,7 +114,7 @@ def main():
             mirror.update_endpoints(wl.endpoint_states())
             mirror.index_reserve(2 * E * C)
         elif variant == "hetero":
-            mirror = CapacityOracle(cfg)
+            mirror = ExtOracle(cfg)
             mirror.update_endpoints(wl.endpoint_states())
             mirror.index_reserve(2 * E * C)
             mirror.set_lru_capacities(all_eps, hetero)

@@ -6,7 +6,7 @@ pick at k = 1, the subset call with NULL subsets (k = 1), random per-request sub
 k = 1, and 64-endpoint subsets at k = 4.  The variants are alternated round by round, so clock or thermal drift hits
 them all alike; the median, min and max per variant are reported.  The card's name, power limit and SM clock are read
 in the same run.  After timing, each variant's picks of the first --check requests are compared bit for bit with the
-subset CPU oracle (tests/subset_oracle.cpp, built by `make`).
+CPU oracle's subset pick (tests/ext_oracle.cpp, built by `make`).
 
     python tools/bench_subset.py [--cfg 3] [--rounds 30] [--check 512]
 """
@@ -113,10 +113,10 @@ def main():
 
     checked = {}
     if args.check:
-        from tests.subset_oracle import SubsetOracle
+        from tests.ext_oracle import ExtOracle
 
         n = min(args.check, R)
-        cpu = SubsetOracle(cfg)
+        cpu = ExtOracle(cfg)
         cpu.update_endpoints(states)
         for ops in wl.index_ops():
             cpu.index_apply(ops)
