@@ -166,6 +166,7 @@ class fi_epp_stats(C.Structure):
         ("n_index_apply", C.c_uint64),
         ("n_other", C.c_uint64),
         ("probed_blocks", C.c_uint64),
+        ("hashed_blocks", C.c_uint64),
     ]
 
 

@@ -1178,15 +1178,29 @@ int lru_device_resize(fi_epp* h, const std::vector<uint32_t>& local, const std::
   return FI_OK;
 }
 
-// hash kernels for the request slice [r0, r0+R): prompts → chain (device buffers), on stream s
+// Whether a pick may hash each request only up to its first block the index does not hold (hash_kernels.cu "early
+// exit"): the pick reads nothing past that block, and here nothing else reads the chains either.  That needs a single
+// rank (a sharded pool gathers and merges over whole chains), hash_chain (block_bytes % 32 == 0), no chains_out, and
+// no LRU (lru_capacity == 0: no device-LRU Add can take the batch's chains from the handle's buffers; the index is fed
+// by fi_epp_index_apply alone).  Every other batch, and fi_epp_hash_batch, hashes whole chains.
+bool early_exit_hashing(const fi_epp* h, bool chains_wanted) {
+  return h->world == 1 && h->fast_hash && !chains_wanted && h->cfg.lru_capacity == 0;
+}
+
+// blocks hash_chain read the prompt bytes of, while profiling (slot 6 of d_probed; 0 is N_probe, 1-5 the
+// FI_MATCH_TIMING sums)
+unsigned long long* hashed_counter(fi_epp* h) { return h->profiling ? h->d_probed.get() + 6 : nullptr; }
+
+// hash kernels for the request slice [r0, r0+R): prompts → chain (device buffers), on stream s.  early: the index
+// view the batch's match reads, when early_exit_hashing allows it (s must already wait for ev_index), else null
 int run_hash(fi_epp* h, const uint8_t* d_prompts, const uint64_t* d_offsets, const uint64_t* d_h0, uint32_t r0,
-             uint32_t R, cudaStream_t s) {
+             uint32_t R, cudaStream_t s, const IndexView* early) {
   uint64_t* chain = h->d_chain.get() + (size_t)r0 * h->MP;
   uint32_t* nb = h->d_nblocks.get() + r0;
   LaunchScope ls(h, s, K_HASH);
   if (h->fast_hash) {  // block hashing and chain walk in one kernel, no pre-states in HBM
     FI_CUDA(launch_hash_chain(d_prompts, d_offsets + r0, d_h0 + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP,
-                              chain, nb, h->sm_count, s));
+                              chain, nb, h->sm_count, s, early, hashed_counter(h)));
   } else {
     FI_CUDA(launch_hash_generic(d_prompts, d_offsets + r0, d_h0 + r0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP,
                                 chain, nb, s));
@@ -1449,6 +1463,8 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
   if (rc != FI_OK) return rc;
   rc = claim_chain_slot0(h, h->s_main.get());
   if (rc != FI_OK) return rc;
+  // (s_main already waits for ev_index: the hashing reads the same index view as the match)
+  const IndexView* early = early_exit_hashing(h, c.chains_out || (feed && feed->chains_out)) ? &mp.ix : nullptr;
 
   const uint32_t S = h->feed_slices;
   if (feed && !sharded && h->fast_hash && S > 1 && R >= 64 * S && feed->offsets[R] >= (8ull << 20)) {
@@ -1467,7 +1483,7 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
     for (uint32_t k = 0; k < used; ++k) {
       const uint32_t r0 = k * per, Rk = std::min(per, R - r0);
       FI_CUDA(cudaStreamWaitEvent(h->s_main.get(), h->ev_copy[k].get(), 0));
-      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, Rk, h->s_main.get());
+      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, Rk, h->s_main.get(), early);
       if (rc != FI_OK) return rc;
       MatchParams ms = mp;
       ms.chain = mp.chain + (size_t)r0 * h->MP;
@@ -1493,7 +1509,7 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
     // (A sub-batch pipeline over several streams was tried and measured slower on device-resident
     // inputs — DESIGN.md "What did not work": the chain walk costs a flat serial latency at any batch
     // size and small slices pay launch/ramp overheads.)
-    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main.get());
+    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main.get(), early);
     if (rc != FI_OK) return rc;
     LaunchScope ls(h, h->s_main.get(), K_MATCH);
     FI_CUDA(launch_match_pick(mp, h->sm_count, h->s_main.get()));
@@ -1508,7 +1524,7 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
     const uint32_t per = (((R + h->world - 1) / h->world) + 31) & ~31u;  // ≤ chain_rows / world
     const uint32_t r0 = std::min(R, h->rank * per), r1 = std::min(R, r0 + per);
     if (r1 > r0) {
-      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, r1 - r0, h->s_main.get());
+      rc = run_hash(h, c.prompts, c.offsets, c.h0, r0, r1 - r0, h->s_main.get(), nullptr);
       if (rc != FI_OK) return rc;
     }
     rc = nccl_allgather(h, h->d_chain.get() + (size_t)h->rank * per * h->MP, h->d_chain.get(), (size_t)per * h->MP * sizeof(uint64_t));
@@ -1517,7 +1533,7 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
     if (rc != FI_OK) return rc;
     h->stats.n_other += 2;  // two collectives of the step (not kernels of this library)
   } else {
-    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main.get());
+    rc = run_hash(h, c.prompts, c.offsets, c.h0, 0, R, h->s_main.get(), nullptr);
     if (rc != FI_OK) return rc;
   }
   const bool p2p = h->px.enabled != 0;
@@ -1628,6 +1644,14 @@ int submit_pick(fi_epp* h, const PickCall& c, cudaStream_t us, uint64_t* ticket,
   FI_CUDA(cudaStreamWaitEvent(h->s_a.get(), h->ev_plain.get(), 0));
   rc = wait_slot_readers(h, slot, h->s_a.get());
   if (rc != FI_OK) return rc;
+  // stage B's parameters first: stage A's early exit reads the same index view (one per call: a rebuild swaps tables)
+  MatchParams mp;
+  rc = prepare_match(h, c, chain, nb, mp);
+  if (rc != FI_OK) return rc;
+  const bool early = early_exit_hashing(h, c.chains_out != nullptr);
+  // Early exit reads the index in stage A: every op submitted before this batch is applied first, as for its match.
+  // Updates submitted after it wait for ev_pick, which follows this batch's match and so its stage A.
+  if (early) FI_CUDA(cudaStreamWaitEvent(h->s_a.get(), h->ev_index.get(), 0));
   {
     // Block hashing and chain walk in one kernel (hash_kernels.cu hash_chain).  It does not wait for the previous
     // batch's match_pick: a full batch runs half-SM CTAs, and one starts on an SM as soon as two of match's three
@@ -1635,13 +1659,10 @@ int submit_pick(fi_epp* h, const PickCall& c, cudaStream_t us, uint64_t* ticket,
     // every SM for the whole step was measured slower: §7).
     LaunchScope ls(h, h->s_a.get(), K_HASH);
     FI_CUDA(launch_hash_chain(c.prompts, c.offsets, c.h0, R, h->cfg.block_bytes, h->cfg.max_blocks, h->MP, chain, nb,
-                              h->sm_count, h->s_a.get()));
+                              h->sm_count, h->s_a.get(), early ? &mp.ix : nullptr, hashed_counter(h)));
   }
   FI_CUDA(cudaEventRecord(h->ev_a[slot].get(), h->s_a.get()));
   // ---- stage B
-  MatchParams mp;
-  rc = prepare_match(h, c, chain, nb, mp);
-  if (rc != FI_OK) return rc;
   FI_CUDA(cudaStreamWaitEvent(h->s_main.get(), h->ev_a[slot].get(), 0));
   mp.work_counter = h->d_work.get() + 8 + slot;
   {
@@ -2396,7 +2417,7 @@ int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets
   rc = claim_chain_slot0(h, h->s_main.get());
   if (rc != FI_OK) return rc;
   h->last_plain_R = 0;  // d_chain no longer holds a pick batch's chains
-  rc = run_hash(h, h->d_prompts.get(), h->d_offsets.get(), h->d_h0.get(), 0, R, h->s_main.get());
+  rc = run_hash(h, h->d_prompts.get(), h->d_offsets.get(), h->d_h0.get(), 0, R, h->s_main.get(), nullptr);
   if (rc != FI_OK) return rc;
   rc = copy_chains_out(h, h->d_chain.get(), chains_out, R, cudaMemcpyDeviceToHost, h->s_main.get());
   if (rc != FI_OK) return rc;
@@ -2791,6 +2812,7 @@ int fi_epp_get_stats(fi_epp* h, fi_epp_stats* out) {
     unsigned long long pb[8] = {0};
     FI_CUDA(cudaMemcpy(pb, h->d_probed.get(), sizeof(pb), cudaMemcpyDeviceToHost));
     h->stats.probed_blocks = pb[0];
+    h->stats.hashed_blocks = pb[6];
     if (pb[5] && h->verbose)  // FI_MATCH_TIMING build: where a request's time goes inside match_pick
       std::fprintf(stderr, "[fi_epp] match_pick phases, cycles per request over %llu requests: stage %.0f, first lookup %.0f, "
                    "chunks %.0f, score+pick %.0f\n", pb[5], (double)pb[1] / pb[5], (double)pb[2] / pb[5], (double)pb[3] / pb[5],

@@ -13,6 +13,7 @@
 #include "kernels.cuh"
 #include "xxh64.cuh"
 #include "xxh64_sm100.cuh"
+#include "index_device.cuh"
 
 namespace fi {
 
@@ -130,21 +131,46 @@ __device__ __forceinline__ uint64_t pre_unaligned(const uint8_t* blk, uint32_t B
   return xacc2_finish(a, (uint64_t)B + 8);
 }
 
-template <int STRIPES, int WALK, int WARPS>
+// ---- early exit: hash a request only up to its first block no endpoint holds -----------------------------------
+// A pick reads a request's chain up to a, its first block that no endpoint holds (match_kernels.cu
+// resolve_request_nodes: both match modes stop there), plus chain[0] for the tie seed.  When nothing else reads the
+// chain (no chains_out, no device-LRU Add: the host decides, engine.cu early_exit_hashing) hash_chain runs with
+// MODE = kHashEarly, and one warp of the tile, the checker, looks up each request's latest stored hash in the index
+// (index_find, the presence test match_pick uses).  A miss at block i proves a <= i, and i's group is already hashed,
+// so the request stops after that group: hashers issue no prompt loads for its later groups and the walkers store
+// zeros there.  A hit proves nothing about the blocks before it (a hole), so the request simply goes on.
+// Contract: chain[r][0 .. min(n, a+1)) is the true chain, nblocks[r] = n, and every later entry is either true or 0.
+// A zero never verifies in the match (key_is_special), and entries past a cannot change its walk
+// (resolve_request_nodes returns at a whatever they hold), so the picks are those of the full chain.
+// The checker needs no run of consecutive nodes, so an index built out of chain order stops requests as early.
+enum : int { kHashFull = 0, kHashFullCounted = 1, kHashEarly = 2 };
+
+__device__ __forceinline__ uint32_t ld_volatile_shared(const uint32_t* p) { return *reinterpret_cast<const volatile uint32_t*>(p); }
+// a chain entry a walker warp of this CTA stored (ordered by the walker's fence before it counted the group and the
+// checker's after it read the count)
+__device__ __forceinline__ uint64_t ld_chain_cta(const uint64_t* p) {
+  uint64_t v;
+  asm volatile("ld.relaxed.cta.global.u64 %0, [%1];\n" : "=l"(v) : "l"(p) : "memory");
+  return v;
+}
+
+template <int STRIPES, int WALK, int WARPS, int MODE>
 __global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(const uint8_t* __restrict__ prompts,
                                                                    const uint64_t* __restrict__ offsets,
                                                                    const uint64_t* __restrict__ h0, uint32_t R,
                                                                    uint32_t M, uint32_t MP,
                                                                    uint64_t* __restrict__ chain,
                                                                    uint32_t* __restrict__ nblocks,
-                                                                   uint32_t block_bytes) {
+                                                                   uint32_t block_bytes, const IndexView ix,
+                                                                   unsigned long long* hashed) {
+  constexpr bool EARLY = MODE == kHashEarly;
   const uint32_t B = STRIPES ? STRIPES * 32 : block_bytes;
   // A hashing warp's job: 8 blocks of 4 * BPL requests, BPL blocks per lane (two blocks' loads in flight per
   // thread, one at 128-byte blocks and at run-time stripe counts, blocks of 96 bytes or more).  Lanes 8j .. 8j+7
   // read one request's 8 blocks: 512 contiguous bytes at 64-byte blocks.
   constexpr uint32_t BPL = STRIPES == 4 || STRIPES == 0 ? 1 : 2;
   constexpr uint32_t kFuseReq = 32 * WALK;  // requests per CTA
-  constexpr uint32_t kFuseHashWarps = WARPS - WALK;
+  constexpr uint32_t kFuseHashWarps = WARPS - WALK - (EARLY ? 1 : 0);  // (early exit: warp WALK is the checker)
   constexpr uint32_t kFuseRing = WARPS * kFuseRingBytesPerWarp / (WALK * 4 * 32 * 16);
   constexpr uint32_t kJobs = kFuseReq / (4 * BPL);  // jobs per group
   __shared__ __align__(16) ulonglong2 s_ring[kFuseRing][WALK][4][32];
@@ -152,6 +178,10 @@ __global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(cons
   __shared__ const uint8_t* s_base[kFuseReq];
   __shared__ uint32_t s_n[kFuseReq];
   __shared__ uint32_t s_groups;
+  // early exit: s_stop[q] = first group of request q not to hash (~0: none yet; written by the checker only, once);
+  // s_walked[w] = groups walker warp w has stored
+  // s_hashed = the tile's hashed blocks (profiling)
+  __shared__ uint32_t s_stop[EARLY ? kFuseReq : 1], s_walked[EARLY ? WALK : 1], s_hashed;
 
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t r_tile = blockIdx.x * kFuseReq;
@@ -161,6 +191,9 @@ __global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(cons
       mbar_init(&s_full[s], kJobs * 32);
       mbar_init(&s_empty[s], WALK * 32);
     }
+    if constexpr (EARLY)
+      for (uint32_t w = 0; w < WALK; ++w) s_walked[w] = 0;
+    if constexpr (MODE != kHashFull) s_hashed = 0;
   }
   __syncthreads();
   if (tid < kFuseReq) {
@@ -176,17 +209,78 @@ __global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(cons
     }
     s_n[tid] = n;
     s_base[tid] = base;
+    if constexpr (EARLY) s_stop[tid] = 0xFFFFFFFFu;
+    if constexpr (MODE == kHashFullCounted)
+      if (n) atomicAdd(&s_hashed, n);
     atomicMax(&s_groups, (n + 7) / 8);
   }
   __syncthreads();
   const uint32_t ng = s_groups;  // groups of the tile's longest request: every slot up to it is produced and consumed
+  if constexpr (MODE == kHashFullCounted)
+    if (tid == 0 && s_hashed) atomicAdd(hashed, (unsigned long long)s_hashed);
+
+  if constexpr (EARLY) {
+    if (warp == WALK) {
+      // ---------------- checker warp: lane l looks after requests l, l + 32, .. (one per walker warp).  Each round
+      // probes the last stored block of every live request's latest walked group, the lane's requests in flight
+      // together: one 8-byte read of the chain row, then the home bucket.  It checks the newest group rather than
+      // every group so that it never falls behind the walkers by more than a round.
+      uint32_t done_g[WALK];  // groups of the request already probed
+      bool live[WALK];
+#pragma unroll
+      for (int j = 0; j < WALK; ++j) {
+        done_g[j] = 0;
+        live[j] = r_tile + j * 32 + lane < R && s_n[j * 32 + lane] > 0;
+      }
+#pragma unroll 1
+      for (;;) {
+        uint32_t gw[WALK];  // groups walker warp j has stored
+        bool any = false, fresh = false;
+#pragma unroll
+        for (int j = 0; j < WALK; ++j) {
+          gw[j] = ld_volatile_shared(&s_walked[j]);
+          live[j] = live[j] && done_g[j] * 8 < s_n[j * 32 + lane];  // not yet stored in full
+          any = any || live[j];
+          fresh = fresh || (live[j] && gw[j] > done_g[j]);
+        }
+        if (!__any_sync(0xFFFFFFFFu, any)) break;
+        if (!__any_sync(0xFFFFFFFFu, fresh)) {
+          __nanosleep(64);
+          continue;
+        }
+        __threadfence_block();
+        uint64_t hk[WALK];
+#pragma unroll
+        for (int j = 0; j < WALK; ++j) {
+          const uint32_t q = j * 32 + lane;
+          hk[j] = 0;
+          if (live[j] && gw[j] > done_g[j]) {
+            const uint32_t i = min(gw[j] * 8, s_n[q]) - 1;  // last stored block
+            hk[j] = ld_chain_cta(chain + (uint64_t)(r_tile + q) * MP + i);
+          }
+        }
+#pragma unroll
+        for (int j = 0; j < WALK; ++j) {
+          const uint32_t q = j * 32 + lane;
+          if (live[j] && gw[j] > done_g[j]) {
+            if (index_find(ix, hk[j]) == SLOT_MISS) {  // a <= the probed block, whose group gw - 1 is hashed
+              *reinterpret_cast<volatile uint32_t*>(&s_stop[q]) = gw[j];
+              live[j] = false;
+            }
+            done_g[j] = gw[j];
+          }
+        }
+      }
+      return;
+    }
+  }
 
   if (warp >= WALK) {
     // ---------------- hashing warps
     const uint64_t pol = make_evict_first_policy();
     const uint32_t b = lane & 7;
 #pragma unroll 1
-    for (uint32_t t = warp - WALK; t < ng * kJobs; t += kFuseHashWarps) {
+    for (uint32_t t = warp - WALK - (EARLY ? 1 : 0); t < ng * kJobs; t += kFuseHashWarps) {
       const uint32_t g = t / kJobs, job = t % kJobs;
       const uint32_t i = g * 8 + b;  // block index within the row
       uint32_t q[BPL];
@@ -197,6 +291,7 @@ __global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(cons
       for (uint32_t k = 0; k < BPL; ++k) {
         q[k] = job * 4 * BPL + k * 4 + (lane >> 3);
         ok[k] = i < s_n[q[k]];
+        if constexpr (EARLY) ok[k] = ok[k] && g < ld_volatile_shared(&s_stop[q[k]]);
         src[k] = s_base[q[k]] + (uint64_t)i * B;
         al[k] = (reinterpret_cast<uintptr_t>(src[k]) & 15) == 0;
         mis = mis || (ok[k] && !al[k]);
@@ -228,6 +323,14 @@ __global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(cons
                                       v[k][2 * s + 1].y, v[k][2 * s + 1].z, v[k][2 * s + 1].w}});
             pre[k] = xacc2_finish(a, (uint64_t)B + 8);
           }
+      }
+      if constexpr (EARLY) {
+        if (hashed) {  // profiling: the job's hashed blocks (counted before the arrive: the walkers add them up)
+          uint32_t c = 0;
+#pragma unroll
+          for (uint32_t k = 0; k < BPL; ++k) c += __popc(__ballot_sync(0xFFFFFFFFu, ok[k]));
+          if (lane == 0) atomicAdd(&s_hashed, c);
+        }
       }
       const uint32_t slot = g % kFuseRing;
       if (g >= kFuseRing) mbar_wait(&s_empty[slot], ((g / kFuseRing) + 1) & 1);  // the walkers took use g/kFuseRing - 1
@@ -267,6 +370,22 @@ __global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(cons
     mbar_arrive(&s_empty[slot]);
   };
 
+  // early exit: the group's hashes are in the row; tell the checker (the fence orders every lane's stores before the
+  // count, __syncwarp the other lanes' before lane 0's fence)
+  auto publish = [&](uint32_t g) {
+    if constexpr (EARLY) {
+      __syncwarp();
+      if (lane == 0) {
+        __threadfence_block();
+        *reinterpret_cast<volatile uint32_t*>(&s_walked[warp]) = g + 1;
+      }
+    }
+  };
+  // early exit: false once the checker stopped this request before group g.  Read after take(g): every hasher of
+  // the group read s_stop before it arrived, so a stop they saw is seen here too and the ring's stale entries of a
+  // stopped request are never stored (a stop they missed only costs the group's hashing).
+  auto hashed_group = [&](uint32_t g) { return !EARLY || g < ld_volatile_shared(&s_stop[warp * 32 + lane]); };
+
   uint32_t g = 0;
 #pragma unroll 1
   for (; g < ng_full; ++g) {
@@ -278,9 +397,15 @@ __global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(cons
       h = chain_step(in[k].y, h);
       res[k].y = h;
     }
+    if constexpr (EARLY) {
+      if (!hashed_group(g))  // (h goes on over the ring's stale entries: it is never stored again)
+#pragma unroll
+        for (int k = 0; k < 4; ++k) res[k] = make_ulonglong2(0, 0);
+    }
     ulonglong2* o = out + g * 4;
 #pragma unroll
     for (int k = 0; k < 4; ++k) st_row16(o + k, res[k]);  // (ng_full > 0: every lane is valid)
+    publish(g);
   }
   // ragged groups up to the tile's longest request: some lane's chain ends inside, or has ended (zeros stored)
 #pragma unroll 1
@@ -288,23 +413,29 @@ __global__ void __launch_bounds__(WARPS * 32, 32 / WARPS) hash_chain_kernel(cons
     take(g);
     ulonglong2* o = out + g * 4;
     const uint32_t i0 = g * 8;
+    const bool hg = hashed_group(g);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       ulonglong2 v;
       uint64_t t = chain_step(in[k].x, h);
-      const bool v0 = i0 + 2 * k < n;
+      const bool v0 = i0 + 2 * k < n && hg;
       h = v0 ? t : h;
       v.x = v0 ? t : 0;
       t = chain_step(in[k].y, h);
-      const bool v1 = i0 + 2 * k + 1 < n;
+      const bool v1 = i0 + 2 * k + 1 < n && hg;
       h = v1 ? t : h;
       v.y = v1 ? t : 0;
       if (valid) st_row16(o + k, v);
     }
+    publish(g);
   }
   if (valid) {
     const ulonglong2 z = make_ulonglong2(0, 0);
     for (uint32_t u = g * 4; u < MP2; ++u) st_row16(out + u, z);
+  }
+  if constexpr (EARLY) {
+    // every job arrived on its full barrier after counting, and this warp has waited on all of them
+    if (hashed && warp == 0 && lane == 0 && s_hashed) atomicAdd(hashed, (unsigned long long)s_hashed);
   }
 }
 
@@ -335,32 +466,53 @@ __global__ void __launch_bounds__(128) hash_generic_kernel(const uint8_t* __rest
 }  // namespace
 
 // One tile shape: WALK = 1 or 2 on a whole SM, or the half-SM tile (16 warps, WALK = 2).
-template <int STRIPES>
+template <int STRIPES, int MODE>
 static void launch_hash_chain_tile(uint32_t walk, uint32_t warps, uint32_t grid, cudaStream_t s, const uint8_t* prompts,
                                    const uint64_t* offsets, const uint64_t* h0, uint32_t R, uint32_t B, uint32_t M,
-                                   uint32_t MP, uint64_t* chain, uint32_t* nblocks) {
+                                   uint32_t MP, uint64_t* chain, uint32_t* nblocks, const IndexView& ix,
+                                   unsigned long long* hashed) {
   if (warps == 16)
-    hash_chain_kernel<STRIPES, 2, 16><<<grid, 512, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B);
+    hash_chain_kernel<STRIPES, 2, 16, MODE><<<grid, 512, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B, ix, hashed);
   else if (walk == 2)
-    hash_chain_kernel<STRIPES, 2, 32><<<grid, 1024, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B);
+    hash_chain_kernel<STRIPES, 2, 32, MODE><<<grid, 1024, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B, ix, hashed);
   else
-    hash_chain_kernel<STRIPES, 1, 32><<<grid, 1024, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B);
+    hash_chain_kernel<STRIPES, 1, 32, MODE><<<grid, 1024, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B, ix, hashed);
+}
+
+// Early exit runs in half-SM tiles only.  A whole-SM tile's ring is 8 or 16 groups deep (64 or 128 blocks), so its
+// hashers run that far ahead of the walkers and the checker, and the warp the checker takes costs more than the
+// stops save: at cfg 2 (4 096 requests of 128 blocks, whole-SM tiles of 32) the stream-ordered step took 49.6-50.3 us
+// with early exit against 49.1-49.3 us without (one H100 80GB HBM3 at 700 W, three runs of each alternated).
+template <int STRIPES>
+static void launch_hash_chain_mode(uint32_t walk, uint32_t warps, uint32_t grid, cudaStream_t s, const uint8_t* prompts,
+                                   const uint64_t* offsets, const uint64_t* h0, uint32_t R, uint32_t B, uint32_t M,
+                                   uint32_t MP, uint64_t* chain, uint32_t* nblocks, const IndexView* early,
+                                   unsigned long long* hashed) {
+  if (early && warps == 16)
+    hash_chain_kernel<STRIPES, 2, 16, kHashEarly><<<grid, 512, 0, s>>>(prompts, offsets, h0, R, M, MP, chain, nblocks, B,
+                                                                        *early, hashed);
+  else if (hashed)
+    launch_hash_chain_tile<STRIPES, kHashFullCounted>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks,
+                                                      IndexView{}, hashed);
+  else
+    launch_hash_chain_tile<STRIPES, kHashFull>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks,
+                                               IndexView{}, nullptr);
 }
 
 cudaError_t launch_hash_chain_shape(uint32_t walk, uint32_t warps, const uint8_t* prompts, const uint64_t* offsets,
                                     const uint64_t* h0, uint32_t R, uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain,
-                                    uint32_t* nblocks, cudaStream_t s) {
+                                    uint32_t* nblocks, cudaStream_t s, const IndexView* early, unsigned long long* hashed) {
   if (R == 0) return cudaSuccess;
   if (!((warps == 32 && (walk == 1 || walk == 2)) || (warps == 16 && walk == 2))) return cudaErrorInvalidValue;
   const uint32_t grid = (R + 32 * walk - 1) / (32 * walk);
   if (B == 64)
-    launch_hash_chain_tile<2>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
+    launch_hash_chain_mode<2>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks, early, hashed);
   else if (B == 32)
-    launch_hash_chain_tile<1>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
+    launch_hash_chain_mode<1>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks, early, hashed);
   else if (B == 128)
-    launch_hash_chain_tile<4>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
+    launch_hash_chain_mode<4>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks, early, hashed);
   else if (B % 32 == 0)
-    launch_hash_chain_tile<0>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks);
+    launch_hash_chain_mode<0>(walk, warps, grid, s, prompts, offsets, h0, R, B, M, MP, chain, nblocks, early, hashed);
   else
     return cudaErrorInvalidValue;
   return cudaGetLastError();
@@ -368,11 +520,11 @@ cudaError_t launch_hash_chain_shape(uint32_t walk, uint32_t warps, const uint8_t
 
 cudaError_t launch_hash_chain(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
                               uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain, uint32_t* nblocks, int sm_count,
-                              cudaStream_t s) {
+                              cudaStream_t s, const IndexView* early, unsigned long long* hashed) {
   // the smallest whole-SM tile whose grid still fits one CTA per SM; half-SM tiles beyond that
   const uint32_t walk = (R + 31) / 32 > (uint32_t)sm_count ? 2 : 1;
   const uint32_t warps = (R + 63) / 64 > (uint32_t)sm_count ? 16 : 32;
-  return launch_hash_chain_shape(walk, warps, prompts, offsets, h0, R, B, M, MP, chain, nblocks, s);
+  return launch_hash_chain_shape(walk, warps, prompts, offsets, h0, R, B, M, MP, chain, nblocks, s, early, hashed);
 }
 
 cudaError_t launch_hash_generic(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,

@@ -188,13 +188,18 @@ struct MergeParams {
 // block hashing and chain walk in one kernel, for block_bytes % 32 == 0 (cudaErrorInvalidValue otherwise).
 // sm_count sets the tile: 32 or 64 requests per whole-SM CTA, the smallest whose grid fits one CTA per SM, and
 // half-SM CTAs of 64 requests for larger batches
+// early (optional): the index the batch's match reads; hash_chain may then leave a request's chain after its
+// first block that index does not hold unhashed (zeros; hash_kernels.cu "early exit").  hashed (optional): += the
+// blocks whose prompt bytes were read (profiling).
 cudaError_t launch_hash_chain(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
                               uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain, uint32_t* nblocks,
-                              int sm_count, cudaStream_t s);
+                              int sm_count, cudaStream_t s, const IndexView* early = nullptr,
+                              unsigned long long* hashed = nullptr);
 // the same with the tile shape given: walk = 1 or 2 with warps = 32 (whole SM), walk = 2 with warps = 16 (half SM)
 cudaError_t launch_hash_chain_shape(uint32_t walk, uint32_t warps, const uint8_t* prompts, const uint64_t* offsets,
                                     const uint64_t* h0, uint32_t R, uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain,
-                                    uint32_t* nblocks, cudaStream_t s);
+                                    uint32_t* nblocks, cudaStream_t s, const IndexView* early = nullptr,
+                                    unsigned long long* hashed = nullptr);
 cudaError_t launch_hash_generic(const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
                                 uint32_t R, uint32_t B, uint32_t M, uint32_t MP, uint64_t* chain,
                                 uint32_t* nblocks, cudaStream_t s);

@@ -218,6 +218,10 @@ typedef struct fi_epp_stats {
   double ms_hash_blocks, ms_chain_probe, ms_match_pick, ms_index_apply, ms_other;
   uint64_t n_hash_blocks, n_chain_probe, n_match_pick, n_index_apply, n_other;
   uint64_t probed_blocks; /* sum over requests of N_probe (SURVEY.md §8d), profiling only */
+  uint64_t hashed_blocks; /* blocks whose prompt bytes were read, summed over requests; profiling only, counted when
+                           * block_bytes % 32 == 0.  A pick without chains_out on a single-rank handle with
+                           * lru_capacity == 0 stops hashing each request after its first block the index does not
+                           * hold, so it reads fewer blocks than its requests' n_blocks */
 } fi_epp_stats;
 
 typedef struct fi_epp fi_epp;
