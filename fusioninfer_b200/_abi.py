@@ -216,6 +216,7 @@ SYMBOLS = [
     ("fi_epp_endpoints_lora_update", C.c_int, [_P, _P, C.c_uint32]),
     ("fi_epp_index_apply", C.c_int, [_P, _P, C.c_uint64]),
     ("fi_epp_index_remove_endpoints", C.c_int, [_P, _P, C.c_uint32, _P]),
+    ("fi_epp_resize_pool", C.c_int, [_P, C.c_uint32, _P]),
     ("fi_epp_set_lru_capacities", C.c_int, [_P, _P, _P, C.c_uint32, _P]),
     ("fi_epp_index_add_chain", C.c_int, [_P, C.c_uint32, _P, C.c_uint32]),
     ("fi_epp_index_add_chains", C.c_int, [_P, _P, _P, C.c_uint32, _P, C.c_uint32]),

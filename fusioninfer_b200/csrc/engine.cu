@@ -34,6 +34,7 @@
 #include "lru_batch.h"
 #include "lru_device.cuh"
 #include "lru_plan.h"
+#include "pool_shape.h"
 #include "xxh64.cuh"
 
 using namespace fi;
@@ -99,11 +100,6 @@ enum KernelKind { K_HASH = 0, K_MATCH = 1, K_INDEX = 2, K_OTHER = 3, K_KINDS = 4
 
 uint32_t pow2_ceil32(uint32_t v) {
   uint32_t p = 1;
-  while (p < v) p <<= 1;
-  return p;
-}
-uint64_t pow2_ceil64(uint64_t v) {
-  uint64_t p = 1;
   while (p < v) p <<= 1;
   return p;
 }
@@ -256,6 +252,7 @@ struct fi_epp {
 
   // index
   IndexTables ix;
+  uint64_t index_slots_given = 0;  // index_slots as passed to fi_epp_create (0: the default for the pool, pool_shape.h)
   std::unique_ptr<IndexTables> ix_spare;  // rebuild target, allocated at the first rebuild and reused alternately
   DevPtr<IndexCounters> d_ctr;
   PinnedPtr<IndexCounters> h_ctr;
@@ -438,13 +435,13 @@ int clear_index(fi_epp* h, IndexView& v) {
   return FI_OK;
 }
 
-// empty index tables of `slots` slots into `out`, which is left as it was on failure
-int alloc_index(fi_epp* h, uint64_t slots, IndexTables& out) {
+// empty index tables of `slots` slots and rows of W words into `out`, which is left as it was on failure
+int alloc_index(fi_epp* h, uint64_t slots, uint32_t W, IndexTables& out) {
   IndexTables t;
   IndexView& v = t.v;
   v.C = slots;
   v.bmask = slots / BUCKET_KEYS - 1;
-  v.W = h->W;
+  v.W = W;
   v.logW = 0;
   while ((1u << v.logW) < v.W) ++v.logW;
   const uint64_t total = slots + 3;  // + slots for hash 0, hash ~0, and a permanently-zero row
@@ -485,7 +482,7 @@ int alloc_index(fi_epp* h, uint64_t slots, IndexTables& out) {
 int rebuild_index(fi_epp* h) {
   if (!h->ix_spare) {
     auto spare = std::make_unique<IndexTables>();
-    int rc = alloc_index(h, h->ix.v.C, *spare);  // clears it too
+    int rc = alloc_index(h, h->ix.v.C, h->ix.v.W, *spare);  // clears it too
     if (rc != FI_OK) return rc;
     h->ix_spare = std::move(spare);
   } else {
@@ -720,12 +717,10 @@ int check_add_requests(fi_epp* h, const uint32_t* endpoints, const uint32_t* nbl
   return FI_OK;
 }
 
-// the device LRU's buffers, all or nothing: `s` is filled only as far as it got when a step fails
-int alloc_dev_lru(fi_epp* h, DevLruStore& s) {
+// The device LRU's table size TS and log size L, chosen at its first Add and kept for its life (fi_epp_resize_pool
+// keeps them too).
+int size_dev_lru(fi_epp* h, uint32_t* TS, uint32_t* L) {
   const uint32_t EL = h->cfg.endpoint_count, C = h->cfg.lru_capacity;
-  DevLru& d = s.v;
-  d.EL = EL;
-  d.capacity = C;
   size_t free_b = 0, total_b = 0;
   FI_CUDA(cudaMemGetInfo(&free_b, &total_b));
   // Log: at least 4 C records (a sub-batch appends at most C; more room = rarer compaction).  Table: at least 4 C slots (C entries + C new keys of a
@@ -733,17 +728,31 @@ int alloc_dev_lru(fi_epp* h, DevLruStore& s) {
   // endpoint that attracts a popular prefix can receive a large share of a batch — so the tables get as much as
   // a quarter of the free HBM buys, up to 32 C slots (1 Mi slots = 16 MiB per endpoint at lruCapacityPerServer
   // 31 250: 17 GB for 1 024 endpoints, a fifth of an H100's 80).  Option "lru_table_slots" / FI_EPP_LRU_TABLE_SLOTS pins it.
-  d.L = std::max<uint32_t>(pow2_ceil32(4u * C), 64u);
-  const uint32_t ts_min = d.L;
+  const uint32_t log_min = std::max<uint32_t>(pow2_ceil32(4u * C), 64u);
+  const uint32_t ts_min = log_min;
   uint32_t ts = pow2_ceil32(32u * C);
   while (ts > ts_min && (size_t)EL * (ts + 2) * sizeof(LruSlot) > free_b / 4) ts >>= 1;
   uint32_t want = h->lru_table_slots;
   if (!want)
     if (const char* ev = std::getenv("FI_EPP_LRU_TABLE_SLOTS")) want = (uint32_t)std::strtoul(ev, nullptr, 10);
   if (want) ts = std::max(ts_min, pow2_ceil32(want));
-  d.TS = ts;
-  d.L = std::max(d.L, d.TS / 4);
+  *TS = ts;
+  *L = std::max(log_min, ts / 4);
+  return FI_OK;
+}
+
+// the device LRU's buffers for EL local endpoints, tables of TS slots and logs of L records, all or nothing: `s` is
+// filled only as far as it got when a step fails.  Every LRU starts empty, endpoint e with capacity caps[e] (a
+// pageable host array: taken when the call returns).
+int alloc_dev_lru(fi_epp* h, DevLruStore& s, uint32_t EL, uint32_t TS, uint32_t L, const uint32_t* caps) {
+  DevLru& d = s.v;
+  d.EL = EL;
+  d.capacity = h->cfg.lru_capacity;
+  d.TS = TS;
+  d.L = L;
   d.insert_limit = (uint32_t)((uint64_t)d.TS * 85 / 100);
+  size_t free_b = 0, total_b = 0;
+  FI_CUDA(cudaMemGetInfo(&free_b, &total_b));
   const size_t slots = (size_t)EL * (d.TS + 2), log_records = (size_t)EL * d.L;
   s.touch_cap = std::max<uint64_t>((uint64_t)h->cfg.max_batch * h->MP, 1u << 16);
   const size_t scratch = (size_t)s.touch_cap * (sizeof(uint32_t) + 3 * sizeof(fi_index_op));
@@ -779,9 +788,7 @@ int alloc_dev_lru(fi_epp* h, DevLruStore& s) {
   d.any_ovf = d.ovf + EL;
   d.error = d.any_ovf + 1;
   d.cap = d.error + 1;
-  // the capacities set so far (possibly before this first Add); pageable source: taken when the call returns
-  if (h->lru_caps.size() != EL) h->lru_caps.assign(EL, C);
-  FI_CUDA(cudaMemcpyAsync(d.cap, h->lru_caps.data(), (size_t)EL * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
+  FI_CUDA(cudaMemcpyAsync(d.cap, caps, (size_t)EL * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
   d.n_sets = s.ctr.get();
   d.n_maintained = s.ctr.get() + 1;
   d.n_clears = s.ctr.get() + 3;
@@ -793,8 +800,14 @@ int alloc_dev_lru(fi_epp* h, DevLruStore& s) {
 // succeed, e.g. with the host LRU freed)
 int ensure_dev_lru(fi_epp* h) {
   if (h->dlru) return FI_OK;
+  const uint32_t EL = h->cfg.endpoint_count;
+  uint32_t TS = 0, L = 0;
+  int rc = size_dev_lru(h, &TS, &L);
+  if (rc != FI_OK) return rc;
+  // the capacities set so far (possibly before this first Add)
+  if (h->lru_caps.size() != EL) h->lru_caps.assign(EL, h->cfg.lru_capacity);
   auto s = std::make_unique<DevLruStore>();
-  const int rc = alloc_dev_lru(h, *s);
+  rc = alloc_dev_lru(h, *s, EL, TS, L, h->lru_caps.data());
   if (rc != FI_OK) {
     cudaGetLastError();
     return rc;
@@ -1683,6 +1696,55 @@ int submit_pick(fi_epp* h, const PickCall& c, cudaStream_t us, uint64_t* ticket,
   return FI_OK;
 }
 
+// Upstream indexer.RemovePod for the distinct local endpoints `local` (fi_epp_index_remove_endpoints, and the endpoints
+// a shrink of fi_epp_resize_pool drops): one sweep over the index rows clears their bits whatever put them there (LRU
+// Adds or direct SETs), keys nobody holds any more are retired (tombstones, like a CLEAR), and the endpoints' LRUs
+// start empty.  Ordered like fi_epp_index_apply: behind the ops staged so far and the picks called so far, ahead of
+// every later pick.  pairs_removed != null: wait for the sweep and write how many pairs left the index.
+int remove_local_endpoints(fi_epp* h, const std::vector<uint32_t>& local, uint64_t* pairs_removed) {
+  RemoveSet rs{};
+  for (uint32_t e : local) rs.row[e >> 5] |= 1u << (e & 31);
+  for (uint32_t w = 0; w < h->W; ++w)
+    if (rs.row[w]) {
+      rs.word[rs.m] = w;
+      rs.bits[rs.m] = rs.row[w];
+      ++rs.m;
+    }
+  int rc = flush_ops(h);  // staged SET / CLEAR groups and host-LRU deltas go first
+  if (rc != FI_OK) return rc;
+  rc = check_counters(h);
+  if (rc != FI_OK) return rc;
+  if (!h->d_rm) FI_CUDA(cuda_alloc(h->d_rm, 1 + ((size_t)h->cfg.endpoint_count + 1) / 2));
+  uint32_t* d_eps = reinterpret_cast<uint32_t*>(h->d_rm.get() + 1);
+  // picks called before this one must not see the removal
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
+  FI_CUDA(cudaMemsetAsync(h->d_rm.get(), 0, sizeof(unsigned long long), h->s_index.get()));
+  {
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_index_remove_sweep(h->ix.v, h->d_ctr.get(), rs, remove_whole_rows(rs, h->W), h->rank, h->d_rm.get(), h->sm_count, h->s_index.get()));
+  }
+  if (h->lru_mode == 1 && h->dlru) {
+    // (pageable source: the copy has taken the data when cudaMemcpyAsync returns)
+    FI_CUDA(cudaMemcpyAsync(d_eps, local.data(), local.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
+    h->stats.h2d_bytes += local.size() * sizeof(uint32_t);
+    LaunchScope ls(h, h->s_index.get(), K_INDEX);
+    FI_CUDA(launch_lru_reset(h->dlru->v, d_eps, (uint32_t)local.size(), h->s_index.get()));
+  }
+  for (uint32_t e : local)
+    if (e < h->lrus.size()) h->lrus[e].clear();
+  // the sweep's tombstones reach the rebuild decision of the next index update
+  rc = read_counters(h);
+  if (rc != FI_OK) return rc;
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
+  if (pairs_removed) {
+    unsigned long long c = 0;
+    FI_CUDA(cudaMemcpyAsync(&c, h->d_rm.get(), sizeof(c), cudaMemcpyDeviceToHost, h->s_index.get()));
+    FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
+    *pairs_removed = c;
+  }
+  return FI_OK;
+}
+
 int validate_config(const fi_epp_config& c, std::string* err) {
   auto bad = [&](const char* m) {
     *err = m;
@@ -1840,19 +1902,14 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
   h->sm_count = prop.multiProcessorCount;
   h->P = cfg->n_profiles;
   h->MP = (cfg->max_blocks + 7) & ~7u;  // whole groups of 8 links for the chain walker
-  h->W = pow2_ceil32((cfg->endpoint_count + 31) / 32);
+  h->W = pool_row_words(cfg->endpoint_count);
   h->fast_hash = (cfg->block_bytes % 32) == 0;
   if (const char* e = std::getenv("FI_EPP_TRACE")) h->trace_call = std::strtol(e, nullptr, 10);
   h->verbose = std::getenv("FI_EPP_VERBOSE") != nullptr;
   if (h->cfg.max_prompt_bytes == 0)
     h->cfg.max_prompt_bytes = (uint64_t)cfg->max_batch * cfg->block_bytes * cfg->max_blocks;
-  if (h->cfg.index_slots == 0) {
-    // load <= 0.5; an endpoint-range shard is a directory of the WHOLE pool's keys (rows for its own endpoints)
-    uint64_t want = 2ull * cfg->num_endpoints * (cfg->lru_capacity ? cfg->lru_capacity : 1024);
-    if (want < 4096) want = 4096;
-    h->cfg.index_slots = pow2_ceil64(want);
-    if (h->cfg.index_slots > 0x80000000ull) h->cfg.index_slots = 0x80000000ull;
-  }
+  h->index_slots_given = cfg->index_slots;
+  if (h->cfg.index_slots == 0) h->cfg.index_slots = pool_default_slots(cfg->num_endpoints, cfg->lru_capacity);
 
   for (Stream* s : {&h->s_main, &h->s_index, &h->s_copy, &h->s_a}) FI_TRY(cuda_create(*s));
   for (Event* e : {&h->ev_in, &h->ev_a[0], &h->ev_a[1], &h->ev_b[0], &h->ev_b[1], &h->ev_pick, &h->ev_plain,
@@ -1894,7 +1951,7 @@ int fi_epp_create(const fi_epp_config* cfg, fi_epp** out) {
   FI_TRY(cuda_alloc(h->h_ctr, 1));
   std::memset(h->h_ctr.get(), 0, sizeof(IndexCounters));
   {
-    int rc = alloc_index(h, h->cfg.index_slots, h->ix);
+    int rc = alloc_index(h, h->cfg.index_slots, h->W, h->ix);
     if (rc != FI_OK) return die(rc);
   }
   for (int b = 0; b < 2; ++b) {
@@ -2022,10 +2079,6 @@ int fi_epp_index_apply(fi_epp* h, const fi_index_op* ops, uint64_t n) {
   });
 }
 
-// Upstream indexer.RemovePod for a list of endpoints: one sweep over the index rows clears their bits whatever put
-// them there (LRU Adds or direct SETs), keys nobody holds any more are retired (tombstones, like a CLEAR), and the
-// endpoints' LRUs start empty.  Ordered like fi_epp_index_apply: behind the ops staged so far and the picks called
-// so far, ahead of every later pick.
 int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t n, uint64_t* pairs_removed) {
   if (!h || (!endpoints && n)) return FI_ERR_INVALID;
   std::lock_guard<std::mutex> lk(h->mu);
@@ -2035,53 +2088,158 @@ int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t
     if (endpoints[i] >= h->cfg.num_endpoints) return fail(h, FI_ERR_INVALID, "endpoint out of range");
   if (h->world > 1) return fail(h, FI_ERR_STATE, "sharded pool: fi_epp_index_remove_endpoints needs a single-rank handle");
   const uint32_t lo = h->cfg.endpoint_begin, EL = h->cfg.endpoint_count;
-  RemoveSet rs{};
-  std::vector<uint32_t> local;  // distinct local endpoints, for the device LRU
+  std::vector<uint32_t> local;  // distinct local endpoints
+  std::vector<uint8_t> listed(EL, 0);
   for (uint32_t i = 0; i < n; ++i) {
     const uint32_t e = endpoints[i] - lo;
-    if (e >= EL || (rs.row[e >> 5] >> (e & 31)) & 1u) continue;
-    rs.row[e >> 5] |= 1u << (e & 31);
+    if (e >= EL || listed[e]) continue;
+    listed[e] = 1;
     local.push_back(e);
   }
   if (local.empty()) return FI_OK;
-  for (uint32_t w = 0; w < h->W; ++w)
-    if (rs.row[w]) {
-      rs.word[rs.m] = w;
-      rs.bits[rs.m] = rs.row[w];
-      ++rs.m;
-    }
-  int rc = flush_ops(h);  // staged SET / CLEAR groups and host-LRU deltas go first
+  return remove_local_endpoints(h, local, pairs_removed);
+}
+
+// Resize the pool of a single-rank handle over the whole pool (docs/SPEC.md S.2c).  Blocking: every call before it
+// completes against the old pool first.  Every buffer the new pool needs is allocated before anything of the handle
+// changes, so FI_ERR_NOMEM leaves the handle as it was; after the allocations only a CUDA error can fail the call.  The
+// old and new copies of what is reallocated are both held until the end.
+int fi_epp_resize_pool(fi_epp* h, uint32_t num_endpoints, uint64_t* pairs_removed) {
+  if (!h) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  if (pairs_removed) *pairs_removed = 0;
+  const uint32_t E = h->cfg.num_endpoints, En = num_endpoints, C = h->cfg.lru_capacity;
+  if (En == 0 || En > 4096) return fail(h, FI_ERR_INVALID, "num_endpoints must be in 1 .. 4096");
+  if (h->world > 1) return fail(h, FI_ERR_STATE, "sharded pool: fi_epp_resize_pool needs a single-rank handle");
+  if (h->cfg.endpoint_begin != 0 || h->cfg.endpoint_count != E)
+    return fail(h, FI_ERR_STATE, "fi_epp_resize_pool needs a handle over the whole pool");
+  if (h->lru_mode == 0) return fail(h, FI_ERR_STATE, "fi_epp_resize_pool: the host LRU serves the handle");
+  if (En == E) return FI_OK;
+  int rc = flush_ops(h);
   if (rc != FI_OK) return rc;
   rc = check_counters(h);
   if (rc != FI_OK) return rc;
-  if (!h->d_rm) FI_CUDA(cuda_alloc(h->d_rm, 1 + ((size_t)EL + 1) / 2));
-  uint32_t* d_eps = reinterpret_cast<uint32_t*>(h->d_rm.get() + 1);
-  // picks called before this one must not see the removal
-  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
-  FI_CUDA(cudaMemsetAsync(h->d_rm.get(), 0, sizeof(unsigned long long), h->s_index.get()));
-  {
-    LaunchScope ls(h, h->s_index.get(), K_INDEX);
-    FI_CUDA(launch_index_remove_sweep(h->ix.v, h->d_ctr.get(), rs, remove_whole_rows(rs, h->W), h->rank, h->d_rm.get(), h->sm_count, h->s_index.get()));
+  for (cudaStream_t s : {h->s_main.get(), h->s_index.get(), h->s_copy.get(), h->s_a.get()}) FI_CUDA(cudaStreamSynchronize(s));
+  // The slot floor counts the live keys before a shrink's removal: an upper bound of those after it, known before
+  // anything changes.
+  IndexCounters ctr;
+  FI_CUDA(cudaMemcpy(&ctr, h->d_ctr.get(), sizeof(ctr), cudaMemcpyDeviceToHost));
+  const uint32_t Wn = pool_row_words(En), Epad = Wn * 32, keep = std::min(E, En);
+  const uint64_t slots = pool_resized_slots(h->index_slots_given, En, C, ctr.used - ctr.tombstones);
+  const bool rebuild = pool_needs_rebuild(h->W, h->ix.v.C, Wn, slots);
+
+  // ---- allocations: nothing of the handle changes before all of them are in place
+  IndexTables nix;
+  if (rebuild) {
+    rc = alloc_index(h, slots, Wn, nix);
+    if (rc != FI_OK) return rc;
   }
-  if (h->lru_mode == 1 && h->dlru) {
-    // (pageable source: the copy has taken the data when cudaMemcpyAsync returns)
-    FI_CUDA(cudaMemcpyAsync(d_eps, local.data(), local.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
-    h->stats.h2d_bytes += local.size() * sizeof(uint32_t);
-    LaunchScope ls(h, h->s_index.get(), K_INDEX);
-    FI_CUDA(launch_lru_reset(h->dlru->v, d_eps, (uint32_t)local.size(), h->s_index.get()));
+  std::vector<uint32_t> caps;  // the new pool's LRU capacities: the kept endpoints', then lru_capacity
+  if (C) {
+    caps.assign(h->lru_caps.begin(), h->lru_caps.begin() + keep);
+    caps.resize(En, C);
   }
-  for (uint32_t e : local)
-    if (e < h->lrus.size()) h->lrus[e].clear();
-  // the sweep's tombstones reach the rebuild decision of the next index update
+  std::unique_ptr<DevLruStore> nlru;
+  if (h->dlru) {
+    nlru = std::make_unique<DevLruStore>();
+    rc = alloc_dev_lru(h, *nlru, En, h->dlru->v.TS, h->dlru->v.L, caps.data());
+    if (rc != FI_OK) {
+      cudaGetLastError();
+      return rc;
+    }
+  }
+  DevPtr<EndpointDev> d_eps;
+  DevPtr<double> d_sc;
+  DevPtr<uint32_t> d_elig, d_ztie;
+  DevPtr<LoraDev> d_lora;
+  const size_t n_sc = (size_t)FI_EPP_MAX_PROFILES * FI_EPP_MAX_SCORERS * Epad, n_bits = (size_t)FI_EPP_MAX_PROFILES * Wn;
+  cudaError_t e = cuda_alloc(d_eps, En);
+  if (e == cudaSuccess) e = cuda_alloc(d_sc, n_sc);
+  if (e == cudaSuccess) e = cuda_alloc(d_elig, n_bits);
+  if (e == cudaSuccess) e = cuda_alloc(d_ztie, n_bits);
+  if (e == cudaSuccess) e = cuda_alloc(d_lora, Epad);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(h, e == cudaErrorMemoryAllocation ? FI_ERR_NOMEM : FI_ERR_CUDA, std::string("endpoint tables: ") + cudaGetErrorString(e));
+  }
+  cudaStream_t si = h->s_index.get();
+  FI_CUDA(cudaMemsetAsync(d_sc.get(), 0, n_sc * sizeof(double), si));
+  FI_CUDA(cudaMemsetAsync(d_elig.get(), 0, n_bits * sizeof(uint32_t), si));
+  FI_CUDA(cudaMemsetAsync(d_ztie.get(), 0, n_bits * sizeof(uint32_t), si));
+
+  // ---- the dropped endpoints leave the index and their LRUs, exactly as fi_epp_index_remove_endpoints removes them
+  if (En < E) {
+    std::vector<uint32_t> gone;
+    for (uint32_t x = En; x < E; ++x) gone.push_back(x);
+    rc = remove_local_endpoints(h, gone, pairs_removed);
+    if (rc != FI_OK) return rc;
+  }
+  // ---- the index in its new shape: rebuilt only when the row width or the slot count changes
+  if (rebuild) {
+    FI_CUDA(cudaMemsetAsync(h->d_ctr.get(), 0, sizeof(IndexCounters), si));
+    LaunchScope ls(h, si, K_INDEX);
+    FI_CUDA(launch_index_rebuild(h->ix.v, nix.v, h->d_ctr.get(), si));
+  }
+  // ---- the device LRU: its regions are endpoint-major, so the kept endpoints move with one prefix copy per array;
+  // the new ones start empty (alloc_dev_lru), and the totals carry over
+  if (nlru) {
+    const DevLru& o = h->dlru->v;
+    const DevLru& n = nlru->v;
+    FI_CUDA(cudaMemcpyAsync(n.slots, o.slots, (size_t)keep * (o.TS + 2) * sizeof(LruSlot), cudaMemcpyDeviceToDevice, si));
+    FI_CUDA(cudaMemcpyAsync(n.log, o.log, (size_t)keep * o.L * sizeof(uint64_t), cudaMemcpyDeviceToDevice, si));
+    const std::pair<uint32_t*, const uint32_t*> arrays[] = {{n.head, o.head}, {n.tail, o.tail},   {n.count, o.count}, {n.used, o.used},
+                                                            {n.hold, o.hold}, {n.dcount, o.dcount}, {n.ovf, o.ovf}};
+    for (const auto& a : arrays) FI_CUDA(cudaMemcpyAsync(a.first, a.second, (size_t)keep * sizeof(uint32_t), cudaMemcpyDeviceToDevice, si));
+    FI_CUDA(cudaMemcpyAsync(n.any_ovf, o.any_ovf, 2 * sizeof(uint32_t), cudaMemcpyDeviceToDevice, si));  // any_ovf, error
+    FI_CUDA(cudaMemcpyAsync(nlru->ctr.get(), h->dlru->ctr.get(), 8 * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, si));
+    *nlru->stat = *h->dlru->stat;
+    FI_CUDA(cudaEventRecord(nlru->ev.get(), si));
+  }
+
+  // ---- swap in the new pool (the old buffers stay allocated until the work above is done)
+  if (rebuild) {
+    std::swap(h->ix, nix);
+    h->ix_spare.reset();  // a later rebuild allocates it in the new shape
+  }
+  if (nlru) std::swap(h->dlru, nlru);
+  h->eps.resize(keep);
+  h->eps.resize(En, EndpointDev{0.0, 0, 0, 0, 0});
+  h->lora.resize(keep);
+  h->lora.resize(Epad, LoraDev{});
+  std::swap(h->d_eps, d_eps);
+  std::swap(h->d_sc, d_sc);
+  std::swap(h->d_elig, d_elig);
+  std::swap(h->d_ztie, d_ztie);
+  std::swap(h->d_lora, d_lora);
+  h->st.Epad = Epad;
+  h->st.sc = h->d_sc.get();
+  h->st.elig = h->d_elig.get();
+  h->st.ztie = h->d_ztie.get();
+  h->st.lora = h->d_lora.get();
+  h->eps_dirty = h->lora_dirty = true;
+  if (C) {
+    // no Add has run through the host LRUs (lru_mode != 0): they are empty and only carry the capacities
+    h->lrus.clear();
+    LruArena* arena = h->lru_arena.reserve((size_t)En * LruSet::bytes_needed(C)) ? &h->lru_arena : nullptr;
+    h->lrus = std::vector<LruSet>(En, LruSet(C, arena));
+    for (uint32_t x = 0; x < En; ++x)
+      if (caps[x] != C) h->lrus[x].shrink(caps[x], [](uint64_t) {});
+    h->lru_caps.swap(caps);
+  }
+  // lazily created buffers sized by the pool: their next use allocates them anew
+  h->d_rm.reset();
+  h->subsets = Staging<uint32_t>{};
+  h->lru_plan_buf = Staging<uint32_t>{};
+  h->lru_resize = Staging<uint32_t>{};
+  for (fi_epp::PipeAdd& pa : h->padd) pa.plan = Staging<uint32_t>{};
+  h->cfg.num_endpoints = h->cfg.endpoint_count = En;
+  h->cfg.index_slots = h->ix.v.C;
+  h->W = Wn;
   rc = read_counters(h);
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
-  if (pairs_removed) {
-    unsigned long long c = 0;
-    FI_CUDA(cudaMemcpyAsync(&c, h->d_rm.get(), sizeof(c), cudaMemcpyDeviceToHost, h->s_index.get()));
-    FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
-    *pairs_removed = c;
-  }
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), si));
+  FI_CUDA(cudaStreamSynchronize(si));
   return FI_OK;
 }
 

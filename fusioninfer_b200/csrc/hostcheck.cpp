@@ -13,6 +13,7 @@
 #include "lru.h"
 #include "lru_batch.h"
 #include "lru_plan.h"
+#include "pool_shape.h"
 #include "tiebreak.cuh"
 #include "xxh64.cuh"
 
@@ -456,6 +457,18 @@ int fihc_lru_bound_check(uint32_t E, uint32_t cap, uint32_t TS, const uint32_t* 
   if (max_pct) *max_pct = 100.0 * (double)peak / TS;
   if (subs) *subs = (uint32_t)nsubs;
   return 0;
+}
+
+// the index shape of a pool (pool_shape.h), as fi_epp_create and fi_epp_resize_pool derive it
+uint32_t fihc_pool_row_words(uint32_t endpoint_count) { return fi::pool_row_words(endpoint_count); }
+uint64_t fihc_pool_default_slots(uint32_t num_endpoints, uint32_t lru_capacity) {
+  return fi::pool_default_slots(num_endpoints, lru_capacity);
+}
+uint64_t fihc_pool_resized_slots(uint64_t pinned, uint32_t num_endpoints, uint32_t lru_capacity, uint64_t live_keys) {
+  return fi::pool_resized_slots(pinned, num_endpoints, lru_capacity, live_keys);
+}
+int fihc_pool_needs_rebuild(uint32_t W, uint64_t slots, uint32_t new_W, uint64_t new_slots) {
+  return fi::pool_needs_rebuild(W, slots, new_W, new_slots) ? 1 : 0;
 }
 
 }  // extern "C"

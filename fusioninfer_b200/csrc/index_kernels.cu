@@ -237,8 +237,12 @@ __global__ void __launch_bounds__(256) index_clear_kernel(IndexView ix, IndexCou
 }
 
 // Re-insert every live node of `from` into the (fresh) index `to`, in node order, so that runs of
-// consecutive nodes stay consecutive (each CTA pass compacts 256 consecutive old nodes into one range).
+// consecutive nodes stay consecutive (each CTA pass compacts 256 consecutive old nodes into one range).  The two
+// tables may differ in slots and row width (fi_epp_resize_pool): a row copies min(from.W, to.W) words — a wider
+// target's extra words are zero from alloc_index, and a narrower one drops only words the removal sweep of the
+// dropped endpoints has already cleared.
 __global__ void __launch_bounds__(256) index_rebuild_kernel(IndexView from, IndexView to, IndexCounters* ctr) {
+  const uint32_t W = from.W < to.W ? from.W : to.W;
   for (uint64_t base = blockIdx.x * (uint64_t)blockDim.x; base < from.C; base += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t s = base + threadIdx.x;
     uint64_t h = 0;
@@ -254,16 +258,16 @@ __global__ void __launch_bounds__(256) index_rebuild_kernel(IndexView from, Inde
       to.rmask[d] = from.rmask[s];
       const uint32_t* src = from.rows + (s << from.logW);
       uint32_t* dst = to.rows + (d << to.logW);
-      for (uint32_t w = 0; w < from.W; ++w) dst[w] = src[w];
+      for (uint32_t w = 0; w < W; ++w) dst[w] = src[w];
     }
   }
-  // the two special nodes keep their place
+  // the two special nodes keep their place: the first two past the regular slots
   if (blockIdx.x == 0 && threadIdx.x < 2) {
-    const uint64_t s = from.C + threadIdx.x;
+    const uint64_t s = from.C + threadIdx.x, d = to.C + threadIdx.x;
     if (from.rmask[s]) {
-      to.cnt[s] = from.cnt[s];
-      to.rmask[s] = from.rmask[s];
-      for (uint32_t w = 0; w < from.W; ++w) to.rows[(s << to.logW) + w] = from.rows[(s << from.logW) + w];
+      to.cnt[d] = from.cnt[s];
+      to.rmask[d] = from.rmask[s];
+      for (uint32_t w = 0; w < W; ++w) to.rows[(d << to.logW) + w] = from.rows[(s << from.logW) + w];
     }
   }
 }

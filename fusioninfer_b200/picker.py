@@ -203,6 +203,19 @@ class EndpointPicker:
                     "fi_epp_index_remove_endpoints")
         return out.value if count else None
 
+    def resize_pool(self, num_endpoints: int, count: bool = False) -> Optional[int]:
+        """Grow or shrink the pool to num_endpoints endpoints, keeping the prefixes the kept endpoints [0, min(old,
+        new)) have cached: a shrink drops the tail endpoints as remove_endpoints would, a grow appends endpoints that
+        are not alive and hold nothing yet.  Blocks until every earlier call is done against the old pool.
+        count=True returns how many (endpoint, hash) pairs a shrink removed."""
+        out = C.c_uint64(0)
+        self._check(self._lib.fi_epp_resize_pool(self._h, int(num_endpoints), C.byref(out) if count else None),
+                    "fi_epp_resize_pool")
+        # a copy: the caller's config (which created the handle) stays as it was
+        self.cfg = abi.fi_epp_config.from_buffer_copy(self.cfg)
+        self.cfg.num_endpoints = self.cfg.endpoint_count = int(num_endpoints)
+        return out.value if count else None
+
     def set_lru_capacities(self, endpoints, capacities, want_evicted: bool = False) -> Optional[int]:
         """Per-endpoint LRU capacities (upstream autoTune: a pod's LRU sized from its KV-cache block count).
         capacities[i] is endpoints[i]'s new capacity, 0 meaning lru_capacity; an LRU above its new capacity evicts its

@@ -287,6 +287,28 @@ int fi_epp_index_apply(fi_epp* h, const fi_index_op* ops, uint64_t n);
  * applied); FI_ERR_STATE on a sharded pool. */
 int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t n, uint64_t* pairs_removed);
 
+/* Resize the pool of a single-rank handle over the whole pool to num_endpoints endpoints (docs/SPEC.md S.2c), keeping
+ * what the kept endpoints [0, min(E, num_endpoints)) have cached.  Afterwards the handle behaves exactly like one
+ * created with num_endpoints = endpoint_count = num_endpoints and everything else the same, fed the same calls, except
+ * that everything ever addressed to an endpoint a shrink dropped is left out of that history, and that index_slots
+ * stays as given at create (0: the default, now computed for the new pool, but never below what the live keys need).
+ *   Shrink: endpoints [num_endpoints, E) leave the pool; their pairs leave the index as fi_epp_index_remove_endpoints
+ *   removes them, and their state, adapters, LRUs and LRU capacities are forgotten.  pairs_removed != NULL receives
+ *   how many (endpoint, hash) pairs left.
+ *   Grow: endpoints [E, num_endpoints) are new: not alive, no adapters, max_active 0, an empty LRU of capacity
+ *   lru_capacity.  An endpoint a shrink dropped comes back this way.
+ *   The kept endpoints keep their index pairs, LRU contents and recency order, capacities, states and adapters.  The
+ *   tie rotation, the subset row width (ceil(num_endpoints / 32) words), every endpoint range check and the queue
+ *   scorer's min / max follow the new pool from the next call on.  num_endpoints == E is a no-op.
+ * Blocking: every call issued before it completes on the device against the old pool (fi_epp_pick_submit batches in
+ * flight and staged index ops included), every later call sees the new pool.  Tickets stay valid; the chains a ticket
+ * holds are not released, and fi_epp_index_add_submitted checks the ticket's endpoints against the new pool.  Errors
+ * change nothing: FI_ERR_INVALID if num_endpoints is 0 or above 4096; FI_ERR_STATE on a sharded pool, on a handle over
+ * part of the pool, or on a handle the host LRU already serves (before the first Add both LRUs stay ready for the
+ * new pool); FI_ERR_NOMEM if the new tables do not fit (everything is allocated before anything changes, so the old
+ * and the new tables are both held while the call runs). */
+int fi_epp_resize_pool(fi_epp* h, uint32_t num_endpoints, uint64_t* pairs_removed);
+
 /* Per-endpoint LRU capacities (docs/SPEC.md S.2b; upstream's autoTune sizes a pod's LRU from the KV-cache blocks the
  * pod reports).  Every endpoint's LRU capacity starts at lru_capacity; this sets it to capacities[i] for endpoints[i]
  * (0 = lru_capacity; the last entry of an endpoint listed twice wins).  An LRU that holds more keys than its new
