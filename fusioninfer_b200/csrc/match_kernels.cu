@@ -33,6 +33,9 @@
 // the rank's (score, endpoint) pick, stored straight into every rank's memory (PeerXchg) and reduced by
 // merge_picks_kernel.
 #include <climits>
+#include <map>
+#include <mutex>
+#include <utility>
 
 #include "bitslice.cuh"
 #include "index_device.cuh"
@@ -900,34 +903,43 @@ __global__ void __launch_bounds__(1024) prepare_endpoints_kernel(const EndpointD
   }
 }
 
+// Handles on one device share the match variants, and different handles may launch from different threads at once
+// (each handle's mutex covers only itself), so the variants' launch state is process-wide, under this one mutex.
+std::mutex g_match_launch_mu;
+
 // One instantiation per kernel variant: the shared-memory opt-in (cudaFuncSetAttribute) applies to one function
-// only, and occupancy differs between variants, so each variant keeps its own cache, per device.
+// only, and occupancy differs between variants, so each variant keeps its own state, per device.
 template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false>
 cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_t s) {
   const auto kern = match_pick_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET>;
   const size_t smem = (size_t)kWarps * p.MP * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
-  // occupancy is a property of (kernel, smem): query once per distinct smem size
-  static size_t cached_smem_dev[64];
-  static int cached_per_sm_dev[64];
+  static std::map<int, size_t> opted_in;                // device -> the variant's max dynamic smem attribute
+  static std::map<std::pair<int, size_t>, int> per_sm;  // (device, smem) -> resident CTAs per SM
   int dev = 0;
   cudaError_t e = cudaGetDevice(&dev);
   if (e != cudaSuccess) return e;
-  dev &= 63;
-  size_t& cached_smem = cached_smem_dev[dev];
-  int& cached_per_sm = cached_per_sm_dev[dev];
-  if (cached_smem != smem + 1) {  // +1: zero-initialised statics mean "not cached"
-    if (smem > 48 * 1024) {
+  int ctas_per_sm = 1;
+  {
+    std::lock_guard<std::mutex> lk(g_match_launch_mu);
+    // The attribute is only ever raised: another handle may be launching this variant, on another thread, with the
+    // larger size it opted in to, and lowering it under that launch would make the launch fail.
+    size_t& attr = opted_in[dev];
+    if (smem > 48 * 1024 && smem > attr) {
       e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
       if (e != cudaSuccess) return e;
+      attr = smem;
     }
-    int per_sm = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kWarps * 32, smem);
-    if (e != cudaSuccess) return e;
-    cached_per_sm = per_sm < 1 ? 1 : per_sm;
-    cached_smem = smem + 1;
+    auto it = per_sm.find({dev, smem});
+    if (it == per_sm.end()) {
+      int n = 0;
+      e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kern, kWarps * 32, smem);
+      if (e != cudaSuccess) return e;
+      it = per_sm.emplace(std::make_pair(dev, smem), n < 1 ? 1 : n).first;
+    }
+    ctas_per_sm = it->second;
   }
   uint32_t grid = (p.R + kWarps - 1) / kWarps;
-  const uint32_t cap = (uint32_t)sm_count * (uint32_t)cached_per_sm;
+  const uint32_t cap = (uint32_t)sm_count * (uint32_t)ctas_per_sm;
   if (grid > cap) grid = cap;
   if (grid == 0) grid = 1;
   e = cudaMemsetAsync(p.work_counter, 0, sizeof(uint32_t), s);

@@ -37,8 +37,11 @@
  * Conventions (cgo-safe): every function returns 0 (FI_OK) or a negative
  * fi_status; nothing throws across the ABI; the caller owns every buffer and
  * no pointer is retained after a call returns; one fi_epp handle is internally
- * serialised by a mutex (concurrency comes from batching); library threads
- * never call back into the host language.  There is NO CPU fallback: without
+ * serialised by a mutex (concurrency comes from batching); calls on different
+ * handles may run concurrently, also on handles of one device; library threads
+ * never call back into the host language.  fi_epp_last_error is the message of
+ * the handle's latest failing call, and is not meaningful while other threads
+ * use the handle (read the status instead).  There is NO CPU fallback: without
  * a CUDA device fi_epp_create fails with FI_ERR_CUDA.
  *
  * Ties.  Upstream's MaxScorePicker shuffles the candidates before its stable sort, i.e. equal totals are
