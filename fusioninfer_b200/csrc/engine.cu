@@ -475,9 +475,9 @@ int alloc_index(fi_epp* h, uint64_t slots, uint32_t W, IndexTables& out) {
 }
 
 // Compact the live nodes into the spare table and swap.  Everything is queued on the index stream — no host
-// synchronisation: picks submitted later wait for ev_index (recorded by the flush that called us) and are
-// launched with the new view; picks already in flight keep reading the old tables, which are not touched again
-// before the NEXT rebuild, and that one is ordered behind them (flush_ops makes s_index wait for ev_pick).
+// synchronisation: picks submitted later wait for ev_index and are launched with the new view; picks already in
+// flight keep reading the old tables, which are not touched again before the NEXT rebuild, and that one is ordered
+// behind them (the rebuild is an update: update_begin).
 // The spare is allocated once, at the first rebuild (the only point where memory doubles), and then reused.
 int rebuild_index(fi_epp* h) {
   if (!h->ix_spare) {
@@ -499,6 +499,64 @@ int rebuild_index(fi_epp* h) {
   return FI_OK;
 }
 
+// queue the copy of the index counters that the next check_counters reads
+int read_counters(fi_epp* h) {
+  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
+  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
+  h->ctr_pending = true;
+  return FI_OK;
+}
+
+int check_counters(fi_epp* h);
+int check_counters_lagged(fi_epp* h, uint64_t extra);
+int flush_ops(fi_epp* h);
+
+// ---- the ordering rule of index updates -------------------------------------------------------------------------
+// Every change to the GPU index or to the device LRU runs on s_index as one update, between update_begin and
+// update_end:
+//  1. the ops staged earlier (fi_epp_index_apply, the host LRU) are flushed first;
+//  2. the counters of the previous update are checked, which may rebuild the index or report it full;
+//  3. s_index waits for ev_pick: a pick sees the index as it was when it was called, so an update queued after a pick
+//     must not overtake it on the GPU;
+//  -- the update's work --
+//  4. the index counters are copied back for the next rebuild decision, and the device LRU's status too when the work
+//     ran LRU kernels that count or flag errors;
+//  5. ev_index is recorded, so that every later pick waits for this update.
+// A missing step is a silent race between the streams.  A pick takes steps 1 and 2 (settle_updates) before it reads
+// the index.  Settle says which of steps 1 and 2 update_begin takes: both (kLagged: with check_counters_lagged(h,
+// extra)), step 2 only (flush_ops, which is the flush) or neither (the callers say why); Readback what step 4 copies.
+enum class Settle { kAll, kLagged, kCheck, kNone };
+enum class Readback { kIndex, kIndexAndLru, kNone };
+
+int settle_updates(fi_epp* h, bool lagged = false, uint64_t extra = 0) {
+  int rc = flush_ops(h);
+  if (rc != FI_OK) return rc;
+  return lagged ? check_counters_lagged(h, extra) : check_counters(h);
+}
+
+int update_begin(fi_epp* h, Settle settle = Settle::kAll, uint64_t extra = 0) {
+  int rc = FI_OK;
+  if (settle == Settle::kAll || settle == Settle::kLagged) rc = settle_updates(h, settle == Settle::kLagged, extra);
+  if (settle == Settle::kCheck) rc = check_counters(h);
+  if (rc != FI_OK) return rc;
+  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
+  return FI_OK;
+}
+
+// done (optional) is recorded behind the update's work and copies, before ev_index
+int update_end(fi_epp* h, Readback rb = Readback::kIndex, cudaEvent_t done = nullptr) {
+  cudaStream_t si = h->s_index.get();
+  if (rb == Readback::kIndexAndLru) {
+    FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->error, h->dlru->v.error, sizeof(uint32_t), cudaMemcpyDeviceToHost, si));
+    FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->n_sets, h->dlru->ctr.get(), 5 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, si));
+  }
+  const int rc = rb == Readback::kNone ? FI_OK : read_counters(h);  // (ev_ctr covers the status copies too)
+  if (rc != FI_OK) return rc;
+  if (done) FI_CUDA(cudaEventRecord(done, si));
+  FI_CUDA(cudaEventRecord(h->ev_index.get(), si));
+  return FI_OK;
+}
+
 // look at the counters copied back after the previous flush; rebuild if the table is
 // clogged with tombstones, fail if it is genuinely full
 int check_counters(fi_epp* h) {
@@ -515,12 +573,10 @@ int check_counters(fi_epp* h) {
   const uint64_t used = h->h_ctr->used, tomb = h->h_ctr->tombstones;
   if (used * 10 > h->ix.v.C * 7) {
     if ((used - tomb) * 10 > h->ix.v.C * 6) return fail(h, FI_ERR_CAPACITY, "index above 60% live keys: raise index_slots");
-    // the rebuild reads the old tables on s_index: every pick that still uses them must be ordered before the
-    // NEXT rebuild clears them — flush_ops (our only caller that launches work) waits for ev_pick first
-    FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
-    int rc = rebuild_index(h);
+    int rc = update_begin(h, Settle::kNone);  // (inside the check already)
+    if (rc == FI_OK) rc = rebuild_index(h);
     if (rc != FI_OK) return rc;
-    FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
+    return update_end(h, Readback::kNone);  // (a rebuild leaves the table below the rebuild threshold)
   }
   return FI_OK;
 }
@@ -550,24 +606,14 @@ GossipLog gossip_log(fi_epp* h) {
   return g;
 }
 
-// queue the copy of the index counters that the next check_counters reads
-int read_counters(fi_epp* h) {
-  FI_CUDA(cudaMemcpyAsync(h->h_ctr.get(), h->d_ctr.get(), sizeof(IndexCounters), cudaMemcpyDeviceToHost, h->s_index.get()));
-  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
-  h->ctr_pending = true;
-  return FI_OK;
-}
-
 // launch the staged SET then CLEAR ops of the current group on the index stream.
 // Asynchronous: the only waits are for the *previous* group's counters (rebuild /
 // overflow decisions lag one group) and for the staging buffer being reused.
 int flush_ops(fi_epp* h) {
   if (h->n_sets == 0 && h->n_clears == 0) return FI_OK;
-  int rc = check_counters(h);  // may rebuild (swaps tables) — only ever between groups
+  int rc = update_begin(h, Settle::kCheck);  // may rebuild (swaps tables) — only ever between groups
   if (rc != FI_OK) return rc;
   const int b = h->cur_buf;
-  // ops submitted after a pick returned must not overtake it on the GPU: the pick sees the index as of its call
-  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
   const GossipLog gl = gossip_log(h);
   if (h->n_sets) {
     FI_CUDA(cudaMemcpyAsync(h->d_sets[b].get(), h->h_sets[b].get(), h->n_sets * sizeof(fi_index_op), cudaMemcpyHostToDevice, h->s_index.get()));
@@ -586,9 +632,8 @@ int flush_ops(fi_epp* h) {
   h->ops_applied += h->n_sets + h->n_clears;
   h->ctr_unchecked += h->n_sets;
   FI_CUDA(cudaEventRecord(h->ev_buf[b].get(), h->s_index.get()));
-  rc = read_counters(h);
+  rc = update_end(h);
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   h->n_sets = h->n_clears = 0;
   h->cleared.clear();
   h->clears_untracked = false;
@@ -608,7 +653,9 @@ int gossip_round(fi_epp* h) {
   ShardState& sh = *h->shard;
   const unsigned long long* hdr = sh.h_ghdr.get();
   const uint32_t Wd = h->world;
-  int rc = nccl_allgather_on(h, sh.comm, sh.d_glog_n.get(), sh.d_ghdr.get(), 2 * sizeof(unsigned long long), h->s_index.get());
+  int rc = update_begin(h, Settle::kNone);  // (a check could fail this rank before the collectives, or make it wait)
+  if (rc != FI_OK) return rc;
+  rc = nccl_allgather_on(h, sh.comm, sh.d_glog_n.get(), sh.d_ghdr.get(), 2 * sizeof(unsigned long long), h->s_index.get());
   if (rc != FI_OK) return rc;
   FI_CUDA(cudaMemcpyAsync(sh.h_ghdr.get(), sh.d_ghdr.get(), (size_t)Wd * 2 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->s_index.get()));
   FI_CUDA(cudaStreamSynchronize(h->s_index.get()));
@@ -637,12 +684,7 @@ int gossip_round(fi_epp* h) {
     }
   }
   FI_CUDA(cudaMemsetAsync(sh.d_glog_n.get(), 0, 2 * sizeof(unsigned long long), h->s_index.get()));
-  if (na || nv) {  // the replays allocate nodes too: refresh the counters the rebuild decision reads
-    rc = read_counters(h);
-    if (rc != FI_OK) return rc;
-  }
-  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
-  return FI_OK;
+  return update_end(h, na || nv ? Readback::kIndex : Readback::kNone);  // (only the replays change the counters)
 }
 
 // One collective index update of a sharded pool = `rounds` gossip rounds on every rank: the ranks agree on the
@@ -816,13 +858,6 @@ int ensure_dev_lru(fi_epp* h) {
   return FI_OK;
 }
 
-// queue the refresh of the pinned LRU status (error flag + totals) behind everything submitted so far
-int lru_refresh_stat(fi_epp* h) {
-  FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->error, h->dlru->v.error, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
-  FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->n_sets, h->dlru->ctr.get(), 5 * sizeof(unsigned long long), cudaMemcpyDeviceToHost, h->s_index.get()));
-  return FI_OK;
-}
-
 // One sub-batch of a planned Add (the plan packed at `dp` by lru_plan_pack): the view the LRU kernels take, and the
 // kernels themselves.  Both Add paths (lru_device_add, lru_add_submitted) enqueue a sub-batch through these two.
 LruBatch lru_sub_batch(fi_epp* h, const uint32_t* dp, const LruPlan& pl, size_t sb, const uint64_t* chains, uint32_t pitch,
@@ -858,8 +893,9 @@ int lru_enqueue_touch(fi_epp* h, const LruBatch& b, const uint32_t* inc) {
 }
 
 // the rest of one sub-batch after its touch: winners, log records, index SETs, evictions, index CLEARs (clear_ovf:
-// then the overflow flags of the touch are reset); the index counters are copied back for the next rebuild decision
-int lru_enqueue_apply(fi_epp* h, const LruBatch& b, uint64_t touches, const GossipLog& glog, bool clear_ovf) {
+// then the overflow flags of the touch are reset); unless it is the update's last sub-batch, the index counters are
+// copied back for the rebuild decision before the next one
+int lru_enqueue_apply(fi_epp* h, const LruBatch& b, uint64_t touches, const GossipLog& glog, bool clear_ovf, bool last) {
   const uint32_t EL = h->cfg.endpoint_count, lo = h->cfg.endpoint_begin;
   FI_CUDA(cudaMemsetAsync(h->dlru->ctr.get() + 2, 0, sizeof(unsigned long long), h->s_index.get()));
   {
@@ -891,43 +927,29 @@ int lru_enqueue_apply(fi_epp* h, const LruBatch& b, uint64_t touches, const Goss
   }
   if (clear_ovf) FI_CUDA(cudaMemsetAsync(h->dlru->v.ovf, 0, ((size_t)EL + 1) * sizeof(uint32_t), h->s_index.get()));  // ovf[] and any_ovf
   h->ctr_unchecked += touches;
-  return read_counters(h);
+  return last ? FI_OK : read_counters(h);
 }
 
-// The prologue of both device-LRU Adds: the LRU exists, every local chain fits lru_capacity, and the ops staged
-// through fi_epp_index_apply go first.
-int lru_add_begin(fi_epp* h, const uint32_t* endpoints, const uint32_t* nblocks, uint32_t R) {
+// What both device-LRU Adds need before they plan: the LRU exists and every local chain fits lru_capacity.
+int lru_add_prepare(fi_epp* h, const uint32_t* endpoints, const uint32_t* nblocks, uint32_t R) {
   int rc = ensure_dev_lru(h);
   if (rc != FI_OK) return rc;
   for (uint32_t r = 0; r < R; ++r)
     if (nblocks[r] > h->cfg.lru_capacity && endpoints[r] - h->cfg.endpoint_begin < h->cfg.endpoint_count)
       return fail(h, FI_ERR_INVALID, "device LRU: a chain longer than lru_capacity");
-  return flush_ops(h);
+  return FI_OK;
 }
 
 // Pack plan `pl` into `buf` once `done` says the device has consumed the plan staged there before, and upload it on
-// the index stream.  Like every index update, ordered behind the picks submitted so far (a pick sees the index as of
-// its call).
+// the index stream.
 int lru_stage_plan(fi_epp* h, Staging<uint32_t>& buf, const LruPlan& pl, cudaEvent_t done) {
   const size_t words = lru_plan_words(pl, h->cfg.endpoint_count);
   FI_CUDA(cudaEventSynchronize(done));
   int rc = grow_staging(h, buf, words, words + words / 2 + 1024, true);  // room to spare: plans vary in size
   if (rc != FI_OK) return rc;
   lru_plan_pack(pl, buf.h.get());
-  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
   if (words) FI_CUDA(cudaMemcpyAsync(buf.d.get(), buf.h.get(), words * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
   h->stats.h2d_bytes += words * sizeof(uint32_t);
-  return FI_OK;
-}
-
-// The epilogue of both device-LRU Adds, behind their sub-batches: the LRU status refresh, then ev_ctr (which covers
-// the status copies), `done` (if given) and ev_index.
-int lru_add_end(fi_epp* h, cudaEvent_t done) {
-  int rc = lru_refresh_stat(h);
-  if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_ctr.get(), h->s_index.get()));
-  if (done) FI_CUDA(cudaEventRecord(done, h->s_index.get()));
-  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   return FI_OK;
 }
 
@@ -961,13 +983,12 @@ int lru_stage_chains(fi_epp* h, const uint64_t* chains, uint32_t pitch, uint32_t
 // (my_err) with no sub-batches.
 int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains, bool on_device, uint32_t pitch,
                    const uint32_t* nblocks, uint32_t R, int my_err) {
-  if (my_err == FI_OK) my_err = lru_add_begin(h, endpoints, nblocks, R);
+  if (my_err == FI_OK) my_err = lru_add_prepare(h, endpoints, nblocks, R);
   const uint32_t EL = h->cfg.endpoint_count, lo = h->cfg.endpoint_begin;
   const bool sharded = h->world > 1;
   LruPlan& pl = h->lru_plan;
   std::vector<uint32_t> ep2;  // the conservative pass's endpoints: the deferred requests' (FI_NO_ENDPOINT elsewhere)
   for (const bool conservative : {false, true}) {
-    if (my_err == FI_OK) my_err = check_counters(h);
     const auto t0 = std::chrono::steady_clock::now();
     size_t K = 0, nsub = 0;
     if (my_err == FI_OK) {
@@ -975,10 +996,11 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
       // per touch; CLEARs: evictions <= keys added, plus doomed entries <= touches)
       const uint64_t cap_touches = sharded ? std::min<uint64_t>(h->dlru->touch_cap, kOpChunk / 2) : h->dlru->touch_cap;
       lru_plan_batch(endpoints, nblocks, R, lo, EL, conservative ? h->cfg.lru_capacity : 0xFFFFFFFFu, cap_touches, h->cfg.max_batch, &pl);
-      if (pl.subs.empty() && !sharded) return FI_OK;
+      if (pl.subs.empty() && !sharded) return settle_updates(h);
       K = pl.req_id.size();
       nsub = pl.subs.size();
-      my_err = lru_stage_plan(h, h->lru_plan_buf, pl, h->dlru->ev.get());  // (dlru->ev covers the chain staging too)
+      my_err = update_begin(h);
+      if (my_err == FI_OK) my_err = lru_stage_plan(h, h->lru_plan_buf, pl, h->dlru->ev.get());  // (dlru->ev covers the chain staging too)
     }
     if (my_err == FI_OK && !on_device && K) my_err = lru_stage_chains(h, chains, pitch, R, pl, &chains);
     if (my_err == FI_OK) h->lru_sub_batches += nsub;
@@ -1018,11 +1040,11 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
             ++n_deferred;
           }
       }
-      return lru_enqueue_apply(h, b, sbt.touches, glog, any_ovf);
+      return lru_enqueue_apply(h, b, sbt.touches, glog, any_ovf, sb + 1 == nsub);
     });
     if (rc != (sharded ? my_err : FI_OK)) return rc;  // (a sharded rank with my_err goes on to the second pass)
     if (my_err != FI_OK) continue;
-    rc = lru_add_end(h, h->dlru->ev.get());
+    rc = update_end(h, Readback::kIndexAndLru, h->dlru->ev.get());
     if (rc != FI_OK) return rc;
     if (h->verbose) {
       const auto t1 = std::chrono::steady_clock::now();
@@ -1043,7 +1065,7 @@ int lru_device_add(fi_epp* h, const uint32_t* endpoints, const uint64_t* chains,
 }
 
 // the index-stream part of lru_add_submitted behind the plan upload: the chain copy out of the slot, the sub-batches,
-// the status copies
+// the copy of the touch kernel's overflow flag
 int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, fi_epp::PipeAdd& pa, uint32_t R) {
   const uint64_t* slot_chain = slot ? h->d_chain2.get() : h->d_chain.get();
   FI_CUDA(cudaStreamWaitEvent(h->s_copy.get(), h->ev_a[slot].get(), 0));  // the batch's chains are written
@@ -1054,17 +1076,17 @@ int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, fi_ep
   h->lru_sub_batches += pl.subs.size();
   for (size_t sb = 0; sb < pl.subs.size(); ++sb) {
     const uint64_t touches = pl.subs[sb].touches;
-    int rc = check_counters_lagged(h, touches);  // may rebuild the index (on s_index, before this sub-batch)
+    int rc = sb ? check_counters_lagged(h, touches) : FI_OK;  // may rebuild the index (update_begin checked the first)
     if (rc != FI_OK) return rc;
     const uint32_t* inc = nullptr;
     const LruBatch b = lru_sub_batch(h, pa.plan.d.get(), pl, sb, pa.d_chains.get(), h->MP, &inc);
     rc = lru_enqueue_touch(h, b, inc);
     if (rc != FI_OK) return rc;
-    rc = lru_enqueue_apply(h, b, touches, glog, false);
+    rc = lru_enqueue_apply(h, b, touches, glog, false, sb + 1 == pl.subs.size());
     if (rc != FI_OK) return rc;
   }
   FI_CUDA(cudaMemcpyAsync(&h->dlru->stat->planned_ovf, h->dlru->v.any_ovf, sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_index.get()));
-  return lru_add_end(h, nullptr);
+  return FI_OK;
 }
 
 // fi_epp_index_add_submitted: indexer.Add(chain_r, endpoints[r]) for the batch whose chains pipeline slot `slot`
@@ -1078,12 +1100,12 @@ int lru_add_submitted_enqueue(fi_epp* h, uint32_t slot, const LruPlan& pl, fi_ep
 //  - the chains are first copied out of the slot on s_copy, as soon as the batch's hashing is done, so that the submit
 //    that reuses the slot waits for that copy only and not for this Add, which runs behind the picks in flight.
 int lru_add_submitted(fi_epp* h, uint32_t slot, const uint32_t* endpoints, const uint32_t* nblocks, uint32_t R) {
-  int rc = lru_add_begin(h, endpoints, nblocks, R);
+  int rc = lru_add_prepare(h, endpoints, nblocks, R);
   if (rc != FI_OK) return rc;
   LruPlan& pl = h->lru_plan;
   lru_plan_batch(endpoints, nblocks, R, h->cfg.endpoint_begin, h->cfg.endpoint_count, lru_touch_bound(h->dlru->v.TS, h->dlru->v.capacity),
                  h->dlru->touch_cap, h->cfg.max_batch, &pl);
-  if (pl.subs.empty()) return FI_OK;
+  if (pl.subs.empty()) return flush_ops(h);
   fi_epp::PipeAdd& pa = h->padd[h->padd_seq & 1];
   if (!pa.ev_done) {
     Event ev;
@@ -1093,17 +1115,17 @@ int lru_add_submitted(fi_epp* h, uint32_t slot, const uint32_t* endpoints, const
     pa.ev_done = std::move(ev);
     pa.d_chains = std::move(chains);
   }
-  rc = lru_stage_plan(h, pa.plan, pl, pa.ev_done.get());  // waits for the Add before the previous one
+  rc = update_begin(h, Settle::kLagged, pl.subs[0].touches);
+  if (rc == FI_OK) rc = lru_stage_plan(h, pa.plan, pl, pa.ev_done.get());  // waits for the Add before the previous one
   if (rc != FI_OK) return rc;
   // From here on work that reads pa's buffers is queued: whatever happens, pa.ev_done marks its end (the s_index wait
   // on the chain copy makes it cover that copy too), and the next call takes the other buffers.
   rc = lru_add_submitted_enqueue(h, slot, pl, pa, R);
-  cudaError_t e = cudaStreamWaitEvent(h->s_index.get(), h->ev_slot_read[slot].get(), 0);
-  if (e == cudaSuccess) e = cudaEventRecord(pa.ev_done.get(), h->s_index.get());
+  if (rc == FI_OK) rc = update_end(h, Readback::kIndexAndLru, pa.ev_done.get());
+  if (rc != FI_OK && cudaStreamWaitEvent(h->s_index.get(), h->ev_slot_read[slot].get(), 0) == cudaSuccess)
+    cudaEventRecord(pa.ev_done.get(), h->s_index.get());
   h->padd_seq++;
-  if (rc != FI_OK) return rc;
-  if (e != cudaSuccess) return fail(h, FI_ERR_CUDA, cudaGetErrorString(e));
-  return FI_OK;
+  return rc;
 }
 
 // fi_epp_set_lru_capacities on the device LRU: upload the new capacities `caps`, then evict the listed local endpoints
@@ -1159,8 +1181,8 @@ int lru_device_resize(fi_epp* h, const std::vector<uint32_t>& local, const std::
     std::memcpy(h->lru_resize.h.get(), r_eps.data(), pairs * sizeof(uint32_t));
     std::memcpy(h->lru_resize.h.get() + pairs, r_quota.data(), pairs * sizeof(uint32_t));
   }
-  // picks called before this one must not see its evictions
-  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
+  int rc = update_begin(h, Settle::kNone);  // (the caller settled before the readback, which must not wait for picks)
+  if (rc != FI_OK) return rc;
   // (pageable source: the copy has taken the data when cudaMemcpyAsync returns)
   FI_CUDA(cudaMemcpyAsync(h->dlru->v.cap, caps.data(), (size_t)EL * sizeof(uint32_t), cudaMemcpyHostToDevice, h->s_index.get()));
   h->stats.h2d_bytes += (size_t)EL * sizeof(uint32_t);
@@ -1182,13 +1204,7 @@ int lru_device_resize(fi_epp* h, const std::vector<uint32_t>& local, const std::
     FI_CUDA(launch_index_clear_counted(h->ix.v, h->d_ctr.get(), h->dlru->clears.get(), r_total[k], h->dlru->ctr.get() + 2, lo, EL, h->rank, glog,
                                        h->s_index.get()));
   }
-  int rc = lru_refresh_stat(h);
-  if (rc != FI_OK) return rc;
-  // the CLEARs' tombstones reach the rebuild decision of the next index update (ev_ctr covers the status copy too)
-  rc = read_counters(h);
-  if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
-  return FI_OK;
+  return update_end(h, Readback::kIndexAndLru);
 }
 
 // Whether a pick may hash each request only up to its first block the index does not hold (hash_kernels.cu "early
@@ -1461,9 +1477,7 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
   const bool sharded = h->world > 1;
   if (sharded && (h->n_sets || h->n_clears))
     return fail(h, FI_ERR_STATE, "sharded pool: index updates are collective (fi_epp_index_apply / fi_epp_index_add_chains)");
-  int rc = flush_ops(h);
-  if (rc != FI_OK) return rc;
-  rc = check_counters(h);
+  int rc = settle_updates(h);
   if (rc != FI_OK) return rc;
   h->tracing = !h->profiling && h->trace_call >= 0 && (long)h->stats.pick_calls == h->trace_call;
   if (h->tracing) {
@@ -1619,9 +1633,7 @@ int issue_ticket(fi_epp* h, uint64_t* t) {
 // fi_epp::s_a).  lagged: the index counters may lag (check_counters_lagged, fi_epp_pick_submit_ex).
 int submit_pick(fi_epp* h, const PickCall& c, cudaStream_t us, uint64_t* ticket, bool lagged) {
   const uint32_t R = c.R;
-  int rc = flush_ops(h);
-  if (rc != FI_OK) return rc;
-  rc = lagged ? check_counters_lagged(h, 0) : check_counters(h);
+  int rc = settle_updates(h, lagged);
   if (rc != FI_OK) return rc;
   if (!h->d_chain2) {  // slot 1's buffers, both or neither
     DevPtr<uint64_t> chain;
@@ -1699,8 +1711,7 @@ int submit_pick(fi_epp* h, const PickCall& c, cudaStream_t us, uint64_t* ticket,
 // Upstream indexer.RemovePod for the distinct local endpoints `local` (fi_epp_index_remove_endpoints, and the endpoints
 // a shrink of fi_epp_resize_pool drops): one sweep over the index rows clears their bits whatever put them there (LRU
 // Adds or direct SETs), keys nobody holds any more are retired (tombstones, like a CLEAR), and the endpoints' LRUs
-// start empty.  Ordered like fi_epp_index_apply: behind the ops staged so far and the picks called so far, ahead of
-// every later pick.  pairs_removed != null: wait for the sweep and write how many pairs left the index.
+// start empty.  pairs_removed != null: wait for the sweep and write how many pairs left the index.
 int remove_local_endpoints(fi_epp* h, const std::vector<uint32_t>& local, uint64_t* pairs_removed) {
   RemoveSet rs{};
   for (uint32_t e : local) rs.row[e >> 5] |= 1u << (e & 31);
@@ -1710,14 +1721,10 @@ int remove_local_endpoints(fi_epp* h, const std::vector<uint32_t>& local, uint64
       rs.bits[rs.m] = rs.row[w];
       ++rs.m;
     }
-  int rc = flush_ops(h);  // staged SET / CLEAR groups and host-LRU deltas go first
-  if (rc != FI_OK) return rc;
-  rc = check_counters(h);
-  if (rc != FI_OK) return rc;
   if (!h->d_rm) FI_CUDA(cuda_alloc(h->d_rm, 1 + ((size_t)h->cfg.endpoint_count + 1) / 2));
   uint32_t* d_eps = reinterpret_cast<uint32_t*>(h->d_rm.get() + 1);
-  // picks called before this one must not see the removal
-  FI_CUDA(cudaStreamWaitEvent(h->s_index.get(), h->ev_pick.get(), 0));
+  int rc = update_begin(h);
+  if (rc != FI_OK) return rc;
   FI_CUDA(cudaMemsetAsync(h->d_rm.get(), 0, sizeof(unsigned long long), h->s_index.get()));
   {
     LaunchScope ls(h, h->s_index.get(), K_INDEX);
@@ -1732,10 +1739,8 @@ int remove_local_endpoints(fi_epp* h, const std::vector<uint32_t>& local, uint64
   }
   for (uint32_t e : local)
     if (e < h->lrus.size()) h->lrus[e].clear();
-  // the sweep's tombstones reach the rebuild decision of the next index update
-  rc = read_counters(h);
+  rc = update_end(h);  // (the reset changes no LRU status)
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_index.get(), h->s_index.get()));
   if (pairs_removed) {
     unsigned long long c = 0;
     FI_CUDA(cudaMemcpyAsync(&c, h->d_rm.get(), sizeof(c), cudaMemcpyDeviceToHost, h->s_index.get()));
@@ -2116,9 +2121,7 @@ int fi_epp_resize_pool(fi_epp* h, uint32_t num_endpoints, uint64_t* pairs_remove
     return fail(h, FI_ERR_STATE, "fi_epp_resize_pool needs a handle over the whole pool");
   if (h->lru_mode == 0) return fail(h, FI_ERR_STATE, "fi_epp_resize_pool: the host LRU serves the handle");
   if (En == E) return FI_OK;
-  int rc = flush_ops(h);
-  if (rc != FI_OK) return rc;
-  rc = check_counters(h);
+  int rc = update_begin(h);
   if (rc != FI_OK) return rc;
   for (cudaStream_t s : {h->s_main.get(), h->s_index.get(), h->s_copy.get(), h->s_a.get()}) FI_CUDA(cudaStreamSynchronize(s));
   // The slot floor counts the live keys before a shrink's removal: an upper bound of those after it, known before
@@ -2236,18 +2239,16 @@ int fi_epp_resize_pool(fi_epp* h, uint32_t num_endpoints, uint64_t* pairs_remove
   h->cfg.num_endpoints = h->cfg.endpoint_count = En;
   h->cfg.index_slots = h->ix.v.C;
   h->W = Wn;
-  rc = read_counters(h);
+  rc = update_end(h);
   if (rc != FI_OK) return rc;
-  FI_CUDA(cudaEventRecord(h->ev_index.get(), si));
   FI_CUDA(cudaStreamSynchronize(si));
   return FI_OK;
 }
 
 // Per-endpoint LRU capacities (SPEC S.2b; upstream's autoTune).  The listed endpoints' LRUs evict their least recently
 // used keys down to the new capacities, each evicted pair CLEARed as an eviction inside an Add would be; later Adds
-// evict against them.  Ordered like fi_epp_index_apply: behind the ops staged so far and the picks called so far,
-// ahead of every later pick.  The host LRU's limits are set whichever LRU serves the handle (before the first Add it
-// is not chosen yet, and both are empty then); the device LRU reads h->lru_caps when it is allocated.
+// evict against them.  The host LRU's limits are set whichever LRU serves the handle (before the first Add it is not
+// chosen yet, and both are empty then); the device LRU reads h->lru_caps when it is allocated.
 int fi_epp_set_lru_capacities(fi_epp* h, const uint32_t* endpoints, const uint32_t* capacities, uint32_t n,
                               uint64_t* entries_evicted) {
   if (!h || ((!endpoints || !capacities) && n)) return FI_ERR_INVALID;
@@ -2276,17 +2277,15 @@ int fi_epp_set_lru_capacities(fi_epp* h, const uint32_t* endpoints, const uint32
     }
   }
   if (local.empty()) return FI_OK;
-  int rc = flush_ops(h);  // staged SET / CLEAR groups and host-LRU deltas go first
-  if (rc != FI_OK) return rc;
-  rc = check_counters(h);
+  int rc = settle_updates(h);
   if (rc != FI_OK) return rc;
   uint64_t evicted = 0;
   if (h->lru_mode == 1 && h->dlru) {
     rc = lru_device_resize(h, local, caps, &evicted);
     if (rc != FI_OK) return rc;
   }
-  // host LRU: the evictions are staged like the deltas of an Add (fi_epp_index_apply's ordering); the sets of a
-  // device-LRU handle are empty and only take the limit
+  // host LRU: the evictions are staged like the deltas of an Add; the sets of a device-LRU handle are empty and only
+  // take the limit
   for (uint32_t e : local) {
     rc = FI_OK;
     h->lrus[e].shrink(caps[e], [&](uint64_t key) {
