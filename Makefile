@@ -14,8 +14,9 @@ HDRS := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/fi_epp.h
 
 EXT_ORACLE := $(OBJDIR)/libepp_ext_oracle.so
 RESIZE_ORACLE := $(OBJDIR)/libepp_resize_oracle.so
+SNAPSHOT_ORACLE := $(OBJDIR)/libepp_snapshot_oracle.so
 
-all: $(LIB) $(HOSTCHECK) oracle $(EXT_ORACLE) $(RESIZE_ORACLE)
+all: $(LIB) $(HOSTCHECK) oracle $(EXT_ORACLE) $(RESIZE_ORACLE) $(SNAPSHOT_ORACLE)
 
 $(OBJDIR)/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -30,7 +31,7 @@ $(LIB): $(CU_OBJS) $(OBJDIR)/epp_config.o
 	$(NVCC) $(ARCH) -shared -o $@ $^ -ldl
 
 # host-only build of the shared host/device arithmetic, for CPU unit tests
-$(HOSTCHECK): $(CSRC)/hostcheck.cpp $(CSRC)/xxh64.cuh $(CSRC)/bitslice.cuh $(CSRC)/lru.h $(CSRC)/lru_batch.h $(CSRC)/lru_plan.h $(CSRC)/pool_shape.h $(CSRC)/tiebreak.cuh
+$(HOSTCHECK): $(CSRC)/hostcheck.cpp $(CSRC)/xxh64.cuh $(CSRC)/bitslice.cuh $(CSRC)/lru.h $(CSRC)/lru_batch.h $(CSRC)/lru_plan.h $(CSRC)/pool_shape.h $(CSRC)/snapshot_format.h $(CSRC)/tiebreak.cuh
 	@mkdir -p $(dir $(HOSTCHECK))
 	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -shared -pthread -x c++ $(CSRC)/hostcheck.cpp -o $@
 
@@ -44,6 +45,8 @@ $(OBJDIR)/libepp_%.so: tests/%.cpp oracle/epp_oracle.cpp include/fi_epp.h
 	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ $<
 # tests/resize_oracle.cpp adds the pool resize on top of tests/ext_oracle.cpp
 $(RESIZE_ORACLE): tests/ext_oracle.cpp
+# tests/snapshot_oracle.cpp adds the state of an index snapshot on top of tests/resize_oracle.cpp
+$(SNAPSHOT_ORACLE): tests/ext_oracle.cpp tests/resize_oracle.cpp
 
 clean:
 	rm -rf $(OBJDIR) $(LIB) $(HOSTCHECK)

@@ -18,6 +18,7 @@ from .picker import (  # noqa: F401
     default_config,
     make_config,
     model_seed,
+    snapshot_info,
     subset_bitsets,
 )
 
@@ -30,6 +31,7 @@ __all__ = [
     "default_config",
     "make_config",
     "model_seed",
+    "snapshot_info",
     "subset_bitsets",
     "PICK_DTYPE",
     "OP_DTYPE",

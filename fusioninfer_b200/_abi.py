@@ -148,6 +148,19 @@ class fi_index_stats(C.Structure):
     ]
 
 
+class fi_epp_snapshot_info(C.Structure):
+    _fields_ = [
+        ("block_bytes", C.c_uint32),
+        ("max_blocks", C.c_uint32),
+        ("lru_capacity", C.c_uint32),
+        ("num_endpoints", C.c_uint32),
+        ("n_nodes", C.c_uint64),
+        ("n_lru", C.c_uint64),
+        ("pairs", C.c_uint64),
+        ("bytes", C.c_uint64),
+    ]
+
+
 class fi_epp_stats(C.Structure):
     _fields_ = [
         ("kernel_launches", C.c_uint64),
@@ -217,6 +230,9 @@ SYMBOLS = [
     ("fi_epp_index_apply", C.c_int, [_P, _P, C.c_uint64]),
     ("fi_epp_index_remove_endpoints", C.c_int, [_P, _P, C.c_uint32, _P]),
     ("fi_epp_resize_pool", C.c_int, [_P, C.c_uint32, _P]),
+    ("fi_epp_snapshot_save", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
+    ("fi_epp_snapshot_load", C.c_int, [_P, _P, C.c_uint64]),
+    ("fi_epp_snapshot_info", C.c_int, [_P, C.c_uint64, C.POINTER(fi_epp_snapshot_info)]),
     ("fi_epp_set_lru_capacities", C.c_int, [_P, _P, _P, C.c_uint32, _P]),
     ("fi_epp_index_add_chain", C.c_int, [_P, C.c_uint32, _P, C.c_uint32]),
     ("fi_epp_index_add_chains", C.c_int, [_P, _P, _P, C.c_uint32, _P, C.c_uint32]),

@@ -35,6 +35,7 @@
 #include "lru_device.cuh"
 #include "lru_plan.h"
 #include "pool_shape.h"
+#include "snapshot_format.h"
 #include "xxh64.cuh"
 
 using namespace fi;
@@ -2242,6 +2243,357 @@ int fi_epp_resize_pool(fi_epp* h, uint32_t num_endpoints, uint64_t* pairs_remove
   rc = update_end(h);
   if (rc != FI_OK) return rc;
   FI_CUDA(cudaStreamSynchronize(si));
+  return FI_OK;
+}
+
+// ---- index snapshots (docs/SPEC.md S.2d) -----------------------------------------------------------------------
+namespace {
+
+// Both directions move the blob between the caller's pageable buffer and device buffers through two pinned buffers of
+// kSnapStage bytes: the copy engine fills (drains) one while the host copies the other.  Nothing larger is pinned.
+constexpr uint64_t kSnapStage = 32ull << 20;
+
+struct SnapStager {
+  PinnedPtr<uint8_t> buf[2];
+  Event ev[2];
+  int k = 0;
+};
+
+int snap_stager(fi_epp* h, SnapStager& st) {
+  for (int i = 0; i < 2; ++i) {
+    if (cuda_alloc(st.buf[i], kSnapStage) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(h, FI_ERR_NOMEM, "cannot allocate the pinned snapshot staging");
+    }
+    FI_CUDA(cuda_create(st.ev[i]));
+  }
+  return FI_OK;
+}
+
+// device [src, src + bytes) -> host dst, on s_index (returns when dst is written)
+int snap_d2h(fi_epp* h, SnapStager& st, uint8_t* dst, const void* src, uint64_t bytes) {
+  cudaStream_t si = h->s_index.get();
+  int prev = -1;
+  uint64_t prev_off = 0, prev_n = 0;
+  for (uint64_t off = 0; off < bytes; off += kSnapStage) {
+    const uint64_t n = std::min(kSnapStage, bytes - off);
+    const int k = st.k;
+    st.k ^= 1;
+    // (buf[k] was drained by the previous iteration's host copy)
+    FI_CUDA(cudaMemcpyAsync(st.buf[k].get(), static_cast<const uint8_t*>(src) + off, n, cudaMemcpyDeviceToHost, si));
+    FI_CUDA(cudaEventRecord(st.ev[k].get(), si));
+    if (prev >= 0) {
+      FI_CUDA(cudaEventSynchronize(st.ev[prev].get()));
+      std::memcpy(dst + prev_off, st.buf[prev].get(), prev_n);
+    }
+    prev = k;
+    prev_off = off;
+    prev_n = n;
+  }
+  if (prev >= 0) {
+    FI_CUDA(cudaEventSynchronize(st.ev[prev].get()));
+    std::memcpy(dst + prev_off, st.buf[prev].get(), prev_n);
+  }
+  h->stats.d2h_bytes += bytes;
+  return FI_OK;
+}
+
+// host [src, src + bytes) -> device dst, queued on s_index (src may be reused when the call returns)
+int snap_h2d(fi_epp* h, SnapStager& st, void* dst, const uint8_t* src, uint64_t bytes) {
+  cudaStream_t si = h->s_index.get();
+  for (uint64_t off = 0; off < bytes; off += kSnapStage) {
+    const uint64_t n = std::min(kSnapStage, bytes - off);
+    const int k = st.k;
+    st.k ^= 1;
+    FI_CUDA(cudaEventSynchronize(st.ev[k].get()));  // the copy out of buf[k] two pieces ago is done
+    std::memcpy(st.buf[k].get(), src + off, n);
+    FI_CUDA(cudaMemcpyAsync(static_cast<uint8_t*>(dst) + off, st.buf[k].get(), n, cudaMemcpyHostToDevice, si));
+    FI_CUDA(cudaEventRecord(st.ev[k].get(), si));
+  }
+  h->stats.h2d_bytes += bytes;
+  return FI_OK;
+}
+
+// nodes per chunk of the device staging of node keys and rows (at least one export tile)
+uint64_t snap_chunk_nodes(uint32_t We) { return std::max<uint64_t>(1024, (64ull << 20) / (8 + 4ull * We)); }
+
+unsigned snap_threads() { return std::min(usable_cores(), 16u); }
+
+// save and load need a single-rank handle over the whole pool whose LRU, if it has one, is the device LRU
+int snapshot_handle_ok(fi_epp* h, const char* what) {
+  if (h->world > 1) return fail(h, FI_ERR_STATE, std::string("sharded pool: ") + what + " needs a single-rank handle");
+  if (h->cfg.endpoint_begin != 0 || h->cfg.endpoint_count != h->cfg.num_endpoints)
+    return fail(h, FI_ERR_STATE, std::string(what) + " needs a handle over the whole pool");
+  if (h->cfg.lru_capacity) {
+    int rc = choose_lru_mode(h);
+    if (rc != FI_OK) return rc;
+    if (h->lru_mode == 0) return fail(h, FI_ERR_STATE, std::string(what) + ": the host LRU serves the handle");
+  }
+  return FI_OK;
+}
+
+int sync_all_streams(fi_epp* h) {
+  for (cudaStream_t s : {h->s_main.get(), h->s_index.get(), h->s_copy.get(), h->s_a.get()}) FI_CUDA(cudaStreamSynchronize(s));
+  return FI_OK;
+}
+
+}  // namespace
+
+// Save (S.2d).  Blocking; the handle is not changed.  Sizes first: the live nodes per export tile and the LRUs' entry
+// counts are read back, which gives the header.  Then the sections are written in payload order: the capacities and
+// LRU lengths from the host, every LRU's keys from one dump of all endpoints, the nodes chunk by chunk through the
+// device staging; last the checksum, over the caller's buffer on host threads.
+int fi_epp_snapshot_save(fi_epp* h, void* buf, uint64_t cap, uint64_t* bytes) {
+  if (!h || !bytes) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  int rc = snapshot_handle_ok(h, "fi_epp_snapshot_save");
+  if (rc != FI_OK) return rc;
+  rc = settle_updates(h);
+  if (rc != FI_OK) return rc;
+  rc = sync_all_streams(h);  // (picks in flight included: the state saved is the one every earlier call left)
+  if (rc != FI_OK) return rc;
+  cudaStream_t si = h->s_index.get();
+  const uint32_t E = h->cfg.num_endpoints, C = h->cfg.lru_capacity, We = snap_row_words(E);
+  IndexCounters ctr;
+  FI_CUDA(cudaMemcpy(&ctr, h->d_ctr.get(), sizeof(ctr), cudaMemcpyDeviceToHost));
+  const uint64_t n = std::min<uint64_t>(ctr.used, h->ix.v.C);
+  const uint32_t tiles = index_snap_tiles(n);
+  DevPtr<uint32_t> d_tile;
+  DevPtr<uint64_t> d_tile_off;
+  if (cuda_alloc(d_tile, tiles) != cudaSuccess || cuda_alloc(d_tile_off, (size_t)tiles + 1) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(h, FI_ERR_NOMEM, "cannot allocate the snapshot's tile counts");
+  }
+  {
+    LaunchScope ls(h, si, K_OTHER);
+    FI_CUDA(launch_index_snap_count(h->ix.v, n, d_tile.get(), si));
+  }
+  std::vector<uint32_t> tile(tiles);
+  FI_CUDA(cudaMemcpyAsync(tile.data(), d_tile.get(), (size_t)tiles * sizeof(uint32_t), cudaMemcpyDeviceToHost, si));
+  std::vector<uint32_t> caps(E, 0), lens(E, 0);
+  if (C) caps = h->lru_caps;
+  if (h->dlru) FI_CUDA(cudaMemcpyAsync(lens.data(), h->dlru->v.count, (size_t)E * sizeof(uint32_t), cudaMemcpyDeviceToHost, si));
+  FI_CUDA(cudaStreamSynchronize(si));
+  std::vector<uint64_t> tile_off(tiles + 1, 0), lru_off(E + 1, 0);
+  for (uint32_t t = 0; t < tiles; ++t) tile_off[t + 1] = tile_off[t] + tile[t];
+  for (uint32_t e = 0; e < E; ++e) lru_off[e + 1] = lru_off[e] + lens[e];
+  const uint64_t n_nodes = tile_off[tiles], n_lru = lru_off[E];
+  const SnapLayout l = snap_layout(E, n_nodes, n_lru);
+  *bytes = kSnapHeaderBytes + l.end;
+  if (!buf) return FI_OK;
+  if (cap < *bytes) return fail(h, FI_ERR_CAPACITY, "snapshot buffer of " + std::to_string(cap) + " bytes, " + std::to_string(*bytes) + " needed");
+
+  SnapStager st;
+  rc = snap_stager(h, st);
+  if (rc != FI_OK) return rc;
+  uint8_t* out = static_cast<uint8_t*>(buf);
+  uint8_t* pay = out + kSnapHeaderBytes;
+  SnapHeader hd{};
+  std::memcpy(hd.magic, kSnapMagic, 8);
+  hd.version = kSnapVersion;
+  hd.header_bytes = kSnapHeaderBytes;
+  hd.block_bytes = h->cfg.block_bytes;
+  hd.max_blocks = h->cfg.max_blocks;
+  hd.lru_capacity = C;
+  hd.num_endpoints = E;
+  hd.n_nodes = n_nodes;
+  hd.n_lru = n_lru;
+  hd.payload_bytes = l.end;
+  std::memcpy(pay + l.caps, caps.data(), 4ull * E);
+  std::memcpy(pay + l.lru_len, lens.data(), 4ull * E);
+  // every LRU, oldest first, in one launch
+  if (n_lru) {
+    DevPtr<uint64_t> d_keys, d_off;
+    DevPtr<uint32_t> d_n;
+    if (cuda_alloc(d_keys, n_lru) != cudaSuccess || cuda_alloc(d_off, E) != cudaSuccess || cuda_alloc(d_n, E) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(h, FI_ERR_NOMEM, "cannot allocate the snapshot's LRU staging");
+    }
+    FI_CUDA(cudaMemcpyAsync(d_off.get(), lru_off.data(), (size_t)E * sizeof(uint64_t), cudaMemcpyHostToDevice, si));
+    {
+      LaunchScope ls(h, si, K_OTHER);
+      FI_CUDA(launch_lru_dump_all(h->dlru->v, d_off.get(), d_keys.get(), d_n.get(), si));
+    }
+    std::vector<uint32_t> got(E);
+    FI_CUDA(cudaMemcpyAsync(got.data(), d_n.get(), (size_t)E * sizeof(uint32_t), cudaMemcpyDeviceToHost, si));
+    rc = snap_d2h(h, st, pay + l.lru_keys, d_keys.get(), 8 * n_lru);
+    if (rc != FI_OK) return rc;
+    if (got != lens) return fail(h, FI_ERR_STATE, "device LRU: live records differ from the entry counts (broken invariant)");
+  }
+  // the nodes, a range of tiles per chunk of the device staging
+  if (n_nodes) {
+    const uint64_t chunk = snap_chunk_nodes(We);
+    DevPtr<uint64_t> d_keys;
+    DevPtr<uint32_t> d_rows;
+    if (cuda_alloc(d_keys, chunk) != cudaSuccess || cuda_alloc(d_rows, chunk * We) != cudaSuccess) {
+      cudaGetLastError();
+      return fail(h, FI_ERR_NOMEM, "cannot allocate the snapshot's node staging");
+    }
+    FI_CUDA(cudaMemcpyAsync(d_tile_off.get(), tile_off.data(), ((size_t)tiles + 1) * sizeof(uint64_t), cudaMemcpyHostToDevice, si));
+    for (uint32_t t0 = 0; t0 < tiles;) {
+      uint32_t t1 = t0;
+      while (t1 < tiles && tile_off[t1 + 1] - tile_off[t0] <= chunk) ++t1;
+      const uint64_t base = tile_off[t0], m = tile_off[t1] - base;
+      {
+        LaunchScope ls(h, si, K_OTHER);
+        FI_CUDA(launch_index_snap_export(h->ix.v, n, t0, t1, d_tile_off.get(), base, We, d_keys.get(), d_rows.get(), si));
+      }
+      rc = snap_d2h(h, st, pay + l.node_keys + 8 * base, d_keys.get(), 8 * m);
+      if (rc == FI_OK) rc = snap_d2h(h, st, pay + l.node_rows + 4ull * We * base, d_rows.get(), 4ull * We * m);
+      if (rc != FI_OK) return rc;
+      t0 = t1;
+    }
+  }
+  hd.checksum = snap_checksum(&hd, pay, l.end, snap_threads());
+  std::memcpy(out, &hd, sizeof(hd));
+  return FI_OK;
+}
+
+// Load (S.2d).  The blob is checked on the host first (snap_check, marker keys, the configuration, room in the index);
+// then, with every earlier call complete, new index tables and a new device LRU are built from it on s_index and
+// checked for duplicate keys; only then are they swapped in.  Until the swap nothing of the handle changes.
+int fi_epp_snapshot_load(fi_epp* h, const void* buf, uint64_t len) {
+  if (!h || (!buf && len)) return FI_ERR_INVALID;
+  std::lock_guard<std::mutex> lk(h->mu);
+  if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
+  int rc = snapshot_handle_ok(h, "fi_epp_snapshot_load");
+  if (rc != FI_OK) return rc;
+  SnapHeader hd;
+  uint64_t pairs = 0;
+  std::string why;
+  if (!snap_check(buf, len, snap_threads(), &hd, &pairs, &why)) return fail(h, FI_ERR_INVALID, why);
+  const uint32_t E = h->cfg.num_endpoints, C = h->cfg.lru_capacity, We = snap_row_words(E);
+  if (hd.block_bytes != h->cfg.block_bytes || hd.max_blocks != h->cfg.max_blocks || hd.lru_capacity != C || hd.num_endpoints != E)
+    return fail(h, FI_ERR_INVALID, "snapshot of another configuration (block_bytes, max_blocks, lru_capacity or num_endpoints)");
+  const uint8_t* pay = static_cast<const uint8_t*>(buf) + kSnapHeaderBytes;
+  const SnapLayout l = snap_layout(E, hd.n_nodes, hd.n_lru);
+  uint64_t m0 = kSnapNone, m1 = kSnapNone;
+  if (!snap_markers(pay + l.node_keys, hd.n_nodes, &m0, &m1)) return fail(h, FI_ERR_INVALID, "snapshot repeats a node key");
+  const uint64_t regular = hd.n_nodes - (m0 != kSnapNone) - (m1 != kSnapNone);
+  const uint64_t slots = pool_resized_slots(h->index_slots_given, E, C, regular);
+  if (regular * 10 > slots * 6) return fail(h, FI_ERR_CAPACITY, "snapshot keys above 60% of index_slots: raise index_slots");
+  std::vector<uint32_t> caps(E), lens(E);
+  std::memcpy(caps.data(), pay + l.caps, 4ull * E);
+  std::memcpy(lens.data(), pay + l.lru_len, 4ull * E);
+  std::vector<uint64_t> lru_off(E + 1, 0);
+  for (uint32_t e = 0; e < E; ++e) lru_off[e + 1] = lru_off[e] + lens[e];
+
+  rc = update_begin(h);
+  if (rc != FI_OK) return rc;
+  rc = sync_all_streams(h);
+  if (rc != FI_OK) return rc;
+  cudaStream_t si = h->s_index.get();
+  // ---- allocations: nothing of the handle changes before all of them are in place
+  IndexTables nix;
+  rc = alloc_index(h, slots, h->W, nix);
+  if (rc != FI_OK) return rc;
+  std::unique_ptr<DevLruStore> nlru;
+  if (C) {
+    uint32_t TS = 0, L = 0;
+    if (h->dlru) {
+      TS = h->dlru->v.TS;
+      L = h->dlru->v.L;
+    } else {
+      rc = size_dev_lru(h, &TS, &L);
+      if (rc != FI_OK) return rc;
+    }
+    nlru = std::make_unique<DevLruStore>();
+    rc = alloc_dev_lru(h, *nlru, E, TS, L, caps.data());
+    if (rc != FI_OK) {
+      cudaGetLastError();
+      return rc;
+    }
+  }
+  const uint64_t chunk = snap_chunk_nodes(We);
+  DevPtr<uint64_t> d_keys, d_lkeys, d_loff;
+  DevPtr<uint32_t> d_rows, d_llen, d_dup;
+  DevPtr<IndexCounters> d_sctr;
+  cudaError_t e = cuda_alloc(d_dup, 2);
+  if (e == cudaSuccess) e = cuda_alloc(d_sctr, 1);
+  if (e == cudaSuccess && hd.n_nodes) e = cuda_alloc(d_keys, std::min(chunk, hd.n_nodes));
+  if (e == cudaSuccess && hd.n_nodes) e = cuda_alloc(d_rows, std::min(chunk, hd.n_nodes) * We);
+  if (e == cudaSuccess && hd.n_lru) e = cuda_alloc(d_lkeys, hd.n_lru);
+  if (e == cudaSuccess && C) e = cuda_alloc(d_loff, E);
+  if (e == cudaSuccess && C) e = cuda_alloc(d_llen, E);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(h, e == cudaErrorMemoryAllocation ? FI_ERR_NOMEM : FI_ERR_CUDA, std::string("snapshot staging: ") + cudaGetErrorString(e));
+  }
+  SnapStager st;
+  rc = snap_stager(h, st);
+  if (rc != FI_OK) return rc;
+  FI_CUDA(cudaMemsetAsync(d_dup.get(), 0, 2 * sizeof(uint32_t), si));
+  FI_CUDA(cudaMemsetAsync(d_sctr.get(), 0, sizeof(IndexCounters), si));
+
+  // ---- build: the LRUs, then the nodes in blob order
+  if (nlru) {
+    rc = snap_h2d(h, st, d_lkeys.get(), pay + l.lru_keys, 8 * hd.n_lru);
+    if (rc != FI_OK) return rc;
+    // (pageable sources: the copies have taken the data when cudaMemcpyAsync returns)
+    FI_CUDA(cudaMemcpyAsync(d_loff.get(), lru_off.data(), (size_t)E * sizeof(uint64_t), cudaMemcpyHostToDevice, si));
+    FI_CUDA(cudaMemcpyAsync(d_llen.get(), lens.data(), (size_t)E * sizeof(uint32_t), cudaMemcpyHostToDevice, si));
+    LaunchScope ls(h, si, K_INDEX);
+    FI_CUDA(launch_lru_load(nlru->v, d_lkeys.get(), d_loff.get(), d_llen.get(), d_dup.get(), si));
+  }
+  for (uint64_t g0 = 0; g0 < hd.n_nodes; g0 += chunk) {
+    const uint64_t m = std::min(chunk, hd.n_nodes - g0);
+    // (the staging is rewritten only behind the previous chunk's import: all of it runs on s_index)
+    rc = snap_h2d(h, st, d_keys.get(), pay + l.node_keys + 8 * g0, 8 * m);
+    if (rc == FI_OK) rc = snap_h2d(h, st, d_rows.get(), pay + l.node_rows + 4ull * We * g0, 4ull * We * m);
+    if (rc != FI_OK) return rc;
+    LaunchScope ls(h, si, K_INDEX);
+    FI_CUDA(launch_index_snap_import(nix.v, d_sctr.get(), d_keys.get(), d_rows.get(), m, g0, m0, m1, We, d_dup.get(), si));
+  }
+  // ---- check
+  uint32_t dup = 0, lru_err = 0;
+  IndexCounters sctr;
+  FI_CUDA(cudaMemcpyAsync(&dup, d_dup.get(), sizeof(dup), cudaMemcpyDeviceToHost, si));
+  FI_CUDA(cudaMemcpyAsync(&sctr, d_sctr.get(), sizeof(sctr), cudaMemcpyDeviceToHost, si));
+  if (nlru) FI_CUDA(cudaMemcpyAsync(&lru_err, nlru->v.error, sizeof(lru_err), cudaMemcpyDeviceToHost, si));
+  FI_CUDA(cudaStreamSynchronize(si));
+  if (dup) return fail(h, FI_ERR_INVALID, "snapshot repeats a key in the index or in an LRU");
+  if (sctr.overflow) return fail(h, FI_ERR_CAPACITY, "snapshot keys do not fit the index");
+  if (lru_err) return fail(h, FI_ERR_STATE, "device LRU: invariant " + std::to_string(lru_err) + " broken while loading");
+
+  // ---- swap in the loaded state (the old tables stay allocated until the end of the call)
+  const IndexCounters fresh{regular, 0, 0, 0};
+  FI_CUDA(cudaMemcpyAsync(h->d_ctr.get(), &fresh, sizeof(fresh), cudaMemcpyHostToDevice, si));
+  if (nlru && h->dlru) {  // the statistics keep counting
+    FI_CUDA(cudaMemcpyAsync(nlru->ctr.get(), h->dlru->ctr.get(), 8 * sizeof(unsigned long long), cudaMemcpyDeviceToDevice, si));
+    *nlru->stat = *h->dlru->stat;
+  }
+  if (nlru) FI_CUDA(cudaEventRecord(nlru->ev.get(), si));
+  std::swap(h->ix, nix);
+  h->ix_spare.reset();  // a later rebuild allocates it in the new size
+  h->cfg.index_slots = h->ix.v.C;
+  h->ctr_used_known = regular;
+  h->ctr_unchecked = 0;
+  if (nlru) {
+    std::swap(h->dlru, nlru);
+    h->lru_caps = caps;
+    for (uint32_t x = 0; x < E; ++x) h->lrus[x].shrink(caps[x], [](uint64_t) {});  // (empty: they only take the limit)
+  }
+  rc = update_end(h);
+  if (rc != FI_OK) return rc;
+  FI_CUDA(cudaStreamSynchronize(si));
+  return FI_OK;
+}
+
+int fi_epp_snapshot_info(const void* buf, uint64_t len, struct fi_epp_snapshot_info* out) {
+  if ((!buf && len) || !out) return FI_ERR_INVALID;
+  SnapHeader hd;
+  uint64_t pairs = 0;
+  std::string why;
+  if (!snap_check(buf, len, snap_threads(), &hd, &pairs, &why)) return FI_ERR_INVALID;
+  out->block_bytes = hd.block_bytes;
+  out->max_blocks = hd.max_blocks;
+  out->lru_capacity = hd.lru_capacity;
+  out->num_endpoints = hd.num_endpoints;
+  out->n_nodes = hd.n_nodes;
+  out->n_lru = hd.n_lru;
+  out->pairs = pairs;
+  out->bytes = len;
   return FI_OK;
 }
 

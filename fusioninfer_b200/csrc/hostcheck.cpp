@@ -14,6 +14,7 @@
 #include "lru_batch.h"
 #include "lru_plan.h"
 #include "pool_shape.h"
+#include "snapshot_format.h"
 #include "tiebreak.cuh"
 #include "xxh64.cuh"
 
@@ -470,5 +471,17 @@ uint64_t fihc_pool_resized_slots(uint64_t pinned, uint32_t num_endpoints, uint32
 int fihc_pool_needs_rebuild(uint32_t W, uint64_t slots, uint32_t new_W, uint64_t new_slots) {
   return fi::pool_needs_rebuild(W, slots, new_W, new_slots) ? 1 : 0;
 }
+
+// the snapshot format (snapshot_format.h): its checksum and its structural check (0: well-formed; *pairs = popcount)
+uint64_t fihc_snap_xxh64(const uint8_t* p, uint64_t len) { return fi::snap_xxh64(p, len); }
+uint64_t fihc_snap_checksum(const uint8_t* blob, uint64_t len, unsigned threads) {
+  return fi::snap_checksum(blob, blob + fi::kSnapHeaderBytes, len - fi::kSnapHeaderBytes, threads);
+}
+int fihc_snap_check(const uint8_t* blob, uint64_t len, unsigned threads, uint64_t* pairs) {
+  fi::SnapHeader hd;
+  std::string why;
+  return fi::snap_check(blob, len, threads, &hd, pairs, &why) ? 0 : -1;
+}
+int fihc_snap_markers(const uint8_t* keys, uint64_t n, uint64_t* pos) { return fi::snap_markers(keys, n, pos, pos + 1) ? 0 : -1; }
 
 }  // extern "C"

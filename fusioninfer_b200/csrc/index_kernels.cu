@@ -401,6 +401,97 @@ __global__ void __launch_bounds__(256) index_contains_kernel(IndexView ix, const
   }
 }
 
+// ---- snapshots (fi_epp_snapshot_save / fi_epp_snapshot_load, docs/SPEC.md S.2d) -----------------------------------
+// Export: an order-preserving compaction of the sweep items (the regular nodes [0, n) in order, then the marker nodes
+// C, C+1: sweep_node) that hold a key — klog != 0 for a regular node, rmask != 0 for a marker.  Items come in tiles of
+// kSnapTile, one CTA per tile: a count pass, a prefix sum on the host, then the export of a range of tiles into the
+// staging buffers, each tile's live nodes at its offset.
+constexpr uint32_t kSnapTile = 1024;
+
+__device__ __forceinline__ bool snap_live(const IndexView& ix, uint32_t node) {
+  return node < ix.C ? ix.klog[node] != 0 : ix.rmask[node] != 0;
+}
+
+// this thread's rank among the flagged threads of the CTA (kSnapTile threads)
+__device__ __forceinline__ uint32_t snap_rank(bool flag) {
+  __shared__ uint32_t s_w[kSnapTile / 32];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const unsigned m = __ballot_sync(0xFFFFFFFFu, flag);
+  if (lane == 0) s_w[warp] = __popc(m);
+  __syncthreads();
+  if (warp == 0) {
+    const uint32_t c = s_w[lane];
+    uint32_t inc = c;
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint32_t t = __shfl_up_sync(0xFFFFFFFFu, inc, d);
+      if ((int)lane >= d) inc += t;
+    }
+    s_w[lane] = inc - c;
+  }
+  __syncthreads();
+  return s_w[warp] + __popc(m & ((1u << lane) - 1u));
+}
+
+__global__ void __launch_bounds__(kSnapTile) index_snap_count_kernel(IndexView ix, uint64_t n, uint32_t* tile_live) {
+  const uint64_t t = (uint64_t)blockIdx.x * kSnapTile + threadIdx.x;
+  const bool live = t < n + 2 && snap_live(ix, sweep_node(ix, t, n));
+  const int c = __syncthreads_count(live);
+  if (threadIdx.x == 0) tile_live[blockIdx.x] = (uint32_t)c;
+}
+
+// tiles [t0, t0 + gridDim.x): the live nodes' keys and their rows narrowed to We words, at tile_off[t] - base
+__global__ void __launch_bounds__(kSnapTile) index_snap_export_kernel(IndexView ix, uint64_t n, uint32_t t0,
+                                                                      const uint64_t* __restrict__ tile_off, uint64_t base,
+                                                                      uint32_t We, uint64_t* keys, uint32_t* rows) {
+  const uint32_t tile = t0 + blockIdx.x;
+  const uint64_t t = (uint64_t)tile * kSnapTile + threadIdx.x;
+  const uint32_t node = t < n + 2 ? sweep_node(ix, t, n) : 0u;
+  const bool live = t < n + 2 && snap_live(ix, node);
+  const uint32_t r = snap_rank(live);
+  if (!live) return;
+  const uint64_t d = tile_off[tile] - base + r;
+  keys[d] = node < ix.C ? ix.klog[node] : node == ix.C ? KEY_EMPTY : KEY_TOMB;
+  const uint32_t* src = ix.rows + ((uint64_t)node << ix.logW);
+  for (uint32_t w = 0; w < We; ++w) rows[d * We + w] = src[w];
+}
+
+// Import: nodes [g0, g0 + n) of a snapshot (keys and rows of We words, in staging) into fresh tables, like a rebuild
+// fed from the blob: a regular key gets node g minus the markers before it (m0, m1: the blob positions of the keys 0
+// and ~0, or ~0), so the regular nodes are numbered consecutively in blob order; the markers take their fixed nodes.
+// A key that is already there (a duplicate in the blob) sets *dup.
+__global__ void __launch_bounds__(256) index_snap_import_kernel(IndexView ix, IndexCounters* ctr, const uint64_t* __restrict__ keys,
+                                                                const uint32_t* __restrict__ rows, uint64_t n, uint64_t g0,
+                                                                uint64_t m0, uint64_t m1, uint32_t We, uint32_t* dup) {
+  for (uint64_t i = blockIdx.x * (uint64_t)blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint64_t key = keys[i], g = g0 + i;
+    uint32_t node;
+    if (key_is_special(key)) {
+      node = (uint32_t)(ix.C + (key == KEY_TOMB ? 1 : 0));
+      if (atomicExch(ix.rmask + node, 1u)) atomicExch(dup, 1u);
+    } else {
+      node = (uint32_t)(g - (g > m0 ? 1 : 0) - (g > m1 ? 1 : 0));
+      bool claimed = false;
+      const uint32_t slot = table_find_or_claim(ix, ctr, key, &claimed);
+      if (!claimed) {  // (a full table sets ctr->overflow instead)
+        if (slot != SLOT_MISS) atomicExch(dup, 1u);
+        continue;
+      }
+      ix.klog[node] = key;
+      ix.node_of[slot] = node;
+      ix.rmask[node] = 1u;
+    }
+    const uint32_t* src = rows + i * We;
+    uint32_t* dst = ix.rows + ((uint64_t)node << ix.logW);
+    uint32_t c = 0;
+    for (uint32_t w = 0; w < We; ++w) {
+      dst[w] = src[w];
+      c += __popc(src[w]);
+    }
+    ix.cnt[node] = c;
+  }
+}
+
 inline unsigned grid_for(uint64_t n) {
   uint64_t g = (n + 255) / 256;
   if (g > 132ull * 16) g = 132ull * 16;  // 16 CTAs per SM of an H100
@@ -467,6 +558,27 @@ cudaError_t launch_index_contains(IndexView ix, const fi_index_op* q, uint64_t n
                                   uint32_t ep_count, uint8_t* out, cudaStream_t s) {
   if (n == 0) return cudaSuccess;
   index_contains_kernel<<<grid_for(n), 256, 0, s>>>(ix, q, n, ep_begin, ep_count, out);
+  return cudaGetLastError();
+}
+
+uint32_t index_snap_tiles(uint64_t n) { return (uint32_t)((n + 2 + kSnapTile - 1) / kSnapTile); }
+
+cudaError_t launch_index_snap_count(IndexView ix, uint64_t n, uint32_t* tile_live, cudaStream_t s) {
+  index_snap_count_kernel<<<index_snap_tiles(n), kSnapTile, 0, s>>>(ix, n, tile_live);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_index_snap_export(IndexView ix, uint64_t n, uint32_t t0, uint32_t t1, const uint64_t* tile_off, uint64_t base,
+                                     uint32_t We, uint64_t* keys, uint32_t* rows, cudaStream_t s) {
+  if (t1 <= t0) return cudaSuccess;
+  index_snap_export_kernel<<<t1 - t0, kSnapTile, 0, s>>>(ix, n, t0, tile_off, base, We, keys, rows);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_index_snap_import(IndexView ix, IndexCounters* ctr, const uint64_t* keys, const uint32_t* rows, uint64_t n,
+                                     uint64_t g0, uint64_t m0, uint64_t m1, uint32_t We, uint32_t* dup, cudaStream_t s) {
+  if (n == 0) return cudaSuccess;
+  index_snap_import_kernel<<<grid_for(n), 256, 0, s>>>(ix, ctr, keys, rows, n, g0, m0, m1, We, dup);
   return cudaGetLastError();
 }
 

@@ -477,8 +477,13 @@ __global__ void __launch_bounds__(256) lru_reset_kernel(DevLru lru, const uint32
   if (blockIdx.x == 0 && threadIdx.x == 0) lru.head[e] = lru.tail[e] = lru.count[e] = lru.used[e] = 0;
 }
 
-// diagnostics (tests): the live keys of endpoint e, oldest first
-__global__ void __launch_bounds__(256) lru_dump_kernel(DevLru lru, uint32_t e, uint64_t* out, uint32_t* n_out) {
+// the live keys of endpoints e0 + blockIdx.x, oldest first, one CTA each: to out + off[blockIdx.x] (off == null: out),
+// and their number to n_out[blockIdx.x] (fi_epp_lru_dump: one endpoint; a snapshot: all of them)
+__global__ void __launch_bounds__(256) lru_dump_kernel(DevLru lru, uint32_t e0, const uint64_t* __restrict__ off, uint64_t* out,
+                                                       uint32_t* n_out) {
+  const uint32_t e = e0 + blockIdx.x;
+  if (off) out += off[blockIdx.x];
+  n_out += blockIdx.x;
   const LruSlot* tab = lru.slots + (uint64_t)e * (lru.TS + 2);
   const uint64_t* log = lru.log + (uint64_t)e * lru.L;
   const uint32_t head = lru.head[e];
@@ -498,6 +503,37 @@ __global__ void __launch_bounds__(256) lru_dump_kernel(DevLru lru, uint32_t e, u
     d += tot;
   }
   if (threadIdx.x == 0) *n_out = d;
+}
+
+// ---- load: every endpoint's LRU from a snapshot (fi_epp_snapshot_load), one CTA per endpoint --------------------
+// The store is fresh (alloc_dev_lru: tables zeroed, head = tail = count = used = 0).  Endpoint e's len[e] keys, LRU
+// first, at keys + off[e], become a compacted log (tail 0, head = count = len) and its table is built from the log as
+// maintain's step 2 does, the two special slots included (they are free here).  A key that repeats sets *dup.
+__global__ void __launch_bounds__(kWideCta) lru_load_kernel(DevLru lru, const uint64_t* __restrict__ keys, const uint64_t* __restrict__ off,
+                                                       const uint32_t* __restrict__ len, uint32_t* dup) {
+  const uint32_t e = blockIdx.x, n = len[e];
+  const uint64_t* src = keys + off[e];
+  LruSlot* tab = lru.slots + (uint64_t)e * (lru.TS + 2);
+  uint64_t* log = lru.log + (uint64_t)e * lru.L;
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const uint64_t key = src[i];
+    log[i] = key;
+    bool ins = false;
+    const uint32_t slot = lru_find_or_insert(tab, lru.TS, key, lru.used + e, lru.TS, &ins);
+    if (slot == LRU_MISS) {
+      atomicExch(lru.error, 4u);
+      continue;
+    }
+    if (!ins) {
+      atomicExch(dup, 1u);
+      continue;
+    }
+    tab[slot].posp1 = i + 1;
+  }
+  if (threadIdx.x == 0) {
+    lru.head[e] = lru.count[e] = n;
+    lru.tail[e] = 0;
+  }
 }
 
 }  // namespace
@@ -549,7 +585,16 @@ cudaError_t launch_lru_reset(const DevLru& lru, const uint32_t* eps, uint32_t n,
   return cudaGetLastError();
 }
 cudaError_t launch_lru_dump(const DevLru& lru, uint32_t e, uint64_t* out, uint32_t* n_out, cudaStream_t s) {
-  lru_dump_kernel<<<1, 256, 0, s>>>(lru, e, out, n_out);
+  lru_dump_kernel<<<1, 256, 0, s>>>(lru, e, nullptr, out, n_out);
+  return cudaGetLastError();
+}
+cudaError_t launch_lru_dump_all(const DevLru& lru, const uint64_t* off, uint64_t* out, uint32_t* n_out, cudaStream_t s) {
+  lru_dump_kernel<<<lru.EL, 256, 0, s>>>(lru, 0, off, out, n_out);
+  return cudaGetLastError();
+}
+cudaError_t launch_lru_load(const DevLru& lru, const uint64_t* keys, const uint64_t* off, const uint32_t* len, uint32_t* dup,
+                            cudaStream_t s) {
+  lru_load_kernel<<<lru.EL, kWideCta, 0, s>>>(lru, keys, off, len, dup);
   return cudaGetLastError();
 }
 

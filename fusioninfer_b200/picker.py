@@ -141,6 +141,18 @@ def _ptr(a: Optional[np.ndarray]):
     return None if a is None else a.ctypes.data_as(C.c_void_p)
 
 
+def snapshot_info(buf) -> abi.fi_epp_snapshot_info:
+    """Check a snapshot blob's structure (everything but key distinctness) and return its header; no handle, no GPU.
+    ValueError if the blob is not well-formed."""
+    buf = np.ascontiguousarray(np.frombuffer(buf, dtype=np.uint8) if isinstance(buf, (bytes, bytearray)) else buf,
+                               dtype=np.uint8)
+    out = abi.fi_epp_snapshot_info()
+    rc = abi.load().fi_epp_snapshot_info(_ptr(buf), len(buf), C.byref(out))
+    if rc != abi.FI_OK:
+        raise ValueError("not a well-formed snapshot")
+    return out
+
+
 class EndpointPicker:
     """One handle = one GPU = one endpoint-range shard of the pool."""
 
@@ -215,6 +227,23 @@ class EndpointPicker:
         self.cfg = abi.fi_epp_config.from_buffer_copy(self.cfg)
         self.cfg.num_endpoints = self.cfg.endpoint_count = int(num_endpoints)
         return out.value if count else None
+
+    def save_snapshot(self) -> np.ndarray:
+        """The handle's learned state (docs/SPEC.md S.2d: the index's pairs, every endpoint's LRU and its capacity) as
+        a snapshot blob.  Blocks until every earlier call is applied; the handle is not changed."""
+        n = C.c_uint64(0)
+        self._check(self._lib.fi_epp_snapshot_save(self._h, None, 0, C.byref(n)), "fi_epp_snapshot_save")
+        buf = np.empty(n.value, dtype=np.uint8)
+        self._check(self._lib.fi_epp_snapshot_save(self._h, _ptr(buf), len(buf), C.byref(n)), "fi_epp_snapshot_save")
+        return buf
+
+    def load_snapshot(self, buf) -> None:
+        """Replace the index, the LRUs and their capacities with a snapshot's: afterwards the handle behaves like the
+        one that saved it, except for its own endpoint states and adapters (re-send them).  Blocks like resize_pool;
+        a failing load changes nothing."""
+        buf = np.ascontiguousarray(np.frombuffer(buf, dtype=np.uint8) if isinstance(buf, (bytes, bytearray)) else buf,
+                                   dtype=np.uint8)
+        self._check(self._lib.fi_epp_snapshot_load(self._h, _ptr(buf), len(buf)), "fi_epp_snapshot_load")
 
     def set_lru_capacities(self, endpoints, capacities, want_evicted: bool = False) -> Optional[int]:
         """Per-endpoint LRU capacities (upstream autoTune: a pod's LRU sized from its KV-cache block count).

@@ -312,6 +312,49 @@ int fi_epp_index_remove_endpoints(fi_epp* h, const uint32_t* endpoints, uint32_t
  * and the new tables are both held while the call runs). */
 int fi_epp_resize_pool(fi_epp* h, uint32_t num_endpoints, uint64_t* pairs_removed);
 
+/* Index snapshots (docs/SPEC.md S.2d): what a handle has learned — every (endpoint, hash) pair of the index, whatever
+ * put it there, every endpoint's LRU in recency order, and every endpoint's LRU capacity — as a device-independent byte
+ * blob in host memory, so that a restarted picker (or a new replica) starts warm.  Endpoint states and adapters are
+ * not part of it: the caller re-sends them after a load, as after create.  The blob format (version 1, little-endian)
+ * is part of the ABI: fusioninfer_b200/csrc/snapshot_format.h and S.2d lay it out.  A blob of another format version
+ * is refused, never guessed at.  (The header's struct has no typedef: its tag names it, and the plain name is the
+ * function fi_epp_snapshot_info.) */
+struct fi_epp_snapshot_info {
+  uint32_t block_bytes, max_blocks, lru_capacity, num_endpoints;
+  uint64_t n_nodes; /* keys in the index */
+  uint64_t n_lru;   /* LRU entries, summed over the endpoints */
+  uint64_t pairs;   /* (endpoint, hash) pairs: the total popcount of the rows */
+  uint64_t bytes;   /* 64 + payload bytes */
+};
+
+/* Write h's learned state to buf.  buf == NULL: *bytes = the size the snapshot needs, FI_OK.  cap < that size:
+ * FI_ERR_CAPACITY, *bytes = the size, nothing written.  Blocking: every call issued before it (staged ops, Adds,
+ * removals, capacity changes, fi_epp_pick_submit batches in flight) is applied first; the handle is not changed.  The
+ * index's live nodes are written in node order (insertion order), so a load numbers a cached prefix's nodes
+ * consecutively again.  buf is ordinary pageable memory of any size; it is filled through bounded pinned staging.
+ * FI_ERR_STATE on a sharded pool, on a handle over part of the pool, or on a handle the host LRU serves. */
+int fi_epp_snapshot_save(fi_epp* h, void* buf, uint64_t cap, uint64_t* bytes);
+
+/* Replace h's index, LRUs and LRU capacities with the snapshot's.  h must have the block_bytes, max_blocks,
+ * lru_capacity and num_endpoints of the handle that saved it; its index_slots, LRU table size and device may differ.
+ * Afterwards h behaves exactly like the saved handle at the moment of the save, for every later call sequence, except
+ * that h keeps its own endpoint states and adapters, and its statistics (ops_applied, rebuilds, fi_epp_lru_counters,
+ * fi_epp_get_stats) keep counting; fi_epp_index_stats' used and lru_entries describe the loaded state, without
+ * tombstones.  Before the first Add, the call allocates the device LRU as the first Add would.
+ * Blocking, ordered like fi_epp_resize_pool: every call issued before it completes against the old state (staged ops and
+ * fi_epp_pick_submit batches in flight included), every later call sees the loaded state.  Tickets stay valid:
+ * fi_epp_index_add_submitted of an earlier ticket adds its chains to the loaded state.
+ * Errors change nothing (new tables are built and checked, then swapped in): FI_ERR_INVALID for a blob that is not
+ * well-formed (S.2d; duplicate keys are found on the device while building) or whose block_bytes, max_blocks,
+ * lru_capacity or num_endpoints differ from h's; FI_ERR_CAPACITY if the keys exceed 60 % of an index_slots given at
+ * create (with index_slots 0 the index grows as fi_epp_resize_pool grows it); FI_ERR_STATE as for
+ * fi_epp_snapshot_save; FI_ERR_NOMEM if the old and new tables do not fit together. */
+int fi_epp_snapshot_load(fi_epp* h, const void* buf, uint64_t len);
+
+/* No handle, no device: check a blob's structure (everything S.2d asks except that keys are distinct) and read its
+ * header into *out.  FI_ERR_INVALID if it is not well-formed. */
+int fi_epp_snapshot_info(const void* buf, uint64_t len, struct fi_epp_snapshot_info* out);
+
 /* Per-endpoint LRU capacities (docs/SPEC.md S.2b; upstream's autoTune sizes a pod's LRU from the KV-cache blocks the
  * pod reports).  Every endpoint's LRU capacity starts at lru_capacity; this sets it to capacities[i] for endpoints[i]
  * (0 = lru_capacity; the last entry of an endpoint listed twice wins).  An LRU that holds more keys than its new
