@@ -141,7 +141,9 @@ typedef struct fi_epp_config {
   uint32_t max_blocks;  /* maxPrefixBlocksToMatch (strategy.go:58,148) */
   uint32_t lru_capacity; /* lruCapacityPerServer (strategy.go:59,149); 0: no LRU (fi_epp_index_add_chain* fail) */
   uint32_t num_endpoints;  /* global pool size E */
-  uint32_t endpoint_begin; /* this handle's shard [begin, begin+count) of the pool */
+  uint32_t endpoint_begin; /* this handle's shard [begin, begin+count) of the pool.  Without fi_epp_comm_init such a
+                            * handle indexes, learns and picks only its own endpoints, with the queue scorer's min /
+                            * max and the tie rotation of the whole pool (docs/SPEC.md S.2e) */
   uint32_t endpoint_count;
   uint32_t match_mode; /* fi_match_mode */
   uint32_t max_batch;  /* largest R accepted by one pick/hash call */

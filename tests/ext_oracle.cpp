@@ -4,7 +4,10 @@
 // hashing, index, eligibility, scoring and tie-rotation pieces:
 //   * the ranked pick (docs/SPEC.md S.6a), over each request's candidate subset (S.5a) when one is given;
 //   * per-endpoint LRU capacities (S.2b): a capacity c_e per endpoint, an indexer.Add that evicts against it, the
-//     resize of fi_epp_set_lru_capacities, and the LRU's content for comparisons.
+//     resize of fi_epp_set_lru_capacities, and the LRU's content for comparisons;
+//   * the shard view (S.2e): a handle over endpoints [lo, lo + cnt) of the pool.  Its Adds and capacity changes skip
+//     the other endpoints, and its ranked pick ranks only its own endpoints, with the queue scorer's min / max still
+//     taken over the whole pool.  (Index ops addressed elsewhere are dropped by the wrapper, tests/ext_oracle.py.)
 // The handle is the oracle's own plus the capacities, so every epo_* function of the oracle works on it too.  The
 // oracle itself is left as it is: its single pick stays the yardstick of fi_epp_pick_batch.
 #include "../oracle/epp_oracle.cpp"
@@ -13,6 +16,8 @@ namespace {
 
 struct ExtOracle : Oracle {
   std::vector<uint32_t> cap;  // [num_endpoints] c_e, lru_capacity until set
+  uint32_t lo = 0, cnt = 0;   // the shard [lo, lo + cnt): the whole pool unless epx_set_shard narrowed it
+  bool mine(uint32_t e) const { return e - lo < cnt; }
 };
 
 inline ExtOracle* ext_of(void* h) { return static_cast<ExtOracle*>(static_cast<Oracle*>(h)); }
@@ -26,12 +31,13 @@ struct Ranked {
 
 inline bool in_subset(const uint32_t* row, uint32_t e) { return !row || ((row[e >> 5] >> (e & 31)) & 1u); }
 
-// One request: hash → match (A.3) over the WHOLE pool, exactly as pick_one does (the walk stops at the first block
-// no endpoint of the pool holds, whatever the subset).  Then per profile: the eligible endpoints of the subset (of the
-// pool when row is NULL), the queue scorer's min / max over them (S.4 per request; make_ctx's set without a row),
-// their totals (A.4), partially sorted by (total desc, rotation distance asc), the order whose first element is
-// pick_one's pick, and the PD rule on the decode profile's entry 0 (A.6) applied to the prefill profile's whole list.
-void rank_one(const Oracle& o, const uint8_t* prompt, uint64_t len, uint64_t h0, uint64_t adapter, const uint32_t* row,
+// One request: hash → match (A.3) over the WHOLE index, exactly as pick_one does (the walk stops at the first block
+// no endpoint of the index holds, whatever the subset; a shard view's index holds its own endpoints only).  Then per
+// profile: the eligible endpoints of the subset (of the pool when row is NULL), the queue scorer's min / max over them
+// (S.4 per request; make_ctx's set without a row), the totals (A.4) of those inside the shard, partially sorted by
+// (total desc, rotation distance asc), the order whose first element is pick_one's pick, and the PD rule on the
+// decode profile's entry 0 (A.6) applied to the prefill profile's whole list.
+void rank_one(const ExtOracle& o, const uint8_t* prompt, uint64_t len, uint64_t h0, uint64_t adapter, const uint32_t* row,
               uint32_t r, uint32_t k, fi_pick* out, Scratch& sc, std::vector<Ranked>& cand) {
   const fi_epp_config& cfg = o.cfg;
   const uint32_t E = cfg.num_endpoints;
@@ -78,7 +84,7 @@ void rank_one(const Oracle& o, const uint8_t* prompt, uint64_t len, uint64_t h0,
       ctx.min_q = ctx.any ? std::min(ctx.min_q, q) : q;
       ctx.max_q = ctx.any ? std::max(ctx.max_q, q) : q;
       ctx.any = true;
-      cand.push_back({0.0, tie_distance(e, start, E), e, sc.match[e]});
+      if (o.mine(e)) cand.push_back({0.0, tie_distance(e, start, E), e, sc.match[e]});
     }
     for (Ranked& c : cand) c.total = total_score(prof, ctx, o.eps[c.e], c.match, n, adapter);
     const size_t kk = std::min<size_t>(k, cand.size());
@@ -145,10 +151,21 @@ void* epx_create(const fi_epp_config* cfg) {
   o->eps.assign(cfg->num_endpoints, EpState{});
   if (cfg->lru_capacity) o->lrus.resize(cfg->num_endpoints);
   o->cap.assign(cfg->num_endpoints, cfg->lru_capacity);
+  o->cnt = cfg->num_endpoints;
   return static_cast<Oracle*>(o);
 }
 
 void epx_destroy(void* h) { delete ext_of(h); }
+
+// Narrow a fresh handle to the shard view over endpoints [begin, begin + count) (docs/SPEC.md S.2e).  FI_ERR_INVALID
+// for a range that is empty or leaves the pool.
+int epx_set_shard(void* h, uint32_t begin, uint32_t count) {
+  ExtOracle* o = ext_of(h);
+  if (count == 0 || (uint64_t)begin + count > o->cfg.num_endpoints) return FI_ERR_INVALID;
+  o->lo = begin;
+  o->cnt = count;
+  return FI_OK;
+}
 
 // subsets: R rows of ceil(num_endpoints / 32) words (bit e of row r: e is a candidate of request r), or NULL (every
 // request ranks the whole pool).  out: R*n_profiles*k picks, out[(r*n_profiles + p)*k + j] = rank j of profile p;
@@ -156,7 +173,7 @@ void epx_destroy(void* h) { delete ext_of(h); }
 int epx_pick_batch_ranked(void* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0,
                           const uint64_t* adapters, const uint32_t* subsets, uint32_t R, uint32_t k, fi_pick* out) {
   if (!h || k == 0) return FI_ERR_INVALID;
-  const Oracle* o = (const Oracle*)h;
+  const ExtOracle* o = ext_of(h);
   const uint32_t P = o->cfg.n_profiles;
   const size_t pitch = (o->cfg.num_endpoints + 31) / 32;
   Scratch sc;
@@ -168,11 +185,13 @@ int epx_pick_batch_ranked(void* h, const uint8_t* prompts, const uint64_t* offse
 }
 
 // upstream indexer.Add(hashes, pod) against the pod's own capacity (S.2 with c_e, S.2b): epo_index_add_chain with
-// lru_capacity replaced by c_e, so with every c_e at lru_capacity it makes the same changes step for step
+// lru_capacity replaced by c_e, so with every c_e at lru_capacity it makes the same changes step for step.  An Add
+// to an endpoint outside the shard changes nothing.
 int epx_add_chain(void* h, uint32_t endpoint, const uint64_t* hashes, uint32_t n) {
   ExtOracle* o = ext_of(h);
   if (!o->cfg.lru_capacity) return FI_ERR_STATE;
   if (endpoint >= o->cfg.num_endpoints) return FI_ERR_INVALID;
+  if (!o->mine(endpoint)) return FI_OK;
   PodLRU& l = o->lrus[endpoint];
   for (uint32_t i = 0; i < n; ++i) {
     const uint64_t k = hashes[i];
@@ -209,7 +228,8 @@ int epx_add_chains(void* h, const uint32_t* endpoints, const uint64_t* chains, u
 // fi_epp_set_lru_capacities (S.2b): c_e = capacities[i] (0: lru_capacity; the last entry of an endpoint wins), then
 // each listed endpoint, in order of first appearance, evicts down to c_e.  The evicted pairs are written to
 // ev_hash / ev_ep (at most ev_cap), oldest first per endpoint; *n_evicted = how many.  FI_ERR_INVALID (nothing
-// changes) for an endpoint >= num_endpoints, a capacity above lru_capacity or one in (0, max_blocks).
+// changes) for an endpoint >= num_endpoints, a capacity above lru_capacity or one in (0, max_blocks).  Endpoints
+// outside the shard are checked, then ignored.
 int epx_set_lru_capacities(void* h, const uint32_t* endpoints, const uint32_t* capacities, uint32_t n,
                            uint64_t* ev_hash, uint32_t* ev_ep, uint64_t ev_cap, uint64_t* n_evicted) {
   ExtOracle* o = ext_of(h);
@@ -222,6 +242,7 @@ int epx_set_lru_capacities(void* h, const uint32_t* endpoints, const uint32_t* c
   std::vector<uint32_t> order;
   std::vector<uint8_t> listed(o->cfg.num_endpoints, 0);
   for (uint32_t i = 0; i < n; ++i) {
+    if (!o->mine(endpoints[i])) continue;
     o->cap[endpoints[i]] = capacities[i] ? capacities[i] : C;
     if (!listed[endpoints[i]]) {
       listed[endpoints[i]] = 1;

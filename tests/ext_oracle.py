@@ -4,7 +4,12 @@ infrastructure only.  ExtOracle is the oracle of oracle/epp_oracle.py with:
     rotation), the first k of them, over each request's candidate subset (S.5a) with pick_batch_subset;
   * per-endpoint LRU capacities (S.2b): its Adds evict against each endpoint's own capacity, set_lru_capacities
     resizes, lru(e) dumps an endpoint's LRU.  remove_endpoints (S.2a) CLEARs every hash ever aimed at an endpoint, so
-    the handle has to be created with track_removal=True to use it."""
+    the handle has to be created with track_removal=True to use it;
+  * the shard view (S.2e), ExtOracle(cfg, shard=(b, c)): what a single-rank handle created with endpoint_begin = b,
+    endpoint_count = c computes.  Its index and LRUs hold only pairs of endpoints in [b, b + c): ops, Adds, capacity
+    changes and removals addressed elsewhere are dropped.  Its picks (single, LoRA, ranked) rank only the shard's
+    eligible endpoints, with the queue scorer's min / max over the eligible endpoints of the whole pool, the tie
+    rotation of the whole pool, and the PD rule on the shard's own decode pick."""
 from __future__ import annotations
 
 import ctypes as C
@@ -38,6 +43,7 @@ def load() -> C.CDLL:
     for name, res, args in (
             ("epx_create", _P, [C.POINTER(abi.fi_epp_config)]),
             ("epx_destroy", None, [_P]),
+            ("epx_set_shard", C.c_int, [_P, C.c_uint32, C.c_uint32]),
             ("epx_pick_batch_ranked", C.c_int, [_P, _P, _P, _P, _P, _P, C.c_uint32, C.c_uint32, _P]),
             ("epx_add_chain", C.c_int, [_P, C.c_uint32, _P, C.c_uint32]),
             ("epx_add_chains", C.c_int, [_P, _P, _P, C.c_uint32, _P, C.c_uint32]),
@@ -51,7 +57,9 @@ def load() -> C.CDLL:
 
 
 class ExtOracle(epp_oracle.Oracle):
-    def __init__(self, cfg: abi.fi_epp_config, track_removal: bool = False):
+    shard = None  # (b, c) on a shard view
+
+    def __init__(self, cfg: abi.fi_epp_config, track_removal: bool = False, shard=None):
         self._lib = load()
         self.cfg = abi.fi_epp_config.from_buffer_copy(cfg)
         self._h = self._lib.epx_create(C.byref(self.cfg))
@@ -62,6 +70,25 @@ class ExtOracle(epp_oracle.Oracle):
         self.E = cfg.num_endpoints
         self.C = cfg.lru_capacity
         self._seen = [set() for _ in range(self.E)] if track_removal else None
+        if shard is not None:
+            b, c = int(shard[0]), int(shard[1])
+            if self._lib.epx_set_shard(self._h, b, c) != 0:
+                raise ValueError(f"shard {shard} is not a non-empty range of the {self.E} endpoints")
+            self.shard = (b, c)
+
+    def mine(self, endpoints) -> np.ndarray:
+        """which of the endpoints lie in the shard (all of them without one)"""
+        e = np.asarray(endpoints, dtype=np.int64)
+        if self.shard is None:
+            return np.ones(e.shape, dtype=bool)
+        return (e >= self.shard[0]) & (e < self.shard[0] + self.shard[1])
+
+    # ---- the single pick: on a shard view, rank 0 of the ranked pick -------------------------------------------
+    def pick_batch(self, prompts, offsets, h0, want_chains=False, nthreads=1, adapters=None):
+        if self.shard is None:
+            return super().pick_batch(prompts, offsets, h0, want_chains, nthreads, adapters)
+        picks = np.ascontiguousarray(self.pick_batch_ranked(prompts, offsets, h0, 1, adapters)[:, :, 0])
+        return (picks, self.hash_batch(prompts, offsets, h0)[0]) if want_chains else picks
 
     def close(self):
         if self._h:
@@ -80,6 +107,7 @@ class ExtOracle(epp_oracle.Oracle):
         ad = None if adapters is None else np.ascontiguousarray(np.broadcast_to(np.asarray(adapters, dtype=np.uint64), (R,)))
         sub = None
         if subsets is not None:
+            assert self.shard is None, "a handle over part of the pool takes no subsets"
             sub = np.ascontiguousarray(subsets, dtype=np.uint32)
             assert sub.shape == (R, (self.E + 31) // 32), sub.shape
         rc = self._lib.epx_pick_batch_ranked(self._h, _ptr(prompts), _ptr(offsets), _ptr(h0), _ptr(ad), _ptr(sub), R, k,
@@ -89,11 +117,15 @@ class ExtOracle(epp_oracle.Oracle):
 
     # ---- per-endpoint LRU capacities --------------------------------------------------------------------------------
     def _see(self, e, hashes):
-        if self._seen is not None:
+        if self._seen is not None and self.mine(e):
             self._seen[int(e)].update(int(h) for h in hashes)
 
     def index_apply(self, ops):
         ops = np.ascontiguousarray(ops, dtype=epp_oracle.OP_DTYPE)
+        if self.shard is not None:
+            bad = ops["endpoint"] >= self.E
+            assert not bad.any(), "index op endpoint out of range"
+            ops = np.ascontiguousarray(ops[self.mine(ops["endpoint"])])
         for e in np.unique(ops["endpoint"]):
             self._see(e, ops["hash"][ops["endpoint"] == e])
         super().index_apply(ops)

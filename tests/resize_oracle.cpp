@@ -22,6 +22,7 @@ int epx_resize(void* h, uint32_t num_endpoints) {
   o->cap.resize(keep);
   o->cap.resize(num_endpoints, o->cfg.lru_capacity);
   o->cfg.num_endpoints = o->cfg.endpoint_count = num_endpoints;
+  o->cnt = num_endpoints;  // (a resized handle covers the whole pool: lo is 0)
   return FI_OK;
 }
 

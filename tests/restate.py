@@ -17,6 +17,8 @@ Semantics restated:
   A.5 pick         max total over alive endpoints passing the profile's role filter; ties by the request's
                    rotation (fi_epp.h "Ties")
   A.6 PD           decode first; prefill stands iff (1 - m_dec/n)·len >= threshold
+  shard view       (docs/SPEC.md S.2e) a handle over endpoints [b, b + c): ops and Adds for other endpoints are
+                   dropped, only its own endpoints are candidates; queue min/max and the rotation stay pool-wide
 """
 from __future__ import annotations
 
@@ -51,9 +53,11 @@ def tie_start(n_blocks: int, first_hash: int, h0: int, r: int, E: int) -> int:
 
 
 class Restatement:
-    def __init__(self, num_endpoints, block_bytes, max_blocks, profiles, pd=None, lpm=False, lru_capacity=0):
-        """profiles: [{"filters": [label-bit masks, ANDed], "scorers": [(kind, weight), ...]}]; pd: {"decode", "prefill", "threshold"}"""
+    def __init__(self, num_endpoints, block_bytes, max_blocks, profiles, pd=None, lpm=False, lru_capacity=0, shard=None):
+        """profiles: [{"filters": [label-bit masks, ANDed], "scorers": [(kind, weight), ...]}]; pd: {"decode", "prefill", "threshold"};
+        shard: (b, c) for the view of a handle over endpoints [b, b + c)"""
         self.E, self.B, self.M = num_endpoints, block_bytes, max_blocks
+        self.own = range(num_endpoints) if shard is None else range(shard[0], shard[0] + shard[1])
         self.profiles, self.pd, self.lpm = profiles, pd, lpm
         self.index = {}  # hash -> set of endpoints
         self.state = {}  # endpoint -> dict(role_mask, kv_util, queue, flags)
@@ -64,6 +68,8 @@ class Restatement:
     # ---- A.2
     def apply(self, ops):
         for h, e, op in zip(ops["hash"].tolist(), ops["endpoint"].tolist(), ops["op"].tolist()):
+            if e not in self.own:
+                continue
             if op == 1:
                 self.index.setdefault(h, set()).add(e)
             else:
@@ -72,6 +78,8 @@ class Restatement:
                     s.discard(e)
 
     def add_chain(self, endpoint, hashes):
+        if endpoint not in self.own:
+            return
         d = self.lru.setdefault(endpoint, OrderedDict())
         for h in hashes:
             h = int(h)
@@ -152,7 +160,7 @@ class Restatement:
             for pi, prof in enumerate(self.profiles):
                 best = None
                 mn, mx = qctx[pi]
-                for e in range(self.E):
+                for e in self.own:
                     if not self._eligible(e, prof):
                         continue
                     st = self.state[e]
@@ -184,7 +192,7 @@ class Restatement:
         return out
 
 
-def from_config(cfg, lpm=None):
+def from_config(cfg, lpm=None, shard=None):
     """Build a Restatement from an abi.fi_epp_config (ctypes struct: layout only, no library call)."""
     profiles = []
     for i in range(cfg.n_profiles):
@@ -196,4 +204,4 @@ def from_config(cfg, lpm=None):
     if cfg.pd_enabled:
         pd = {"decode": int(cfg.pd_decode_profile), "prefill": int(cfg.pd_prefill_profile), "threshold": float(cfg.pd_threshold)}
     return Restatement(cfg.num_endpoints, cfg.block_bytes, cfg.max_blocks, profiles, pd,
-                       lpm=bool(cfg.match_mode) if lpm is None else lpm, lru_capacity=int(cfg.lru_capacity))
+                       lpm=bool(cfg.match_mode) if lpm is None else lpm, lru_capacity=int(cfg.lru_capacity), shard=shard)
