@@ -15,8 +15,9 @@ HDRS := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/fi_epp.h
 EXT_ORACLE := $(OBJDIR)/libepp_ext_oracle.so
 RESIZE_ORACLE := $(OBJDIR)/libepp_resize_oracle.so
 SNAPSHOT_ORACLE := $(OBJDIR)/libepp_snapshot_oracle.so
+COUNTS_ORACLE := $(OBJDIR)/libepp_counts_oracle.so
 
-all: $(LIB) $(HOSTCHECK) oracle $(EXT_ORACLE) $(RESIZE_ORACLE) $(SNAPSHOT_ORACLE)
+all: $(LIB) $(HOSTCHECK) oracle $(EXT_ORACLE) $(RESIZE_ORACLE) $(SNAPSHOT_ORACLE) $(COUNTS_ORACLE)
 
 $(OBJDIR)/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -47,6 +48,8 @@ $(OBJDIR)/libepp_%.so: tests/%.cpp oracle/epp_oracle.cpp include/fi_epp.h
 $(RESIZE_ORACLE): tests/ext_oracle.cpp
 # tests/snapshot_oracle.cpp adds the state of an index snapshot on top of tests/resize_oracle.cpp
 $(SNAPSHOT_ORACLE): tests/ext_oracle.cpp tests/resize_oracle.cpp
+# tests/counts_oracle.cpp adds the match counts of fi_epp_match_counts on top of tests/ext_oracle.cpp
+$(COUNTS_ORACLE): tests/ext_oracle.cpp
 
 clean:
 	rm -rf $(OBJDIR) $(LIB) $(HOSTCHECK)

@@ -255,6 +255,8 @@ SYMBOLS = [
     ("fi_epp_pick_batch_subset", C.c_int, [_P, _P, _P, _P, _P, _P, C.c_uint32, C.c_uint32, _P, _P]),
     ("fi_epp_pick_batch_device_subset", C.c_int,
      [_P, _P, _P, _P, _P, _P, C.c_uint32, C.c_uint64, C.c_uint32, _P, _P, _P]),
+    ("fi_epp_match_counts", C.c_int, [_P, _P, _P, _P, C.c_uint32, _P, _P, _P]),
+    ("fi_epp_match_counts_device", C.c_int, [_P, _P, _P, _P, C.c_uint32, C.c_uint64, _P, _P, _P, _P]),
     ("fi_epp_pinned_alloc", _P, [C.c_size_t]),
     ("fi_epp_pinned_free", None, [_P]),
     ("fi_epp_comm_unique_id", C.c_int, [_P]),

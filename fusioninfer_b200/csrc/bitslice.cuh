@@ -103,4 +103,31 @@ FI_HD uint32_t bc_get(const BitCounter& b, uint32_t bit) {
   return v;
 }
 
+// out[j] = count of endpoint bit0 + j for j < NB (NB a power of two <= 32, bit0 + NB <= 32).  Two counts per pass
+// over the planes: bit q and bit q + NB/2 are gathered into the low and high half of one word, so the transpose
+// costs half of NB bc_get calls.
+template <int NB>
+FI_HD void bc_unpack(const BitCounter& b, uint32_t bit0, uint16_t* out) {
+  static_assert(NB == 1 || NB == 2 || NB == 4 || NB == 8 || NB == 16 || NB == 32, "NB must be a power of two <= 32");
+  if (NB == 1) {
+    out[0] = (uint16_t)bc_get(b, bit0);
+    return;
+  }
+  constexpr int H = NB > 1 ? NB / 2 : 1;
+  uint32_t c[NPLANES];
+#pragma unroll
+  for (int pl = 0; pl < NPLANES; ++pl) c[pl] = b.c[pl] >> bit0;
+#pragma unroll
+  for (int q = 0; q < H; ++q) {
+    uint32_t v = 0;
+#pragma unroll
+    for (int pl = 0; pl < NPLANES; ++pl) {
+      const uint32_t x = c[pl] >> q;
+      v |= ((x & 1u) | ((x << (16 - H)) & 0x10000u)) << pl;
+    }
+    out[q] = (uint16_t)(v & 0xFFFFu);
+    out[q + H] = (uint16_t)(v >> 16);
+  }
+}
+
 }  // namespace fi

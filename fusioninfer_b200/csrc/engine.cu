@@ -236,6 +236,7 @@ struct fi_epp {
   DevPtr<fi_pick> d_picks;      // [R][P] final
   Staging<fi_pick> ranked;      // [R][P][k] of the host ranked pick: allocated by the first such call, grown with k
   Staging<uint32_t> subsets;    // [max_batch][ceil(E/32)] staging of fi_epp_pick_batch_subset: allocated by its first call
+  Staging<uint16_t> counts;     // [max_batch][endpoint_count] of fi_epp_match_counts: allocated by its first call
   std::unique_ptr<ShardState> shard;  // sharded mode only
   PeerXchg px{};                 // px.enabled == 0: NCCL all-gathers are used
   // sharded mode: every rank hashes every prompt (the default: hashing 16 KiB from local HBM is expected to cost
@@ -1381,6 +1382,9 @@ struct PickCall {
   uint32_t k;                // 0: out is [R][P]; else [R][P][k]
   fi_pick* out;
   uint64_t* chains_out;      // [R][max_blocks], or null
+  // match counts (S.3a) instead of picks: out is null, counts [R][endpoint_count]; nblocks_out [R] or null
+  uint16_t* counts;
+  uint32_t* nblocks_out;
 };
 
 // the same from the untyped pointers the device entry points take
@@ -1440,6 +1444,7 @@ int prepare_match(fi_epp* h, const PickCall& c, const uint64_t* chain, const uin
   mp.probed_blocks = h->profiling ? h->d_probed.get() : nullptr;
   mp.work_counter = h->d_work.get();
   mp.k = c.k;
+  mp.counts = c.counts;
   if (c.subsets) {
     mp.subsets = c.subsets;
     mp.sub_pitch = (h->cfg.num_endpoints + 31) / 32;
@@ -1522,7 +1527,8 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
       ms.h0 = mp.h0 + r0;
       ms.r_base = r0;
       ms.R = Rk;
-      ms.out = mp.out + (size_t)r0 * h->P * std::max(c.k, 1u);
+      ms.out = mp.out ? mp.out + (size_t)r0 * h->P * std::max(c.k, 1u) : nullptr;
+      ms.counts = mp.counts ? mp.counts + (size_t)r0 * h->cfg.endpoint_count : nullptr;
       ms.work_counter = h->d_work.get() + k;
       LaunchScope ls(h, h->s_main.get(), K_MATCH);
       FI_CUDA(launch_match_pick(ms, h->sm_count, h->s_main.get()));
@@ -2943,8 +2949,8 @@ int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets
 // the argument checks of every pick call, before the handle is touched (FI_ERR_INVALID); the ranked entry points, which
 // take k >= 1, reject k == 0 themselves
 static bool bad_pick_args(const PickCall& c, bool host) {
-  return !c.offsets || (!c.h0 && c.R) || (!c.out && (c.R || c.k)) || c.k > FI_EPP_MAX_RANKED || (c.k == 0 && c.subsets) ||
-         (host && !c.prompts && c.R && c.offsets[c.R]);
+  return !c.offsets || (!c.h0 && c.R) || (!c.out && !c.counts && (c.R || c.k)) || c.k > FI_EPP_MAX_RANKED ||
+         (c.k == 0 && c.subsets) || (host && !c.prompts && c.R && c.offsets[c.R]);
 }
 
 // The handle's checks of every pick call, under its lock and before an empty batch returns (a batch over max_batch is
@@ -2953,6 +2959,7 @@ static bool bad_pick_args(const PickCall& c, bool host) {
 static int check_pick_handle(fi_epp* h, const PickCall& c) {
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   if (c.k && h->world > 1) return fail(h, FI_ERR_STATE, "ranked picks need a single-rank pool");
+  if (c.counts && h->world > 1) return fail(h, FI_ERR_STATE, "match counts need a single-rank pool");
   if (c.subsets && (h->cfg.endpoint_begin != 0 || h->cfg.endpoint_count != h->cfg.num_endpoints))
     return fail(h, FI_ERR_STATE, "subset picks need a single handle over the whole pool");
   if (c.R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
@@ -2981,6 +2988,15 @@ static int pick_host(fi_epp* h, const PickCall& c) {
     d.out = h->ranked.d.get();
     h_out = h->ranked.h.get();
   }
+  if (c.counts) {
+    // the count rows exist only on handles that ask for counts; sized for max_batch rows of the pool as it is now
+    const size_t need = (size_t)h->cfg.max_batch * h->cfg.endpoint_count;
+    if (need > h->counts.cap) FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
+    rc = grow_staging(h, h->counts, need, need, true);
+    if (rc != FI_OK) return rc;
+    d.out = nullptr;
+    d.counts = h->counts.d.get();
+  }
   rc = stage_inputs(h, c.prompts, c.offsets, c.h0, R, total, /*copy_prompts=*/false);
   if (rc != FI_OK) return rc;
   if (c.adapters) {
@@ -3002,18 +3018,30 @@ static int pick_host(fi_epp* h, const PickCall& c) {
   }
   rc = run_pick(h, d, &c);
   if (rc != FI_OK) return rc;
-  const size_t pb = (size_t)R * h->P * std::max(c.k, 1u) * sizeof(fi_pick);
-  FI_CUDA(cudaMemcpyAsync(h_out, d.out, pb, cudaMemcpyDeviceToHost, h->s_main.get()));
+  void* h_res = h_out;
+  const void* d_res = d.out;
+  size_t pb = (size_t)R * h->P * std::max(c.k, 1u) * sizeof(fi_pick);
+  if (c.counts) {
+    h_res = h->counts.h.get();
+    d_res = d.counts;
+    pb = (size_t)R * h->cfg.endpoint_count * sizeof(uint16_t);
+  }
+  FI_CUDA(cudaMemcpyAsync(h_res, d_res, pb, cudaMemcpyDeviceToHost, h->s_main.get()));
   h->stats.d2h_bytes += pb;
   rc = copy_chains_out(h, h->d_chain.get(), c.chains_out, R, cudaMemcpyDeviceToHost, h->s_main.get());
   if (rc != FI_OK) return rc;
+  if (c.nblocks_out) {
+    FI_CUDA(cudaMemcpyAsync(h->h_nblocks.get(), h->d_nblocks.get(), (size_t)R * sizeof(uint32_t), cudaMemcpyDeviceToHost, h->s_main.get()));
+    h->stats.d2h_bytes += (size_t)R * sizeof(uint32_t);
+  }
   FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
   volatile uint32_t* xerr = h->shard ? h->shard->h_xerr.get() : nullptr;
   if (xerr && *xerr) {  // (sharded) reported once; the tags are monotonic, so later steps can succeed again
     *xerr = 0;
     return fail(h, FI_ERR_COMM, "peer exchange timed out waiting for another rank");
   }
-  std::memcpy(c.out, h_out, pb);
+  std::memcpy(c.counts ? (void*)c.counts : (void*)c.out, h_res, pb);
+  if (c.nblocks_out) std::memcpy(c.nblocks_out, h->h_nblocks.get(), (size_t)R * sizeof(uint32_t));
   return FI_OK;
 }
 
@@ -3031,6 +3059,8 @@ static int pick_device(fi_epp* h, const PickCall& c, void* stream) {
   if (rc != FI_OK) return rc;
   rc = copy_chains_out(h, h->d_chain.get(), c.chains_out, c.R, cudaMemcpyDeviceToDevice, h->s_main.get());
   if (rc != FI_OK) return rc;
+  if (c.nblocks_out)
+    FI_CUDA(cudaMemcpyAsync(c.nblocks_out, h->d_nblocks.get(), (size_t)c.R * sizeof(uint32_t), cudaMemcpyDeviceToDevice, h->s_main.get()));
   FI_CUDA(cudaEventRecord(h->ev_done.get(), h->s_main.get()));
   FI_CUDA(cudaStreamWaitEvent(us, h->ev_done.get(), 0));
   return FI_OK;
@@ -3112,6 +3142,22 @@ int fi_epp_pick_batch_device_subset(fi_epp* h, const void* d_prompts, const void
                                     void* stream) {
   if (k == 0) return FI_ERR_INVALID;
   return pick_device(h, device_call(d_prompts, d_offsets, d_h0, d_adapters, d_subsets, R, k, d_out, d_chains_out), stream);
+}
+
+int fi_epp_match_counts(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
+                        uint16_t* counts, uint32_t* nblocks_out, uint64_t* chains_out) {
+  if (!counts && R) return FI_ERR_INVALID;
+  return pick_host(h, PickCall{prompts, offsets, h0, nullptr, nullptr, R, 0, nullptr, chains_out, counts, nblocks_out});
+}
+
+int fi_epp_match_counts_device(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
+                               uint64_t total_prompt_bytes, void* d_counts, void* d_nblocks_out, void* d_chains_out,
+                               void* stream) {
+  if (!d_counts && R) return FI_ERR_INVALID;
+  PickCall c = device_call(d_prompts, d_offsets, d_h0, nullptr, nullptr, R, 0, nullptr, d_chains_out);
+  c.counts = (uint16_t*)d_counts;
+  c.nblocks_out = (uint32_t*)d_nblocks_out;
+  return pick_device(h, c, stream);
 }
 
 int fi_epp_pick_submit(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,

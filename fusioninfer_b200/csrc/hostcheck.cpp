@@ -73,6 +73,25 @@ void fihc_bitcount(const uint32_t* words, uint32_t n, uint32_t K, uint32_t* coun
   for (uint32_t bit = 0; bit < 32; ++bit) counts[bit] = fi::bc_get(b, bit);
 }
 
+// bc_unpack<nb>(planes, bit0) and bc_get of the same bits: out_unpack[j], out_get[j] for j < nb; -1 for an nb that is
+// not a power of two <= 32 or a range past bit 31
+int fihc_bc_unpack(const uint32_t* planes, uint32_t bit0, uint32_t nb, uint16_t* out_unpack, uint16_t* out_get) {
+  if (bit0 + nb > 32) return -1;
+  fi::BitCounter b;
+  for (int pl = 0; pl < fi::NPLANES; ++pl) b.c[pl] = planes[pl];
+  switch (nb) {
+    case 1: fi::bc_unpack<1>(b, bit0, out_unpack); break;
+    case 2: fi::bc_unpack<2>(b, bit0, out_unpack); break;
+    case 4: fi::bc_unpack<4>(b, bit0, out_unpack); break;
+    case 8: fi::bc_unpack<8>(b, bit0, out_unpack); break;
+    case 16: fi::bc_unpack<16>(b, bit0, out_unpack); break;
+    case 32: fi::bc_unpack<32>(b, bit0, out_unpack); break;
+    default: return -1;
+  }
+  for (uint32_t j = 0; j < nb; ++j) out_get[j] = (uint16_t)fi::bc_get(b, bit0 + j);
+  return 0;
+}
+
 // merge of two counters built from two word streams
 void fihc_bitcount_merge(const uint32_t* wa, uint32_t na, const uint32_t* wb, uint32_t nb, uint32_t* counts,
                          uint32_t* nonzero) {

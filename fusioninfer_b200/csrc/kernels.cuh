@@ -158,7 +158,7 @@ struct MatchParams {
   // pd-profile-handler
   uint32_t apply_pd, pd_decode, pd_prefill;
   double pd_threshold;
-  fi_pick* out;                       // [R][P], or [R][P][k] when k > 0
+  fi_pick* out;                       // [R][P], or [R][P][k] when k > 0 (null for match counts)
   unsigned long long* probed_blocks;  // optional Σ N_probe
   uint32_t* work_counter;             // dynamic request queue of the launch (the launcher zeroes it first)
   uint32_t lane_zero;                 // always 0: makes the ticket address formally lane-dependent (match_kernels.cu take_ticket)
@@ -168,6 +168,9 @@ struct MatchParams {
   const uint32_t* subsets;  // [R][sub_pitch] candidate bitset of each request over the pool, or null (unrestricted)
   uint32_t sub_pitch;       // words per subset row: ceil(E_global / 32); words past it read as 0
   const EndpointDev* eps;   // [E_global] raw endpoint state: the per-request queue min / max of a subset pick
+  // match counts (docs/SPEC.md S.3a), appended like the subset fields: non-null selects the COUNTS variant, which
+  // writes every local endpoint's match count instead of picks (out, k, PD and the score tables are not read)
+  uint16_t* counts;  // [R][ep_count], dense, 2-byte aligned
 };
 
 struct MergeParams {

@@ -23,6 +23,8 @@
 //      request's candidate subset, S.5a); equal totals are resolved by the request's tie rotation (tiebreak.cuh — upstream's
 //      MaxScorePicker shuffles, Appendix A.5), then the pd-profile-handler threshold rule (Appendix A.6,
 //      /root/reference/pkg/router/strategy.go:129-133).
+//   The COUNTS variant (fi_epp_match_counts, docs/SPEC.md S.3a) replaces 4./5. with counts_row: every local endpoint's
+//   match count, written as the request's row of a dense [R][ep_count] u16 matrix.
 //
 // Rows narrower than 32 words (fewer than 1024 local endpoints, e.g. an
 // endpoint-range shard of a multi-GPU pool) are read G = 32/L rows per load
@@ -380,6 +382,49 @@ __device__ __forceinline__ void ranked_profile(const MatchParams& p, uint32_t pi
   }
 }
 
+// docs/SPEC.md S.3a, the epilogue of the COUNTS variant: request r's row counts[r * ep_count + j] = the match count of
+// local endpoint j.  After the merge every lane group holds the full counters, so group g unpacks bits
+// [g*32/G, (g+1)*32/G) of its lanes' words (as the LoRA branch splits them) into the warp's staging row in shared
+// memory, placed at the offset the row has in its first 32-byte sector of global memory.  The warp then stores 16
+// bytes per lane from that sector on: whole sectors, except the row's first and last, which it shares with the rows
+// before and after it and writes with 2-byte stores (any 2-byte aligned counts pointer works).  Words without a
+// matched endpoint store zeros without unpacking; a request without a matched block skips the staging row.
+template <int VEC, int G>
+__device__ __forceinline__ void counts_row(const MatchParams& p, const BitCounter (&cnt)[VEC], uint32_t r, bool nothing,
+                                           uint16_t* __restrict__ s_row, int lane, int t, int g) {
+  constexpr int BPG = 32 / G;
+  const uint64_t a = reinterpret_cast<uint64_t>(p.counts + (uint64_t)r * p.ep_count);
+  const uint32_t shift = (uint32_t)(a & 31u) >> 1;  // counts of the rows before this one in its first sector
+  uint16_t* const base = reinterpret_cast<uint16_t*>(a - 2u * shift);
+  const uint32_t end = shift + p.ep_count;
+  if (!nothing) {
+#pragma unroll
+    for (int x = 0; x < VEC; ++x) {
+      uint16_t* o = s_row + shift + (uint32_t)(t * VEC + x) * 32u + (uint32_t)(g * BPG);
+      if (bc_nonzero(cnt[x])) {
+        bc_unpack<BPG>(cnt[x], (uint32_t)(g * BPG), o);
+      } else {
+#pragma unroll
+        for (int i = 0; i < BPG; ++i) o[i] = 0;
+      }
+    }
+    __syncwarp();  // the staging row is written by each lane group and read by every lane
+  }
+  for (uint32_t c = lane; c < (end + 7) / 8; c += 32) {
+    const uint32_t j0 = c * 8;
+    uint4 v = make_uint4(0, 0, 0, 0);
+    if (!nothing) v = *reinterpret_cast<const uint4*>(s_row + j0);
+    if (j0 >= shift && j0 + 8 <= end) {
+      *reinterpret_cast<uint4*>(base + j0) = v;
+    } else {  // the row's first or last 16 bytes
+      const uint32_t w[4] = {v.x, v.y, v.z, v.w};
+#pragma unroll
+      for (int i = 0; i < 8; ++i)
+        if (j0 + i >= shift && j0 + i < end) base[j0 + i] = (uint16_t)(w[i >> 1] >> (16 * (i & 1)));
+    }
+  }
+}
+
 // LPR lanes read one row (VEC words each, LPR*VEC = words per row); a load
 // instruction therefore covers G = 32/LPR rows.  E = 1024 → LPR 16, VEC 2: a 128-byte
 // row is 16 × 8-byte loads and one instruction brings in 2 rows; 16 rows in flight.
@@ -388,7 +433,9 @@ __device__ __forceinline__ void ranked_profile(const MatchParams& p, uint32_t pi
 // SUBSET (with RANKED only): every request carries a candidate bitset (docs/SPEC.md S.5a).  Steps 1-3 do not look
 // at it — the walk and the counts stay pool-wide — and its words are loaded when the request starts, so they
 // arrive under the walk; only the scoring of ranked_profile uses them.
-template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false>
+// COUNTS (not with LORA / RANKED): steps 1-3 as for a pick, then counts_row writes the request's match counts instead
+// of steps 4-5 and the PD rule.  Its staging rows follow the node buffers in shared memory, Epad + 16 counts per warp.
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
 __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MIN_BLOCKS : FI_MATCH_MIN_BLOCKS + 1))
     match_pick_kernel(const MatchParams p) {
   constexpr int G = 32 / LPR;                 // rows per load instruction
@@ -406,8 +453,12 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
   // per warp: two chain buffers (the next request's chain is staged while this one is matched) and the nodes
   uint64_t* const s_chain_base = s_mem + (size_t)(2 * warp) * p.MP;  // buffer b at s_chain_base + b * MP
   uint32_t* s_node = reinterpret_cast<uint32_t*>(s_mem + (size_t)2 * kWarps * p.MP) + (size_t)warp * p.MP;  // node of every block
+  uint16_t* s_row = nullptr;  // COUNTS: the warp's staging row
+  if constexpr (COUNTS)
+    s_row = reinterpret_cast<uint16_t*>(s_mem + (size_t)2 * kWarps * p.MP) + (size_t)2 * kWarps * p.MP +
+            (size_t)warp * (p.st.Epad + 16);
   const IndexView ix = p.ix;
-  const uint32_t P = p.st.n_profiles;
+  const uint32_t P = COUNTS ? 0u : p.st.n_profiles;  // COUNTS: no profile is scored
   const char* row_base = reinterpret_cast<const char*>(ix.rows + t * VEC);
   const uint32_t row_bytes = 4u << ix.logW;
   const uint32_t zero_slot = (uint32_t)(ix.C + 2);  // never written: all-zero row
@@ -571,6 +622,7 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
         }
       }
     }
+    if constexpr (COUNTS) counts_row<VEC, G>(p, cnt, r, nothing, s_row, lane, t, g);
 
     // ---- 4./5. score candidates, argmax, PD rule ---------------------------------
     TieRot tr;
@@ -700,7 +752,7 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
       }
     }
     if (lane == 0) {
-      if (p.apply_pd) {  // pd-profile-handler: the prefill pick stands only if the threshold test passes
+      if (!COUNTS && p.apply_pd) {  // pd-profile-handler: the prefill pick stands only if the threshold test passes
         const uint64_t len = p.offsets[r + 1] - p.offsets[r];
         if (!pd_prefill_runs(dec_e, dec_m, n, len, p.pd_threshold)) {
           fi_pick pk;
@@ -909,10 +961,11 @@ std::mutex g_match_launch_mu;
 
 // One instantiation per kernel variant: the shared-memory opt-in (cudaFuncSetAttribute) applies to one function
 // only, and occupancy differs between variants, so each variant keeps its own state, per device.
-template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false>
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
 cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_t s) {
-  const auto kern = match_pick_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET>;
-  const size_t smem = (size_t)kWarps * p.MP * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
+  const auto kern = match_pick_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS>;
+  size_t smem = (size_t)kWarps * p.MP * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
+  if (COUNTS) smem += (size_t)kWarps * (p.st.Epad + 16) * sizeof(uint16_t);        // + the staging rows
   static std::map<int, size_t> opted_in;                // device -> the variant's max dynamic smem attribute
   static std::map<std::pair<int, size_t>, int> per_sm;  // (device, smem) -> resident CTAs per SM
   int dev = 0;
@@ -951,6 +1004,9 @@ cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_
 template <int LPR, int VEC>
 cudaError_t launch_match_t(const MatchParams& p, int sm_count, cudaStream_t s) {
   const bool lpm = p.lpm == FI_MATCH_LPM;
+  if (p.counts)  // match counts (S.3a): no profile is scored
+    return lpm ? launch_match_variant<LPR, VEC, true, false, false, false, true>(p, sm_count, s)
+               : launch_match_variant<LPR, VEC, false, false, false, false, true>(p, sm_count, s);
   if (p.k && p.subsets)  // ranked pick over per-request candidate subsets
     return lpm ? launch_match_variant<LPR, VEC, true, false, true, true>(p, sm_count, s)
                : launch_match_variant<LPR, VEC, false, false, true, true>(p, sm_count, s);

@@ -388,6 +388,30 @@ class EndpointPicker:
         self._check(rc, "fi_epp_pick_batch_subset")
         return (picks, chains) if want_chains else picks
 
+    def match_counts(self, prompts, offsets, h0, want_chains: bool = False):
+        """The prefix-cache-scorer alone (docs/SPEC.md S.3a): every local endpoint's prefix match count, for a host
+        framework that runs the configuration's other plugins itself.  -> (counts uint16 [R, endpoint_count],
+        nblocks uint32 [R][, chains]); counts[r, j] / nblocks[r] is upstream's prefix score of endpoint
+        endpoint_begin + j.  After the host's pick, index_add_chains_device(endpoints, 0, 0, nblocks) adds the chains."""
+        prompts, offsets, h0, R = self._inputs(prompts, offsets, h0)
+        counts = np.zeros((R, int(self.cfg.endpoint_count)), dtype=np.uint16)
+        nb = np.zeros(R, dtype=np.uint32)
+        chains = np.zeros((R, self.max_blocks), dtype=np.uint64) if want_chains else None
+        self._check(self._lib.fi_epp_match_counts(self._h, _ptr(prompts), _ptr(offsets), _ptr(h0), R, _ptr(counts),
+                                                  _ptr(nb), _ptr(chains)),
+                    "fi_epp_match_counts")
+        return (counts, nb, chains) if want_chains else (counts, nb)
+
+    def match_counts_device(self, d_prompts: int, d_offsets: int, d_h0: int, R: int, total_bytes: int, d_counts: int,
+                            d_nblocks: int = 0, d_chains: int = 0, stream: int = 0):
+        """match_counts on device buffers: d_counts holds R * endpoint_count uint16 (2-byte aligned), d_nblocks R uint32
+        (optional), d_chains R * max_blocks hashes (optional)."""
+        self._check(
+            self._lib.fi_epp_match_counts_device(self._h, d_prompts, d_offsets, d_h0, R, total_bytes, d_counts,
+                                                 d_nblocks or None, d_chains or None, stream or None),
+            "fi_epp_match_counts_device",
+        )
+
     def pick_batch_raw(self, prompts_ptr: int, offsets_ptr: int, h0_ptr: int, R: int, out_ptr: int, chains_ptr: int = 0):
         """Host-pointer variant without numpy marshalling (pinned buffers from pinned_alloc)."""
         self._check(

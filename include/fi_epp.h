@@ -31,6 +31,8 @@
  *   KV-cache block count)
  *   datastore pod metrics refresh (kv, queue, role) → fi_epp_endpoints_update
  *   SchedulerProfile.Run: filter → scorers → picker → fi_epp_pick_batch
+ *   prefix.Plugin.Score alone (matchLen / total per  → fi_epp_match_counts (the host runs
+ *   pod; the other plugins run in the framework)       the rest of any config)
  *   pd-profile-handler (decode then prefill)        → fi_epp_pick_batch with
  *                                                     cfg.pd_enabled
  *
@@ -483,6 +485,27 @@ int fi_epp_pick_batch_device_subset(fi_epp* h, const void* d_prompts, const void
                                     const void* d_adapters, const void* d_subsets, uint32_t R,
                                     uint64_t total_prompt_bytes, uint32_t k, void* d_out, void* d_chains_out,
                                     void* stream);
+
+/* Match counts: the prefix-cache-scorer on its own (docs/SPEC.md S.3a), for a configuration whose other plugins run on
+ * the host (a picker, filter or scorer this library does not implement).  counts[r*endpoint_count + j] = the number
+ * of prefix blocks of request r that local endpoint endpoint_begin + j holds, in the handle's match mode: S.3's
+ * match[e], the match_blocks every pick of any variant would report for that endpoint on the same index.  It ignores
+ * endpoint state, adapters, profiles, filters and PD: the host filters after the call and scores counts / n_blocks.
+ * counts is dense [R][endpoint_count] uint16 with no row padding (any 2-byte aligned pointer); nblocks_out [R]
+ * (optional) = the requests' n_blocks; chains_out (optional) as fi_epp_pick_batch's.  A handle over part of the pool
+ * returns its own columns with the shard-local walk of S.2e.  Ordered and counted like the stream-ordered picks:
+ * every index update issued before the call is seen, it is a pick call in fi_epp_stats and for the chain retention of
+ * fi_epp_index_add_submitted, and fi_epp_index_add_chains_device(.., NULL, ..) afterwards adds this call's chains (the
+ * PreRequest step after the host's own pick).  Errors write nothing: FI_ERR_INVALID for a NULL handle, offsets, h0 or
+ * counts with R > 0; FI_ERR_CAPACITY for R > max_batch or (host call) prompt bytes above max_prompt_bytes;
+ * FI_ERR_STATE on a sharded pool.  The host call stages the rows through buffers of max_batch * endpoint_count counts
+ * allocated by its first call. */
+int fi_epp_match_counts(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
+                        uint16_t* counts, uint32_t* nblocks_out, uint64_t* chains_out);
+/* The same on device buffers, in `stream` order like fi_epp_pick_batch_device. */
+int fi_epp_match_counts_device(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
+                               uint64_t total_prompt_bytes, void* d_counts, void* d_nblocks_out, void* d_chains_out,
+                               void* stream);
 
 /* Pipelined device path.  fi_epp_pick_submit enqueues one batch exactly like fi_epp_pick_batch_device (inputs
  * ready in `stream` order at the call) but does NOT order `stream` behind the result: batch k+1's block
