@@ -17,7 +17,7 @@ FI_EPP_MAX_SCORERS = 4
 FI_EPP_MAX_FILTERS = 4
 FI_EPP_MAX_LABELS = 24
 FI_ROLE_FIRST_FREE = 8
-FI_EPP_MAX_BLOCKS = 1023
+FI_EPP_MAX_BLOCKS = 4095
 FI_EPP_MAX_RANKED = 16
 FI_NO_ENDPOINT = 0xFFFFFFFF
 FI_EPP_UNIQUE_ID_BYTES = 128

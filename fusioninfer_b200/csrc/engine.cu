@@ -1429,6 +1429,7 @@ int prepare_match(fi_epp* h, const PickCall& c, const uint64_t* chain, const uin
   mp.adapters = c.adapters;
   mp.R = c.R;
   mp.MP = h->MP;
+  mp.max_blocks = h->cfg.max_blocks;
   mp.ix = h->ix.v;
   mp.st = h->st;
   mp.ep_begin = h->cfg.endpoint_begin;
@@ -3253,6 +3254,8 @@ int fi_epp_comm_init(fi_epp* h, const uint8_t id_bytes[FI_EPP_UNIQUE_ID_BYTES], 
   std::lock_guard<std::mutex> lk(h->mu);
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   if (h->shard) return fail(h, FI_ERR_STATE, "communicator already initialised");
+  // the sharded pick is tested only with chains that fit one match window (DESIGN.md §4.9)
+  if (h->cfg.max_blocks > 1023) return fail(h, FI_ERR_STATE, "sharded pools need max_blocks <= 1023");
   if (world > 32) return fail(h, FI_ERR_INVALID, "more than 32 ranks: the directory keeps one presence bit per rank");
   if (h->ops_applied || h->n_sets || h->n_clears)
     return fail(h, FI_ERR_STATE, "fi_epp_comm_init must precede the first index update (the directory is built by gossip)");

@@ -18,6 +18,58 @@
 #include "tiebreak.cuh"
 #include "xxh64.cuh"
 
+namespace {
+
+template <int NP>
+void bitcount(const uint32_t* words, uint32_t n, uint32_t K, uint32_t* counts) {
+  fi::BitCounter<NP> b;
+  fi::bc_clear(b);
+  for (uint32_t i = 0; i < n; i += K) {
+    uint32_t w[16] = {0};
+    for (uint32_t j = 0; j < K && i + j < n; ++j) w[j] = words[i + j];
+    switch (K) {
+      case 1: { uint32_t t[1] = {w[0]}; fi::bc_add<1>(b, t); break; }
+      case 2: { uint32_t t[2] = {w[0], w[1]}; fi::bc_add<2>(b, t); break; }
+      case 4: { uint32_t t[4]; std::memcpy(t, w, sizeof(t)); fi::bc_add<4>(b, t); break; }
+      case 8: { uint32_t t[8]; std::memcpy(t, w, sizeof(t)); fi::bc_add<8>(b, t); break; }
+      default: { uint32_t t[16]; std::memcpy(t, w, sizeof(t)); fi::bc_add<16>(b, t); break; }
+    }
+  }
+  for (uint32_t bit = 0; bit < 32; ++bit) counts[bit] = fi::bc_get(b, bit);
+}
+
+template <int NP>
+int bc_unpack_check(const uint32_t* planes, uint32_t bit0, uint32_t nb, uint16_t* out_unpack, uint16_t* out_get) {
+  if (bit0 + nb > 32) return -1;
+  fi::BitCounter<NP> b;
+  for (int pl = 0; pl < NP; ++pl) b.c[pl] = planes[pl];
+  switch (nb) {
+    case 1: fi::bc_unpack<1>(b, bit0, out_unpack); break;
+    case 2: fi::bc_unpack<2>(b, bit0, out_unpack); break;
+    case 4: fi::bc_unpack<4>(b, bit0, out_unpack); break;
+    case 8: fi::bc_unpack<8>(b, bit0, out_unpack); break;
+    case 16: fi::bc_unpack<16>(b, bit0, out_unpack); break;
+    case 32: fi::bc_unpack<32>(b, bit0, out_unpack); break;
+    default: return -1;
+  }
+  for (uint32_t j = 0; j < nb; ++j) out_get[j] = (uint16_t)fi::bc_get(b, bit0 + j);
+  return 0;
+}
+
+template <int NP>
+void bitcount_merge(const uint32_t* wa, uint32_t na, const uint32_t* wb, uint32_t nb, uint32_t* counts, uint32_t* nonzero) {
+  fi::BitCounter<NP> a, b;
+  fi::bc_clear(a);
+  fi::bc_clear(b);
+  for (uint32_t i = 0; i < na; ++i) { uint32_t t[1] = {wa[i]}; fi::bc_add<1>(a, t); }
+  for (uint32_t i = 0; i < nb; ++i) { uint32_t t[1] = {wb[i]}; fi::bc_add<1>(b, t); }
+  fi::bc_merge(a, b);
+  for (uint32_t bit = 0; bit < 32; ++bit) counts[bit] = fi::bc_get(a, bit);
+  *nonzero = fi::bc_nonzero(a);
+}
+
+}  // namespace
+
 extern "C" {
 
 uint64_t fihc_xxh64(const uint8_t* p, uint32_t len) { return fi::xxh64_bytes(p, len); }
@@ -56,53 +108,28 @@ uint32_t fihc_chain_split(const uint8_t* p, uint64_t len, uint64_t h0, uint32_t 
 }
 
 // bit-sliced counting: add n words K at a time (zero padded), return the 32 counts
-void fihc_bitcount(const uint32_t* words, uint32_t n, uint32_t K, uint32_t* counts) {
-  fi::BitCounter b;
-  fi::bc_clear(b);
-  for (uint32_t i = 0; i < n; i += K) {
-    uint32_t w[16] = {0};
-    for (uint32_t j = 0; j < K && i + j < n; ++j) w[j] = words[i + j];
-    switch (K) {
-      case 1: { uint32_t t[1] = {w[0]}; fi::bc_add<1>(b, t); break; }
-      case 2: { uint32_t t[2] = {w[0], w[1]}; fi::bc_add<2>(b, t); break; }
-      case 4: { uint32_t t[4]; std::memcpy(t, w, sizeof(t)); fi::bc_add<4>(b, t); break; }
-      case 8: { uint32_t t[8]; std::memcpy(t, w, sizeof(t)); fi::bc_add<8>(b, t); break; }
-      default: { uint32_t t[16]; std::memcpy(t, w, sizeof(t)); fi::bc_add<16>(b, t); break; }
-    }
-  }
-  for (uint32_t bit = 0; bit < 32; ++bit) counts[bit] = fi::bc_get(b, bit);
-}
+void fihc_bitcount(const uint32_t* words, uint32_t n, uint32_t K, uint32_t* counts) { bitcount<fi::NPLANES>(words, n, K, counts); }
 
 // bc_unpack<nb>(planes, bit0) and bc_get of the same bits: out_unpack[j], out_get[j] for j < nb; -1 for an nb that is
 // not a power of two <= 32 or a range past bit 31
 int fihc_bc_unpack(const uint32_t* planes, uint32_t bit0, uint32_t nb, uint16_t* out_unpack, uint16_t* out_get) {
-  if (bit0 + nb > 32) return -1;
-  fi::BitCounter b;
-  for (int pl = 0; pl < fi::NPLANES; ++pl) b.c[pl] = planes[pl];
-  switch (nb) {
-    case 1: fi::bc_unpack<1>(b, bit0, out_unpack); break;
-    case 2: fi::bc_unpack<2>(b, bit0, out_unpack); break;
-    case 4: fi::bc_unpack<4>(b, bit0, out_unpack); break;
-    case 8: fi::bc_unpack<8>(b, bit0, out_unpack); break;
-    case 16: fi::bc_unpack<16>(b, bit0, out_unpack); break;
-    case 32: fi::bc_unpack<32>(b, bit0, out_unpack); break;
-    default: return -1;
-  }
-  for (uint32_t j = 0; j < nb; ++j) out_get[j] = (uint16_t)fi::bc_get(b, bit0 + j);
-  return 0;
+  return bc_unpack_check<fi::NPLANES>(planes, bit0, nb, out_unpack, out_get);
 }
 
 // merge of two counters built from two word streams
 void fihc_bitcount_merge(const uint32_t* wa, uint32_t na, const uint32_t* wb, uint32_t nb, uint32_t* counts,
                          uint32_t* nonzero) {
-  fi::BitCounter a, b;
-  fi::bc_clear(a);
-  fi::bc_clear(b);
-  for (uint32_t i = 0; i < na; ++i) { uint32_t t[1] = {wa[i]}; fi::bc_add<1>(a, t); }
-  for (uint32_t i = 0; i < nb; ++i) { uint32_t t[1] = {wb[i]}; fi::bc_add<1>(b, t); }
-  fi::bc_merge(a, b);
-  for (uint32_t bit = 0; bit < 32; ++bit) counts[bit] = fi::bc_get(a, bit);
-  *nonzero = fi::bc_nonzero(a);
+  bitcount_merge<fi::NPLANES>(wa, na, wb, nb, counts, nonzero);
+}
+
+// the same three with the 12 bit-planes of the windowed match kernel (counts up to 4095)
+void fihc_bitcount12(const uint32_t* words, uint32_t n, uint32_t K, uint32_t* counts) { bitcount<12>(words, n, K, counts); }
+int fihc_bc_unpack12(const uint32_t* planes, uint32_t bit0, uint32_t nb, uint16_t* out_unpack, uint16_t* out_get) {
+  return bc_unpack_check<12>(planes, bit0, nb, out_unpack, out_get);
+}
+void fihc_bitcount_merge12(const uint32_t* wa, uint32_t na, const uint32_t* wb, uint32_t nb, uint32_t* counts,
+                           uint32_t* nonzero) {
+  bitcount_merge<12>(wa, na, wb, nb, counts, nonzero);
 }
 
 // tie rotation (tiebreak.cuh): start of a request's rotation, rotated distance of an endpoint, and the first

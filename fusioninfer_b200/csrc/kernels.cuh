@@ -171,6 +171,9 @@ struct MatchParams {
   // match counts (docs/SPEC.md S.3a), appended like the subset fields: non-null selects the COUNTS variant, which
   // writes every local endpoint's match count instead of picks (out, k, PD and the score tables are not read)
   uint16_t* counts;  // [R][ep_count], dense, 2-byte aligned
+  // the handle's max_blocks (appended like the fields above): above 1023 a count needs more than the 10 bit-planes of
+  // one match window, and launch_match_pick runs the windowed variant (DESIGN.md §4.9)
+  uint32_t max_blocks;
 };
 
 struct MergeParams {

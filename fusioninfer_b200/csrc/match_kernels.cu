@@ -49,6 +49,9 @@ namespace fi {
 namespace {
 
 constexpr int kWarps = 8;
+// match_window_kernel: blocks per window (the chain staged at once), and counter planes for counts up to 4095
+constexpr int kWindow = 1024;
+constexpr int kWindowPlanes = 12;
 #ifndef FI_MATCH_MIN_BLOCKS
 #define FI_MATCH_MIN_BLOCKS 2
 #endif
@@ -270,8 +273,8 @@ __device__ __forceinline__ uint32_t take_ticket(uint32_t* counter, uint32_t opaq
 // SUBSET (S.5a): sub[x] is the request's candidate word t*VEC + x.  The eligible words become elig & sub, and the
 // queue scorer is normalised by the min / max queue depth over those endpoints (a warp reduction over the raw
 // endpoint state), in prepare_endpoints' arithmetic; the per-batch queue column does not apply.
-template <int VEC, int G, bool SUBSET>
-__device__ __forceinline__ void ranked_profile(const MatchParams& p, uint32_t pi, const BitCounter (&cnt)[VEC],
+template <int VEC, int G, bool SUBSET, int NP>
+__device__ __forceinline__ void ranked_profile(const MatchParams& p, uint32_t pi, const BitCounter<NP> (&cnt)[VEC],
                                                const uint32_t (&sub)[VEC], const TieRot& tr, uint32_t n, uint32_t r,
                                                int lane, int t, int g, uint32_t& dec_e, uint32_t& dec_m) {
   const ProfileDev& pr = p.st.prof[pi];
@@ -389,8 +392,8 @@ __device__ __forceinline__ void ranked_profile(const MatchParams& p, uint32_t pi
 // bytes per lane from that sector on: whole sectors, except the row's first and last, which it shares with the rows
 // before and after it and writes with 2-byte stores (any 2-byte aligned counts pointer works).  Words without a
 // matched endpoint store zeros without unpacking; a request without a matched block skips the staging row.
-template <int VEC, int G>
-__device__ __forceinline__ void counts_row(const MatchParams& p, const BitCounter (&cnt)[VEC], uint32_t r, bool nothing,
+template <int VEC, int G, int NP>
+__device__ __forceinline__ void counts_row(const MatchParams& p, const BitCounter<NP> (&cnt)[VEC], uint32_t r, bool nothing,
                                            uint16_t* __restrict__ s_row, int lane, int t, int g) {
   constexpr int BPG = 32 / G;
   const uint64_t a = reinterpret_cast<uint64_t>(p.counts + (uint64_t)r * p.ep_count);
@@ -435,10 +438,12 @@ __device__ __forceinline__ void counts_row(const MatchParams& p, const BitCounte
 // arrive under the walk; only the scoring of ranked_profile uses them.
 // COUNTS (not with LORA / RANKED): steps 1-3 as for a pick, then counts_row writes the request's match counts instead
 // of steps 4-5 and the PD rule.  Its staging rows follow the node buffers in shared memory, Epad + 16 counts per warp.
-template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
-__global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MIN_BLOCKS : FI_MATCH_MIN_BLOCKS + 1))
-    match_pick_kernel(const MatchParams p) {
+// WIN (match_window_kernel, handles with max_blocks > 1023; DESIGN.md §4.9): steps 1-3 run once per window of up to
+// kWindow blocks, in staging buffers of kWindow entries, and the counters have 12 bit-planes; steps 4-5 are the same.
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET, bool COUNTS, bool WIN>
+__device__ __forceinline__ void match_pick_body(const MatchParams& p) {
   constexpr int G = 32 / LPR;                 // rows per load instruction
+  constexpr int NP = WIN ? kWindowPlanes : NPLANES;
 #ifndef FI_MATCH_BATCH
 #define FI_MATCH_BATCH 16
 #endif
@@ -451,11 +456,14 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
   const int t = lane % LPR;  // position within the row
   const int g = lane / LPR;  // row group
   // per warp: two chain buffers (the next request's chain is staged while this one is matched) and the nodes
-  uint64_t* const s_chain_base = s_mem + (size_t)(2 * warp) * p.MP;  // buffer b at s_chain_base + b * MP
-  uint32_t* s_node = reinterpret_cast<uint32_t*>(s_mem + (size_t)2 * kWarps * p.MP) + (size_t)warp * p.MP;  // node of every block
+  // entries per buffer: a whole chain row, or one window.  An expression at each use, not a local: a local holding
+  // p.MP moved the register allocation of several unwindowed instantiations.
+#define SP (WIN ? (uint32_t)kWindow : p.MP)
+  uint64_t* const s_chain_base = s_mem + (size_t)(2 * warp) * SP;  // buffer b at s_chain_base + b * SP
+  uint32_t* s_node = reinterpret_cast<uint32_t*>(s_mem + (size_t)2 * kWarps * SP) + (size_t)warp * SP;  // node of every block
   uint16_t* s_row = nullptr;  // COUNTS: the warp's staging row
   if constexpr (COUNTS)
-    s_row = reinterpret_cast<uint16_t*>(s_mem + (size_t)2 * kWarps * p.MP) + (size_t)2 * kWarps * p.MP +
+    s_row = reinterpret_cast<uint16_t*>(s_mem + (size_t)2 * kWarps * SP) + (size_t)2 * kWarps * SP +
             (size_t)warp * (p.st.Epad + 16);
   const IndexView ix = p.ix;
   const uint32_t P = COUNTS ? 0u : p.st.n_profiles;  // COUNTS: no profile is scored
@@ -473,11 +481,21 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
     const uint64_t* crow = p.chain + (uint64_t)rr * p.MP;
     for (uint32_t u = lane; u < row_units; u += 32) cp_async16(dst + 2 * u, crow + 2 * u);
   };
+  // WIN: entries [w0, w0 + kWindow) of the row (w0 a multiple of kWindow; MP - w0 is even)
+  auto stage_window = [&](uint32_t rr, uint32_t w0, uint64_t* dst) {
+    const uint64_t* crow = p.chain + (uint64_t)rr * p.MP + w0;
+    const uint32_t units = min(p.MP - w0, (uint32_t)kWindow) / 2;
+    for (uint32_t u = lane; u < units; u += 32) cp_async16(dst + 2 * u, crow + 2 * u);
+  };
   uint32_t r_next = 0;
   if (lane == 0) r_next = take_ticket(p.work_counter, threadIdx.x & p.lane_zero);
   r_next = __shfl_sync(FULL, r_next, 0);
   int buf = 0;
-  if (r_next < p.R) stage(r_next, s_chain_base);
+  if constexpr (WIN) {
+    if (r_next < p.R) stage_window(r_next, 0, s_chain_base);
+  } else {
+    if (r_next < p.R) stage(r_next, s_chain_base);
+  }
   // prefetched home bucket of the current request's first block (valid when pf_ok)
   bool pf_ok = false;
   uint64_t pf_h = 0, pf_key = 0;
@@ -496,7 +514,7 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
         if (wi < p.sub_pitch) sub[x] = __ldg(p.subsets + (uint64_t)r * p.sub_pitch + wi);
       }
     }
-    uint64_t* s_chain = s_chain_base + (size_t)buf * p.MP;
+    uint64_t* s_chain = s_chain_base + (size_t)buf * SP;
 #ifdef FI_MATCH_TIMING
     const long long tm0 = clock64();
 #endif
@@ -519,8 +537,9 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
 
 #ifdef FI_MATCH_TIMING
     const long long tm1 = clock64();
+    long long tm2 = 0;
 #endif
-    BitCounter cnt[VEC];
+    BitCounter<NP> cnt[VEC];
     uint32_t alive[VEC];
 #pragma unroll
     for (int x = 0; x < VEC; ++x) {
@@ -529,71 +548,178 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
     }
     uint32_t matched_rows = 0;
     bool real_miss = false;
+    uint64_t h_first = 0;  // WIN: block 0's hash (the tie seed), read before the buffer holds a later window
+    if constexpr (WIN) h_first = n ? s_chain[0] : 0ull;
 
-    // ---- 2. the index node of every block up to the first one no endpoint holds ---------------
-    const uint32_t m_rows = resolve_request_nodes(ix, s_chain, s_node, n, lane, have_first, first_node);
-    real_miss = m_rows < n;
-    __syncwarp();  // s_node is written by some lanes and read by others
-    // ---- the next request: its ticket has long arrived; stage its chain and read its first hash
-    r_next = __shfl_sync(FULL, r_next, 0);
-    pf_ok = false;
-    if (r_next < p.R) {
-      stage(r_next, s_chain_base + (size_t)(buf ^ 1) * p.MP);
-      pf_h = __ldg(p.chain + (uint64_t)r_next * p.MP);
-    }
-#ifdef FI_MATCH_TIMING
-    const long long tm2 = clock64();
-#endif
-    // ---- 3. the rows of those blocks: independent loads, BATCH instructions (BATCH * G rows) in flight --
-#pragma unroll 1
-    for (uint32_t b0 = 0; b0 < m_rows; b0 += BATCH * G) {
-      uint32_t w[VEC][BATCH];
-#pragma unroll
-      for (int qi = 0; qi < BATCH; ++qi) {
-        const uint32_t j = b0 + qi * G + g;  // row this lane helps read; rows past the end read the permanently
-        const uint32_t sn = j < m_rows ? s_node[j] : zero_slot;  // zero row instead of being predicated off
-        uint32_t tmp[VEC];
-        load_row_words<VEC>(reinterpret_cast<const uint32_t*>(row_base + (uint64_t)sn * row_bytes), true, tmp);
-#pragma unroll
-        for (int x = 0; x < VEC; ++x) w[x][qi] = tmp[x];
+    if constexpr (!WIN) {
+      // ---- 2. the index node of every block up to the first one no endpoint holds ---------------
+      const uint32_t m_rows = resolve_request_nodes(ix, s_chain, s_node, n, lane, have_first, first_node);
+      real_miss = m_rows < n;
+      __syncwarp();  // s_node is written by some lanes and read by others
+      // ---- the next request: its ticket has long arrived; stage its chain and read its first hash
+      r_next = __shfl_sync(FULL, r_next, 0);
+      pf_ok = false;
+      if (r_next < p.R) {
+        stage(r_next, s_chain_base + (size_t)(buf ^ 1) * p.MP);
+        pf_h = __ldg(p.chain + (uint64_t)r_next * p.MP);
       }
-      if (LPM) {
+#ifdef FI_MATCH_TIMING
+      tm2 = clock64();
+#endif
+      // ---- 3. the rows of those blocks: independent loads, BATCH instructions (BATCH * G rows) in flight --
+#pragma unroll 1
+      for (uint32_t b0 = 0; b0 < m_rows; b0 += BATCH * G) {
+        uint32_t w[VEC][BATCH];
 #pragma unroll
         for (int qi = 0; qi < BATCH; ++qi) {
+          const uint32_t j = b0 + qi * G + g;  // row this lane helps read; rows past the end read the permanently
+          const uint32_t sn = j < m_rows ? s_node[j] : zero_slot;  // zero row instead of being predicated off
+          uint32_t tmp[VEC];
+          load_row_words<VEC>(reinterpret_cast<const uint32_t*>(row_base + (uint64_t)sn * row_bytes), true, tmp);
 #pragma unroll
-          for (int x = 0; x < VEC; ++x) {
-            uint32_t v = w[x][qi];
-            if (G > 1) {  // prefix-AND over the G rows of this instruction
+          for (int x = 0; x < VEC; ++x) w[x][qi] = tmp[x];
+        }
+        if (LPM) {
 #pragma unroll
-              for (int d = 1; d < G; d <<= 1) {
-                const uint32_t o = __shfl_up_sync(FULL, v, d * LPR);
-                if (g >= d) v &= o;
+          for (int qi = 0; qi < BATCH; ++qi) {
+#pragma unroll
+            for (int x = 0; x < VEC; ++x) {
+              uint32_t v = w[x][qi];
+              if (G > 1) {  // prefix-AND over the G rows of this instruction
+#pragma unroll
+                for (int d = 1; d < G; d <<= 1) {
+                  const uint32_t o = __shfl_up_sync(FULL, v, d * LPR);
+                  if (g >= d) v &= o;
+                }
+                v &= alive[x];
+                alive[x] = __shfl_sync(FULL, v, (G - 1) * LPR + t);
+              } else {
+                v &= alive[x];
+                alive[x] = v;
               }
-              v &= alive[x];
-              alive[x] = __shfl_sync(FULL, v, (G - 1) * LPR + t);
-            } else {
-              v &= alive[x];
-              alive[x] = v;
+              w[x][qi] = v;
             }
-            w[x][qi] = v;
           }
         }
+#pragma unroll
+        for (int x = 0; x < VEC; ++x) {
+          // membership rows are sparse: most 32-endpoint words of a batch are zero for every lane,
+          // and adding zeros is a no-op — skip the carry-save tree then (warp-uniform branch)
+          uint32_t any = 0;
+#pragma unroll
+          for (int qi = 0; qi < BATCH; ++qi) any |= w[x][qi];
+          if (__any_sync(FULL, any != 0)) bc_add<BATCH>(cnt[x], w[x]);
+        }
+        matched_rows = min(m_rows, b0 + BATCH * G);
+        if (LPM) {  // every local endpoint already dropped out: nothing more can match
+          bool any = false;
+#pragma unroll
+          for (int x = 0; x < VEC; ++x) any |= alive[x] != 0;
+          if (!__ballot_sync(FULL, any)) break;
+        }
       }
+    } else {
+      // the next request: its ticket has long arrived; stage its first window and read its first hash
+      auto stage_next_request = [&]() {
+        r_next = __shfl_sync(FULL, r_next, 0);
+        pf_ok = false;
+        if (r_next < p.R) {
+          stage_window(r_next, 0, s_chain_base + (size_t)(buf ^ 1) * SP);
+          pf_h = __ldg(p.chain + (uint64_t)r_next * p.MP);
+        }
+      };
+      // ---- 3. the rows of s_node[0, m_rows) (blocks w0 ..), as above.  Returns true when LPM has dropped every
+      // local endpoint.
+      auto read_rows = [&](uint32_t m_rows, uint32_t w0) -> bool {
+#pragma unroll 1
+        for (uint32_t b0 = 0; b0 < m_rows; b0 += BATCH * G) {
+          uint32_t w[VEC][BATCH];
 #pragma unroll
-      for (int x = 0; x < VEC; ++x) {
-        // membership rows are sparse: most 32-endpoint words of a batch are zero for every lane,
-        // and adding zeros is a no-op — skip the carry-save tree then (warp-uniform branch)
-        uint32_t any = 0;
+          for (int qi = 0; qi < BATCH; ++qi) {
+            const uint32_t j = b0 + qi * G + g;  // row this lane helps read; rows past the end read the permanently
+            const uint32_t sn = j < m_rows ? s_node[j] : zero_slot;  // zero row instead of being predicated off
+            uint32_t tmp[VEC];
+            load_row_words<VEC>(reinterpret_cast<const uint32_t*>(row_base + (uint64_t)sn * row_bytes), true, tmp);
 #pragma unroll
-        for (int qi = 0; qi < BATCH; ++qi) any |= w[x][qi];
-        if (__any_sync(FULL, any != 0)) bc_add<BATCH>(cnt[x], w[x]);
-      }
-      matched_rows = min(m_rows, b0 + BATCH * G);
-      if (LPM) {  // every local endpoint already dropped out: nothing more can match
-        bool any = false;
+            for (int x = 0; x < VEC; ++x) w[x][qi] = tmp[x];
+          }
+          if (LPM) {
 #pragma unroll
-        for (int x = 0; x < VEC; ++x) any |= alive[x] != 0;
-        if (!__ballot_sync(FULL, any)) break;
+            for (int qi = 0; qi < BATCH; ++qi) {
+#pragma unroll
+              for (int x = 0; x < VEC; ++x) {
+                uint32_t v = w[x][qi];
+                if (G > 1) {  // prefix-AND over the G rows of this instruction
+#pragma unroll
+                  for (int d = 1; d < G; d <<= 1) {
+                    const uint32_t o = __shfl_up_sync(FULL, v, d * LPR);
+                    if (g >= d) v &= o;
+                  }
+                  v &= alive[x];
+                  alive[x] = __shfl_sync(FULL, v, (G - 1) * LPR + t);
+                } else {
+                  v &= alive[x];
+                  alive[x] = v;
+                }
+                w[x][qi] = v;
+              }
+            }
+          }
+#pragma unroll
+          for (int x = 0; x < VEC; ++x) {
+            // membership rows are sparse: most 32-endpoint words of a batch are zero for every lane,
+            // and adding zeros is a no-op — skip the carry-save tree then (warp-uniform branch)
+            uint32_t any = 0;
+#pragma unroll
+            for (int qi = 0; qi < BATCH; ++qi) any |= w[x][qi];
+            if (__any_sync(FULL, any != 0)) bc_add<BATCH>(cnt[x], w[x]);
+          }
+          matched_rows = w0 + min(m_rows, b0 + BATCH * G);
+          if (LPM) {  // every local endpoint already dropped out: nothing more can match
+            bool any = false;
+#pragma unroll
+            for (int x = 0; x < VEC; ++x) any |= alive[x] != 0;
+            if (!__ballot_sync(FULL, any)) return true;
+          }
+        }
+        return false;
+      };
+
+      // blocks [w0, w0 + nw) are in s_chain
+      uint32_t w0 = 0;
+#pragma unroll 1
+      for (;;) {
+        const uint32_t nw = min(n - w0, (uint32_t)kWindow);
+        const uint32_t m_rows = resolve_request_nodes(ix, s_chain, s_node, nw, lane, have_first, first_node);
+        real_miss = m_rows < nw;
+        __syncwarp();
+        // the walk goes on into the next window (every block of this one is cached): stage that window instead
+        const bool more = !real_miss && w0 + nw < n;
+        if (more)
+          stage_window(r, w0 + kWindow, s_chain_base + (size_t)(buf ^ 1) * SP);
+        else
+          stage_next_request();
+#ifdef FI_MATCH_TIMING
+        tm2 = clock64();
+#endif
+        const bool dead = read_rows(m_rows, w0);
+        if (!more) break;
+        if (LPM && dead) {  // the staged window goes unread: the next request's first window takes its buffer
+          cp_async_wait_all();  // (lane u % 32 writes unit u in both stagings, so each lane orders its own copies)
+          stage_next_request();
+          break;
+        }
+        // the next window.  Its block 0 continues the run of consecutive nodes (index_device.cuh) when klog holds
+        // its hash at the previous block's node + 1; else resolve_request_nodes looks it up in the table.
+        const uint32_t prev = s_node[kWindow - 1];
+        w0 += kWindow;
+        buf ^= 1;
+        s_chain = s_chain_base + (size_t)buf * SP;
+        cp_async_wait_all();
+        __syncwarp();  // the window is staged for every lane, and this window's s_node reads are done
+        const uint64_t h = s_chain[0];
+        first_node = prev + 1;
+        have_first = first_node < ix.C && !key_is_special(h) && __ldg(ix.klog + first_node) == h;
       }
     }
 
@@ -615,26 +741,26 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
       for (int x = 0; x < VEC; ++x) {
 #pragma unroll
         for (int d = LPR; d < 32; d <<= 1) {
-          BitCounter o;
+          BitCounter<NP> o;
 #pragma unroll
-          for (int pl = 0; pl < NPLANES; ++pl) o.c[pl] = __shfl_xor_sync(FULL, cnt[x].c[pl], d);
+          for (int pl = 0; pl < NP; ++pl) o.c[pl] = __shfl_xor_sync(FULL, cnt[x].c[pl], d);
           bc_merge(cnt[x], o);
         }
       }
     }
-    if constexpr (COUNTS) counts_row<VEC, G>(p, cnt, r, nothing, s_row, lane, t, g);
+    if constexpr (COUNTS) counts_row<VEC, G, NP>(p, cnt, r, nothing, s_row, lane, t, g);
 
     // ---- 4./5. score candidates, argmax, PD rule ---------------------------------
     TieRot tr;
     tr.E = p.E_global;
     tr.ep_begin = p.ep_begin;
-    tr.start = tie_start(tie_seed(n, n ? s_chain[0] : 0ull, n ? 0ull : p.h0[r], p.r_base + r), p.E_global);
+    tr.start = tie_start(tie_seed(n, WIN ? h_first : (n ? s_chain[0] : 0ull), n ? 0ull : p.h0[r], p.r_base + r), p.E_global);
     uint32_t dec_e = FI_NO_ENDPOINT, dec_m = 0;
 #pragma unroll
     for (int pi = 0; pi < (int)FI_EPP_MAX_PROFILES; ++pi) {
       if (pi < (int)P) {
         if constexpr (RANKED) {
-          ranked_profile<VEC, G, SUBSET>(p, (uint32_t)pi, cnt, sub, tr, n, r, lane, t, g, dec_e, dec_m);
+          ranked_profile<VEC, G, SUBSET, NP>(p, (uint32_t)pi, cnt, sub, tr, n, r, lane, t, g, dec_e, dec_m);
           continue;
         }
         const ProfileDev& pr = p.st.prof[pi];
@@ -782,6 +908,22 @@ __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MI
     buf ^= 1;
     __syncwarp();  // this request's s_chain / s_node reads are done before the buffers are written again
   }
+}
+
+#undef SP
+
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
+__global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MIN_BLOCKS : FI_MATCH_MIN_BLOCKS + 1))
+    match_pick_kernel(const MatchParams p) {
+  match_pick_body<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS, false>(p);
+}
+
+// chains longer than one window (max_blocks > 1023): the same CTA shape, warps and shared memory per warp as
+// match_pick_kernel at MP = kWindow
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
+__global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MIN_BLOCKS : FI_MATCH_MIN_BLOCKS + 1))
+    match_window_kernel(const MatchParams p) {
+  match_pick_body<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS, true>(p);
 }
 
 // multi-GPU: reduce the ranks' local picks (score desc, then the request's tie rotation), then the PD rule
@@ -961,10 +1103,12 @@ std::mutex g_match_launch_mu;
 
 // One instantiation per kernel variant: the shared-memory opt-in (cudaFuncSetAttribute) applies to one function
 // only, and occupancy differs between variants, so each variant keeps its own state, per device.
-template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
+template <bool WIN, int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
 cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_t s) {
-  const auto kern = match_pick_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS>;
-  size_t smem = (size_t)kWarps * p.MP * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
+  const auto kern = WIN ? match_window_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS>
+                        : match_pick_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS>;
+  const size_t sp = WIN ? (size_t)kWindow : p.MP;  // entries per staging buffer
+  size_t smem = (size_t)kWarps * sp * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
   if (COUNTS) smem += (size_t)kWarps * (p.st.Epad + 16) * sizeof(uint16_t);        // + the staging rows
   static std::map<int, size_t> opted_in;                // device -> the variant's max dynamic smem attribute
   static std::map<std::pair<int, size_t>, int> per_sm;  // (device, smem) -> resident CTAs per SM
@@ -1001,44 +1145,52 @@ cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_
   return cudaGetLastError();
 }
 
-template <int LPR, int VEC>
+template <int LPR, int VEC, bool WIN>
 cudaError_t launch_match_t(const MatchParams& p, int sm_count, cudaStream_t s) {
   const bool lpm = p.lpm == FI_MATCH_LPM;
   if (p.counts)  // match counts (S.3a): no profile is scored
-    return lpm ? launch_match_variant<LPR, VEC, true, false, false, false, true>(p, sm_count, s)
-               : launch_match_variant<LPR, VEC, false, false, false, false, true>(p, sm_count, s);
+    return lpm ? launch_match_variant<WIN, LPR, VEC, true, false, false, false, true>(p, sm_count, s)
+               : launch_match_variant<WIN, LPR, VEC, false, false, false, false, true>(p, sm_count, s);
   if (p.k && p.subsets)  // ranked pick over per-request candidate subsets
-    return lpm ? launch_match_variant<LPR, VEC, true, false, true, true>(p, sm_count, s)
-               : launch_match_variant<LPR, VEC, false, false, true, true>(p, sm_count, s);
+    return lpm ? launch_match_variant<WIN, LPR, VEC, true, false, true, true>(p, sm_count, s)
+               : launch_match_variant<WIN, LPR, VEC, false, false, true, true>(p, sm_count, s);
   if (p.k)  // ranked pick: the LoRA scorer is handled at run time inside the variant
-    return lpm ? launch_match_variant<LPR, VEC, true, false, true>(p, sm_count, s)
-               : launch_match_variant<LPR, VEC, false, false, true>(p, sm_count, s);
+    return lpm ? launch_match_variant<WIN, LPR, VEC, true, false, true>(p, sm_count, s)
+               : launch_match_variant<WIN, LPR, VEC, false, false, true>(p, sm_count, s);
   if (p.st.has_lora)
-    return lpm ? launch_match_variant<LPR, VEC, true, true, false>(p, sm_count, s)
-               : launch_match_variant<LPR, VEC, false, true, false>(p, sm_count, s);
-  return lpm ? launch_match_variant<LPR, VEC, true, false, false>(p, sm_count, s)
-             : launch_match_variant<LPR, VEC, false, false, false>(p, sm_count, s);
+    return lpm ? launch_match_variant<WIN, LPR, VEC, true, true, false>(p, sm_count, s)
+               : launch_match_variant<WIN, LPR, VEC, false, true, false>(p, sm_count, s);
+  return lpm ? launch_match_variant<WIN, LPR, VEC, true, false, false>(p, sm_count, s)
+             : launch_match_variant<WIN, LPR, VEC, false, false, false>(p, sm_count, s);
+}
+
+template <bool WIN>
+cudaError_t launch_match_w(const MatchParams& p, int sm_count, cudaStream_t s) {
+  // Words per row = LPR * VEC.  Two words per lane (half the counter registers of VEC = 4 -> three CTAs
+  // = 24 warps per SM instead of 16): the kernel is bound by per-warp instruction latency and wants warps, not
+  // wide loads (E = 1024, cfg 3 on one H100 SXM, 700 W: match_pick 74.5 us with two words per lane vs 98.1-98.4 us
+  // with four, two runs each).
+  switch (p.ix.W) {
+    case 1: return launch_match_t<1, 1, WIN>(p, sm_count, s);
+    case 2: return launch_match_t<1, 2, WIN>(p, sm_count, s);
+    case 4: return launch_match_t<2, 2, WIN>(p, sm_count, s);
+    case 8: return launch_match_t<4, 2, WIN>(p, sm_count, s);
+    case 16: return launch_match_t<8, 2, WIN>(p, sm_count, s);
+    case 32: return launch_match_t<16, 2, WIN>(p, sm_count, s);
+    case 64: return launch_match_t<32, 2, WIN>(p, sm_count, s);
+    case 128: return launch_match_t<32, 4, WIN>(p, sm_count, s);
+    default: return cudaErrorInvalidValue;
+  }
 }
 
 }  // namespace
 
 cudaError_t launch_match_pick(const MatchParams& p, int sm_count, cudaStream_t s) {
   if (p.R == 0) return cudaSuccess;
-  // Words per row = LPR * VEC.  Two words per lane (half the counter registers of VEC = 4 -> three CTAs
-  // = 24 warps per SM instead of 16): the kernel is bound by per-warp instruction latency and wants warps, not
-  // wide loads (E = 1024, cfg 3 on one H100 SXM, 700 W: match_pick 74.5 us with two words per lane vs 98.1-98.4 us
-  // with four, two runs each).
-  switch (p.ix.W) {
-    case 1: return launch_match_t<1, 1>(p, sm_count, s);
-    case 2: return launch_match_t<1, 2>(p, sm_count, s);
-    case 4: return launch_match_t<2, 2>(p, sm_count, s);
-    case 8: return launch_match_t<4, 2>(p, sm_count, s);
-    case 16: return launch_match_t<8, 2>(p, sm_count, s);
-    case 32: return launch_match_t<16, 2>(p, sm_count, s);
-    case 64: return launch_match_t<32, 2>(p, sm_count, s);
-    case 128: return launch_match_t<32, 4>(p, sm_count, s);
-    default: return cudaErrorInvalidValue;
-  }
+  // A handle whose chains can be longer than 1023 blocks runs the windowed variant: a count of 1024 or more needs
+  // its 12 bit-planes, and a longer chain does not fit one staging buffer (DESIGN.md §4.9).
+  if (p.max_blocks > (1u << NPLANES) - 1) return launch_match_w<true>(p, sm_count, s);
+  return launch_match_w<false>(p, sm_count, s);
 }
 
 cudaError_t launch_merge_picks(const MergeParams& p, cudaStream_t s) {

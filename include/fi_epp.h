@@ -71,7 +71,8 @@ extern "C" {
 #define FI_EPP_MAX_SCORERS 4u
 #define FI_EPP_MAX_FILTERS 4u /* by-label filters per profile */
 #define FI_EPP_MAX_LABELS 24u /* (label, value) pairs a configuration can filter on */
-#define FI_EPP_MAX_BLOCKS 1023u /* counts are kept in 10 bit-planes on the GPU */
+#define FI_EPP_MAX_BLOCKS 4095u /* counts are kept in 12 bit-planes on the GPU.  A handle with max_blocks > 1023
+                                 * serves every single-rank call; fi_epp_comm_init refuses it (FI_ERR_STATE). */
 #define FI_NO_ENDPOINT 0xFFFFFFFFu
 #define FI_EPP_UNIQUE_ID_BYTES 128u
 
@@ -555,7 +556,8 @@ void* fi_epp_pinned_alloc(size_t bytes);
 void fi_epp_pinned_free(void* p);
 
 /* Multi-GPU (one handle per GPU, endpoint-range shards).  Rank 0 makes an id,
- * the host distributes it out of band, every rank calls comm_init. */
+ * the host distributes it out of band, every rank calls comm_init.  A handle with max_blocks > 1023 cannot be
+ * sharded: comm_init returns FI_ERR_STATE. */
 int fi_epp_comm_unique_id(uint8_t out[FI_EPP_UNIQUE_ID_BYTES]);
 int fi_epp_comm_init(fi_epp* h, const uint8_t id[FI_EPP_UNIQUE_ID_BYTES], uint32_t rank, uint32_t world);
 /* Must precede the first index update of the handle.  How the sharded pick reduces the ranks' local
