@@ -13,6 +13,7 @@ from .picker import (  # noqa: F401
     EndpointPicker,
     FiEppError,
     PinnedBuffer,
+    SnapshotCapture,
     config_from_yaml,
     config_picker_endpoints,
     default_config,
@@ -26,6 +27,7 @@ __all__ = [
     "EndpointPicker",
     "FiEppError",
     "PinnedBuffer",
+    "SnapshotCapture",
     "config_from_yaml",
     "config_picker_endpoints",
     "default_config",

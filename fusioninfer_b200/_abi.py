@@ -233,6 +233,9 @@ SYMBOLS = [
     ("fi_epp_snapshot_save", C.c_int, [_P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
     ("fi_epp_snapshot_load", C.c_int, [_P, _P, C.c_uint64]),
     ("fi_epp_snapshot_info", C.c_int, [_P, C.c_uint64, C.POINTER(fi_epp_snapshot_info)]),
+    ("fi_epp_snapshot_capture", C.c_int, [_P, C.POINTER(_P), C.POINTER(C.c_uint64)]),
+    ("fi_epp_snapshot_read", C.c_int, [_P, _P, C.c_uint64]),
+    ("fi_epp_snapshot_free", None, [_P]),
     ("fi_epp_set_lru_capacities", C.c_int, [_P, _P, _P, C.c_uint32, _P]),
     ("fi_epp_index_add_chain", C.c_int, [_P, C.c_uint32, _P, C.c_uint32]),
     ("fi_epp_index_add_chains", C.c_int, [_P, _P, _P, C.c_uint32, _P, C.c_uint32]),

@@ -433,7 +433,10 @@ __device__ __forceinline__ uint32_t snap_rank(bool flag) {
   return s_w[warp] + __popc(m & ((1u << lane) - 1u));
 }
 
-__global__ void __launch_bounds__(kSnapTile) index_snap_count_kernel(IndexView ix, uint64_t n, uint32_t* tile_live) {
+// (n = min(ctr->used, C) is read here, so that the host learns it in the same readback as the tile counts; the grid
+// covers the tiles of C + 2 items, and the tiles past n + 2 count 0)
+__global__ void __launch_bounds__(kSnapTile) index_snap_count_kernel(IndexView ix, const IndexCounters* ctr, uint32_t* tile_live) {
+  const uint64_t used = ctr->used, n = used < ix.C ? used : ix.C;
   const uint64_t t = (uint64_t)blockIdx.x * kSnapTile + threadIdx.x;
   const bool live = t < n + 2 && snap_live(ix, sweep_node(ix, t, n));
   const int c = __syncthreads_count(live);
@@ -563,8 +566,8 @@ cudaError_t launch_index_contains(IndexView ix, const fi_index_op* q, uint64_t n
 
 uint32_t index_snap_tiles(uint64_t n) { return (uint32_t)((n + 2 + kSnapTile - 1) / kSnapTile); }
 
-cudaError_t launch_index_snap_count(IndexView ix, uint64_t n, uint32_t* tile_live, cudaStream_t s) {
-  index_snap_count_kernel<<<index_snap_tiles(n), kSnapTile, 0, s>>>(ix, n, tile_live);
+cudaError_t launch_index_snap_count(IndexView ix, const IndexCounters* ctr, uint32_t* tile_live, cudaStream_t s) {
+  index_snap_count_kernel<<<index_snap_tiles(ix.C), kSnapTile, 0, s>>>(ix, ctr, tile_live);
   return cudaGetLastError();
 }
 

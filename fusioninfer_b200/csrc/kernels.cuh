@@ -249,11 +249,13 @@ inline bool remove_whole_rows(const RemoveSet& rs, uint32_t W) {
 cudaError_t launch_index_contains(IndexView ix, const fi_index_op* q, uint64_t n, uint32_t ep_begin,
                                   uint32_t ep_count, uint8_t* out, cudaStream_t s);
 // Snapshots (index_kernels.cu).  Export walks the regular nodes [0, n) (n = min(used, C)) and the markers C, C+1 in
-// index_snap_tiles(n) tiles: the count pass writes every tile's live nodes; the export of tiles [t0, t1) writes their
-// keys and their rows narrowed to We words at tile_off[t] - base.  Import inserts n blob nodes starting at blob
-// position g0 into fresh tables (m0, m1: the blob positions of the keys 0 and ~0, or ~0); *dup != 0: a key repeats.
+// index_snap_tiles(n) tiles: the count pass reads n from ctr and writes the live nodes of each of the
+// index_snap_tiles(C) tiles (0 past the walk); the export of tiles [t0, t1) writes their keys and their rows narrowed
+// to We words at tile_off[t] - base (64-bit offsets: one export may cover every tile).  Import inserts n blob nodes
+// starting at blob position g0 into fresh tables (m0, m1: the blob positions of the keys 0 and ~0, or ~0); *dup != 0:
+// a key repeats.
 uint32_t index_snap_tiles(uint64_t n);
-cudaError_t launch_index_snap_count(IndexView ix, uint64_t n, uint32_t* tile_live, cudaStream_t s);
+cudaError_t launch_index_snap_count(IndexView ix, const IndexCounters* ctr, uint32_t* tile_live, cudaStream_t s);
 cudaError_t launch_index_snap_export(IndexView ix, uint64_t n, uint32_t t0, uint32_t t1, const uint64_t* tile_off, uint64_t base,
                                      uint32_t We, uint64_t* keys, uint32_t* rows, cudaStream_t s);
 cudaError_t launch_index_snap_import(IndexView ix, IndexCounters* ctr, const uint64_t* keys, const uint32_t* rows, uint64_t n,

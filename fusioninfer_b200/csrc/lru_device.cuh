@@ -69,9 +69,11 @@ cudaError_t launch_lru_shrink(const DevLru& lru, const uint32_t* eps, const uint
 cudaError_t launch_lru_reset(const DevLru& lru, const uint32_t* eps, uint32_t n, cudaStream_t s);
 // diagnostics: the live keys of local endpoint e, least recently used first
 cudaError_t launch_lru_dump(const DevLru& lru, uint32_t e, uint64_t* out, uint32_t* n_out, cudaStream_t s);
-// snapshots: every endpoint's live keys, oldest first, endpoint e's at out + off[e] (n_out[e]: how many); and the load
-// of every endpoint's LRU into a fresh store from len[e] keys at keys + off[e] (*dup != 0: a key repeats in an LRU)
-cudaError_t launch_lru_dump_all(const DevLru& lru, const uint64_t* off, uint64_t* out, uint32_t* n_out, cudaStream_t s);
+// snapshots: every endpoint's live keys, oldest first, endpoint e's at out + off[e] (n_out[e]: how many; bad != null:
+// *bad = 1 where that differs from count[e], a broken invariant); and the load of every endpoint's LRU into a fresh
+// store from len[e] keys at keys + off[e] (*dup != 0: a key repeats in an LRU)
+cudaError_t launch_lru_dump_all(const DevLru& lru, const uint64_t* off, uint64_t* out, uint32_t* n_out, uint32_t* bad,
+                                cudaStream_t s);
 cudaError_t launch_lru_load(const DevLru& lru, const uint64_t* keys, const uint64_t* off, const uint32_t* len, uint32_t* dup,
                             cudaStream_t s);
 

@@ -478,9 +478,10 @@ __global__ void __launch_bounds__(256) lru_reset_kernel(DevLru lru, const uint32
 }
 
 // the live keys of endpoints e0 + blockIdx.x, oldest first, one CTA each: to out + off[blockIdx.x] (off == null: out),
-// and their number to n_out[blockIdx.x] (fi_epp_lru_dump: one endpoint; a snapshot: all of them)
+// and their number to n_out[blockIdx.x] (fi_epp_lru_dump: one endpoint; a snapshot: all of them); bad != null: *bad = 1
+// if that number is not count[e]
 __global__ void __launch_bounds__(256) lru_dump_kernel(DevLru lru, uint32_t e0, const uint64_t* __restrict__ off, uint64_t* out,
-                                                       uint32_t* n_out) {
+                                                       uint32_t* n_out, uint32_t* bad) {
   const uint32_t e = e0 + blockIdx.x;
   if (off) out += off[blockIdx.x];
   n_out += blockIdx.x;
@@ -502,7 +503,10 @@ __global__ void __launch_bounds__(256) lru_dump_kernel(DevLru lru, uint32_t e0, 
     if (live) out[d + rank] = key;
     d += tot;
   }
-  if (threadIdx.x == 0) *n_out = d;
+  if (threadIdx.x == 0) {
+    *n_out = d;
+    if (bad && d != lru.count[e]) atomicExch(bad, 1u);
+  }
 }
 
 // ---- load: every endpoint's LRU from a snapshot (fi_epp_snapshot_load), one CTA per endpoint --------------------
@@ -585,11 +589,12 @@ cudaError_t launch_lru_reset(const DevLru& lru, const uint32_t* eps, uint32_t n,
   return cudaGetLastError();
 }
 cudaError_t launch_lru_dump(const DevLru& lru, uint32_t e, uint64_t* out, uint32_t* n_out, cudaStream_t s) {
-  lru_dump_kernel<<<1, 256, 0, s>>>(lru, e, nullptr, out, n_out);
+  lru_dump_kernel<<<1, 256, 0, s>>>(lru, e, nullptr, out, n_out, nullptr);
   return cudaGetLastError();
 }
-cudaError_t launch_lru_dump_all(const DevLru& lru, const uint64_t* off, uint64_t* out, uint32_t* n_out, cudaStream_t s) {
-  lru_dump_kernel<<<lru.EL, 256, 0, s>>>(lru, 0, off, out, n_out);
+cudaError_t launch_lru_dump_all(const DevLru& lru, const uint64_t* off, uint64_t* out, uint32_t* n_out, uint32_t* bad,
+                                cudaStream_t s) {
+  lru_dump_kernel<<<lru.EL, 256, 0, s>>>(lru, 0, off, out, n_out, bad);
   return cudaGetLastError();
 }
 cudaError_t launch_lru_load(const DevLru& lru, const uint64_t* keys, const uint64_t* off, const uint32_t* len, uint32_t* dup,

@@ -153,6 +153,44 @@ def snapshot_info(buf) -> abi.fi_epp_snapshot_info:
     return out
 
 
+class SnapshotCapture:
+    """A snapshot taken on the device by EndpointPicker.capture_snapshot() (docs/SPEC.md S.2d).  read() gives the
+    bytes save_snapshot() would have returned at the capture's point; it never touches the picker, so it may run on
+    another thread, and after the picker is resized, loaded or closed.  close() frees the device image."""
+
+    def __init__(self, lib, c: C.c_void_p, nbytes: int):
+        self._lib = lib
+        self._c = c
+        self.nbytes = nbytes
+
+    def read(self) -> np.ndarray:
+        """The snapshot blob; blocks until the device image is complete.  Repeatable: the same bytes every time."""
+        if not self._c:
+            raise ValueError("snapshot capture is closed")
+        buf = np.empty(self.nbytes, dtype=np.uint8)
+        rc = self._lib.fi_epp_snapshot_read(self._c, _ptr(buf), len(buf))
+        if rc != abi.FI_OK:
+            raise FiEppError(rc, "fi_epp_snapshot_read")
+        return buf
+
+    def close(self):
+        if getattr(self, "_c", None):
+            self._lib.fi_epp_snapshot_free(self._c)
+            self._c = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 class EndpointPicker:
     """One handle = one GPU = one endpoint-range shard of the pool."""
 
@@ -236,6 +274,16 @@ class EndpointPicker:
         buf = np.empty(n.value, dtype=np.uint8)
         self._check(self._lib.fi_epp_snapshot_save(self._h, _ptr(buf), len(buf), C.byref(n)), "fi_epp_snapshot_save")
         return buf
+
+    def capture_snapshot(self) -> SnapshotCapture:
+        """Take a snapshot on the device at this point of the call order, without waiting for picks in flight; copy
+        it out with .read() (any thread, the picker not needed) and free it with .close().  The device image (the
+        blob's size) is held until then; FiEppError(FI_ERR_NOMEM) when it does not fit, where save_snapshot() still
+        works."""
+        c = C.c_void_p()
+        n = C.c_uint64(0)
+        self._check(self._lib.fi_epp_snapshot_capture(self._h, C.byref(c), C.byref(n)), "fi_epp_snapshot_capture")
+        return SnapshotCapture(self._lib, c, n.value)
 
     def load_snapshot(self, buf) -> None:
         """Replace the index, the LRUs and their capacities with a snapshot's: afterwards the handle behaves like the

@@ -340,6 +340,34 @@ struct fi_epp_snapshot_info {
  * FI_ERR_STATE on a sharded pool, on a handle over part of the pool, or on a handle the host LRU serves. */
 int fi_epp_snapshot_save(fi_epp* h, void* buf, uint64_t cap, uint64_t* bytes);
 
+/* Snapshot captures (docs/SPEC.md S.2d): a snapshot taken on the device at a point in h's call order, copied out
+ * later without h, so that periodic saves do not stall the serving loop.  Owned by the library. */
+typedef struct fi_epp_capture fi_epp_capture;
+
+/* Take a snapshot of h on the device.  *bytes = the size of its blob, *out = the capture.  Point in time: every call
+ * issued on h before it is in the blob (staged ops, stream-ordered and fi_epp_index_add_submitted Adds, removals,
+ * capacity changes, resizes, loads); no later call is.  It does not wait for pick batches in flight, and later picks
+ * do not wait for it; later index updates run after its device work, in s_index order.  It holds h only to flush the
+ * staged ops, for one synchronisation of the index stream (the sizes), to allocate the device image (one buffer of
+ * the payload size, held until fi_epp_snapshot_free) and to queue the export.  Errors leave *out NULL, allocate
+ * nothing and leave h unchanged: FI_ERR_INVALID for NULL arguments; FI_ERR_STATE as for fi_epp_snapshot_save;
+ * FI_ERR_NOMEM if the image does not fit on the device (fi_epp_snapshot_save, which needs only bounded staging, is
+ * the fallback). */
+int fi_epp_snapshot_capture(fi_epp* h, fi_epp_capture** out, uint64_t* bytes);
+
+/* Write the capture's blob to buf: exactly the bytes fi_epp_snapshot_save would have written had it been called in
+ * place of fi_epp_snapshot_capture.  Never takes or touches the handle, so it may run on any thread while others use
+ * h, and after fi_epp_resize_pool, fi_epp_snapshot_load or fi_epp_destroy(h).  Blocks until the device image is
+ * complete; buf is ordinary pageable memory, filled through bounded pinned staging; the checksum is computed on host
+ * threads.  Repeatable: every read gives the same bytes.  cap < the blob's size: FI_ERR_CAPACITY, nothing written.
+ * FI_ERR_STATE (nothing written) if the device LRU's invariant was found broken, as the save reports it.  Calls on one
+ * capture must not overlap. */
+int fi_epp_snapshot_read(fi_epp_capture* c, void* buf, uint64_t cap);
+
+/* Release a capture (NULL: no-op).  Allowed while its device work still runs, with or without a read, and after h is
+ * destroyed; it does not stall h's streams. */
+void fi_epp_snapshot_free(fi_epp_capture* c);
+
 /* Replace h's index, LRUs and LRU capacities with the snapshot's.  h must have the block_bytes, max_blocks,
  * lru_capacity and num_endpoints of the handle that saved it; its index_slots, LRU table size and device may differ.
  * Afterwards h behaves exactly like the saved handle at the moment of the save, for every later call sequence, except
