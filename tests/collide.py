@@ -72,7 +72,7 @@ def pow2_ceil(x: int) -> int:
 
 
 def dlru_table_slots(C: int, lru_table_slots: int) -> int:
-    """TS of a device LRU of capacity C with the option lru_table_slots pinned (engine.cu, alloc_dev_lru:
+    """TS of a device LRU of capacity C with the option lru_table_slots pinned (engine_lru.cu, alloc_dev_lru:
     L = max(pow2_ceil(4 C), 64); TS = max(L, pow2_ceil(lru_table_slots)))"""
     assert lru_table_slots > 0, "the tests pin lru_table_slots: unpinned, TS depends on the free HBM"
     return max(max(pow2_ceil(4 * C), 64), pow2_ceil(lru_table_slots))

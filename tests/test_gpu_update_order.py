@@ -9,7 +9,7 @@ the pinned ones below, and index membership (index_contains) and every pick must
 (tests/resize_oracle.py).
 
 The pinned deltas are what the library gave before every update was ordered through update_begin / update_end
-(engine.cu), measured by running this file with FI_EPP_LIB=<that build of libfi_epp.so>: the same kernels and the
+(engine_index.cu), measured by running this file with FI_EPP_LIB=<that build of libfi_epp.so>: the same kernels and the
 same copies in the same order.
 """
 import numpy as np
