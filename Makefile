@@ -15,11 +15,8 @@ CU_OBJS := $(patsubst $(CSRC)/%.cu,$(OBJDIR)/%.o,$(CU_SRCS))
 HDRS := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/fi_epp.h
 
 EXT_ORACLE := $(OBJDIR)/libepp_ext_oracle.so
-RESIZE_ORACLE := $(OBJDIR)/libepp_resize_oracle.so
-SNAPSHOT_ORACLE := $(OBJDIR)/libepp_snapshot_oracle.so
-COUNTS_ORACLE := $(OBJDIR)/libepp_counts_oracle.so
 
-all: $(LIB) $(HOSTCHECK) oracle $(EXT_ORACLE) $(RESIZE_ORACLE) $(SNAPSHOT_ORACLE) $(COUNTS_ORACLE)
+all: $(LIB) $(HOSTCHECK) oracle $(EXT_ORACLE)
 
 $(OBJDIR)/%.o: $(CSRC)/%.cu $(HDRS)
 	@mkdir -p $(OBJDIR)
@@ -42,16 +39,11 @@ oracle:
 	$(MAKE) -C oracle
 
 # a test-side extension of the CPU oracle, tests/<name>.cpp -> build/libepp_<name>.so (test infrastructure only):
-# tests/ext_oracle.cpp adds the ranked / subset pick and per-endpoint LRU capacities
+# tests/ext_oracle.cpp adds the ranked / subset pick, per-endpoint LRU capacities, the shard view, match counts, the
+# pool resize and the state of an index snapshot
 $(OBJDIR)/libepp_%.so: tests/%.cpp oracle/epp_oracle.cpp include/fi_epp.h
 	@mkdir -p $(OBJDIR)
 	$(CXX) -O2 -std=c++17 -ffp-contract=off -fPIC -Wall -Wextra -pthread -shared -o $@ $<
-# tests/resize_oracle.cpp adds the pool resize on top of tests/ext_oracle.cpp
-$(RESIZE_ORACLE): tests/ext_oracle.cpp
-# tests/snapshot_oracle.cpp adds the state of an index snapshot on top of tests/resize_oracle.cpp
-$(SNAPSHOT_ORACLE): tests/ext_oracle.cpp tests/resize_oracle.cpp
-# tests/counts_oracle.cpp adds the match counts of fi_epp_match_counts on top of tests/ext_oracle.cpp
-$(COUNTS_ORACLE): tests/ext_oracle.cpp
 
 clean:
 	rm -rf $(OBJDIR) $(LIB) $(HOSTCHECK)

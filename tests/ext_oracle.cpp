@@ -8,6 +8,10 @@
 //   * the shard view (S.2e): a handle over endpoints [lo, lo + cnt) of the pool.  Its Adds and capacity changes skip
 //     the other endpoints, and its ranked pick ranks only its own endpoints, with the queue scorer's min / max still
 //     taken over the whole pool.  (Index ops addressed elsewhere are dropped by the wrapper, tests/ext_oracle.py.)
+//   * the match counts of fi_epp_match_counts (S.3a), from the ranked pick's own walk;
+//   * the per-endpoint part of fi_epp_resize_pool (S.2c);
+//   * the state of an index snapshot (S.2d), read and written whole: the pair set, every endpoint's capacity and,
+//     with the LRU lists of epx_lru_dump, epx_load_state, which replaces all three.
 // The handle is the oracle's own plus the capacities, so every epo_* function of the oracle works on it too.  The
 // oracle itself is left as it is: its single pick stays the yardstick of fi_epp_pick_batch.
 #include "../oracle/epp_oracle.cpp"
@@ -133,6 +137,28 @@ void shrink_to_cap(ExtOracle* o, uint32_t e, Emit&& emit) {
     emit(old);
   }
 }
+
+// The oracle's index keeps its slots private.  An explicit instantiation may name a private member, which lets the pair
+// enumeration read them without changing the oracle.
+using SlotsMember = std::vector<Slot> PodIndex::*;
+SlotsMember slots_member();
+template <SlotsMember M>
+struct SlotsAccess {
+  friend SlotsMember slots_member() { return M; }
+};
+template struct SlotsAccess<&PodIndex::slots_>;
+
+template <class Visit>
+void for_each_pair(const ExtOracle& o, Visit&& visit) {
+  for (const Slot& s : o.index.*slots_member()) {
+    if (!s.used) continue;
+    const uint32_t* m = s.ext ? s.ext->data() : s.inl;
+    for (uint32_t j = 0; j < s.n; ++j) visit(s.key, m[j]);
+  }
+}
+
+// a resize or a load needs a handle over the whole pool (the product's check_whole_pool)
+inline bool whole_pool(const ExtOracle& o) { return o.lo == 0 && o.cnt == o.cfg.num_endpoints; }
 
 }  // namespace
 
@@ -280,6 +306,110 @@ int epx_lru_clear(void* h, uint32_t e) {
   if (e >= o->cfg.num_endpoints) return FI_ERR_INVALID;
   o->lrus[e].order.clear();
   o->lrus[e].pos.clear();
+  return FI_OK;
+}
+
+// fi_epp_match_counts (S.3a): counts[r * cnt + j] = match[lo + j] of request r, nblocks[r] = N.  For the call the
+// handle's configuration is one profile without filters or PD and its endpoints are all alive, so rank_one's one
+// list holds every endpoint of the shard; configuration and states are restored before the call returns.  The count
+// reads neither, as S.3a says.  A probe that makes every endpoint a candidate and ranks all of the shard's endpoints
+// reports each one's match_blocks, so the walk of S.3 is the one the ranked and subset tests already check.
+int epx_match_counts(void* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
+                     uint16_t* counts, uint32_t* nblocks) {
+  if (!h) return FI_ERR_INVALID;
+  ExtOracle* o = ext_of(h);
+  const fi_epp_config saved_cfg = o->cfg;
+  std::vector<EpState> saved_eps;
+  saved_eps.swap(o->eps);
+  o->eps.assign(saved_cfg.num_endpoints, EpState{});
+  for (EpState& s : o->eps) s.flags = FI_ENDPOINT_ALIVE;
+  fi_profile probe{};
+  probe.n_scorers = 1;
+  probe.scorers[0].kind = FI_SCORER_PREFIX;
+  probe.scorers[0].weight = 1;
+  o->cfg.n_profiles = 1;
+  o->cfg.profiles[0] = probe;
+  o->cfg.pd_enabled = 0;
+  Scratch sc;
+  std::vector<Ranked> cand;
+  std::vector<fi_pick> list(o->cnt);
+  for (uint32_t r = 0; r < R; ++r) {
+    rank_one(*o, prompts + offsets[r], offsets[r + 1] - offsets[r], h0[r], 0, nullptr, r, o->cnt, list.data(), sc, cand);
+    for (const fi_pick& pk : list) counts[(size_t)r * o->cnt + (pk.endpoint - o->lo)] = pk.match_blocks;
+    nblocks[r] = list[0].n_blocks;
+  }
+  o->cfg = saved_cfg;
+  o->eps.swap(saved_eps);
+  return FI_OK;
+}
+
+// fi_epp_resize_pool (S.2c) on the oracle's per-endpoint state: endpoints [E', E) are truncated away, [E, E') are
+// appended fresh (not alive, no adapters, an empty LRU of capacity lru_capacity), and E becomes E'.  A shrink's index
+// pairs are the caller's to remove first (ExtOracle.resize: remove_endpoints of the tail).  FI_ERR_STATE on a shard
+// view, as the product refuses a handle over part of the pool.
+int epx_resize(void* h, uint32_t num_endpoints) {
+  ExtOracle* o = ext_of(h);
+  if (!whole_pool(*o)) return FI_ERR_STATE;
+  if (num_endpoints == 0 || num_endpoints > 4096) return FI_ERR_INVALID;
+  const uint32_t keep = std::min(o->cfg.num_endpoints, num_endpoints);
+  o->eps.resize(keep);
+  o->eps.resize(num_endpoints, EpState{});
+  if (o->cfg.lru_capacity) {
+    o->lrus.resize(keep);
+    o->lrus.resize(num_endpoints);
+  }
+  o->cap.resize(keep);
+  o->cap.resize(num_endpoints, o->cfg.lru_capacity);
+  o->cfg.num_endpoints = o->cfg.endpoint_count = num_endpoints;
+  o->cnt = num_endpoints;  // (a resized handle covers the whole pool: lo is 0)
+  return FI_OK;
+}
+
+// the pair set: (hashes[i], endpoints[i]) for i < the returned count (at most cap written), in no particular order
+uint64_t epx_index_pairs(void* h, uint64_t* hashes, uint32_t* endpoints, uint64_t cap) {
+  uint64_t n = 0;
+  for_each_pair(*ext_of(h), [&](uint64_t key, uint32_t e) {
+    if (n < cap) {
+      hashes[n] = key;
+      endpoints[n] = e;
+    }
+    ++n;
+  });
+  return n;
+}
+
+// every endpoint's LRU capacity c_e (0 without an LRU)
+int epx_lru_capacities(void* h, uint32_t* out) {
+  ExtOracle* o = ext_of(h);
+  for (uint32_t e = 0; e < o->cfg.num_endpoints; ++e) out[e] = o->cfg.lru_capacity ? o->cap[e] : 0;
+  return FI_OK;
+}
+
+// Replace the state of S.2d: the pair set becomes the n pairs (hashes[i], endpoints[i]); endpoint e's LRU becomes its
+// lens[e] keys, least recently used first, taken in endpoint order from `keys`; its capacity becomes caps[e].
+// Endpoint states and adapters are left as they are.  FI_ERR_STATE on a shard view, as for epx_resize.
+int epx_load_state(void* h, uint64_t n, const uint64_t* hashes, const uint32_t* endpoints, const uint32_t* lens,
+                   const uint64_t* keys, const uint32_t* caps) {
+  ExtOracle* o = ext_of(h);
+  if (!whole_pool(*o)) return FI_ERR_STATE;
+  const uint32_t E = o->cfg.num_endpoints;
+  for (uint64_t i = 0; i < n; ++i)
+    if (endpoints[i] >= E) return FI_ERR_INVALID;
+  std::vector<std::pair<uint64_t, uint32_t>> old;
+  for_each_pair(*o, [&](uint64_t key, uint32_t e) { old.emplace_back(key, e); });
+  for (const auto& p : old) o->index.clear(p.first, p.second);
+  for (uint64_t i = 0; i < n; ++i) o->index.set(hashes[i], endpoints[i]);
+  if (!o->cfg.lru_capacity) return FI_OK;
+  for (uint32_t e = 0; e < E; ++e) {
+    PodLRU& l = o->lrus[e];
+    l.order.clear();
+    l.pos.clear();
+    for (uint32_t j = 0; j < lens[e]; ++j) {  // oldest first: each key goes in front of the older ones
+      l.order.push_front(*keys++);
+      l.pos[l.order.front()] = l.order.begin();
+    }
+    o->cap[e] = caps[e];
+  }
   return FI_OK;
 }
 

@@ -9,7 +9,15 @@ infrastructure only.  ExtOracle is the oracle of oracle/epp_oracle.py with:
     endpoint_count = c computes.  Its index and LRUs hold only pairs of endpoints in [b, b + c): ops, Adds, capacity
     changes and removals addressed elsewhere are dropped.  Its picks (single, LoRA, ranked) rank only the shard's
     eligible endpoints, with the queue scorer's min / max over the eligible endpoints of the whole pool, the tie
-    rotation of the whole pool, and the PD rule on the shard's own decode pick."""
+    rotation of the whole pool, and the PD rule on the shard's own decode pick;
+  * match_counts: fi_epp_match_counts (S.3a), every endpoint's match count of the picks' walk, one column per endpoint
+    of the shard (of the pool without one);
+  * resize(E'), the pool resize of S.2c: a shrink is remove_endpoints of the tail followed by truncating the
+    per-endpoint state, a grow appends fresh endpoints.  A shrink removes, so it needs track_removal=True;
+  * the state of an index snapshot (S.2d): state() reads the pair set, every endpoint's LRU (least recently used
+    first) and every capacity, and load_state(...) replaces them, leaving endpoint states and adapters as they are.
+A shard view refuses resize, state and load_state with ValueError, as the product refuses a handle over part of the
+pool."""
 from __future__ import annotations
 
 import ctypes as C
@@ -49,7 +57,12 @@ def load() -> C.CDLL:
             ("epx_add_chains", C.c_int, [_P, _P, _P, C.c_uint32, _P, C.c_uint32]),
             ("epx_set_lru_capacities", C.c_int, [_P, _P, _P, C.c_uint32, _P, _P, C.c_uint64, C.POINTER(C.c_uint64)]),
             ("epx_lru_dump", C.c_uint32, [_P, C.c_uint32, _P, C.c_uint32]),
-            ("epx_lru_clear", C.c_int, [_P, C.c_uint32])):
+            ("epx_lru_clear", C.c_int, [_P, C.c_uint32]),
+            ("epx_match_counts", C.c_int, [_P, _P, _P, _P, C.c_uint32, _P, _P]),
+            ("epx_resize", C.c_int, [_P, C.c_uint32]),
+            ("epx_index_pairs", C.c_uint64, [_P, _P, _P, C.c_uint64]),
+            ("epx_lru_capacities", C.c_int, [_P, _P]),
+            ("epx_load_state", C.c_int, [_P, C.c_uint64, _P, _P, _P, _P, _P])):
         f = getattr(lib, name)
         f.restype, f.argtypes = res, args
     _lib = lib
@@ -190,3 +203,72 @@ class ExtOracle(epp_oracle.Oracle):
         out = np.zeros(max(n, 1), dtype=np.uint64)
         self._lib.epx_lru_dump(self._h, e, _ptr(out), n)
         return out[:n].copy()
+
+    # ---- match counts -----------------------------------------------------------------------------------------------
+    def match_counts(self, prompts, offsets, h0):
+        """-> (counts uint16 [R, c], nblocks uint32 [R]) of fi_epp_match_counts"""
+        prompts, offsets, h0, R = self._inputs(prompts, offsets, h0)
+        c = self.E if self.shard is None else self.shard[1]
+        counts = np.zeros((R, c), dtype=np.uint16)
+        nb = np.zeros(R, dtype=np.uint32)
+        rc = self._lib.epx_match_counts(self._h, _ptr(prompts), _ptr(offsets), _ptr(h0), R, _ptr(counts), _ptr(nb))
+        assert rc == 0, rc
+        return counts, nb
+
+    # ---- pool resize and snapshot state: a handle over the whole pool -------------------------------------------
+    def _whole_pool(self, what):
+        if self.shard is not None:
+            raise ValueError(f"{what} needs a handle over the whole pool, not a shard view")
+
+    def resize(self, num_endpoints: int) -> int:
+        """fi_epp_resize_pool (S.2c).  -> the (endpoint, hash) pairs a shrink removed."""
+        self._whole_pool("resize")
+        En = int(num_endpoints)
+        if En < 1 or En > 4096:
+            raise ValueError("num_endpoints out of range")
+        removed = 0
+        if En < self.E:
+            removed = sum(self.index_contains(e, h) for e in range(En, self.E) for h in self._seen[e])
+            self.remove_endpoints(range(En, self.E))
+        rc = self._lib.epx_resize(self._h, En)
+        assert rc == 0, rc
+        if self._seen is not None:
+            self._seen = self._seen[:En] + [set() for _ in range(En - len(self._seen))]
+        self.E = self.cfg.num_endpoints = self.cfg.endpoint_count = En
+        return int(removed)
+
+    def index_pairs(self) -> set:
+        """{(endpoint, hash)}"""
+        n = int(self._lib.epx_index_pairs(self._h, None, None, 0))
+        hs = np.zeros(max(n, 1), dtype=np.uint64)
+        es = np.zeros(max(n, 1), dtype=np.uint32)
+        self._lib.epx_index_pairs(self._h, _ptr(hs), _ptr(es), n)
+        return set(zip(es[:n].tolist(), hs[:n].tolist()))
+
+    def capacities(self) -> list:
+        out = np.zeros(self.E, dtype=np.uint32)
+        self._lib.epx_lru_capacities(self._h, _ptr(out))
+        return out.tolist()
+
+    def state(self):
+        """(pair set, [LRU of each endpoint, least recently used first], [capacity of each endpoint])"""
+        self._whole_pool("state")
+        lrus = [self.lru(e) if self.C else np.zeros(0, np.uint64) for e in range(self.E)]
+        return self.index_pairs(), lrus, self.capacities()
+
+    def load_state(self, pairs, lrus, caps):
+        self._whole_pool("load_state")
+        pairs = sorted(pairs)
+        es = np.array([e for e, _ in pairs], dtype=np.uint32)
+        hs = np.array([h for _, h in pairs], dtype=np.uint64)
+        lens = np.array([len(x) for x in lrus], dtype=np.uint32)
+        keys = np.concatenate([np.asarray(x, dtype=np.uint64) for x in lrus] + [np.zeros(1, np.uint64)])
+        caps = np.ascontiguousarray(caps, dtype=np.uint32)
+        rc = self._lib.epx_load_state(self._h, len(pairs), _ptr(hs), _ptr(es), _ptr(lens), _ptr(keys), _ptr(caps))
+        assert rc == 0, rc
+        if self._seen is not None:
+            self._seen = [set() for _ in range(self.E)]
+            for e, h in pairs:
+                self._seen[e].add(int(h))
+            for e, x in enumerate(lrus):
+                self._seen[e].update(int(h) for h in x)

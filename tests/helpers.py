@@ -3,6 +3,7 @@ from __future__ import annotations
 
 import json
 import os
+from collections import OrderedDict
 
 import numpy as np
 
@@ -57,6 +58,55 @@ def describe_diff(got, want, limit=5):
         i = tuple(idx)
         lines.append(f"  {i}: got {got[i]} want {want[i]}")
     return "\n".join(lines)
+
+
+class OrderedLrus:
+    """hashicorp/golang-lru, the plainest way: one ordered dict per endpoint (lru[e], oldest first) with its own
+    capacity (cap[e], C until resized), and the index as the set of (endpoint, hash) pairs"""
+
+    def __init__(self, E, cap):
+        self.C = cap
+        self.cap = [cap] * E
+        self.lru = [OrderedDict() for _ in range(E)]
+        self.pairs = set()
+
+    def apply(self, ops):
+        """direct SET / CLEAR ops [(hash, endpoint, op)]: the pair set only"""
+        for h, e, o in ops:
+            (self.pairs.add if o == abi.FI_OP_SET else self.pairs.discard)((int(e), int(h)))
+
+    def add_chain(self, e, keys):
+        """upstream indexer.Add: a hit becomes the most recent, a miss is inserted and SET, evicting (and CLEARing)
+        the oldest key past the capacity"""
+        e, d = int(e), self.lru[int(e)]
+        for k in (int(x) for x in keys):
+            if k in d:
+                d.move_to_end(k)
+                continue
+            d[k] = True
+            self.pairs.add((e, k))
+            if len(d) > self.cap[e]:
+                old, _ = d.popitem(last=False)
+                self.pairs.discard((e, old))
+
+    def resize(self, e, c):
+        """capacity c (0: C) -> the keys evicted, oldest first"""
+        self.cap[e] = c or self.C
+        d, gone = self.lru[e], []
+        while len(d) > self.cap[e]:
+            old, _ = d.popitem(last=False)
+            self.pairs.discard((e, old))
+            gone.append(old)
+        return gone
+
+    def remove(self, eps):
+        """upstream indexer.RemovePod: every pair of the endpoints leaves and their LRUs empty -> pairs dropped"""
+        drop = {int(e) for e in eps}
+        gone = {p for p in self.pairs if p[0] in drop}
+        self.pairs -= gone
+        for e in drop:
+            self.lru[e].clear()
+        return len(gone)
 
 
 def small_workload(**kw):

@@ -2,7 +2,7 @@
 
 S.2c defines a resize by a history: after a resize to E', the handle behaves like one created at E' and fed the same
 calls, with everything ever addressed to an endpoint a shrink dropped left out.  History keeps those calls and replays
-them, so filtered, into a fresh ResizeOracle: what tests/test_resize_cpu.py holds ResizeOracle.resize to.  CallStream makes
+them, so filtered, into a fresh ExtOracle: what tests/test_resize_cpu.py holds ExtOracle.resize to.  CallStream makes
 the calls: endpoint states with label bits, adapters, direct SETs and CLEARs (the index markers 0 and ~0 included),
 batched Adds and per-endpoint LRU capacities, over prompts that share prefixes so that picks match across endpoints.
 """
@@ -13,7 +13,7 @@ import numpy as np
 from fusioninfer_b200 import _abi as abi
 from fusioninfer_b200 import make_config, subset_bitsets
 from tests import helpers as H
-from tests.resize_oracle import ResizeOracle
+from tests.ext_oracle import ExtOracle
 
 P, K, Q, L = H.P, H.K, H.Q, abi.FI_SCORER_LORA
 U64_MAX = 0xFFFFFFFFFFFFFFFF
@@ -58,17 +58,17 @@ class History:
                     log.append((kind, a[0][keep], a[1][keep]))
         self.log = log
 
-    def replay(self, E) -> ResizeOracle:
+    def replay(self, E) -> ExtOracle:
         cfg = abi.fi_epp_config.from_buffer_copy(self.cfg)
         cfg.num_endpoints = cfg.endpoint_count = E
-        ora = ResizeOracle(cfg, track_removal=True)
+        ora = ExtOracle(cfg, track_removal=True)
         for entry in self.log:
             apply(ora, entry)
         return ora
 
 
 def apply(target, entry):
-    """one call on an EndpointPicker or a ResizeOracle"""
+    """one call on an EndpointPicker or an ExtOracle"""
     kind, *a = entry
     if kind == "states":
         target.update_endpoints(a[0])
@@ -98,7 +98,7 @@ class CallStream:
         self.tok, self.offs = H.pack_prompts(blobs)
         self.h0 = 0x5EED
         self.R = R
-        ora = ResizeOracle(cfg)
+        ora = ExtOracle(cfg)
         self.chains, self.nb = ora.hash_batch(self.tok, self.offs, self.h0)
         ora.close()
         self.hashes = np.unique(np.concatenate([self.chains[r, : self.nb[r]] for r in range(R)] +

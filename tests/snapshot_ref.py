@@ -110,7 +110,7 @@ def resealed(blob: bytes) -> bytes:
 
 
 def from_oracle(ora, rng=None) -> bytes:
-    """a blob of a SnapshotOracle's state; rng: the node order shuffled"""
+    """a blob of an ExtOracle's state; rng: the node order shuffled"""
     cfg = ora.cfg
     pairs, lrus, caps = ora.state()
     keys = np.array(sorted({h for _, h in pairs}), dtype=np.uint64)

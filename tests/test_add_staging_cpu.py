@@ -7,7 +7,6 @@ applied SETs-then-CLEARs, against sequential Adds.
 """
 import ctypes as C
 import os
-from collections import OrderedDict
 
 import numpy as np
 import pytest
@@ -124,22 +123,6 @@ class _Index:
         return (self.pairs | set(self.sets)) - set(self.clears)
 
 
-class _Lrus:
-    def __init__(self, E, cap):
-        self.cap, self.lru, self.pairs = cap, [OrderedDict() for _ in range(E)], set()
-
-    def add_chain(self, e, keys):
-        d = self.lru[e]
-        for k in (int(x) for x in keys):
-            if k in d:
-                d.move_to_end(k)
-                continue
-            d[k] = True
-            self.pairs.add((e, k))
-            if len(d) > self.cap:
-                self.pairs.discard((e, d.popitem(last=False)[0]))
-
-
 def _add_chains(hc, pool, index, eps, chains, nb, chunk, leading_flush=True):
     """one fi_epp_index_add_chains: its groups go to `index` (leading_flush=False: the old rule, which staged the
     call's ops behind the open group's CLEARs without a flush)"""
@@ -166,7 +149,7 @@ def test_clear_in_tail_then_re_set(hc, leading_flush):
     """a call evicts (1, e) and leaves the CLEAR in its tail; the next call adds key 1 again: only the leading flush
     keeps the pair in the index"""
     pool = hc.fihc_lrupool_new(1, 2, 1)
-    index, model = _Index(), _Lrus(1, 2)
+    index, model = _Index(), H.OrderedLrus(1, 2)
     for keys in ([1, 2, 3], [1]):
         _add_chains(hc, pool, index, *_one(0, keys, 3), chunk=1 << 16, leading_flush=leading_flush)
         model.add_chain(0, keys)
@@ -185,7 +168,7 @@ def test_consecutive_calls_match_sequential_adds(hc, workers):
     E, cap, mb, R, chunk = 6, 8, 6, 12, 16
     rng = np.random.default_rng(workers)
     pool = hc.fihc_lrupool_new(E, cap, workers)
-    index, model = _Index(), _Lrus(E, cap)
+    index, model = _Index(), H.OrderedLrus(E, cap)
     for step in range(40):
         hot = int(rng.integers(0, E))
         eps = np.where(rng.random(R) < 0.5, hot, rng.integers(0, E, size=R)).astype(np.uint32)

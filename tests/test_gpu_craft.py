@@ -15,8 +15,6 @@ Every scene asserts that the crafting happened (fi_epp_hash_batch holds the mark
 the markers the scene designed, early exit really stopped requests, the rotation really decided), so a scene that
 degenerates fails instead of checking nothing.
 """
-from collections import OrderedDict
-
 import numpy as np
 import pytest
 
@@ -323,39 +321,12 @@ def test_markers_at_every_block_size(size, mode):
 
 
 # ---- B. markers entering the index from hashed chains (device LRU) ------------------------------------------------------
-class _Lru:
-    """ordered dicts (oldest first) with per-endpoint capacities: hashicorp/golang-lru, plainly"""
-
-    def __init__(self, E, cap):
-        self.cap = [cap] * E
-        self.d = [OrderedDict() for _ in range(E)]
-
-    def add(self, e, keys):
-        d = self.d[e]
-        for k in keys:
-            k = int(k)
-            if k in d:
-                d.move_to_end(k)
-            else:
-                d[k] = True
-                while len(d) > self.cap[e]:
-                    d.popitem(last=False)
-
-    def resize(self, e, cap):
-        self.cap[e] = cap
-        while len(self.d[e]) > cap:
-            self.d[e].popitem(last=False)
-
-    def clear(self, e):
-        self.d[e].clear()
-
-
 def test_markers_through_the_device_lru_and_two_rebuilds():
     torch = _torch()
     E, C, M, B = 8, 48, 32, 64
     cfg = make_config(num_endpoints=E, block_bytes=B, max_blocks=M, lru_capacity=C, max_batch=256, index_slots=1 << 12,
                       profiles=[{"name": "default", "scorers": [(H.P, 100), (H.K, 13), (H.Q, 7)]}])
-    gpu, ref, model = EndpointPicker(cfg), ExtOracle(cfg, track_removal=True), _Lru(E, C)
+    gpu, ref, model = EndpointPicker(cfg), ExtOracle(cfg, track_removal=True), H.OrderedLrus(E, C)
     gpu.set_option("device_lru", 1)
     rng = np.random.default_rng(77)
     st = H.states_array(E, kv=rng.integers(0, 1024, E) / 1024.0, queue=rng.integers(0, 8, E))
@@ -371,7 +342,7 @@ def test_markers_through_the_device_lru_and_two_rebuilds():
         for e in range(E):
             got = gpu.lru_dump(e)
             assert np.array_equal(got, ref.lru(e)), f"{what}: LRU of endpoint {e} vs the oracle"
-            assert np.array_equal(got, np.array(list(model.d[e]), dtype=np.uint64)), f"{what}: LRU {e} vs the model"
+            assert np.array_equal(got, np.array(list(model.lru[e]), dtype=np.uint64)), f"{what}: LRU {e} vs the model"
         _check_markers(gpu, ref, E, design, what)
         _eq(gpu.pick_batch(sc.tok, sc.offs, sc.h0), ref.pick_batch(sc.tok, sc.offs, sc.h0), f"{what}: picks")
         _eq(gpu.pick_batch_ranked(sc.tok, sc.offs, sc.h0, 3), ref.pick_batch_ranked(sc.tok, sc.offs, sc.h0, 3),
@@ -381,7 +352,7 @@ def test_markers_through_the_device_lru_and_two_rebuilds():
         ref.index_add_chains(eps, ch, nbk)
         for r, e in enumerate(eps):
             if e != NOEP:
-                model.add(int(e), ch[r, : nbk[r]])
+                model.add_chain(e, ch[r, : nbk[r]])
 
     # 1. the chains_out of a crafted device pick, added through fi_epp_index_add_chains_device
     R = sc.R
@@ -428,8 +399,7 @@ def test_markers_through_the_device_lru_and_two_rebuilds():
     # 5. removing holders of both markers
     gpu.remove_endpoints([2, 6])
     ref.remove_endpoints([2, 6])
-    model.clear(2)
-    model.clear(6)
+    model.remove([2, 6])
     check("endpoints 2 and 6 removed", {Z: [3, 5, 7], T: [1, 3]})
 
     # 6. two rebuilds: junk keys SET and CLEARed on endpoint 7 (outside the LRU) fill the table with tombstones
@@ -448,8 +418,7 @@ def test_markers_through_the_device_lru_and_two_rebuilds():
     check("after the first rebuild, markers held", {Z: [3, 5, 7], T: [1, 3]})
     gpu.remove_endpoints([1, 3, 5, 7])
     ref.remove_endpoints([1, 3, 5, 7])
-    for e in (1, 3, 5, 7):
-        model.clear(e)
+    model.remove([1, 3, 5, 7])
     check("markers held by nobody", {Z: [], T: []})
     churn("second rebuild")  # into the spare, whose special rows were live before the first
     check("after the second rebuild, markers held by nobody", {Z: [], T: []})

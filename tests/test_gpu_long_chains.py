@@ -19,7 +19,6 @@ from fusioninfer_b200 import _abi as abi
 from fusioninfer_b200.picker import FiEppError
 from oracle import epp_oracle as eo
 from tests import helpers as H
-from tests.counts_oracle import CountsOracle
 from tests.ext_oracle import ExtOracle
 
 pytestmark = pytest.mark.gpu
@@ -146,7 +145,7 @@ def test_window_counts_at_every_boundary(mode):
     for shuffled in (False, True):
         o_ops = ops[np.random.default_rng(9).permutation(len(ops))] if shuffled else ops
         cfg = _cfg(E, M, len(h0), offs, mode, index_slots=_slots(ops))
-        g, o = _pair(cfg, st, [o_ops], oracle=CountsOracle)
+        g, o = _pair(cfg, st, [o_ops], oracle=ExtOracle)
         got, _ = g.match_counts(tok, offs, h0)
         want, _ = o.match_counts(tok, offs, h0)
         pg, po = g.pick_batch(tok, offs, h0), eo.Oracle.pick_batch(o, tok, offs, h0)

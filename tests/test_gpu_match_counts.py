@@ -1,5 +1,5 @@
 """GPU (-m gpu): fi_epp_match_counts / _device (docs/SPEC.md S.3a), bit-exact against the oracle's match_counts
-(tests/counts_oracle.cpp) on every row shape of the match kernel, and consistent with the picks of the same handle.
+(tests/ext_oracle.cpp) on every row shape of the match kernel, and consistent with the picks of the same handle.
 
 Rows are checked where they are least aligned: the device call writes at an odd 2-byte offset of a guarded buffer,
 so rows start anywhere inside a 32-byte sector, and the guards must come back untouched."""
@@ -16,7 +16,7 @@ from tests import collide, craft
 from tests import helpers as H
 from tests import match_counts_cases as MC
 from tests import shard_view as SV
-from tests.counts_oracle import CountsOracle
+from tests.ext_oracle import ExtOracle
 from tests.test_match_counts_cpu import check_picks_against_matrix
 
 pytestmark = pytest.mark.gpu
@@ -80,7 +80,7 @@ def _world(E, B, M, R, mode, lru, seed, shard=None, **kw):
         kw.update(endpoint_begin=shard[0], endpoint_count=shard[1])
     cfg = _cfg(E, B, M, R, mode, lru, **kw)
     p = EndpointPicker(cfg)
-    o = CountsOracle(_cfg(E, B, M, R, mode, lru), shard=shard, track_removal=lru > 0)
+    o = ExtOracle(_cfg(E, B, M, R, mode, lru), shard=shard, track_removal=lru > 0)
     st = SV.tie_states(E, rng)
     p.update_endpoints(st)
     o.update_endpoints(st)
@@ -208,7 +208,7 @@ def test_crafted_marker_hashes_and_collisions():
                 blocks = [bytes(raw[int(offs[r]) + i * B: int(offs[r]) + (i + 1) * B]) for i in range(3)]
                 h0[r] = craft.h0_for(blocks, 1 + (r // 4) % 2, craft.MARKERS[(r // 8) % 2])
         cfg = _cfg(E, B, M, R, mode, 0, index_slots=slots)
-        p, o = EndpointPicker(cfg), CountsOracle(cfg)
+        p, o = EndpointPicker(cfg), ExtOracle(cfg)
         x = Inputs(tok, offs, h0)
         chains, nb = o.hash_batch(x.tok, x.offs, x.h0)
         valid = np.arange(M)[None, :] < nb[:, None]
@@ -292,7 +292,7 @@ def test_full_size_batch():
     """max_batch 16 384 requests over 1 024 endpoints (32 MiB of counts), bit-exact"""
     wl = synth.Workload(R=16384, E=1024, T=1024, lru_capacity=160, groups_per_endpoint=4, max_blocks=64, holes=True)
     cfg = H.config_for(wl, profiles=PROFILES)
-    p, o = EndpointPicker(cfg), CountsOracle(cfg)
+    p, o = EndpointPicker(cfg), ExtOracle(cfg)
     for ops in wl.index_ops():
         p.index_apply(ops)
         o.index_apply(ops)

@@ -672,25 +672,6 @@ def test_chained_label_filters_third_label():
     gpu.close()
 
 
-class _PyLru:
-    """hashicorp/golang-lru semantics, the plainest way: an ordered dict per endpoint (oldest first)."""
-
-    def __init__(self, cap):
-        from collections import OrderedDict
-
-        self.cap, self.d = cap, OrderedDict()
-
-    def add_chain(self, keys):
-        for k in keys:
-            k = int(k)
-            if k in self.d:
-                self.d.move_to_end(k)
-            else:
-                self.d[k] = True
-                if len(self.d) > self.cap:
-                    self.d.popitem(last=False)
-
-
 def _device_lru_handle(E, cap, max_blocks, max_batch=256):
     wl = H.small_workload(E=E, R=8, T=max_blocks * 16, max_blocks=max_blocks, lru_capacity=0)
     cfg = H.config_for(wl, lru_capacity=cap, index_slots=1 << 17, max_batch=max_batch)
@@ -704,15 +685,15 @@ def _check_lru_state(gpu, ref, E):
     """recency order AND index membership equal the sequential reference"""
     for e in range(E):
         got = gpu.lru_dump(e)
-        want = np.array(list(ref[e].d.keys()), dtype=np.uint64)
+        want = np.array(list(ref.lru[e]), dtype=np.uint64)
         assert np.array_equal(got, want), f"endpoint {e}: {len(got)} vs {len(want)} entries"
     # membership: every key ever seen, at every endpoint
-    seen = np.array(sorted({k for l in ref for k in l.d} | getattr(_check_lru_state, "extra", set())), dtype=np.uint64)
+    seen = np.array(sorted({k for l in ref.lru for k in l} | getattr(_check_lru_state, "extra", set())), dtype=np.uint64)
     q = np.zeros(len(seen) * E, dtype=H.OP_DTYPE)  # every (key, endpoint) pair, key-major
     q["hash"] = np.repeat(seen, E)
     q["endpoint"] = np.tile(np.arange(E, dtype=np.uint32), len(seen))
     have = gpu.index_contains(q)
-    want = np.stack([np.isin(seen, np.array(list(ref[e].d), dtype=np.uint64)) for e in range(E)], axis=1).ravel()
+    want = np.stack([np.isin(seen, np.array(list(ref.lru[e]), dtype=np.uint64)) for e in range(E)], axis=1).ravel()
     assert np.array_equal(have.astype(bool), want)
 
 
@@ -733,7 +714,7 @@ def test_device_lru_random_batches_long_chains(cap, M):
 def _device_lru_random_batches(cap, M):
     E = 6
     gpu = _device_lru_handle(E, cap, M)
-    ref = [_PyLru(cap) for _ in range(E)]
+    ref = H.OrderedLrus(E, cap)
     rng = np.random.default_rng(2024)
     ever = set()
     # a pool of prefix chains; requests take a prefix of a pool chain plus a private tail
@@ -756,7 +737,7 @@ def _device_lru_random_batches(cap, M):
         gpu.index_add_chains(eps, chains, nb)
         for r in range(R):
             if eps[r] != abi.FI_NO_ENDPOINT:
-                ref[eps[r]].add_chain(chains[r, : nb[r]])
+                ref.add_chain(eps[r], chains[r, : nb[r]])
                 ever.update(int(k) for k in chains[r, : nb[r]])
         if step % 4 == 3 or step < 3:
             _check_lru_state.extra = set(list(ever)[:: max(1, len(ever) // 400)])
@@ -764,7 +745,7 @@ def _device_lru_random_batches(cap, M):
     _check_lru_state.extra = ever
     _check_lru_state(gpu, ref, E)
     st = gpu.index_stats()
-    assert st.lru_entries == sum(len(l.d) for l in ref) and st.tombstones > 0
+    assert st.lru_entries == sum(len(l) for l in ref.lru) and st.tombstones > 0
     c = gpu.lru_counters()
     # every path ran: keys gone again within their batch, an endpoint whose table refused a batch (rolled back and
     # re-run in capacity-sized sub-batches), log compactions / table rebuilds
@@ -788,7 +769,7 @@ def test_device_lru_edge_cases_long_chains(cap, M):
 def _device_lru_edge_cases(cap, M):
     E = 3
     gpu = _device_lru_handle(E, cap, M)
-    ref = [_PyLru(cap) for _ in range(E)]
+    ref = H.OrderedLrus(E, cap)
     ever = set()
 
     def add(eps, chains, nb):
@@ -797,7 +778,7 @@ def _device_lru_edge_cases(cap, M):
         nb = np.asarray(nb, dtype=np.uint32)
         gpu.index_add_chains(eps, chains, nb)
         for r in range(len(eps)):
-            ref[eps[r]].add_chain(chains[r, : nb[r]])
+            ref.add_chain(eps[r], chains[r, : nb[r]])
             ever.update(int(k) for k in chains[r, : nb[r]])
         _check_lru_state.extra = ever
         _check_lru_state(gpu, ref, E)
@@ -812,7 +793,7 @@ def _device_lru_edge_cases(cap, M):
     for i in range(cap + 4):                 # push them out again, one new key per call (single-chain entry point)
         k = np.array([1000 + i], dtype=np.uint64)
         gpu.index_add_chain(1, k)
-        ref[1].add_chain(k)
+        ref.add_chain(1, k)
         ever.add(1000 + i)
     _check_lru_state.extra = ever
     _check_lru_state(gpu, ref, E)

@@ -5,7 +5,6 @@ After every removal the picks are bit-equal to the oracle's after the same calls
 oracle's, and index membership is false for every removed pair and unchanged for every other one.
 """
 import threading
-from collections import OrderedDict
 
 import numpy as np
 import pytest
@@ -159,21 +158,6 @@ def test_direct_sets_and_special_hashes_are_removed():
     gpu.close()
 
 
-class _PyLru:
-    def __init__(self, cap):
-        self.cap = cap
-        self.d = OrderedDict()
-
-    def add_chain(self, keys):
-        for k in (int(x) for x in keys):
-            if k in self.d:
-                self.d.move_to_end(k)
-            else:
-                self.d[k] = True
-                if len(self.d) > self.cap:
-                    self.d.popitem(last=False)
-
-
 @pytest.mark.parametrize("device_lru", [0, 1])
 def test_remove_resets_the_lru(device_lru):
     """The removed endpoints' LRUs are empty (lru_dump, lru_entries); re-adding the same chains SETs them again; churn
@@ -186,7 +170,7 @@ def test_remove_resets_the_lru(device_lru):
     st = wl.endpoint_states()
     gpu.update_endpoints(st)
     cpu.update_endpoints(st)
-    ref = [_PyLru(cap) for _ in range(wl.E)]
+    ref = H.OrderedLrus(wl.E, cap)
     ever = set()
 
     def step(batch):
@@ -198,29 +182,28 @@ def test_remove_resets_the_lru(device_lru):
         gpu.index_add_chains(eps, ch, nb)
         cpu.index_add_chains(eps, ch, nb)
         for r in range(wl.R):
-            ref[eps[r]].add_chain(ch[r, : nb[r]])
+            ref.add_chain(eps[r], ch[r, : nb[r]])
             ever.update(int(k) for k in ch[r, : nb[r]])
         return eps, ch, nb
 
     def check():
         keys = sorted(ever)
         _check_membership(gpu, cpu, _membership_queries(keys[:: max(1, len(keys) // 300)], np.arange(wl.E)))
-        assert gpu.index_stats().lru_entries == sum(len(l.d) for l in ref)
+        assert gpu.index_stats().lru_entries == sum(len(l) for l in ref.lru)
         if device_lru:
             for e in range(wl.E):
-                assert np.array_equal(gpu.lru_dump(e), np.array(list(ref[e].d), dtype=np.uint64)), e
+                assert np.array_equal(gpu.lru_dump(e), np.array(list(ref.lru[e]), dtype=np.uint64)), e
 
     for b in range(3):
         step(b)
     check()
     eps, ch, nb = step(3)
     victims = sorted(set(int(e) for e in eps[:6]))
-    sizes = sum(len(ref[e].d) for e in victims)
+    sizes = sum(len(ref.lru[e]) for e in victims)
     assert sizes > 0
     entries = gpu.index_stats().lru_entries
     _remove_both(gpu, cpu, victims)
-    for e in victims:
-        ref[e].d.clear()
+    ref.remove(victims)
     assert gpu.index_stats().lru_entries == entries - sizes
     if device_lru:
         for e in victims:
@@ -230,7 +213,7 @@ def test_remove_resets_the_lru(device_lru):
     gpu.index_add_chains(eps, ch, nb)
     cpu.index_add_chains(eps, ch, nb)
     for r in range(wl.R):
-        ref[eps[r]].add_chain(ch[r, : nb[r]])
+        ref.add_chain(eps[r], ch[r, : nb[r]])
     q = _membership_queries([int(ch[r, 0]) for r in range(wl.R) if eps[r] in victims and nb[r]], victims)
     assert _check_membership(gpu, cpu, q).any()
     check()

@@ -1,6 +1,6 @@
 """GPU (-m gpu): fi_epp_resize_pool (docs/SPEC.md S.2c) against the extended CPU oracle.
 
-The oracle resizes with ResizeOracle.resize, which tests/test_resize_cpu.py holds to S.2c's definition (a fresh pool fed
+The oracle resizes with ExtOracle.resize, which tests/test_resize_cpu.py holds to S.2c's definition (a fresh pool fed
 the history without the dropped endpoints).  Here the GPU is compared with it bit for bit after every resize and after
 further calls: single, ranked and subset picks (PD config, by-label filter, LoRA), index membership of every hash the
 calls ever aimed anywhere, the device LRU's content, the LRU entry total and the pairs a shrink removed.  The sharded
@@ -14,13 +14,13 @@ from fusioninfer_b200 import _abi as abi
 from fusioninfer_b200.picker import FiEppError
 from tests import helpers as H
 from tests import resize_ref as RR
-from tests.resize_oracle import ResizeOracle
+from tests.ext_oracle import ExtOracle
 
 pytestmark = pytest.mark.gpu
 
 
 def _pair(cfg):
-    return EndpointPicker(cfg), ResizeOracle(cfg, track_removal=True)
+    return EndpointPicker(cfg), ExtOracle(cfg, track_removal=True)
 
 
 def _both(gpu, ora, entries):

@@ -2,7 +2,7 @@
 
 A snapshot stores the pair set, the LRU lists and the capacities; tests/test_snapshot_cpu.py shows on the oracle that
 these carry every later call.  Here the GPU's blobs are read with the independent reader of tests/snapshot_ref.py and
-held to the extended oracle (tests/snapshot_oracle.py) after a churn history; loaded handles of other internal sizes are
+held to the extended oracle (tests/ext_oracle.py) after a churn history; loaded handles of other internal sizes are
 compared bit for bit with the source and the oracle, also over further pick + Add steps; a save of a load gives the
 same bytes (node order is kept); failing loads change nothing; loads are ordered against submitted batches and tickets;
 and an aged cfg 3 handle round-trips.
@@ -19,7 +19,7 @@ from tests import craft
 from tests import helpers as H
 from tests import resize_ref as RR
 from tests import snapshot_ref as SR
-from tests.snapshot_oracle import SnapshotOracle
+from tests.ext_oracle import ExtOracle
 
 pytestmark = pytest.mark.gpu
 U64_MAX = 0xFFFFFFFFFFFFFFFF
@@ -44,7 +44,7 @@ class Aged:
         self.E = E
         self.cs = RR.CallStream(seed, RR.config(E, match_mode=mode))
         self.gpu = _handle(self.cfg)
-        self.ora = SnapshotOracle(self.cfg, track_removal=True)
+        self.ora = ExtOracle(self.cfg, track_removal=True)
         self.hist = [("states", H.states_array(E, roles=abi.FI_ROLE_WORKER | RR.LABEL))]
         self.both(self.hist[0])
         calls = self.cs.calls(E, n=n)
@@ -234,7 +234,7 @@ def test_errors_change_nothing():
         struct.pack_into(fmt, bad, off, value)
         return SR.resealed(bytes(bad))
 
-    other = SnapshotOracle(RR.config(E + 1))
+    other = ExtOracle(RR.config(E + 1))
     cases = [
         ("block_bytes", abi.FI_ERR_INVALID, patched(16, "<I", 64)),
         ("max_blocks", abi.FI_ERR_INVALID, patched(20, "<I", a.cfg.max_blocks + 1)),

@@ -19,7 +19,7 @@ from tests import craft
 from tests import helpers as H
 from tests import resize_ref as RR
 from tests import snapshot_ref as SR
-from tests.snapshot_oracle import SnapshotOracle
+from tests.ext_oracle import ExtOracle
 from tests.test_gpu_snapshot import Aged, _device, _handle, _same
 from tests.test_gpu_stream_order import Rig, _device_call, _eq, _held, _want
 
@@ -54,7 +54,7 @@ class Small:
         self.E = E
         self.cfg = RR.config(E, lru_capacity=lru_capacity, index_slots=index_slots)
         self.cs = RR.CallStream(seed, RR.config(E))
-        self.gpu, self.ora = EndpointPicker(self.cfg), SnapshotOracle(self.cfg, track_removal=True)
+        self.gpu, self.ora = EndpointPicker(self.cfg), ExtOracle(self.cfg, track_removal=True)
         self.both(("states", H.states_array(E, roles=abi.FI_ROLE_WORKER | RR.LABEL)))
         calls = self.cs.calls(E, n=n)
         if not (lru_capacity and add):
@@ -114,7 +114,7 @@ def test_capture_without_lru_before_add_and_empty():
     _same_bytes(b.gpu, b.ora, "before the first Add")
     b.close()
     cfg = RR.config(9)
-    e, ora = EndpointPicker(cfg), SnapshotOracle(cfg)
+    e, ora = EndpointPicker(cfg), ExtOracle(cfg)
     blob = _same_bytes(e, ora, "empty handle")
     info = snapshot_info(blob)
     assert (info.n_nodes, info.n_lru, info.pairs) == (0, 0, 0)

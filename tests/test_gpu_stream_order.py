@@ -18,7 +18,7 @@ import pytest
 from fusioninfer_b200 import EndpointPicker, subset_bitsets
 from fusioninfer_b200 import _abi as abi
 from tests import helpers as H
-from tests.resize_oracle import ResizeOracle
+from tests.ext_oracle import ExtOracle
 from tests.test_gpu_ranked import _lora, _states
 
 pytestmark = pytest.mark.gpu
@@ -61,7 +61,7 @@ class Rig:
         self.wl = wl = H.small_workload(E=E, R=R, T=600, max_blocks=MB, block_tokens=block_bytes // 4, holes=True,
                                         lru_capacity=CAP)
         cfg = H.config_for(wl, profiles=PROFILES, lru_capacity=lru_capacity, max_prompt_bytes=R * wl.T * 4)
-        self.gpu, self.cpu = EndpointPicker(cfg), ResizeOracle(cfg, track_removal=True)
+        self.gpu, self.cpu = EndpointPicker(cfg), ExtOracle(cfg, track_removal=True)
         st, lo = _states(wl, rng, roles=False), _lora(E, rng)
         for g in (self.gpu, self.cpu):
             g.update_endpoints(st)

@@ -20,7 +20,7 @@ import pytest
 from fusioninfer_b200 import EndpointPicker, subset_bitsets
 from fusioninfer_b200 import _abi as abi
 from tests import helpers as H
-from tests.resize_oracle import ResizeOracle
+from tests.ext_oracle import ExtOracle
 from tests.test_gpu_ranked import _lora, _states
 
 pytestmark = pytest.mark.gpu
@@ -181,7 +181,7 @@ def test_handles_on_one_device(threaded):
         wl = H.small_workload(E=E, R=R, T=600, max_blocks=mb, block_tokens=bb // 4, holes=True, lru_capacity=mb + 64,
                               seed=0xA110 + n)
         cfg = H.config_for(wl, profiles=PROFILES, match_mode=mode, lru_capacity=mb + 64, max_prompt_bytes=R * wl.T * 4)
-        g, o = EndpointPicker(cfg), ResizeOracle(cfg)
+        g, o = EndpointPicker(cfg), ExtOracle(cfg)
         rng = np.random.default_rng(n)
         st, lo = _states(wl, rng, roles=False), _lora(E, rng)
         for x in (g, o):
@@ -219,7 +219,7 @@ def test_threads_on_one_handle(threaded):
     g.update_endpoints_lora(lo)
     oracles = []
     for t in range(T):  # each oracle: the common state, then only thread t's calls
-        o = ResizeOracle(cfg, track_removal=True)
+        o = ExtOracle(cfg, track_removal=True)
         o.update_endpoints(st)
         o.update_endpoints_lora(lo)
         oracles.append(o)

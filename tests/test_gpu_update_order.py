@@ -6,7 +6,7 @@ index_add_chain, index_add_chains, index_add_chains_device(.., NULL, ..) and pic
 and growing (device LRU only), an index filled with tombstones until the next update rebuilds it, and picks of every
 kind between them.  After each call the deltas of fi_epp_get_stats' kernel_launches, h2d_bytes and d2h_bytes must be
 the pinned ones below, and index membership (index_contains) and every pick must equal the oracle extension's
-(tests/resize_oracle.py).
+(tests/ext_oracle.py).
 
 The pinned deltas are what the library gave before every update was ordered through update_begin / update_end
 (engine_index.cu), measured by running this file with FI_EPP_LIB=<that build of libfi_epp.so>: the same kernels and the
@@ -18,7 +18,7 @@ import pytest
 from fusioninfer_b200 import EndpointPicker, subset_bitsets
 from fusioninfer_b200 import _abi as abi
 from tests import helpers as H
-from tests.resize_oracle import ResizeOracle
+from tests.ext_oracle import ExtOracle
 
 pytestmark = pytest.mark.gpu
 P, K, Q = H.P, H.K, H.Q
@@ -73,7 +73,7 @@ class _Seq:
     def __init__(self, device_lru):
         self.wl = H.small_workload(E=E, R=R, T=512, max_blocks=MB, lru_capacity=0)
         cfg = H.config_for(self.wl, profiles=PROFILES, lru_capacity=CAP, index_slots=SLOTS)
-        self.g, self.o = EndpointPicker(cfg), ResizeOracle(cfg, track_removal=True)
+        self.g, self.o = EndpointPicker(cfg), ExtOracle(cfg, track_removal=True)
         self.g.set_option("device_lru", device_lru)
         self.st = self.wl.endpoint_states()
         self.g.update_endpoints(self.st)

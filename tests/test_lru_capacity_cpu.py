@@ -8,7 +8,6 @@ batched host walk (lru_batch.h) with mixed limits are driven through libfi_hostc
 import ctypes as C
 import os
 import random
-from collections import OrderedDict
 
 import numpy as np
 import pytest
@@ -17,41 +16,6 @@ from fusioninfer_b200 import _abi as abi
 from oracle import epp_oracle as eo
 from tests import helpers as H
 from tests.ext_oracle import ExtOracle
-
-
-class _Model:
-    """index = {(endpoint, hash)}, one ordered-dict LRU per endpoint, each with its own limit"""
-
-    def __init__(self, E, cap):
-        self.C = cap
-        self.cap = [cap] * E
-        self.pairs = set()
-        self.lru = [OrderedDict() for _ in range(E)]
-
-    def apply(self, ops):
-        for h, e, o in ops:
-            (self.pairs.add if o == abi.FI_OP_SET else self.pairs.discard)((int(e), int(h)))
-
-    def add_chain(self, e, keys):
-        d = self.lru[e]
-        for k in (int(x) for x in keys):
-            if k in d:
-                d.move_to_end(k)
-                continue
-            d[k] = True
-            self.pairs.add((e, k))
-            if len(d) > self.cap[e]:
-                old, _ = d.popitem(last=False)
-                self.pairs.discard((e, old))
-
-    def resize(self, e, c):
-        self.cap[e] = c or self.C
-        d, gone = self.lru[e], []
-        while len(d) > self.cap[e]:
-            old, _ = d.popitem(last=False)
-            self.pairs.discard((e, old))
-            gone.append(old)
-        return gone
 
 
 def _universe(rng, n):
@@ -91,7 +55,7 @@ def test_reference_with_random_capacities_matches_model():
     (shrinks, grows, duplicates in one call) between random Adds and direct ops."""
     E, cap, mb = 8, 24, 4
     cfg = H.make_config(num_endpoints=E, max_batch=8, max_blocks=mb, lru_capacity=cap)
-    ref, model = ExtOracle(cfg), _Model(E, cap)
+    ref, model = ExtOracle(cfg), H.OrderedLrus(E, cap)
     rng = random.Random(11)
     universe = _universe(rng, 120)
     for step in range(60):
@@ -174,7 +138,7 @@ def test_host_lru_shrink_and_grow(hc):
     nothing, and touches afterwards (reusing the nodes the shrink gave back) follow the model at every limit."""
     cap = 64
     l = hc.fihc_lru_new(cap)
-    model = _Model(1, cap)
+    model = H.OrderedLrus(1, cap)
     rng = random.Random(5)
     assert _keys(hc.fihc_lru_shrink, l, 10, cap=cap) == [] and hc.fihc_lru_limit(l) == 10  # never used
     model.resize(0, 10)
@@ -202,7 +166,7 @@ def test_host_batch_walk_with_mixed_limits(hc, workers):
     model's membership, and every LRU's recency order is the model's."""
     E, cap, mb, R = 9, 48, 8, 40
     p = hc.fihc_lrupool_new(E, cap, workers)
-    model = _Model(E, cap)
+    model = H.OrderedLrus(E, cap)
     rng = np.random.default_rng(workers)
     pairs = set()
     for e in range(E):

@@ -1,6 +1,6 @@
 """CPU: the oracle of fi_epp_match_counts (docs/SPEC.md S.3a), the yardstick of tests/test_gpu_match_counts.py.
 
-  * CountsOracle.match_counts equals the independent restatement's match (tests/restate.py) in both match modes, on
+  * ExtOracle.match_counts equals the independent restatement's match (tests/restate.py) in both match modes, on
     indices built from SET / CLEAR ops with holes, from LRU Adds that evict chain fronts and from removals, at block
     sizes 5 and 64, on the whole pool and on shard views.
   * Every pick and ranked entry of the oracle, over filters, every scorer kind, LoRA and PD, reports the matrix's
@@ -20,7 +20,7 @@ from tests import helpers as H
 from tests import match_counts_cases as MC
 from tests import restate
 from tests import shard_view as SV
-from tests.counts_oracle import CountsOracle
+from tests.ext_oracle import ExtOracle
 
 P, K, Q, L = H.P, H.K, H.Q, abi.FI_SCORER_LORA
 MODES = [abi.FI_MATCH_UPSTREAM, abi.FI_MATCH_LPM]
@@ -64,7 +64,7 @@ def test_matrix_equals_restatement(mode, B, how, shard):
     tok, offs = MC.prompts(R, B, M, rng)
     lru = 2 * M if how != "ops" else 0  # below what three batches of Adds touch: chain fronts are evicted
     cfg = _cfg(E, B, M, R, mode, lru=lru)
-    o = CountsOracle(cfg, shard=shard, track_removal=how == "ops+remove")
+    o = ExtOracle(cfg, shard=shard, track_removal=how == "ops+remove")
     py = restate.from_config(cfg, shard=shard)
     chains, nb = o.hash_batch(tok, offs, 0x1234)
     _build(o, how, chains, nb, E, seed=B + mode)
@@ -128,7 +128,7 @@ def test_picks_agree_with_the_matrix(mode, profiles, shard):
     if pd is not None:
         pd = dict(pd, threshold=float(B * M // 3))
     cfg = _cfg(E, B, M, R, mode, profiles=prof, pd=pd)
-    o = CountsOracle(cfg, shard=shard)
+    o = ExtOracle(cfg, shard=shard)
     o.update_endpoints(SV.tie_states(E, rng))
     ad = None
     if profiles == "lora":
@@ -156,7 +156,7 @@ def test_shard_matrices_join_into_the_pool(mode):
     rng = np.random.default_rng(21)
     tok, offs = MC.prompts(R, B, M, rng)
     cfg = _cfg(E, B, M, R, mode)
-    full = CountsOracle(cfg)
+    full = ExtOracle(cfg)
     chains, nb = full.hash_batch(tok, offs, 5)
     ops = MC.family_ops(chains, nb, E, rng, holes=0.1 if mode == abi.FI_MATCH_LPM else 0.0)
     if mode == abi.FI_MATCH_UPSTREAM:
@@ -165,7 +165,7 @@ def test_shard_matrices_join_into_the_pool(mode):
         full.index_apply(o)
     want, _ = full.match_counts(tok, offs, 5)
     for parts in SV.splits(E):
-        views = [CountsOracle(cfg, shard=bc) for bc in parts]
+        views = [ExtOracle(cfg, shard=bc) for bc in parts]
         for v in views:
             for o in ops:
                 v.index_apply(o)
@@ -183,11 +183,11 @@ def test_upstream_hole_does_not_join():
     tok, offs = wl.prompts()
     for mode, e0 in ((abi.FI_MATCH_UPSTREAM, (2, 1)), (abi.FI_MATCH_LPM, (1, 1))):
         cfg = H.config_for(wl, match_mode=mode)
-        full = CountsOracle(cfg)
+        full = ExtOracle(cfg)
         chains, nb = full.hash_batch(tok, offs, wl.h0)
         ops = H.ops_array([(int(chains[0, 0]), 0, 1), (int(chains[0, 2]), 0, 1),
                            (int(chains[0, 0]), 1, 1), (int(chains[0, 1]), 1, 1)])
-        views = [CountsOracle(cfg, shard=(0, 1)), CountsOracle(cfg, shard=(1, 1))]
+        views = [ExtOracle(cfg, shard=(0, 1)), ExtOracle(cfg, shard=(1, 1))]
         for x in [full] + views:
             x.index_apply(ops)
         whole = full.match_counts(tok, offs, wl.h0)[0]
@@ -199,7 +199,7 @@ def test_upstream_hole_does_not_join():
 def test_zero_requests_and_the_matrix_layout():
     wl = H.small_workload(E=3, R=4, T=128, max_blocks=8)
     cfg = H.config_for(wl)
-    o = CountsOracle(cfg)
+    o = ExtOracle(cfg)
     tok, offs = wl.prompts()
     counts, nb = o.match_counts(tok, offs[:1], wl.h0)
     assert counts.shape == (0, 3) and nb.shape == (0,)

@@ -7,7 +7,6 @@ same calls: membership, LRU content and the count of removed pairs.
 import ctypes as C
 import os
 import random
-from collections import OrderedDict
 
 import numpy as np
 import pytest
@@ -15,39 +14,6 @@ import pytest
 from fusioninfer_b200 import _abi as abi
 from tests import helpers as H
 from tests.remove_ref import RemovalOracle
-
-
-class _Model:
-    """index = {(endpoint, hash)}, one ordered-dict LRU per endpoint"""
-
-    def __init__(self, E, cap):
-        self.cap = cap
-        self.pairs = set()
-        self.lru = [OrderedDict() for _ in range(E)]
-
-    def apply(self, ops):
-        for h, e, o in ops:
-            (self.pairs.add if o == abi.FI_OP_SET else self.pairs.discard)((int(e), int(h)))
-
-    def add_chain(self, e, keys):
-        d = self.lru[e]
-        for k in (int(x) for x in keys):
-            if k in d:
-                d.move_to_end(k)
-                continue
-            d[k] = True
-            self.pairs.add((e, k))
-            if len(d) > self.cap:
-                old, _ = d.popitem(last=False)
-                self.pairs.discard((e, old))
-
-    def remove(self, eps):
-        drop = set(int(e) for e in eps)
-        gone = {p for p in self.pairs if p[0] in drop}
-        self.pairs -= gone
-        for e in drop:
-            self.lru[e].clear()
-        return len(gone)
 
 
 def _check(cpu, model, E, universe):
@@ -60,7 +26,7 @@ def test_reference_remove_endpoints_matches_model():
     E, cap = 12, 10
     cfg = H.make_config(num_endpoints=E, max_batch=8, lru_capacity=cap)
     cpu = RemovalOracle(cfg)
-    model = _Model(E, cap)
+    model = H.OrderedLrus(E, cap)
     rng = random.Random(7)
     universe = [0, 0xFFFFFFFFFFFFFFFF] + [rng.randrange(1, 2**63) for _ in range(60)]
     for step in range(30):

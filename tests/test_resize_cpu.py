@@ -1,8 +1,8 @@
 """CPU: fi_epp_resize_pool's reference and its shape rule.
 
-The tests' oracle resizes a pool with ResizeOracle.resize (tests/resize_oracle.py).  docs/SPEC.md S.2c defines a resize by a
+The tests' oracle resizes a pool with ExtOracle.resize (tests/ext_oracle.py).  docs/SPEC.md S.2c defines a resize by a
 history: the resized pool behaves like one created at the new size and fed the same calls, with everything ever aimed
-at an endpoint a shrink dropped left out.  Here ResizeOracle.resize is held to that definition (tests/resize_ref.py replays
+at an endpoint a shrink dropped left out.  Here ExtOracle.resize is held to that definition (tests/resize_ref.py replays
 the filtered history into a fresh oracle) over random call streams with interleaved grows and shrinks.  The shape rule
 (pool_shape.h: row words, default slots and their floor, when a resize rebuilds) is checked through libfi_hostcheck.so.
 """
@@ -15,7 +15,7 @@ import pytest
 from fusioninfer_b200 import _abi as abi
 from tests import helpers as H
 from tests import resize_ref as RR
-from tests.resize_oracle import ResizeOracle
+from tests.ext_oracle import ExtOracle
 
 
 def _compare(ora, ref, cs, E, what):
@@ -49,7 +49,7 @@ def test_oracle_resize_matches_the_filtered_history(mode, seed):
     sizes = [40, 33, 70, 5, 64, 1, 37, 37, 100, 31, 45]  # shrinks, grows (dropped endpoints come back), a no-op
     cfg = RR.config(sizes[0], match_mode=mode)
     cs = RR.CallStream(seed, cfg)
-    ora = ResizeOracle(cfg, track_removal=True)
+    ora = ExtOracle(cfg, track_removal=True)
     hist = RR.History(cfg)
     E = sizes[0]
     for En in sizes[1:]:
@@ -76,7 +76,7 @@ def test_grown_endpoints_start_fresh():
     """A grown endpoint is not alive, has no adapters, an empty LRU and capacity lru_capacity, even one that held all
     of these before a shrink dropped it."""
     cfg = RR.config(8)
-    ora = ResizeOracle(cfg, track_removal=True)
+    ora = ExtOracle(cfg, track_removal=True)
     ora.update_endpoints(H.states_array(8))
     ora.index_add_chain(7, np.arange(1, 31, dtype=np.uint64))
     ora.set_lru_capacities([7], [16])

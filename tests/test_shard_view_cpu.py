@@ -171,7 +171,8 @@ def test_upstream_holes_do_not_compose():
 
 def test_shard_view_drops_what_is_addressed_elsewhere():
     """ops, Adds, capacity changes and removals aimed outside the shard leave it as it was; a range outside the pool
-    is refused"""
+    is refused, and so are a resize and the snapshot state (the product refuses them on a handle over part of the
+    pool)"""
     wl = H.small_workload(E=40, R=8, T=1024, lru_capacity=80, groups_per_endpoint=1)
     cfg = H.config_for(wl, lru_capacity=80)
     with pytest.raises(ValueError):
@@ -194,4 +195,10 @@ def test_shard_view_drops_what_is_addressed_elsewhere():
     assert v.index_contains(12, int(chains[0, 0])) and v.lru_size(11) == min(nb[1], wl.max_blocks)
     v.remove_endpoints([12])
     assert not v.index_contains(12, int(chains[0, 0]))
+    for call in (lambda: v.resize(wl.E + 1), v.state, lambda: v.load_state(set(), [[]] * wl.E, [80] * wl.E)):
+        with pytest.raises(ValueError):
+            call()
+    assert v._lib.epx_resize(v._h, wl.E + 1) == abi.FI_ERR_STATE
+    assert v._lib.epx_load_state(v._h, 0, None, None, None, None, None) == abi.FI_ERR_STATE
+    assert v.lru_size(11) == min(nb[1], wl.max_blocks) and v.capacities()[11] == wl.max_blocks
     v.close()

@@ -19,17 +19,17 @@ from fusioninfer_b200 import snapshot_info
 from tests import helpers as H
 from tests import resize_ref as RR
 from tests import snapshot_ref as SR
-from tests.snapshot_oracle import SnapshotOracle
+from tests.ext_oracle import ExtOracle
 
 U64_MAX = 0xFFFFFFFFFFFFFFFF
 
 
 def _aged(seed, E=40, lru_capacity=48, n=16):
-    """a SnapshotOracle after a churn history: Adds with evictions, direct SETs / CLEARs (markers 0 and ~0 included),
+    """an ExtOracle after a churn history: Adds with evictions, direct SETs / CLEARs (markers 0 and ~0 included),
     capacity changes and a removal; -> (oracle, call stream, the state calls fed to it)"""
     cfg = RR.config(E, lru_capacity=lru_capacity)
     cs = RR.CallStream(seed, RR.config(E))
-    ora = SnapshotOracle(cfg, track_removal=True)
+    ora = ExtOracle(cfg, track_removal=True)
     states = []
     for i, entry in enumerate(cs.calls(E, n=n) if lru_capacity else _no_lru_calls(cs, E, n)):
         RR.apply(ora, entry)
@@ -74,7 +74,7 @@ def test_info_reads_reference_blobs(lru_capacity, shuffle):
 
 def test_info_reads_an_empty_blob():
     cfg = RR.config(5)
-    ora = SnapshotOracle(cfg)
+    ora = ExtOracle(cfg)
     blob = SR.from_oracle(ora)
     info = snapshot_info(blob)
     assert (info.n_nodes, info.n_lru, info.pairs, info.bytes) == (0, 0, 0, 64 + 8 * 5)
@@ -227,7 +227,7 @@ def _same(a, b, cs, E, what):
 def test_the_three_parts_carry_every_later_call(seed):
     E = 40
     src, cs, states = _aged(seed, E=E, n=24)
-    dst = SnapshotOracle(src.cfg, track_removal=True)
+    dst = ExtOracle(src.cfg, track_removal=True)
     for entry in states:  # endpoint states and adapters are not part of the state: the caller re-sends them
         RR.apply(dst, entry)
     dst.load_state(*src.state())
@@ -245,7 +245,7 @@ def test_the_three_parts_carry_every_later_call(seed):
         dst.remove_endpoints(victim)
         _same(src, dst, cs, E, f"after step {step}")
     # and the copy through a blob, in shuffled node order, too
-    again = SnapshotOracle(src.cfg, track_removal=True)
+    again = ExtOracle(src.cfg, track_removal=True)
     for entry in states:
         RR.apply(again, entry)
     s = SR.read(SR.from_oracle(src, np.random.default_rng(seed)))
