@@ -137,6 +137,10 @@ class fi_pick(C.Structure):
     ]
 
 
+class fi_match_entry(C.Structure):
+    _fields_ = [("endpoint", C.c_uint32), ("match_blocks", C.c_uint16), ("reserved", C.c_uint16)]
+
+
 class fi_index_stats(C.Structure):
     _fields_ = [
         ("slots", C.c_uint64),
@@ -201,6 +205,15 @@ def np_dtypes():
     return pick, op, ep
 
 
+def match_entry_dtype():
+    """one entry of fi_epp_match_lists (fi_match_entry, 8 bytes)"""
+    import numpy as np
+
+    dt = np.dtype([("endpoint", "<u4"), ("match_blocks", "<u2"), ("reserved", "<u2")], align=True)
+    assert dt.itemsize == C.sizeof(fi_match_entry) == 8
+    return dt
+
+
 def lora_dtype():
     import numpy as np
 
@@ -260,6 +273,9 @@ SYMBOLS = [
      [_P, _P, _P, _P, _P, _P, C.c_uint32, C.c_uint64, C.c_uint32, _P, _P, _P]),
     ("fi_epp_match_counts", C.c_int, [_P, _P, _P, _P, C.c_uint32, _P, _P, _P]),
     ("fi_epp_match_counts_device", C.c_int, [_P, _P, _P, _P, C.c_uint32, C.c_uint64, _P, _P, _P, _P]),
+    ("fi_epp_match_lists", C.c_int, [_P, _P, _P, _P, C.c_uint32, _P, _P, C.c_uint64, _P, _P]),
+    ("fi_epp_match_lists_device", C.c_int,
+     [_P, _P, _P, _P, C.c_uint32, C.c_uint64, _P, _P, C.c_uint64, _P, _P, _P]),
     ("fi_epp_pinned_alloc", _P, [C.c_size_t]),
     ("fi_epp_pinned_free", None, [_P]),
     ("fi_epp_comm_unique_id", C.c_int, [_P]),

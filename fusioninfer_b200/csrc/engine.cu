@@ -528,6 +528,7 @@ int fi_epp_resize_pool(fi_epp* h, uint32_t num_endpoints, uint64_t* pairs_remove
   // lazily created buffers sized by the pool: their next use allocates them anew
   h->d_rm.reset();
   h->subsets = Staging<uint32_t>{};
+  h->lists = fi_epp::ListScratch{};
   h->lru_plan_buf = Staging<uint32_t>{};
   h->lru_resize = Staging<uint32_t>{};
   for (fi_epp::PipeAdd& pa : h->padd) pa.plan = Staging<uint32_t>{};

@@ -52,6 +52,7 @@ struct PairHash {
 };
 
 constexpr uint64_t kOpChunk = 1ull << 20;  // ops per pinned staging buffer
+constexpr uint64_t kListChunk = 1ull << 20;  // entries per copy of the host match-lists call (8 MiB)
 
 enum KernelKind { K_HASH = 0, K_MATCH = 1, K_INDEX = 2, K_OTHER = 3, K_KINDS = 4 };
 
@@ -195,6 +196,16 @@ struct fi_epp {
   Staging<fi_pick> ranked;      // [R][P][k] of the host ranked pick: allocated by the first such call, grown with k
   Staging<uint32_t> subsets;    // [max_batch][ceil(E/32)] staging of fi_epp_pick_batch_subset: allocated by its first call
   Staging<uint16_t> counts;     // [max_batch][endpoint_count] of fi_epp_match_counts: allocated by its first call
+  // fi_epp_match_lists (docs/SPEC.md S.3b): every request's slot of (column << 12) | count entries and the entry
+  // counts the match kernel writes, allocated together by the first lists call for max_batch requests of the pool as
+  // it is (alloc_list_scratch), and freed by a resize
+  struct ListScratch {
+    DevPtr<uint32_t> slots;  // [max_batch][endpoint_count]
+    DevPtr<uint32_t> nnz;    // [max_batch]
+    size_t cap = 0;          // entries of slots
+  } lists;
+  Staging<uint64_t> list_offsets;       // [max_batch + 1] of the host lists call: allocated by its first call
+  Staging<fi_match_entry> list_chunk;   // the host lists call's entries, copied out kListChunk at most at a time
   std::unique_ptr<ShardState> shard;  // sharded mode only
   PeerXchg px{};                 // px.enabled == 0: NCCL all-gathers are used
   // sharded mode: every rank hashes every prompt (the default: hashing 16 KiB from local HBM is expected to cost

@@ -1,5 +1,5 @@
 // engine_pick.cu — the pick paths: block hashing, the match enqueue, the stream-ordered and pipelined picks, match
-// counts, and their entry points in the C ABI.
+// counts and match lists, and their entry points in the C ABI.
 #include "engine.h"
 
 namespace {
@@ -49,6 +49,11 @@ struct PickCall {
   // match counts (S.3a) instead of picks: out is null, counts [R][endpoint_count]; nblocks_out [R] or null
   uint16_t* counts = nullptr;
   uint32_t* nblocks_out = nullptr;
+  // match lists (S.3b) instead of picks: out and counts are null; list_offsets [R + 1], entries [cap].  The match writes
+  // the handle's list scratch, and run_pick's pack step fills these (the host call's copy-out has entries null).
+  uint64_t* list_offsets = nullptr;
+  fi_match_entry* entries = nullptr;
+  uint64_t cap = 0;
 };
 
 // the same from the untyped pointers the device entry points take
@@ -110,6 +115,10 @@ int prepare_match(fi_epp* h, const PickCall& c, const uint64_t* chain, const uin
   mp.work_counter = h->d_work.get();
   mp.k = c.k;
   mp.counts = c.counts;
+  if (c.list_offsets) {
+    mp.lists = h->lists.slots.get();
+    mp.nnz = h->lists.nnz.get();
+  }
   if (c.subsets) {
     mp.subsets = c.subsets;
     mp.sub_pitch = (h->cfg.num_endpoints + 31) / 32;
@@ -194,6 +203,8 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
       ms.R = Rk;
       ms.out = mp.out ? mp.out + (size_t)r0 * h->P * std::max(c.k, 1u) : nullptr;
       ms.counts = mp.counts ? mp.counts + (size_t)r0 * h->cfg.endpoint_count : nullptr;
+      ms.lists = mp.lists ? mp.lists + (size_t)r0 * h->cfg.endpoint_count : nullptr;  // the slices' own slots
+      ms.nnz = mp.nnz ? mp.nnz + r0 : nullptr;
       ms.work_counter = h->d_work.get() + k;
       LaunchScope ls(h, h->s_main.get(), K_MATCH);
       FI_CUDA(launch_match_pick(ms, h->sm_count, h->s_main.get()));
@@ -282,8 +293,23 @@ int run_pick_impl(fi_epp* h, const PickCall& c, const PickCall* feed) {
   return FI_OK;
 }
 
+// The pack step of match lists (S.3b), behind the match launches on s_main: the offsets, then the entries below c.cap
+int pack_lists(fi_epp* h, const PickCall& c) {
+  {
+    LaunchScope ls(h, h->s_main.get(), K_OTHER);
+    FI_CUDA(launch_list_scan(h->lists.nnz.get(), c.R, c.list_offsets, h->s_main.get()));
+  }
+  if (c.cap && c.entries) {
+    LaunchScope ls(h, h->s_main.get(), K_OTHER);
+    FI_CUDA(launch_list_copy(h->lists.slots.get(), h->cfg.endpoint_count, c.list_offsets, c.R, h->cfg.endpoint_begin, 0,
+                             c.cap, c.entries, h->s_main.get()));
+  }
+  return FI_OK;
+}
+
 int run_pick(fi_epp* h, const PickCall& c, const PickCall* feed) {
   int rc = run_pick_impl(h, c, feed);
+  if (rc == FI_OK && c.list_offsets) rc = pack_lists(h, c);
   if (rc != FI_OK) return rc;
   dump_trace(h, c.R);
   h->stats.pick_calls++;
@@ -439,7 +465,8 @@ int fi_epp_hash_batch(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets
 // the argument checks of every pick call, before the handle is touched (FI_ERR_INVALID); the ranked entry points, which
 // take k >= 1, reject k == 0 themselves
 static bool bad_pick_args(const PickCall& c, bool host) {
-  return !c.offsets || (!c.h0 && c.R) || (!c.out && !c.counts && (c.R || c.k)) || c.k > FI_EPP_MAX_RANKED ||
+  return !c.offsets || (!c.h0 && c.R) || (!c.out && !c.counts && !c.list_offsets && (c.R || c.k)) || c.k > FI_EPP_MAX_RANKED ||
+         (c.cap && !c.entries) ||
          (c.k == 0 && c.subsets) || (host && !c.prompts && c.R && c.offsets[c.R]);
 }
 
@@ -450,11 +477,54 @@ static int check_pick_handle(fi_epp* h, const PickCall& c) {
   if (cudaSetDevice(h->cfg.device) != cudaSuccess) return fail(h, FI_ERR_CUDA, "cudaSetDevice failed");
   if (c.k && h->world > 1) return fail(h, FI_ERR_STATE, "ranked picks need a single-rank pool");
   if (c.counts && h->world > 1) return fail(h, FI_ERR_STATE, "match counts need a single-rank pool");
+  if (c.list_offsets && h->world > 1) return fail(h, FI_ERR_STATE, "match lists need a single-rank pool");
   if (c.subsets) {
     const int rc = check_whole_pool(h, "a subset pick");
     if (rc != FI_OK) return rc;
   }
   if (c.R > h->cfg.max_batch) return fail(h, FI_ERR_CAPACITY, "batch larger than max_batch");
+  return FI_OK;
+}
+
+// The list scratch for max_batch requests of the pool as it is, its slots and counts together or neither (the first
+// lists call, and the first after a resize); a scratch in use by queued work is replaced only after s_main drains.
+static int alloc_list_scratch(fi_epp* h) {
+  const size_t need = (size_t)h->cfg.max_batch * h->cfg.endpoint_count;
+  if (h->lists.slots && need <= h->lists.cap) return FI_OK;
+  FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
+  h->lists = fi_epp::ListScratch{};
+  fi_epp::ListScratch t;
+  cudaError_t e = cuda_alloc(t.slots, need);
+  if (e == cudaSuccess) e = cuda_alloc(t.nnz, h->cfg.max_batch);
+  if (e != cudaSuccess) {
+    alloc_status(e);
+    return fail(h, FI_ERR_NOMEM, "cannot allocate the match-list scratch of " + std::to_string(need * 4) + " bytes");
+  }
+  t.cap = need;
+  h->lists = std::move(t);
+  return FI_OK;
+}
+
+// The host lists call after its offsets have arrived: the first min(total, cap) entries, at most kListChunk per copy
+// through list_chunk; FI_ERR_CAPACITY when the total exceeds cap.
+static int copy_out_lists(fi_epp* h, const PickCall& c) {
+  const uint64_t total = c.list_offsets[c.R], n = std::min(total, c.cap);
+  for (uint64_t lo = 0; lo < n; lo += kListChunk) {
+    const uint64_t hi = std::min(n, lo + kListChunk);
+    int rc = grow_staging(h, h->list_chunk, hi - lo, std::min(n, kListChunk), true);
+    if (rc != FI_OK) return rc;
+    {
+      LaunchScope ls(h, h->s_main.get(), K_OTHER);
+      FI_CUDA(launch_list_copy(h->lists.slots.get(), h->cfg.endpoint_count, h->list_offsets.d.get(), c.R,
+                               h->cfg.endpoint_begin, lo, hi, h->list_chunk.d.get(), h->s_main.get()));
+    }
+    const size_t bytes = (size_t)(hi - lo) * sizeof(fi_match_entry);
+    FI_CUDA(cudaMemcpyAsync(h->list_chunk.h.get(), h->list_chunk.d.get(), bytes, cudaMemcpyDeviceToHost, h->s_main.get()));
+    h->stats.d2h_bytes += bytes;
+    FI_CUDA(cudaStreamSynchronize(h->s_main.get()));
+    std::memcpy(c.entries + lo, h->list_chunk.h.get(), bytes);
+  }
+  if (total > c.cap) return fail(h, FI_ERR_CAPACITY, "match lists: " + std::to_string(total) + " entries, cap " + std::to_string(c.cap));
   return FI_OK;
 }
 
@@ -489,6 +559,13 @@ static int pick_host(fi_epp* h, const PickCall& c) {
     d.out = nullptr;
     d.counts = h->counts.d.get();
   }
+  if (c.list_offsets) {  // the offsets come back here; the entries after them, once their total is known
+    rc = alloc_list_scratch(h);
+    if (rc == FI_OK) rc = grow_staging(h, h->list_offsets, (size_t)h->cfg.max_batch + 1, (size_t)h->cfg.max_batch + 1, true);
+    if (rc != FI_OK) return rc;
+    d.out = nullptr;
+    d.list_offsets = h->list_offsets.d.get();
+  }
   rc = stage_inputs(h, c.prompts, c.offsets, c.h0, R, total, /*copy_prompts=*/false);
   if (rc != FI_OK) return rc;
   if (c.adapters) {
@@ -518,6 +595,11 @@ static int pick_host(fi_epp* h, const PickCall& c) {
     d_res = d.counts;
     pb = (size_t)R * h->cfg.endpoint_count * sizeof(uint16_t);
   }
+  if (c.list_offsets) {
+    h_res = h->list_offsets.h.get();
+    d_res = d.list_offsets;
+    pb = (size_t)(R + 1) * sizeof(uint64_t);
+  }
   FI_CUDA(cudaMemcpyAsync(h_res, d_res, pb, cudaMemcpyDeviceToHost, h->s_main.get()));
   h->stats.d2h_bytes += pb;
   rc = copy_chains_out(h, h->d_chain.get(), c.chains_out, R, cudaMemcpyDeviceToHost, h->s_main.get());
@@ -532,8 +614,9 @@ static int pick_host(fi_epp* h, const PickCall& c) {
     *xerr = 0;
     return fail(h, FI_ERR_COMM, "peer exchange timed out waiting for another rank");
   }
-  std::memcpy(c.counts ? (void*)c.counts : (void*)c.out, h_res, pb);
+  std::memcpy(c.list_offsets ? (void*)c.list_offsets : c.counts ? (void*)c.counts : (void*)c.out, h_res, pb);
   if (c.nblocks_out) std::memcpy(c.nblocks_out, h->h_nblocks.get(), (size_t)R * sizeof(uint32_t));
+  if (c.list_offsets) return copy_out_lists(h, c);
   return FI_OK;
 }
 
@@ -545,6 +628,10 @@ static int pick_device(fi_epp* h, const PickCall& c, void* stream) {
   int rc = check_pick_handle(h, c);
   if (rc != FI_OK || c.R == 0) return rc;
   cudaStream_t us = (cudaStream_t)stream;
+  if (c.list_offsets) {
+    rc = alloc_list_scratch(h);
+    if (rc != FI_OK) return rc;
+  }
   FI_CUDA(cudaEventRecord(h->ev_user.get(), us));
   FI_CUDA(cudaStreamWaitEvent(h->s_main.get(), h->ev_user.get(), 0));
   rc = run_pick(h, c, nullptr);
@@ -650,6 +737,34 @@ int fi_epp_match_counts_device(fi_epp* h, const void* d_prompts, const void* d_o
   c.counts = (uint16_t*)d_counts;
   c.nblocks_out = (uint32_t*)d_nblocks_out;
   return pick_device(h, c, stream);
+}
+
+int fi_epp_match_lists(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
+                       uint64_t* list_offsets, fi_match_entry* entries, uint64_t cap, uint32_t* nblocks_out,
+                       uint64_t* chains_out) {
+  if (!list_offsets && R) return FI_ERR_INVALID;
+  PickCall c{prompts, offsets, h0, nullptr, nullptr, R, 0, nullptr, chains_out, nullptr, nblocks_out};
+  c.list_offsets = list_offsets;
+  c.entries = entries;
+  c.cap = cap;
+  const int rc = pick_host(h, c);
+  if (rc == FI_OK && R == 0 && list_offsets) list_offsets[0] = 0;
+  return rc;
+}
+
+int fi_epp_match_lists_device(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
+                              uint64_t total_prompt_bytes, void* d_list_offsets, void* d_entries, uint64_t cap,
+                              void* d_nblocks_out, void* d_chains_out, void* stream) {
+  if (!d_list_offsets && R) return FI_ERR_INVALID;
+  PickCall c = device_call(d_prompts, d_offsets, d_h0, nullptr, nullptr, R, 0, nullptr, d_chains_out);
+  c.nblocks_out = (uint32_t*)d_nblocks_out;
+  c.list_offsets = (uint64_t*)d_list_offsets;
+  c.entries = (fi_match_entry*)d_entries;
+  c.cap = cap;
+  const int rc = pick_device(h, c, stream);
+  if (rc == FI_OK && R == 0 && d_list_offsets && cudaMemsetAsync(d_list_offsets, 0, sizeof(uint64_t), (cudaStream_t)stream) != cudaSuccess)
+    return fail(h, FI_ERR_CUDA, std::string("cudaMemsetAsync: ") + cudaGetErrorString(cudaGetLastError()));
+  return rc;
 }
 
 int fi_epp_pick_submit(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,

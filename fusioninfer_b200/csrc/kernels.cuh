@@ -174,6 +174,11 @@ struct MatchParams {
   // the handle's max_blocks (appended like the fields above): above 1023 a count needs more than the 10 bit-planes of
   // one match window, and launch_match_pick runs the windowed variant (DESIGN.md §4.9)
   uint32_t max_blocks;
+  // match lists (docs/SPEC.md S.3b), appended like the fields above: non-null selects the LISTS variant, which writes
+  // request r's matched local endpoints as (column << 12) | count into lists[r * ep_count ..] and their number into
+  // nnz[r] (counts is not read)
+  uint32_t* lists;  // [R][ep_count]
+  uint32_t* nnz;    // [R]
 };
 
 struct MergeParams {
@@ -267,5 +272,10 @@ cudaError_t launch_prepare_endpoints(const EndpointDev* eps, uint32_t E_global, 
 
 cudaError_t launch_match_pick(const MatchParams& p, int sm_count, cudaStream_t s);
 cudaError_t launch_merge_picks(const MergeParams& p, cudaStream_t s);
+// the pack step of match lists (S.3b): offsets[R + 1] = the exclusive scan of nnz[R] (one CTA); then the entries of
+// list positions [lo, hi) to out[position - lo], read from the slots lists[r * pitch ..] (one warp per request)
+cudaError_t launch_list_scan(const uint32_t* nnz, uint32_t R, uint64_t* offsets, cudaStream_t s);
+cudaError_t launch_list_copy(const uint32_t* lists, uint32_t pitch, const uint64_t* offsets, uint32_t R, uint32_t ep_begin,
+                             uint64_t lo, uint64_t hi, fi_match_entry* out, cudaStream_t s);
 
 }  // namespace fi

@@ -24,7 +24,9 @@
 //      MaxScorePicker shuffles, Appendix A.5), then the pd-profile-handler threshold rule (Appendix A.6,
 //      /root/reference/pkg/router/strategy.go:129-133).
 //   The COUNTS variant (fi_epp_match_counts, docs/SPEC.md S.3a) replaces 4./5. with counts_row: every local endpoint's
-//   match count, written as the request's row of a dense [R][ep_count] u16 matrix.
+//   match count, written as the request's row of a dense [R][ep_count] u16 matrix.  Its LISTS form (fi_epp_match_lists,
+//   S.3b) writes only the matched endpoints, into the request's slot of a scratch that list_scan_kernel and
+//   list_copy_kernel then pack.
 //
 // Rows narrower than 32 words (fewer than 1024 local endpoints, e.g. an
 // endpoint-range shard of a multi-GPU pool) are read G = 32/L rows per load
@@ -428,6 +430,57 @@ __device__ __forceinline__ void counts_row(const MatchParams& p, const BitCounte
   }
 }
 
+// docs/SPEC.md S.3b, the epilogue of the LISTS variant (a COUNTS variant that writes lists instead of rows): request
+// r's matched local endpoints, ascending, packed as (column << 12) | count into its slot p.lists[r * ep_count ..], and
+// their number into p.nnz[r].  No dense row is staged.  After the merge every lane group holds the full counters, so
+// group g takes bits [g*32/G, (g+1)*32/G) of its lanes' words (as counts_row does) and unpacks only the matched ones.
+// An entry's position in the slot is the number of matched endpoints before it: those of the group's lanes before this
+// one (an inclusive shuffle scan over the LPR lanes of the group, which every group computes alike), of this lane's
+// words before x, and of the bits of word x below the group's range.  The slot index is the request's, so the result
+// does not depend on the order in which the dynamic queue finishes requests.
+template <int VEC, int G, int NP>
+__device__ __forceinline__ void lists_slot(const MatchParams& p, const BitCounter<NP> (&cnt)[VEC], uint32_t r, bool nothing,
+                                           int lane, int t, int g) {
+  constexpr int LPR = 32 / G;
+  constexpr uint32_t BPG = 32 / G;
+  if (!nothing) {  // warp-uniform
+    // a word's matched endpoints: its non-zero counters below ep_count (rows hold no bits past it)
+    auto matched = [&](int x) {
+      const uint32_t e0 = (uint32_t)(t * VEC + x) * 32u;
+      const uint32_t lim = p.ep_count > e0 ? p.ep_count - e0 : 0u;
+      return bc_nonzero(cnt[x]) & (lim >= 32 ? 0xFFFFFFFFu : ((1u << lim) - 1u));
+    };
+    uint32_t mine = 0;
+#pragma unroll
+    for (int x = 0; x < VEC; ++x) mine += __popc(matched(x));
+    uint32_t incl = mine;
+#pragma unroll
+    for (int d = 1; d < LPR; d <<= 1) {
+      const uint32_t o = __shfl_up_sync(FULL, incl, d, LPR);
+      if (t >= d) incl += o;
+    }
+    const uint32_t total = __shfl_sync(FULL, incl, LPR - 1, LPR);
+    if (lane == 0) p.nnz[r] = total;
+    // (32-bit positions within the slot, indexed from the parameter at each store: no 64-bit pointer stays live)
+    uint32_t pos = incl - mine;
+    const uint32_t gmask = (BPG >= 32 ? 0xFFFFFFFFu : ((1u << BPG) - 1u)) << (g * BPG);
+    const uint32_t below = (1u << (g * BPG)) - 1u;  // g * BPG < 32
+#pragma unroll
+    for (int x = 0; x < VEC; ++x) {
+      const uint32_t nz = matched(x);
+      const uint32_t e0 = (uint32_t)(t * VEC + x) * 32u;
+      uint32_t at = pos + __popc(nz & below);
+      for (uint32_t cand = nz & gmask; cand; cand &= cand - 1) {
+        const uint32_t bit = __ffs(cand) - 1;
+        p.lists[(uint64_t)r * p.ep_count + at++] = ((e0 + bit) << 12) | bc_get(cnt[x], bit);
+      }
+      pos += __popc(nz);
+    }
+  } else if (lane == 0) {
+    p.nnz[r] = 0;
+  }
+}
+
 // LPR lanes read one row (VEC words each, LPR*VEC = words per row); a load
 // instruction therefore covers G = 32/LPR rows.  E = 1024 → LPR 16, VEC 2: a 128-byte
 // row is 16 × 8-byte loads and one instruction brings in 2 rows; 16 rows in flight.
@@ -438,9 +491,11 @@ __device__ __forceinline__ void counts_row(const MatchParams& p, const BitCounte
 // arrive under the walk; only the scoring of ranked_profile uses them.
 // COUNTS (not with LORA / RANKED): steps 1-3 as for a pick, then counts_row writes the request's match counts instead
 // of steps 4-5 and the PD rule.  Its staging rows follow the node buffers in shared memory, Epad + 16 counts per warp.
+// LISTS (with COUNTS only): lists_slot writes the request's matched endpoints instead of counts_row's dense row; no
+// staging row.
 // WIN (match_window_kernel, handles with max_blocks > 1023; DESIGN.md §4.9): steps 1-3 run once per window of up to
 // kWindow blocks, in staging buffers of kWindow entries, and the counters have 12 bit-planes; steps 4-5 are the same.
-template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET, bool COUNTS, bool WIN>
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET, bool COUNTS, bool LISTS, bool WIN>
 __device__ __forceinline__ void match_pick_body(const MatchParams& p) {
   constexpr int G = 32 / LPR;                 // rows per load instruction
   constexpr int NP = WIN ? kWindowPlanes : NPLANES;
@@ -462,7 +517,7 @@ __device__ __forceinline__ void match_pick_body(const MatchParams& p) {
   uint64_t* const s_chain_base = s_mem + (size_t)(2 * warp) * SP;  // buffer b at s_chain_base + b * SP
   uint32_t* s_node = reinterpret_cast<uint32_t*>(s_mem + (size_t)2 * kWarps * SP) + (size_t)warp * SP;  // node of every block
   uint16_t* s_row = nullptr;  // COUNTS: the warp's staging row
-  if constexpr (COUNTS)
+  if constexpr (COUNTS && !LISTS)
     s_row = reinterpret_cast<uint16_t*>(s_mem + (size_t)2 * kWarps * SP) + (size_t)2 * kWarps * SP +
             (size_t)warp * (p.st.Epad + 16);
   const IndexView ix = p.ix;
@@ -533,6 +588,13 @@ __device__ __forceinline__ void match_pick_body(const MatchParams& p) {
       } else if (emp) {
         have_first = true;  // definite miss
       }  // else: home bucket full without a match — resolve_request_nodes probes on
+    }
+    if constexpr (LISTS) {
+      // The bucket is read: end its registers' live range here.  Assigned only when a bucket is fetched, they would
+      // otherwise stay live around the whole request for the requests that fetch none, which made
+      // match_window_kernel<16, 2, upstream, .., LISTS> spill pf_node under its 80-register bound.
+      pf_key = 0;
+      pf_node = 0;
     }
 
 #ifdef FI_MATCH_TIMING
@@ -748,7 +810,8 @@ __device__ __forceinline__ void match_pick_body(const MatchParams& p) {
         }
       }
     }
-    if constexpr (COUNTS) counts_row<VEC, G, NP>(p, cnt, r, nothing, s_row, lane, t, g);
+    if constexpr (COUNTS && LISTS) lists_slot<VEC, G, NP>(p, cnt, r, nothing, lane, t, g);
+    else if constexpr (COUNTS) counts_row<VEC, G, NP>(p, cnt, r, nothing, s_row, lane, t, g);
 
     // ---- 4./5. score candidates, argmax, PD rule ---------------------------------
     TieRot tr;
@@ -912,18 +975,18 @@ __device__ __forceinline__ void match_pick_body(const MatchParams& p) {
 
 #undef SP
 
-template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false, bool LISTS = false>
 __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MIN_BLOCKS : FI_MATCH_MIN_BLOCKS + 1))
     match_pick_kernel(const MatchParams p) {
-  match_pick_body<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS, false>(p);
+  match_pick_body<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS, LISTS, false>(p);
 }
 
 // chains longer than one window (max_blocks > 1023): the same CTA shape, warps and shared memory per warp as
 // match_pick_kernel at MP = kWindow
-template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
+template <int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false, bool LISTS = false>
 __global__ void __launch_bounds__(kWarps * 32, (VEC >= 4 || RANKED ? FI_MATCH_MIN_BLOCKS : FI_MATCH_MIN_BLOCKS + 1))
     match_window_kernel(const MatchParams p) {
-  match_pick_body<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS, true>(p);
+  match_pick_body<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS, LISTS, true>(p);
 }
 
 // multi-GPU: reduce the ranks' local picks (score desc, then the request's tie rotation), then the PD rule
@@ -1103,13 +1166,14 @@ std::mutex g_match_launch_mu;
 
 // One instantiation per kernel variant: the shared-memory opt-in (cudaFuncSetAttribute) applies to one function
 // only, and occupancy differs between variants, so each variant keeps its own state, per device.
-template <bool WIN, int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false>
+template <bool WIN, int LPR, int VEC, bool LPM, bool LORA, bool RANKED, bool SUBSET = false, bool COUNTS = false,
+          bool LISTS = false>
 cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_t s) {
-  const auto kern = WIN ? match_window_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS>
-                        : match_pick_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS>;
+  const auto kern = WIN ? match_window_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS, LISTS>
+                        : match_pick_kernel<LPR, VEC, LPM, LORA, RANKED, SUBSET, COUNTS, LISTS>;
   const size_t sp = WIN ? (size_t)kWindow : p.MP;  // entries per staging buffer
   size_t smem = (size_t)kWarps * sp * (2 * sizeof(uint64_t) + sizeof(uint32_t));  // 2 chain buffers + nodes
-  if (COUNTS) smem += (size_t)kWarps * (p.st.Epad + 16) * sizeof(uint16_t);        // + the staging rows
+  if (COUNTS && !LISTS) smem += (size_t)kWarps * (p.st.Epad + 16) * sizeof(uint16_t);  // + the staging rows
   static std::map<int, size_t> opted_in;                // device -> the variant's max dynamic smem attribute
   static std::map<std::pair<int, size_t>, int> per_sm;  // (device, smem) -> resident CTAs per SM
   int dev = 0;
@@ -1148,6 +1212,9 @@ cudaError_t launch_match_variant(const MatchParams& p, int sm_count, cudaStream_
 template <int LPR, int VEC, bool WIN>
 cudaError_t launch_match_t(const MatchParams& p, int sm_count, cudaStream_t s) {
   const bool lpm = p.lpm == FI_MATCH_LPM;
+  if (p.lists)  // match lists (S.3b): the counts' walk, the lists' epilogue
+    return lpm ? launch_match_variant<WIN, LPR, VEC, true, false, false, false, true, true>(p, sm_count, s)
+               : launch_match_variant<WIN, LPR, VEC, false, false, false, false, true, true>(p, sm_count, s);
   if (p.counts)  // match counts (S.3a): no profile is scored
     return lpm ? launch_match_variant<WIN, LPR, VEC, true, false, false, false, true>(p, sm_count, s)
                : launch_match_variant<WIN, LPR, VEC, false, false, false, false, true>(p, sm_count, s);
@@ -1196,6 +1263,102 @@ cudaError_t launch_match_pick(const MatchParams& p, int sm_count, cudaStream_t s
 cudaError_t launch_merge_picks(const MergeParams& p, cudaStream_t s) {
   if (p.R == 0) return cudaSuccess;
   merge_picks_kernel<<<(p.R + 255) / 256, 256, 0, s>>>(p);
+  return cudaGetLastError();
+}
+
+namespace {
+
+// ---- the pack step of match lists (docs/SPEC.md S.3b), on the stream of the match launches it follows ------------------
+// offsets[0] = 0, offsets[r + 1] = offsets[r] + nnz[r] in u64.  One CTA walks the requests in tiles of kScanPer per
+// thread (16 384 requests per tile: one tile at cfg 3): each thread reads its kScanPer consecutive counts with 16-byte
+// loads, all issued before any is used, a two-level shuffle scan over the CTA gives each thread its base, and each
+// thread writes its run of offsets (nnz is 16-byte aligned).
+constexpr int kScanPer = 16;
+__global__ void __launch_bounds__(1024) list_scan_kernel(const uint32_t* __restrict__ nnz, uint32_t R,
+                                                         uint64_t* __restrict__ offsets) {
+  __shared__ uint64_t s_warp[32];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  uint64_t carry = 0;
+  if (tid == 0) offsets[0] = 0;
+  for (uint32_t base = 0; base < R; base += kScanPer * blockDim.x) {
+    const uint32_t r = base + kScanPer * tid;
+    uint32_t v[kScanPer];
+#pragma unroll
+    for (int q = 0; q < kScanPer; q += 4) {
+      if (r + q + 3 < R) {
+        const uint4 w = *reinterpret_cast<const uint4*>(nnz + r + q);
+        v[q] = w.x;
+        v[q + 1] = w.y;
+        v[q + 2] = w.z;
+        v[q + 3] = w.w;
+      } else {
+#pragma unroll
+        for (int i = 0; i < 4; ++i) v[q + i] = r + q + i < R ? nnz[r + q + i] : 0u;
+      }
+    }
+    uint64_t sum = 0;
+#pragma unroll
+    for (int i = 0; i < kScanPer; ++i) sum += v[i];
+    uint64_t x = sum;  // inclusive scan over the warp
+#pragma unroll
+    for (int d = 1; d < 32; d <<= 1) {
+      const uint64_t o = __shfl_up_sync(FULL, x, d);
+      if ((int)lane >= d) x += o;
+    }
+    if (lane == 31) s_warp[warp] = x;
+    __syncthreads();
+    if (warp == 0) {
+      uint64_t w = lane < (blockDim.x >> 5) ? s_warp[lane] : 0;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const uint64_t o = __shfl_up_sync(FULL, w, d);
+        if ((int)lane >= d) w += o;
+      }
+      s_warp[lane] = w;
+    }
+    __syncthreads();
+    uint64_t at = carry + (warp ? s_warp[warp - 1] : 0) + x - sum;
+#pragma unroll
+    for (int i = 0; i < kScanPer; ++i) {
+      at += v[i];
+      if (r + i < R) offsets[r + i + 1] = at;
+    }
+    carry += s_warp[31];
+    __syncthreads();  // s_warp is read above before the next tile writes it
+  }
+}
+
+// One warp per request: the entries of its slot at list positions [offsets[r], offsets[r + 1]) within [lo, hi) go to
+// out[position - lo], widened to fi_match_entry with the global endpoint.  Positions past hi are not written.
+__global__ void __launch_bounds__(256) list_copy_kernel(const uint32_t* __restrict__ lists, uint32_t pitch,
+                                                        const uint64_t* __restrict__ offsets, uint32_t R, uint32_t ep_begin,
+                                                        uint64_t lo, uint64_t hi, fi_match_entry* __restrict__ out) {
+  const uint32_t r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (r >= R) return;
+  const uint64_t a = offsets[r], b = offsets[r + 1];
+  const uint64_t e = b < hi ? b : hi;
+  const uint32_t* src = lists + (uint64_t)r * pitch;
+  for (uint64_t pos = (a > lo ? a : lo) + lane; pos < e; pos += 32) {
+    const uint32_t v = src[pos - a];
+    fi_match_entry m;
+    m.endpoint = ep_begin + (v >> 12);
+    m.match_blocks = (uint16_t)(v & 0xFFFu);
+    m.reserved = 0;
+    out[pos - lo] = m;
+  }
+}
+
+}  // namespace
+
+cudaError_t launch_list_scan(const uint32_t* nnz, uint32_t R, uint64_t* offsets, cudaStream_t s) {
+  list_scan_kernel<<<1, 1024, 0, s>>>(nnz, R, offsets);
+  return cudaGetLastError();
+}
+
+cudaError_t launch_list_copy(const uint32_t* lists, uint32_t pitch, const uint64_t* offsets, uint32_t R, uint32_t ep_begin,
+                             uint64_t lo, uint64_t hi, fi_match_entry* out, cudaStream_t s) {
+  if (R == 0 || hi <= lo) return cudaSuccess;
+  list_copy_kernel<<<(R + 7) / 8, 256, 0, s>>>(lists, pitch, offsets, R, ep_begin, lo, hi, out);
   return cudaGetLastError();
 }
 

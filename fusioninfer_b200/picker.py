@@ -460,6 +460,38 @@ class EndpointPicker:
             "fi_epp_match_counts_device",
         )
 
+    def match_lists(self, prompts, offsets, h0, cap=None, want_chains: bool = False):
+        """match_counts as sparse per-request lists (docs/SPEC.md S.3b): only the endpoints that match.
+        -> (list_offsets uint64 [R + 1], entries [list_offsets[R]] (match_entry_dtype: global endpoint, match_blocks),
+        nblocks uint32 [R][, chains]); request r's entries are entries[list_offsets[r]:list_offsets[r + 1]], in
+        ascending endpoint order.  cap (entries): None allows every list (R * endpoint_count); a smaller cap that falls
+        short raises FiEppError with status FI_ERR_CAPACITY."""
+        prompts, offsets, h0, R = self._inputs(prompts, offsets, h0)
+        if cap is None:
+            cap = R * int(self.cfg.endpoint_count)
+        loff = np.zeros(R + 1, dtype=np.uint64)
+        entries = np.zeros(int(cap), dtype=abi.match_entry_dtype())
+        nb = np.zeros(R, dtype=np.uint32)
+        chains = np.zeros((R, self.max_blocks), dtype=np.uint64) if want_chains else None
+        self._check(self._lib.fi_epp_match_lists(self._h, _ptr(prompts), _ptr(offsets), _ptr(h0), R, _ptr(loff),
+                                                 _ptr(entries) if cap else None, int(cap), _ptr(nb), _ptr(chains)),
+                    "fi_epp_match_lists")
+        out = (loff, entries[: int(loff[R])].copy(), nb)
+        return out + (chains,) if want_chains else out
+
+    def match_lists_device(self, d_prompts: int, d_offsets: int, d_h0: int, R: int, total_bytes: int,
+                           d_list_offsets: int, d_entries: int, cap: int, d_nblocks: int = 0, d_chains: int = 0,
+                           stream: int = 0):
+        """match_lists on device buffers: d_list_offsets holds R + 1 uint64, d_entries cap fi_match_entry (4-byte
+        aligned), d_nblocks R uint32 (optional), d_chains R * max_blocks hashes (optional).  A cap that falls short is
+        not an error here: compare list_offsets[R] with cap once the stream has run."""
+        self._check(
+            self._lib.fi_epp_match_lists_device(self._h, d_prompts, d_offsets, d_h0, R, total_bytes, d_list_offsets,
+                                                d_entries or None, int(cap), d_nblocks or None, d_chains or None,
+                                                stream or None),
+            "fi_epp_match_lists_device",
+        )
+
     def pick_batch_raw(self, prompts_ptr: int, offsets_ptr: int, h0_ptr: int, R: int, out_ptr: int, chains_ptr: int = 0):
         """Host-pointer variant without numpy marshalling (pinned buffers from pinned_alloc)."""
         self._check(

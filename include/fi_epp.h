@@ -206,6 +206,13 @@ typedef struct fi_pick {
   double score;          /* weighted fp64 total of the picked endpoint */
 } fi_pick;
 
+/* One matched endpoint of a request's match list (fi_epp_match_lists, 8 bytes). */
+typedef struct fi_match_entry {
+  uint32_t endpoint;     /* global index */
+  uint16_t match_blocks; /* > 0 */
+  uint16_t reserved;     /* written as 0 */
+} fi_match_entry;
+
 typedef struct fi_index_stats {
   uint64_t slots;      /* key slots */
   uint64_t used;       /* slots holding a key or a tombstone */
@@ -535,6 +542,28 @@ int fi_epp_match_counts(fi_epp* h, const uint8_t* prompts, const uint64_t* offse
 int fi_epp_match_counts_device(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
                                uint64_t total_prompt_bytes, void* d_counts, void* d_nblocks_out, void* d_chains_out,
                                void* stream);
+
+/* Match lists (docs/SPEC.md S.3b): fi_epp_match_counts as one sparse list per request, for the same host-side plugins.
+ * Request r's list holds (endpoint_begin + j, counts[r][j]) for every j with counts[r][j] > 0, in ascending endpoint
+ * order, where counts is the matrix fi_epp_match_counts would return at the same point of the call order: upstream's
+ * map of the pods that matched.  list_offsets [R + 1]: list_offsets[0] = 0 and request r's entries are
+ * entries[list_offsets[r] .. list_offsets[r + 1]).  list_offsets is always written in full; only entries at positions
+ * below cap are written, and cap = R * endpoint_count never falls short.  nblocks_out and chains_out (optional),
+ * ordering, statistics, chains, partial-pool handles and the errors are fi_epp_match_counts': FI_ERR_INVALID also for
+ * NULL list_offsets with R > 0 or NULL entries with cap > 0.  The host call returns FI_ERR_CAPACITY when
+ * list_offsets[R] > cap, having written everything else; it waits once more for the total, and copies the entries
+ * through bounded staging.  The lists run through a device scratch of max_batch * endpoint_count 4-byte slots and
+ * max_batch counts, allocated by the first lists call.  R = 0: FI_OK, and list_offsets[0] = 0 when list_offsets is
+ * not NULL.  Two calls on the same index state give identical bytes. */
+int fi_epp_match_lists(fi_epp* h, const uint8_t* prompts, const uint64_t* offsets, const uint64_t* h0, uint32_t R,
+                       uint64_t* list_offsets, fi_match_entry* entries, uint64_t cap, uint32_t* nblocks_out,
+                       uint64_t* chains_out);
+/* The same on device buffers, in `stream` order like fi_epp_pick_batch_device: d_list_offsets [R + 1] u64, d_entries
+ * cap entries (4-byte aligned).  A cap that falls short still returns FI_OK, with entries at cap and beyond untouched:
+ * the caller compares list_offsets[R] with cap after the stream, and the call never blocks the host. */
+int fi_epp_match_lists_device(fi_epp* h, const void* d_prompts, const void* d_offsets, const void* d_h0, uint32_t R,
+                              uint64_t total_prompt_bytes, void* d_list_offsets, void* d_entries, uint64_t cap,
+                              void* d_nblocks_out, void* d_chains_out, void* stream);
 
 /* Pipelined device path.  fi_epp_pick_submit enqueues one batch exactly like fi_epp_pick_batch_device (inputs
  * ready in `stream` order at the call) but does NOT order `stream` behind the result: batch k+1's block
